@@ -25,10 +25,6 @@ sys.path.insert(0, ROOT)
 
 METRIC = "queries/sec at beam=15, 1k queries, 10M-token index; rank-kernel HBM GB/s"
 BEAM, MIN_LEN, MAX_LEN, LP = 15, 10, 10, 0.0          # SEALSearcher body defaults (retrieval.py:70-83)
-# dram__bytes_read.sum + dram__bytes_write.sum per launch of the fc1-shaped GEMM (M=15000, N=4096, K=1024) from
-# `ncu --set full` (profiles/r01_ncu_2cta_fc1_raw.csv); algorithmic bytes of that launch: A halves 61 MB + W halves
-# 17 MB + C halves 246 MB = 324 MB, of which the activations/weights mostly hit L2.
-TRAFFIC_PER_LAUNCH = {2: 438.3e6, 3: 290.8e6, 5: 296.5e6}      # 5: profiles/r02_c_ncu_2cta_fc1_raw.csv (86.5 MB read + 210.0 MB written)
 TOL = 1e-4                                             # BASELINE.json north_star: beam scores within 1e-4
 
 
@@ -38,11 +34,11 @@ def peaks():
             p = json.load(f)
         return float(p["hbm_gbs"]), float(p["bf16_tflops"]), float(p.get("bf16_tflops_sustained", p["bf16_tflops"])), "measured"
     except Exception:
-        return 6650.0, 1590.0, 1400.0, "fallback"
+        return 3350.0, 989.0, 989.0, "fallback (H100 SXM data sheet, 700 W)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -126,6 +122,32 @@ def decode_trace(rec, max_triples=1 << 22):
         if len(sym) >= max_triples:
             break
     return np.asarray(sym, dtype=np.int64), np.asarray(plo, dtype=np.int64), np.asarray(phi, dtype=np.int64)
+
+
+def dump_outputs(out_dir, full, limit=64 << 20):
+    """The hypothesis records of the last timed step, as the caller of the timed path receives them, one .npy per array.
+    A record slot that holds no hypothesis has score -inf; such slots are marked 0 in filled.npy and every field of
+    theirs (score included) is written as 0, as are the token positions past a hypothesis' length, so that all values
+    are finite and unused entries compare equal between builds.  Scores stay float32; integer fields are stored as float64, which holds token ids, lengths and
+    suffix-array rows (< 2^53) exactly.  Everything fits the 64 MB limit at 1 000 queries (~34 MB); above it a fixed,
+    seeded sample of the queries is written, their row numbers in query_index.npy."""
+    names = ("scores", "lens", "tokens", "valid", "lo", "hi")
+    arrs = {n: np.asarray(full[n]) for n in names}
+    filled = np.isfinite(arrs["scores"])
+    arrs["filled"] = filled
+    conv = {n: (np.float32 if a.dtype == np.float32 else np.float64) for n, a in arrs.items()}
+    Q = arrs["scores"].shape[0]
+    per_query = sum(a[:1].size * np.dtype(conv[n]).itemsize for n, a in arrs.items())
+    keep = np.arange(Q)
+    if Q * per_query > limit:
+        keep = np.sort(np.random.default_rng(0).choice(Q, size=max(1, limit // per_query - 1), replace=False))
+    os.makedirs(out_dir, exist_ok=True)
+    used = {"tokens": filled[..., None] & (np.arange(arrs["tokens"].shape[-1]) < arrs["lens"][..., None])}
+    for n, a in arrs.items():
+        out = np.where(used.get(n, filled)[keep], a[keep], 0).astype(conv[n])
+        assert np.isfinite(out).all(), n
+        np.save(os.path.join(out_dir, n + ".npy"), out)
+    np.save(os.path.join(out_dir, "query_index.npy"), keep.astype(np.float64))
 
 
 # ------------------------------------------------------------------------------------------------
@@ -220,6 +242,8 @@ def run_ours(args):
     full = merge_gathered(gathered, layout) if (world > 1 and rank == 0) else (rec.host() if world == 1 else None)
     errs = rec.host()["errors"] if Q else np.zeros(4, dtype=np.int32)
     assert not errs.any(), f"generate raised error flags {errs.tolist()} (include/sealdec.h)"
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, full)
 
     # ---- end to end through the public host-array API: H2D of the inputs, decode, the gather, D2H of the records ----
     e2e_steps = max(1, min(args.steps, 3))
@@ -283,18 +307,15 @@ def run_ours(args):
     gemm_s = prof["total_us"] * 1e-6
     passes = 3
     ach = prof["flops"] / gemm_s / 1e12
-    roof = {"bound": "tensor", "kernel": {2: "umma_gemm_tf32x3_persistent_kernel", 3: "umma_gemm_f16x3_persistent_kernel",
-                                          5: "umma_gemm_f16x3_2cta_kernel"}[args.gemm_mode],
+    roof = {"bound": "tensor", "kernel": "wgmma_gemm_x3_kernel",
             "achieved": ach, "peak": tf_sus, "unit": "TFLOP/s", "frac": ach / tf_sus,
-            "traffic": TRAFFIC_PER_LAUNCH.get(args.gemm_mode),
             "peak_source": f"MEASURED_PEAKS.json bf16_tflops_sustained ({which}; the kernel runs inside a long step)",
             "avg_launch_us": prof["total_us"] / max(prof["launches"], 1), "launches_per_step": prof["launches"],
             "share_of_step": gemm_s / (phases["total"] * 1e-6),
             "tensor_pipe_TFLOPs": ach * passes, "tensor_pipe_frac": ach * passes / tf_sus,
             "note": "achieved = algorithmic 2MNK flops (fp32-equivalent) of all GEMM launches of one step / their summed "
                     "CUDA-event durations; the kernel issues 3 half-precision tensor-core passes per product "
-                    "(error-compensated split, DESIGN.md section 4), so the tensor pipe itself runs at tensor_pipe_TFLOPs; "
-                    "traffic = dram bytes read+written per launch of the fc1-shaped GEMM (ncu, profiles/)"}
+                    "(error-compensated split, DESIGN.md section 4), so the tensor pipe itself runs at tensor_pipe_TFLOPs"}
     rank_kernel = rank_kernel_report(index, full, dev, hbm, phases, args)
     cpu = cpu_baseline_and_parity(args, full, q_lo) if world == 1 else None
     out = {"metric": METRIC, "value": value, "unit": "queries/s", "n_gpus": world, "steps": args.steps,
@@ -351,7 +372,7 @@ def rank_kernel_report(index, full, dev, hbm, phases, args):
     s1 = time_lf(index, sym, lo_t, hi_t)
     out = {"kernel": "lf_step_kernel", "bytes_per_lf_step": 48 * 16,
            "decode_trace_10M": {"triples": N1, "distinct_trace_triples": n_trace, "us": s1 * 1e6, "steps_per_s": N1 / s1,
-                                "algorithmic_GBps": N1 * 768 / s1 / 1e9, "bound": "L2 (27 MB index resident in the 126 MB L2; "
+                                "algorithmic_GBps": N1 * 768 / s1 / 1e9, "bound": "L2 (27 MB index resident in the 50 MB L2; "
                                 "not an HBM fraction)"},
            "note": "48*L B per LF step (SURVEY 8d); select+expand phase of the step: %.1f ms of %.1f ms"
                    % (phases["select_expand"] / 1e3, phases["total"] / 1e3)}
@@ -484,7 +505,7 @@ def cpu_baseline_and_parity(args, full, q_lo):
                 fm_index_generate_oracle(mg, idx, ids[:20].cuda(), mask[:20].cuda(), **kwb)
                 torch.cuda.synchronize(); dtg = time.perf_counter() - t1
                 gpu_eager = {"value": 20 / dtg, "unit": "queries/s", "batch": 20, "s_per_batch": dtg,
-                             "what": "reference algorithm (oracle decode loop) with eager fp32 HF BART + KV cache on this B200, "
+                             "what": "reference algorithm (oracle decode loop) with eager fp32 HF BART + KV cache on this GPU, "
                                      "sdsl-lite FM-index on the host cores"}
                 del mg
             except Exception as ex:  # pragma: no cover
@@ -542,11 +563,13 @@ def main():
     ap.add_argument("--regime", default="random", choices=["random", "freq"],
                     help="freq: final_logits_bias = log unigram frequency, beams follow frequent continuations (SURVEY 8d)")
     ap.add_argument("--ref-queries", type=int, default=8, help="queries per step of the CPU reference sample / parity check")
-    ap.add_argument("--gemm-mode", type=int, default=int(os.environ.get("SEALB200_GEMM", "5")))
+    ap.add_argument("--gemm-mode", type=int, default=int(os.environ.get("SEALB200_GEMM", "3")))
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-big-index", action="store_true")
     ap.add_argument("--no-gpu-eager-baseline", action="store_true")
     ap.add_argument("--big-index-tokens", type=int, default=200_000_000)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the hypothesis records of the last timed step to DIR/<name>.npy (float32 / float64)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

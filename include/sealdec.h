@@ -1,4 +1,4 @@
-/* sealdec.h — C ABI of the B200-native constrained beam-search decode for SEAL.
+/* sealdec.h — C ABI of the H100-native constrained beam-search decode for SEAL.
  *
  * Replaces, behind the reference's own Python surface (seal_b200/beam_search.py mirrors
  * /root/reference/seal/beam_search.py), the per-step work of
@@ -56,7 +56,7 @@ typedef struct {
     int32_t ffn_dim;           /* 4096                                         */
     int32_t max_positions;     /* 1024 (+2 learned offset)                     */
     int32_t scale_embedding;   /* 0 for bart-large                             */
-    int32_t gemm_mode;         /* 5 = 3xFP16 on CTA pairs (cta_group::2, 256x256 tiles; mode 3's kernel with split-K for small problems; default), 3 = 3xFP16, one CTA per 128x256 tile, 2 = 3xTF32 (fp32 range).  All tcgen05 + TMA + TMEM. */
+    int32_t gemm_mode;         /* 3 = 3xFP16, one CTA per 128x128 tile (split-K for small problems; default), 5 = 3xFP16 in clusters of 2 CTAs sharing the W tile (TMA multicast), 2 = 3xTF32 (fp32 range).  All wgmma + TMA. */
 } sealbart_config_t;
 
 int  sealbart_create(const sealbart_config_t* cfg, int device, sealbart_t** out);

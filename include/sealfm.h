@@ -1,4 +1,4 @@
-/* sealfm.h — C ABI of the B200-native FM-index for SEAL's constrained decoding.
+/* sealfm.h — C ABI of the H100-native FM-index for SEAL's constrained decoding.
  *
  * This is the drop-in boundary for the reference's native module `seal.cpp_modules.fm_index`
  * (SWIG wrapper over class FMIndex, /root/reference/seal/cpp_modules/fm_index.hpp:20-45,

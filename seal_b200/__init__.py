@@ -1,7 +1,7 @@
-"""seal_b200 — B200-native constrained beam-search decode for SEAL.
+"""seal_b200 — H100-native constrained beam-search decode for SEAL.
 
 Mirrors ``seal/__init__.py:7-9`` for the hot path: ``FMIndex``, ``fm_index_generate``,
-``IndexBasedLogitsProcessor``.  Touching any of them loads libsealb200.so (CUDA, sm_100a); there is no CPU
+``IndexBasedLogitsProcessor``.  Touching any of them loads libsealb200.so (CUDA, sm_90a); there is no CPU
 fallback.  The names are resolved lazily (PEP 562) so that the pure-numpy helpers (``seal_b200.synthetic``,
 ``seal_b200.sharding``'s layout code) can be imported by tooling — e.g. the CPU reference arm of ``bench.py`` —
 without mapping the CUDA library into that process.

@@ -1,4 +1,4 @@
-"""Drop-in for ``seal.beam_search`` (/root/reference/seal/beam_search.py) on the B200 kernels.
+"""Drop-in for ``seal.beam_search`` (/root/reference/seal/beam_search.py) on the H100 kernels.
 
 * ``IndexBasedLogitsProcessor`` — same constructor, attributes and HF ``LogitsProcessor`` protocol
   (``__call__(input_ids, scores) -> scores + mask``, beam_search.py:33-140); the FM-index work and
@@ -95,10 +95,10 @@ class SealBartEngine:
     """Device-resident BART weights + workspace (include/sealdec.h `sealbart_t`)."""
 
     def __init__(self, state_dict, config, device=0, gemm_mode=None):
-        # gemm_mode: 5 = 3xFP16 on CTA pairs (cta_group::2; default; small problems use mode 3's split-K kernel), 3 = 3xFP16 with
-        # one CTA per tile, 2 = 3xTF32 (fp32 range, the automatic fallback on fp16 overflow).  $SEALB200_GEMM overrides the default.
+        # gemm_mode: 3 = 3xFP16 with one CTA per tile (default), 5 = 3xFP16 in 2-CTA clusters sharing the W tile, 2 = 3xTF32
+        # (fp32 range, the automatic fallback on fp16 overflow).  $SEALB200_GEMM overrides the default.
         if gemm_mode is None:
-            gemm_mode = int(os.environ.get("SEALB200_GEMM", "5"))
+            gemm_mode = int(os.environ.get("SEALB200_GEMM", "3"))
         self.gemm_mode = int(gemm_mode)
         d = int(config.d_model)
         self.config = config

@@ -1,6 +1,6 @@
 """`seal_b200.compat.install()` registers this package under the reference's module names so that
 unmodified SEAL callers (`from seal.index import FMIndex`, `from seal.beam_search import
-fm_index_generate`, `from seal.cpp_modules.fm_index import load_FMIndex`) resolve to the B200 path.
+fm_index_generate`, `from seal.cpp_modules.fm_index import load_FMIndex`) resolve to the H100 path.
 See INTEGRATION.md."""
 import sys
 import types

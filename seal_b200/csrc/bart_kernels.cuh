@@ -25,7 +25,7 @@ __device__ __forceinline__ float warp_max(float v) {
     return v;
 }
 
-// TF32 split used by the tcgen05 GEMM (umma_gemm.cuh): hi keeps sign/exponent/10 mantissa bits,
+// TF32 split used by the 3xTF32 GEMM (wgmma_gemm.cuh): hi keeps sign/exponent/10 mantissa bits,
 // lo = x - hi exactly.  Producers write the split directly so no separate pass is needed.
 __device__ __forceinline__ void split1(float x, float& h, float& l) {
     h = __uint_as_float(__float_as_uint(x) & 0xFFFFE000u);
@@ -40,7 +40,7 @@ __device__ __forceinline__ void split4(const float4& v, float4& h, float4& l) {
 struct SplitOut { void* a = nullptr; void* b = nullptr; int kind = 0; int* overflow = nullptr; };
 
 // A GEMM output that may still be in split-K form: ks > 1 -> value = (sum_s part[s * stride + off]) * unscale + bias[col],
-// the slices summed in index order exactly like umma_splitk_finish_kernel; ks <= 1 -> plain[off].  Lets the consumer of a
+// the slices summed in index order exactly like gemm_splitk_finish_kernel; ks <= 1 -> plain[off].  Lets the consumer of a
 // small-batch GEMM (add+LN, the attention kernels) do the finish pass itself instead of a separate launch.
 struct SplitSrc { const float* part = nullptr; int ks = 0; int64_t stride = 0; const float* bias = nullptr; float unscale = 1.f; };
 __device__ __forceinline__ float4 load_split4(const float* __restrict__ plain, const SplitSrc& ss, int64_t off, int col) {
@@ -167,8 +167,8 @@ __global__ void __launch_bounds__(128) embed_ln_kernel(int64_t rows, int d, cons
 }
 
 // out[r] = LN(a[r] + b[r])     (residual + sub-layer output, post-LN)
-// (Round 2 tried folding the split-K finish pass of the preceding GEMM into this kernel: at 300 rows it has 75 CTAs and
-// became 21 us per launch against 6 + 3 us for the two separate kernels -- profiles/r02_c_launches_q20.csv -- reverted.)
+// (Folding the split-K finish pass of the preceding GEMM into this kernel was tried: at 300 rows it has 75 CTAs and
+// became slower than the two separate kernels -- reverted.)
 __global__ void __launch_bounds__(128) add_ln_kernel(int64_t rows, int d, const float* __restrict__ a,
                                                      const float* __restrict__ b, const float* __restrict__ gamma,
                                                      const float* __restrict__ beta, float* __restrict__ out,
@@ -190,7 +190,7 @@ __global__ void __launch_bounds__(128) add_ln_kernel(int64_t rows, int d, const 
 
 // add+LN for SMALL row counts (batch 20: 300 rows): one CTA of 128 threads per row instead of one warp per row, so a row's
 // 4 KB are read by 128 threads at once and the kernel is not a chain of 8 dependent 16-byte loads per lane on 75 CTAs
-// (9.6 us per launch under ncu at 300 rows, 312 launches per generate: profiles/r02_f_launches_q20.csv).
+// (312 launches per generate at batch 20).
 // bsrc: b may still be the raw split-K output of the preceding GEMM (SplitSrc) -- the finish launch of o / co / fc2 is folded in
 // (the same fold into the warp-per-row kernel was slower: 75 CTAs at 300 rows; here a row has its own 128 threads).
 __global__ void __launch_bounds__(128) add_ln_row_kernel(int64_t rows, int d, const float* __restrict__ a,
@@ -647,7 +647,7 @@ __global__ void __launch_bounds__(kGAttnWarps * 32) cross_attn_kernel(int64_t G,
 // blocks of 16 query rows in shared memory; scores are register-tiled 4 rows x 1 key per thread (one K read
 // feeds four rows), the softmax runs over the lanes of a warp, and the P.V product is tiled 4 rows x 2 head
 // dims per thread.  About half the instructions per (group, head) of grouped_attention, whose one-row-per-warp
-// sweep spends two shared-memory reads per FMA (profiles/r01_SUMMARY.md).  Same ragged-group arguments as
+// sweep spends two shared-memory reads per FMA.  Same ragged-group arguments as
 // cross_attn_kernel.
 constexpr int kXKeys = 32, kXRows = 16, kXPad = kHeadDim + 4;
 __global__ void __launch_bounds__(128) cross_attn_small_kernel(int64_t G, int d, int heads, int beams, int S_pad,

@@ -59,7 +59,7 @@ inline int sm_count() {
             cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0)
             cached = n;
         else
-            cached = 148;
+            cached = 132;                              // H100 SXM
     }
     return cached;
 }

@@ -5,8 +5,7 @@
 #include "common.cuh"
 #include "decode_kernels.cuh"
 #include "fm_handle.hpp"
-#include "umma_gemm.cuh"
-#include "umma_gemm_2cta.cuh"
+#include "wgmma_gemm.cuh"
 
 #include <cuda_runtime.h>
 
@@ -28,7 +27,7 @@ struct Lin {
     __half* w_h1 = nullptr; __half* w_h2 = nullptr;        // FP16 split copies of W * 2^s (gemm_mode 3)
     float w_unscale = 1.f;                                 // 2^-s
     CUtensorMap map_hi{}, map_lo{}; bool maps_ready = false;
-    CUtensorMap map2_hi{}, map2_lo{}; bool maps2_ready = false;   // 128-row boxes: one CTA's half of a pair's W tile (gemm_mode 5)
+    CUtensorMap map2_hi{}, map2_lo{}; bool maps2_ready = false;   // 64-row boxes: one CTA's half of a cluster's W tile (gemm_mode 5)
 };
 struct LNp { float* g = nullptr; float* b = nullptr; };
 struct EncLayerW { Lin qkv, o, fc1, fc2; LNp ln_attn, ln_final; };
@@ -186,20 +185,17 @@ EncodeTiledFn encode_tiled() {
     return fn;
 }
 // row-major [rows][K] fp32 (or fp16), box = 128 bytes of K x box_rows, 128B swizzle, zero fill out of bounds
-void make_map(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t K, uint64_t ld, uint32_t box_rows, bool half = false,
-              int row_bytes = 128) {
+void make_map(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t K, uint64_t ld, uint32_t box_rows, bool half = false) {
     cuuint64_t dims[2] = {K, rows};
     cuuint64_t strides[1] = {ld * (half ? 2 : 4)};
-    cuuint32_t box[2] = {(cuuint32_t)(row_bytes / (half ? 2 : 4)), box_rows};
+    cuuint32_t box[2] = {(cuuint32_t)(128 / (half ? 2 : 4)), box_rows};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = encode_tiled()(map, half ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(ptr), dims, strides, box, estr,
-                                CU_TENSOR_MAP_INTERLEAVE_NONE, row_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                                CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) throw ApiError(SEALFM_ECUDA, "cuTensorMapEncodeTiled failed (" + std::to_string((int)r) + ")");
 }
 
-constexpr int kUmmaBN = 256;
 constexpr int64_t kAddLnRowMax = 2048;      // up to this many rows add+LN runs one CTA per row
 
 void split_into(cudaStream_t s, const float* x, float* hi, float* lo, uint64_t numel) {
@@ -223,23 +219,23 @@ SplitOut split_of(const Act& a, int* overflow) {
     return so;
 }
 
-void umma_launch(cudaStream_t s, int64_t M, int N, int K, const CUtensorMap& ahi, const CUtensorMap& alo, const CUtensorMap& whi,
-                 const CUtensorMap& wlo, const float* bias, const Act& C, int ldc, bool gelu) {
-    using SMm = UmmaSmem<kUmmaBN>;
-    const int tiles = (int)(((N + kUmmaBN - 1) / kUmmaBN) * ((M + UM - 1) / UM));
-    const int ctas = std::min(tiles, sm_count());
-    const int n_fastest = ((int64_t)M >= (int64_t)N) ? 1 : 0;     // stream the larger operand once
-    if (gelu) {
-        CUDA_CHECK(cudaFuncSetAttribute(umma_gemm_tf32x3_persistent_kernel<kUmmaBN, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMm::kTotal));
-        umma_gemm_tf32x3_persistent_kernel<kUmmaBN, true><<<ctas, UTHREADS2, SMm::kTotal, s>>>(ahi, alo, whi, wlo, (int)M, N, K, bias, C.x, C.hi, C.lo, ldc, n_fastest);
-    } else {
-        CUDA_CHECK(cudaFuncSetAttribute(umma_gemm_tf32x3_persistent_kernel<kUmmaBN, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMm::kTotal));
-        umma_gemm_tf32x3_persistent_kernel<kUmmaBN, false><<<ctas, UTHREADS2, SMm::kTotal, s>>>(ahi, alo, whi, wlo, (int)M, N, K, bias, C.x, C.hi, C.lo, ldc, n_fastest);
-    }
-    CUDA_CHECK(cudaGetLastError());
+template <typename T, bool GELU, int CL>
+void gemm_launch(cudaStream_t s, int ctas, const CUtensorMap& ahi, const CUtensorMap& alo, const CUtensorMap& whi, const CUtensorMap& wlo,
+                 int64_t M, int N, int K, const float* bias, float w_unscale, float* C, T* C1, T* C2, int ldc, int n_fastest, int* ovf,
+                 int k_slices, int64_t slice_stride) {
+    auto kern = wgmma_gemm_x3_kernel<T, GELU, CL>;
+    CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, G_SMEM));
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = CL; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3((unsigned)ctas); cfg.blockDim = dim3(GTHREADS); cfg.dynamicSmemBytes = G_SMEM; cfg.stream = s;
+    cfg.attrs = attr; cfg.numAttrs = 1;
+    CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, ahi, alo, whi, wlo, (int)M, N, K, bias, w_unscale, C, C1, C2, ldc, n_fastest, ovf,
+                                  k_slices, slice_stride));
 }
 
-// C = A W^T + b (+GELU) on the tensor cores: gemm_mode 3 / 5 = 3xFP16 (one CTA per tile / CTA pairs), 2 = 3xTF32 (fp32
+// C = A W^T + b (+GELU) on the tensor cores: gemm_mode 3 / 5 = 3xFP16 (one CTA per tile / clusters of 2 sharing W), 2 = 3xTF32 (fp32
 // range: the fallback when an activation leaves the fp16 range).  Operands arrive pre-split from the producing kernel
 // (A.h1/A.h2 or A.hi/A.lo); they are split here only if the producer did not.
 void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, const Act& C, int ldc, bool gelu);
@@ -259,9 +255,10 @@ void gemm(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, const
 void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, const Act& C, int ldc, bool gelu) {
     if (M == 0) return;
     sealbart* m = cx.m;
+    const int tiles = (int)(((N + GN - 1) / GN) * ((M + GM - 1) / GM));
+    const int n_fastest = ((int64_t)M >= (int64_t)N) ? 1 : 0;     // stream the larger operand once
     if (m->cfg.gemm_mode >= 3 && K % UK16 == 0 && lda == K && l.w_h1) {
-        constexpr int rowb = 128;                              // 128-byte shared-memory rows: 64 K-halves per k-block
-        // 3xFP16 on tcgen05 (persistent); operands pre-split into halves by the producers
+        // 3xFP16; operands pre-split into halves by the producers
         const __half* a1 = A.h1; const __half* a2 = A.h2;
         if (!a1) {
             m->a_hi.ensure((size_t)M * K * 2); m->a_lo.ensure((size_t)M * K * 2);
@@ -271,16 +268,12 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
             a1 = m->a_hi.as<__half>(); a2 = m->a_lo.as<__half>();
         }
         CUtensorMap ma1, ma2;
-        make_map(&ma1, a1, M, K, K, UM, true, rowb); make_map(&ma2, a2, M, K, K, UM, true, rowb);
-        if (!l.maps_ready) { make_map(&l.map_hi, l.w_h1, N, K, K, kUmmaBN, true, rowb); make_map(&l.map_lo, l.w_h2, N, K, K, kUmmaBN, true, rowb); l.maps_ready = true; }
-        using SMm = UmmaSmem<kUmmaBN>;
-        const int tiles = (int)(((N + kUmmaBN - 1) / kUmmaBN) * ((M + UM - 1) / UM));
-        const int ctas = std::min(tiles, sm_count());
-        const int n_fastest = ((int64_t)M >= (int64_t)N) ? 1 : 0;
+        make_map(&ma1, a1, M, K, K, GM, true); make_map(&ma2, a2, M, K, K, GM, true);
+        if (!l.maps_ready) { make_map(&l.map_hi, l.w_h1, N, K, K, GN, true); make_map(&l.map_lo, l.w_h2, N, K, K, GN, true); l.maps_ready = true; }
         int* ovf = m->ovf;
-        // skinny problems (a few tiles for 148 SMs): split K so that the serial K loop of a tile is spread
+        // skinny problems (a few tiles for the whole GPU): split K so that the serial K loop of a tile is spread
         // over up to 8 CTAs, then sum the partial tiles in a fixed order
-        const int kblocks = K / (rowb / 2);
+        const int kblocks = K / UK16;
         int k_slices = 1;
         static const int force_slices = [] { const char* e = std::getenv("SEALB200_KSLICES"); return e ? std::atoi(e) : 0; }();
         if (tiles * 2 <= sm_count() && kblocks >= 4) {
@@ -288,40 +281,14 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
             if (force_slices > 0) k_slices = std::min(force_slices, kblocks);     // experiments only
             while (k_slices > 1 && kblocks % k_slices) --k_slices;
         }
-        if (m->cfg.gemm_mode == 5 && k_slices == 1 && M > UM) {
-            // CTA pairs (cluster of 2, tcgen05.mma.cta_group::2) on 256 x 256 tiles: a third less operand
-            // traffic out of L2 per MMA than the one-CTA kernel (umma_gemm_2cta.cuh)
-            if (!l.maps2_ready) { make_map(&l.map2_hi, l.w_h1, N, K, K, 128, true, 128); make_map(&l.map2_lo, l.w_h2, N, K, K, 128, true, 128); l.maps2_ready = true; }
-            const int m_tiles = (int)((M + UM - 1) / UM), n_tiles = (N + kUmmaBN - 1) / kUmmaBN;
-            const int pair_tiles = ((m_tiles + 1) / 2) * n_tiles;
-            const int pairs = std::min(pair_tiles, sm_count() / 2);
-            // wave quantisation: when the last round of pair-tiles would keep less than half of the pairs busy, those
-            // tiles are cut into K slices (one short round instead of a full one) and summed by a finish kernel
-            int full_items = pair_tiles, tail_s = 1;
-            static const bool tail_split = [] { const char* e = std::getenv("SEALB200_TAIL_SPLIT"); return !e || std::atoi(e) != 0; }();
-            const int rem = pair_tiles % pairs;
-            if (tail_split && pair_tiles > pairs && rem > 0 && rem * 2 <= pairs) {
-                int sl = std::min(8, pairs / rem);
-                const int nk = K / 64;
-                while (sl > 1 && (nk % sl || nk / sl < 2)) --sl;
-                if (sl > 1) { tail_s = sl; full_items = pair_tiles - rem; }
-            }
-            float* part = nullptr;
-            if (tail_s > 1) { m->splitk.ensure((size_t)(pair_tiles - full_items) * tail_s * 65536 * 4); part = m->splitk.as<float>(); }
-            auto launchp = [&](auto kern) {
-                CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, U2_SMEM));
-                launch_k(kern, 2 * pairs, UTHREADS2, U2_SMEM, cx.s, ma1, ma2, l.map2_hi, l.map2_lo, (int)M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, ovf,
-                           full_items, tail_s, part);
-            };
-            if (gelu) launchp(umma_gemm_f16x3_2cta_kernel<true>); else launchp(umma_gemm_f16x3_2cta_kernel<false>);
-            CUDA_CHECK(cudaGetLastError()); m->launches++;
-            if (tail_s > 1) {
-                const int fb = (pair_tiles - full_items) * 64;
-                const int pm_tiles = (m_tiles + 1) / 2;
-                if (gelu) launch_k(umma_tail_finish_kernel<true>, fb, 256, 0, cx.s, (int)M, N, ldc, n_tiles, pm_tiles, n_fastest, full_items, tail_s, part, l.b, l.w_unscale, C.x, C.h1, C.h2, ovf);
-                else launch_k(umma_tail_finish_kernel<false>, fb, 256, 0, cx.s, (int)M, N, ldc, n_tiles, pm_tiles, n_fastest, full_items, tail_s, part, l.b, l.w_unscale, C.x, C.h1, C.h2, ovf);
-                CUDA_CHECK(cudaGetLastError()); m->launches++;
-            }
+        if (m->cfg.gemm_mode == 5 && k_slices == 1 && M > GM) {
+            // clusters of 2 CTAs on vertically adjacent tiles: the W tile is loaded once (TMA multicast) for both
+            if (!l.maps2_ready) { make_map(&l.map2_hi, l.w_h1, N, K, K, GN / 2, true); make_map(&l.map2_lo, l.w_h2, N, K, K, GN / 2, true); l.maps2_ready = true; }
+            const int groups = (int)((M + 2 * GM - 1) / (2 * GM)) * ((N + GN - 1) / GN);
+            const int ctas = 2 * std::min(groups, sm_count() / 2);
+            if (gelu) gemm_launch<__half, true, 2>(cx.s, ctas, ma1, ma2, l.map2_hi, l.map2_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, ovf, 1, 0);
+            else gemm_launch<__half, false, 2>(cx.s, ctas, ma1, ma2, l.map2_hi, l.map2_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, ovf, 1, 0);
+            m->launches++;
             return;
         }
         if (k_slices > 1) {
@@ -329,29 +296,23 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
             m->splitk.ensure((size_t)k_slices * slice_stride * 4);
             float* part = m->splitk.as<float>();
             const int ctas2 = std::min(tiles * k_slices, sm_count());
-            auto launch2 = [&](auto kern) {
-                CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMm::kTotalStaged));
-                launch_k(kern, ctas2, UTHREADS2, SMm::kTotalStaged, cx.s, ma1, ma2, l.map_hi, l.map_lo, (int)M, N, K, nullptr, 1.0f, part, nullptr, nullptr,
-                           ldc, n_fastest, ovf, k_slices, slice_stride);
-            };
-            launch2(umma_gemm_f16x3_persistent_kernel<kUmmaBN, false, 128>);
-            CUDA_CHECK(cudaGetLastError()); m->launches++;
+            gemm_launch<__half, false, 1>(cx.s, ctas2, ma1, ma2, l.map_hi, l.map_lo, M, N, K, nullptr, 1.0f, part, nullptr, nullptr, ldc, n_fastest, ovf,
+                                          k_slices, slice_stride);
+            m->launches++;
             if (M <= cx.defer_rows && !gelu && !C.h1 && !C.hi && ldc == N && l.b) {     // summed by the consumer kernel
                 cx.pending = SplitSrc{part, k_slices, slice_stride, l.b, l.w_unscale};
                 return;
             }
             const int fblocks = (int)std::min<int64_t>((M * (ldc / 4) + 255) / 256, (int64_t)sm_count() * 8);
-            if (gelu) launch_k(umma_splitk_finish_kernel<true>, fblocks, 256, 0, cx.s, M, N, ldc, k_slices, slice_stride, part, l.b, l.w_unscale, C.x, C.h1, C.h2, ovf);
-            else launch_k(umma_splitk_finish_kernel<false>, fblocks, 256, 0, cx.s, M, N, ldc, k_slices, slice_stride, part, l.b, l.w_unscale, C.x, C.h1, C.h2, ovf);
+            if (gelu) launch_k(gemm_splitk_finish_kernel<true>, fblocks, 256, 0, cx.s, M, N, ldc, k_slices, slice_stride, part, l.b, l.w_unscale, C.x, C.h1, C.h2, ovf);
+            else launch_k(gemm_splitk_finish_kernel<false>, fblocks, 256, 0, cx.s, M, N, ldc, k_slices, slice_stride, part, l.b, l.w_unscale, C.x, C.h1, C.h2, ovf);
             CUDA_CHECK(cudaGetLastError()); m->launches++;
             return;
         }
-        auto launch = [&](auto kern) {
-            CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMm::kTotalStaged));
-            launch_k(kern, ctas, UTHREADS2, SMm::kTotalStaged, cx.s, ma1, ma2, l.map_hi, l.map_lo, (int)M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, ovf, 1, (int64_t)0);
-        };
-        if (gelu) launch(umma_gemm_f16x3_persistent_kernel<kUmmaBN, true, 128>); else launch(umma_gemm_f16x3_persistent_kernel<kUmmaBN, false, 128>);
-        CUDA_CHECK(cudaGetLastError()); m->launches++;
+        const int ctas = std::min(tiles, sm_count());
+        if (gelu) gemm_launch<__half, true, 1>(cx.s, ctas, ma1, ma2, l.map_hi, l.map_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, ovf, 1, 0);
+        else gemm_launch<__half, false, 1>(cx.s, ctas, ma1, ma2, l.map_hi, l.map_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, ovf, 1, 0);
+        m->launches++;
         return;
     }
     if (m->cfg.gemm_mode == 2 && K % UK == 0 && lda == K && l.w_hi) {
@@ -362,9 +323,11 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
             ahi = m->a_hi.as<float>(); alo = m->a_lo.as<float>();
         }
         CUtensorMap mah, mal;
-        make_map(&mah, ahi, M, K, K, UM); make_map(&mal, alo, M, K, K, UM);
-        if (!l.maps_ready) { make_map(&l.map_hi, l.w_hi, N, K, K, kUmmaBN); make_map(&l.map_lo, l.w_lo, N, K, K, kUmmaBN); l.maps_ready = true; }
-        umma_launch(cx.s, M, N, K, mah, mal, l.map_hi, l.map_lo, l.b, C, ldc, gelu);
+        make_map(&mah, ahi, M, K, K, GM); make_map(&mal, alo, M, K, K, GM);
+        if (!l.maps_ready) { make_map(&l.map_hi, l.w_hi, N, K, K, GN); make_map(&l.map_lo, l.w_lo, N, K, K, GN); l.maps_ready = true; }
+        const int ctas = std::min(tiles, sm_count());
+        if (gelu) gemm_launch<float, true, 1>(cx.s, ctas, mah, mal, l.map_hi, l.map_lo, M, N, K, l.b, 1.0f, C.x, C.hi, C.lo, ldc, n_fastest, m->ovf, 1, 0);
+        else gemm_launch<float, false, 1>(cx.s, ctas, mah, mal, l.map_hi, l.map_lo, M, N, K, l.b, 1.0f, C.x, C.hi, C.lo, ldc, n_fastest, m->ovf, 1, 0);
         m->launches++;
         return;
     }
@@ -702,7 +665,7 @@ int sealbart_create(const sealbart_config_t* cfg, int device, sealbart_t** out) 
             throw ApiError(SEALFM_EINVAL, "d_model must be a multiple of 128, <= 1024, with 64-wide heads");
         if (cfg->ffn_dim % 64 || cfg->vocab_size <= 0) throw ApiError(SEALFM_EINVAL, "bad ffn_dim / vocab_size");
         if (cfg->gemm_mode != 2 && cfg->gemm_mode != 3 && cfg->gemm_mode != 5)
-            throw ApiError(SEALFM_EINVAL, "gemm_mode must be 5 (3xFP16 on CTA pairs, default), 3 (3xFP16, one CTA per tile) or 2 (3xTF32)");
+            throw ApiError(SEALFM_EINVAL, "gemm_mode must be 3 (3xFP16, one CTA per tile, default), 5 (3xFP16 on 2-CTA clusters) or 2 (3xTF32)");
         int count = 0;
         cudaError_t e = cudaGetDeviceCount(&count);
         if (e != cudaSuccess || count == 0) { cudaGetLastError(); throw ApiError(SEALFM_ENODEVICE, "no CUDA device available"); }

@@ -156,8 +156,8 @@ struct RowScratch {
 
 // ---- step kernel 1 of 2: row statistics + the best K constrained candidates of a GROUP of beams ---------------------
 // grid = Q * groups CTAs; group g of query q covers beams [g * rows_per_cta, ...).  After the first step a group is ONE
-// row (groups = num_beams): 15 000 CTAs stream the 3 GB of logits in parallel (round 1 gave a whole query -- 15 rows,
-// 3 MB -- to one CTA: 1.55 ms per step against a 0.46 ms byte floor, and 20 busy SMs at batch 20).  At the first step a
+// row (groups = num_beams): 15 000 CTAs stream the 3 GB of logits in parallel (a CTA per whole query -- 15 rows,
+// 3 MB -- stayed far from the byte floor and kept only 20 SMs busy at batch 20).  At the first step a
 // group is the whole query (groups = 1): beams 1.. carry -1e9 and are pruned exactly against the running K-th best.
 // Full-vocabulary log-softmax (seal/beam_search.py:251), HF processors (:255), FM-index mask (:260-262), top-2B of
 // the constrained scores restricted to the group (:302-307) -- exact: the query's top-K is the top-K of its groups' top-Ks.

@@ -12,8 +12,8 @@
 // GEMM); everything specific to the index is written here.  Memory: 40 bytes per symbol.
 //
 // Limit: m < 2^32 (32-bit ranks and positions, 64-bit keys, 64-bit item counts in the CUB calls) AND 40 B x m of free
-// device memory: ~4.2e9 symbols on a 180 GB B200, i.e. an NQ-sized text (~3.2e9) fits, a KILT-sized one (~5.5e9, 33-bit
-// rows) does not -- that one goes through the host SA-IS builder; the query kernels are 64-bit throughout.
+// device memory: ~1.9e9 symbols on an 80 GB H100, so NQ-sized (~3.2e9) and KILT-sized (~5.5e9, 33-bit rows) texts go
+// through the host SA-IS builder; the query kernels are 64-bit throughout.
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 

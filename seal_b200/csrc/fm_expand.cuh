@@ -35,7 +35,7 @@ struct PairSink {
 // pair per tree level.  Those live in shared memory ([level][slot], conflict-free), a 32-bit mask says which
 // levels are pending, and the prefix of a popped sibling is rebuilt from the current prefix (the ancestor at that
 // level is the left child).  The previous per-thread `Frame stk[36]` (48-byte frames in local memory) produced
-// ~6x the algorithmic traffic in the wide regime (profiles/r01_expand_kernels_ncu.csv).  The children's node-table
+// several times the algorithmic traffic in the wide regime.  The children's node-table
 // entries share one 32-byte sector and are fetched together with the rank sectors, so a level costs ONE dependent
 // memory round trip; a popped sibling re-reads its entry (once per branching node, top-of-tree entries are cache-hot).
 // Symbols are delivered in ascending order per call, like wt_int::_interval_symbols (sdsl/wt_int.hpp:108-147).

@@ -1,4 +1,4 @@
-// CUDA kernels + C ABI (include/sealfm.h) of the FM-index path.  sm_100a only.
+// CUDA kernels + C ABI (include/sealfm.h) of the FM-index path.  sm_90a only.
 #include "../../include/sealfm.h"
 #include "fm_device.cuh"
 #include "fm_host.hpp"
@@ -53,7 +53,7 @@ namespace {
 
 // Two LF steps walked in lockstep: four dependent rank chains (i, j of both symbols) are in flight per level, and the
 // next level's node entries are fetched with them.  One triple per thread (two chains) left the kernel latency-bound
-// beyond L2 -- 0.43-0.47 of the HBM copy peak at 30 % issue activity (profiles/r01_ncu_lf_200m_raw.csv).
+// beyond L2, with low issue activity.
 __device__ __forceinline__ void lf_step_pair(const FmView& v, uint64_t c0, uint64_t l0, uint64_t r0, uint64_t c1, uint64_t l1, uint64_t r1,
                                              uint64_t& ol0, uint64_t& or0, uint64_t& ol1, uint64_t& or1) {
     const uint32_t L = v.L;
@@ -265,7 +265,7 @@ __global__ void __launch_bounds__(64) extract_kernel(FmView v, uint64_t n, const
 // ------------------------------------------------------------------------------------------------
 int grid_for(uint64_t work_items, int per_block, int max_waves = 8) {
     uint64_t blocks = (work_items + per_block - 1) / per_block;
-    uint64_t cap = (uint64_t)sm_count() * max_waves;       // multiples of the SM count (148 on B200)
+    uint64_t cap = (uint64_t)sm_count() * max_waves;       // multiples of the SM count (132 on H100 SXM)
     if (blocks > cap) blocks = cap;
     if (blocks == 0) blocks = 1;
     return (int)blocks;

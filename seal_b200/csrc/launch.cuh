@@ -1,11 +1,10 @@
 // Typed kernel launch helper: kern<<<grid, block, smem, s>>>(args...) through cudaLaunchKernelEx with the arguments
 // converted to the kernel's parameter types.
 //
-// Round 2 tried programmatic dependent launch here (griddepcontrol.wait / launch_dependents in every kernel of a decode
-// step, the programmatic-serialization launch attribute, also inside the captured CUDA graph): at batch 20 the
-// generate took 21.5 ms with it and 21.2 ms without (profiles/r02_b_bench_q20_{default,nopdl}.json) -- inside a graph
-// the kernel-to-kernel gap is already ~1 us and the ~1 900 kernels are bound by their own 5-12 us, so the attribute
-// and the device-side waits were removed again.
+// Programmatic dependent launch was tried here (griddepcontrol.wait / launch_dependents in every kernel of a decode
+// step, the programmatic-serialization launch attribute, also inside the captured CUDA graph) and gave no gain at
+// batch 20: inside a graph the kernel-to-kernel gap is already ~1 us and the ~1 900 kernels are bound by their own
+// run time, so the attribute and the device-side waits were removed again.
 #pragma once
 #include <cuda_runtime.h>
 

@@ -1,0 +1,401 @@
+// Hopper (sm_90a) GEMM for the BART encoder/decoder linears and the lm_head:
+//   C[M,N] = A[M,K] * W[N,K]^T + bias[N]   (optional exact GELU), fp32 in / fp32 out,
+// computed on the tensor cores as an error-compensated 3-pass product
+//   A*W ~= A_lo*W_hi + A_hi*W_lo + A_hi*W_hi,
+// which keeps the fp32-level accuracy the 1e-4 beam-score parity needs (a single TF32/FP16 pass does not).
+// Two operand splits:
+//   3xFP16 (gemm_mode 3 / 5): x = h1 + h2, h1 = rn_half(x), h2 = rn_half(x - h1).  fp16 products are exact in the
+//     fp32 accumulator, so the accuracy class is that of 3xTF32 at half the operand bytes and twice the tensor rate.
+//     Activations are used unscaled (|x| must stay below 65504; the producers saturate and raise a sticky flag
+//     otherwise); each weight matrix is pre-multiplied by a power of two 2^s so that max|W| ~ 2^14 and the epilogue
+//     multiplies the accumulator by 2^-s (exact).
+//   3xTF32 (gemm_mode 2, fp32 range): hi = x with the 13 low mantissa bits cleared, lo = x - hi (exact).
+//
+// Kernel: persistent, 128 x 128 output tile per CTA, three warpgroups.  Warpgroup 0 is the producer (one thread
+// issues the TMA loads of A hi/lo and W hi/lo into 128B-swizzled K-major shared-memory stages); warpgroups 1 and 2
+// each own 64 rows of the tile and issue wgmma.mma_async (m64n128, both operands from shared memory) into register
+// accumulators.  Stage hand-off uses mbarriers (full: TMA transaction bytes; empty: one arrive per consumer warp).
+// With CL = 2 (gemm_mode 5) two CTAs of a cluster compute vertically adjacent tiles that share the W tile: each CTA
+// loads half of the W rows and multicasts them to both, which halves the W traffic out of L2.
+#pragma once
+#include <cuda.h>
+#include <cuda_fp16.h>
+#include <cuda_runtime.h>
+#include <cstdint>
+
+#include "launch.cuh"
+
+namespace sealb200 {
+
+constexpr int GM = 128;                              // tile rows (two consumer warpgroups of 64)
+constexpr int GN = 128;                              // tile columns (wgmma N)
+constexpr int GSTAGES = 3;
+constexpr int GTHREADS = 384;                        // producer warpgroup + 2 consumer warpgroups
+constexpr int G_AB = GM * 128;                       // one A tile (hi or lo): 128 rows x 128 B of K
+constexpr int G_WB = GN * 128;                       // one W tile (hi or lo)
+constexpr int G_STAGE = 2 * G_AB + 2 * G_WB;         // 64 KB
+constexpr int G_SMEM = GSTAGES * G_STAGE + 1024 /*alignment slack*/ + 256 /*barriers*/;
+constexpr int UK16 = 64;                             // 3xFP16 k-block: 64 halves = one 128-byte swizzle row
+constexpr int UK = 32;                               // 3xTF32 k-block: 32 floats
+
+// Per operand type: K elements per k-block, K per wgmma, and k-blocks per register chunk.  The tensor core adds into
+// its fp32 accumulator with truncation, so a long K loop drifts by ~N_adds * 2^-24 relative, in one direction --
+// enough at K = 1024..4096 to push summed beam scores past the 1e-4 parity bound.  The K loop is therefore cut into
+// chunks (48 tensor-core adds for 3xFP16, 24 for 3xTF32): each chunk accumulates from zero in the wgmma registers
+// and is then added, with round-to-nearest, into a second set of fp32 registers.
+template <typename T> struct GemmElem;
+template <> struct GemmElem<__half> { static constexpr int KE = 64, KSTEP = 16, CHUNK = 4; };
+template <> struct GemmElem<float> { static constexpr int KE = 32, KSTEP = 8, CHUNK = 2; };
+
+// ---- PTX wrappers --------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
+
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
+}
+__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+// Bounded spin: a protocol bug must trap (error code back to the host), never hang the GPU.
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
+    uint32_t done = 0;
+    for (uint32_t spin = 0; !done; ++spin) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+            "selp.u32 %0, 1, 0, p;\n\t}"
+            : "=r"(done) : "r"(bar), "r"(parity) : "memory");
+        if (!done && spin > (1u << 26)) __trap();
+    }
+}
+__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
+__device__ __forceinline__ void cluster_sync_all() {
+    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// shared::cluster address of the same shared-memory offset in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t map_to_cta(uint32_t addr, uint32_t rank) {
+    uint32_t r; asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank)); return r;
+}
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
+    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
+}
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
+                 ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1) : "memory");
+}
+// the box lands at offset dst in every CTA of `mask`, completing bytes on the barrier at offset bar in each of them
+__device__ __forceinline__ void tma_load_2d_multicast(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, uint16_t mask) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+                 ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "h"(mask) : "memory");
+}
+
+// K-major SWIZZLE_128B shared-memory matrix descriptor (sm_90 wgmma): start >> 4 | LBO (unused for swizzled K-major,
+// 1) << 16 | SBO = 1024 B between 8-row groups (>> 4) << 32 | layout SWIZZLE_128B (1) << 62.  Advancing K by 32 bytes
+// inside the 128-byte row adds 2 to the address field.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr) {
+    return static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF) | (1ull << 16) | (64ull << 32) | (1ull << 62);
+}
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of the accumulator registers across a wgmma fence / wait
+__device__ __forceinline__ void acc_fence(float (&d)[64]) {
+#pragma unroll
+    for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+#define SEAL_WG_D64                                                                                              \
+    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, " \
+    "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, "  \
+    "%46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}"
+#define SEAL_WG_OPS(d)                                                                                           \
+    "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),      \
+    "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),          \
+    "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),         \
+    "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),         \
+    "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),         \
+    "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),         \
+    "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),         \
+    "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+
+// D[64 x 128] += A[64 x K] * B[128 x K]^T, both operands K-major in shared memory (scale-d = 1: D is zeroed per chunk)
+__device__ __forceinline__ void wgmma_128(float (&d)[64], uint64_t a, uint64_t b, __half) {
+    asm volatile("wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " SEAL_WG_D64 ", %64, %65, 1, 1, 1, 0, 0;"
+                 : SEAL_WG_OPS(d) : "l"(a), "l"(b));
+}
+__device__ __forceinline__ void wgmma_128(float (&d)[64], uint64_t a, uint64_t b, float) {
+    asm volatile("wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 " SEAL_WG_D64 ", %64, %65, 1, 1, 1;"
+                 : SEAL_WG_OPS(d) : "l"(a), "l"(b));
+}
+#undef SEAL_WG_D64
+#undef SEAL_WG_OPS
+
+__device__ __forceinline__ float gelu_erf_u(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
+
+// x -> (hi, lo): hi keeps the TF32 bits (sign, exponent, 10 mantissa bits), lo = x - hi exactly.
+__global__ void __launch_bounds__(256) split_tf32_kernel(int64_t n4, const float4* __restrict__ x, float4* __restrict__ hi,
+                                                         float4* __restrict__ lo) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
+        const float4 v = x[i];
+        float4 h, l;
+        h.x = __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u); l.x = v.x - h.x;
+        h.y = __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u); l.y = v.y - h.y;
+        h.z = __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u); l.z = v.z - h.z;
+        h.w = __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u); l.w = v.w - h.w;
+        hi[i] = h; lo[i] = l;
+    }
+}
+
+constexpr float kHalfMax = 65504.f;
+
+__device__ __forceinline__ void split_half(float x, __half& h1, __half& h2, int* overflow) {
+    if (fabsf(x) > kHalfMax) { if (overflow) *overflow = 1; x = copysignf(kHalfMax, x); }
+    h1 = __float2half_rn(x);
+    h2 = __float2half_rn(x - __half2float(h1));
+}
+
+// x * scale -> (h1, h2) halves; used for weights (once) and for activations whose producer did not split
+__global__ void __launch_bounds__(256) split_half_kernel(int64_t n, const float* __restrict__ x, float scale,
+                                                         __half* __restrict__ h1, __half* __restrict__ h2,
+                                                         int* __restrict__ overflow) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        __half a, b;
+        int ov = 0;
+        split_half(x[i] * scale, a, b, &ov);
+        if (ov) atomicExch(overflow, 1);
+        h1[i] = a; h2[i] = b;
+    }
+}
+
+__global__ void __launch_bounds__(256) absmax_kernel(int64_t n, const float* __restrict__ x, unsigned int* __restrict__ out) {
+    float m = 0.f;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const float v = fabsf(x[i]);
+        if (v == v && v != INFINITY) m = fmaxf(m, v);
+    }
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((threadIdx.x & 31) == 0) atomicMax(out, __float_as_uint(m));       // non-negative floats order like uints
+}
+
+// Optional in-kernel timeline of CTA 0 (debug ABI sealdec_debug_gemm_trace): SM cycle counter at 0 entry,
+// 1 prologue done, 2 first operands landed, 3 last MMA of the first tile issued, 4 its last chunk complete,
+// 5 tile stored, 6 exit; 7/8 = %globaltimer (ns) at entry / exit.
+__device__ long long g_gemm_trace[20];
+__device__ int g_gemm_trace_on;
+__device__ __forceinline__ void gemm_trace(int i) {
+    if (blockIdx.x == 0 && g_gemm_trace_on) {
+        g_gemm_trace[i] = clock64();
+        if (i == 0 || i == 6) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); g_gemm_trace[i == 0 ? 7 : 8] = (long long)t; }
+    }
+}
+
+// Epilogue store of two adjacent columns (n, n + 1) of one row: fp32 and/or the operand split of the next GEMM.
+__device__ __forceinline__ void store_pair(float* C, __half* S1, __half* S2, int64_t off, int n, int N, float v0, float v1, int& ov) {
+    if (n + 1 < N) {
+        if (C) *reinterpret_cast<float2*>(C + off) = make_float2(v0, v1);
+        if (S1) {
+            __half a0, b0, a1, b1;
+            split_half(v0, a0, b0, &ov); split_half(v1, a1, b1, &ov);
+            *reinterpret_cast<__half2*>(S1 + off) = __halves2half2(a0, a1);
+            *reinterpret_cast<__half2*>(S2 + off) = __halves2half2(b0, b1);
+        }
+    } else if (n < N) {
+        if (C) C[off] = v0;
+        if (S1) { __half a, b; split_half(v0, a, b, &ov); S1[off] = a; S2[off] = b; }
+    }
+}
+__device__ __forceinline__ void store_pair(float* C, float* S1, float* S2, int64_t off, int n, int N, float v0, float v1, int&) {
+    const float h0 = __uint_as_float(__float_as_uint(v0) & 0xFFFFE000u), h1 = __uint_as_float(__float_as_uint(v1) & 0xFFFFE000u);
+    if (n + 1 < N) {
+        if (C) *reinterpret_cast<float2*>(C + off) = make_float2(v0, v1);
+        if (S1) { *reinterpret_cast<float2*>(S1 + off) = make_float2(h0, h1); *reinterpret_cast<float2*>(S2 + off) = make_float2(v0 - h0, v1 - h1); }
+    } else if (n < N) {
+        if (C) C[off] = v0;
+        if (S1) { S1[off] = h0; S2[off] = v0 - h0; }
+    }
+}
+
+// T = __half (3xFP16) or float (3xTF32); CL = CTAs per cluster sharing the W tile (1 or 2).
+// Persistent: work unit u = blockIdx.x / CL walks units u, u + gridDim.x / CL, ...  A unit is (tile group, K slice);
+// a tile group is CL vertically adjacent 128 x 128 tiles.  Tile order is chosen by the host so that the LARGER operand
+// is streamed from HBM once: n fastest when the activations dominate (concurrent CTAs then share A tiles and all of W
+// stays in L2), m fastest when the weights dominate (lm_head).
+// Split-K (CL = 1 only; skinny M, where a handful of tiles would leave most SMs idle): slice s accumulates k-blocks
+// [s*num_k, (s+1)*num_k) and stores its raw fp32 partial tile at C + s*slice_stride (the caller passes bias = nullptr,
+// w_unscale = 1, no split outputs; gemm_splitk_finish_kernel or the consumer kernel sums the slices in a fixed order).
+template <typename T, bool GELU, int CL>
+__global__ void __launch_bounds__(GTHREADS, 1)
+wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
+                     const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo,
+                     int M, int N, int K, const float* __restrict__ bias, float w_unscale, float* __restrict__ C,
+                     T* __restrict__ C_s1, T* __restrict__ C_s2, int ldc, int n_fastest, int* __restrict__ overflow,
+                     int k_slices, int64_t slice_stride) {
+    using E = GemmElem<T>;
+    extern __shared__ uint8_t smem_raw[];
+    const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;          // SWIZZLE_128B wants 1024 B alignment
+    const uint32_t full0 = base + GSTAGES * G_STAGE, empty0 = full0 + 8 * GSTAGES;
+    const int wg = threadIdx.x >> 7;
+    const uint32_t rank = CL > 1 ? cluster_ctarank() : 0;
+    if (threadIdx.x == 0) gemm_trace(0);
+
+    const int m_tiles = (M + GM - 1) / GM, n_tiles = (N + GN - 1) / GN;
+    const int m_groups = (m_tiles + CL - 1) / CL;
+    const int total = m_groups * n_tiles * k_slices;
+    const int num_k = (K / E::KE) / k_slices;
+    const int num_chunks = (num_k + E::CHUNK - 1) / E::CHUNK;
+    const int unit0 = blockIdx.x / CL, n_units = gridDim.x / CL;
+
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < GSTAGES; ++s) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 8 * CL); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    if (CL > 1) cluster_sync_all();                                        // the peer's barriers exist before anything targets them
+    if (threadIdx.x == 0) gemm_trace(1);
+
+    if (wg == 0) {
+        if (threadIdx.x == 0) {
+            uint32_t it = 0;                                               // k-blocks issued so far (all units)
+            for (int u = unit0; u < total; u += n_units) {
+                const int tile = u / k_slices, kb0 = (u % k_slices) * num_k;
+                const int mg = n_fastest ? tile / n_tiles : tile % m_groups, n_tile = n_fastest ? tile % n_tiles : tile / m_groups;
+                const int row_a = (mg * CL + (int)rank) * GM;
+                for (int kb = 0; kb < num_k; ++kb, ++it) {
+                    const int s = it % GSTAGES;
+                    mbar_wait(empty0 + 8 * s, ((it / GSTAGES) & 1) ^ 1);
+                    const uint32_t st = base + s * G_STAGE, fb = full0 + 8 * s;
+                    const int kx = (kb0 + kb) * E::KE;
+                    mbar_expect_tx(fb, G_STAGE);
+                    tma_load_2d(st, &tmA_hi, fb, kx, row_a);
+                    tma_load_2d(st + G_AB, &tmA_lo, fb, kx, row_a);
+                    if (CL == 1) {
+                        tma_load_2d(st + 2 * G_AB, &tmW_hi, fb, kx, n_tile * GN);
+                        tma_load_2d(st + 2 * G_AB + G_WB, &tmW_lo, fb, kx, n_tile * GN);
+                    } else {                                               // this CTA's share of the W rows, to both CTAs
+                        const uint32_t part = rank * (G_WB / CL);
+                        const int row_w = n_tile * GN + (int)rank * (GN / CL);
+                        tma_load_2d_multicast(st + 2 * G_AB + part, &tmW_hi, fb, kx, row_w, (uint16_t)((1u << CL) - 1));
+                        tma_load_2d_multicast(st + 2 * G_AB + G_WB + part, &tmW_lo, fb, kx, row_w, (uint16_t)((1u << CL) - 1));
+                    }
+                }
+            }
+        }
+    } else {
+        const int t = threadIdx.x - 128 * wg, warp = t >> 5, lane = t & 31;
+        const uint32_t a_off = (uint32_t)(wg - 1) * 64 * 128;               // this warpgroup's 64 rows of the A tile
+        uint32_t empty_peer[CL];
+#pragma unroll
+        for (int r = 0; r < CL; ++r) empty_peer[r] = CL > 1 ? map_to_cta(empty0, r) : empty0;
+        uint32_t it = 0;
+        bool first = true;
+        for (int u = unit0; u < total; u += n_units) {
+            const int tile = u / k_slices;
+            float acc[64];
+#pragma unroll
+            for (int j = 0; j < 64; ++j) acc[j] = 0.f;
+            int kb = 0;
+            for (int c = 0; c < num_chunks; ++c) {
+                float d[64];
+#pragma unroll
+                for (int j = 0; j < 64; ++j) d[j] = 0.f;
+                int prev_s = -1;
+                const int kend = (kb + E::CHUNK < num_k) ? kb + E::CHUNK : num_k;
+                for (; kb < kend; ++kb, ++it) {
+                    const int s = it % GSTAGES;
+                    mbar_wait(full0 + 8 * s, (it / GSTAGES) & 1);
+                    if (first && t == 0 && wg == 1) gemm_trace(2);
+                    const uint32_t st = base + s * G_STAGE;
+                    const uint64_t a_hi = gmma_desc_sw128(st + a_off), a_lo = gmma_desc_sw128(st + G_AB + a_off);
+                    const uint64_t w_hi = gmma_desc_sw128(st + 2 * G_AB), w_lo = gmma_desc_sw128(st + 2 * G_AB + G_WB);
+                    acc_fence(d);
+                    wgmma_fence();
+#pragma unroll
+                    for (int k = 0; k < E::KE / E::KSTEP; ++k) {           // KSTEP elements = 32 B -> +2 in the address field
+                        wgmma_128(d, a_lo + 2 * k, w_hi + 2 * k, T{});
+                        wgmma_128(d, a_hi + 2 * k, w_lo + 2 * k, T{});
+                        wgmma_128(d, a_hi + 2 * k, w_hi + 2 * k, T{});
+                    }
+                    wgmma_commit();
+                    wgmma_wait<1>();                                       // the previous k-block's MMAs have retired
+                    acc_fence(d);
+                    if (prev_s >= 0) {
+                        __syncwarp();
+                        if (lane == 0) for (int r = 0; r < CL; ++r) mbar_arrive_cluster(empty_peer[r] + 8 * prev_s);
+                    }
+                    prev_s = s;
+                }
+                wgmma_wait<0>();
+                acc_fence(d);
+                __syncwarp();
+                if (lane == 0) for (int r = 0; r < CL; ++r) mbar_arrive_cluster(empty_peer[r] + 8 * prev_s);
+#pragma unroll
+                for (int j = 0; j < 64; ++j) acc[j] += d[j];              // round-to-nearest promotion
+            }
+            if (first && t == 0 && wg == 1) gemm_trace(4);
+            // accumulator layout of m64n128: warp w holds rows 16w + lane/4 (+8); register 4j + {0,1} / {2,3} holds
+            // columns 8j + 2 (lane % 4) + {0, 1} of the first / second of those rows
+            const int mg = n_fastest ? tile / n_tiles : tile % m_groups, n_tile = n_fastest ? tile % n_tiles : tile / m_groups;
+            const int row0 = (mg * CL + (int)rank) * GM + (wg - 1) * 64 + warp * 16 + (lane >> 2);
+            const int col0 = n_tile * GN + 2 * (lane & 3);
+            float* Cs = C ? C + (int64_t)(u % k_slices) * slice_stride : nullptr;
+            int ov = 0;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = row0 + 8 * h;
+                if (row >= M) continue;
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+                    const int n = col0 + 8 * j;
+                    float v[2];
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const float x = acc[4 * j + 2 * h + e] * w_unscale + ((bias && n + e < N) ? bias[n + e] : 0.f);
+                        v[e] = GELU ? gelu_erf_u(x) : x;
+                    }
+                    store_pair(Cs, C_s1, C_s2, (int64_t)row * ldc + n, n, N, v[0], v[1], ov);
+                }
+            }
+            if (ov) atomicExch(overflow, 1);
+            if (first && t == 0 && wg == 1) gemm_trace(5);
+            first = false;
+        }
+    }
+    __syncthreads();
+    if (CL > 1) cluster_sync_all();                                        // no CTA leaves while the peer may still signal it
+    if (threadIdx.x == 0) gemm_trace(6);
+}
+
+// Finishes a split-K GEMM: out = act((sum_s part[s]) * w_unscale + bias), slices summed in index order
+// (deterministic), written as fp32 and/or as the half split the next GEMM consumes.
+template <bool GELU>
+__global__ void __launch_bounds__(256) gemm_splitk_finish_kernel(int64_t M, int N, int ldc, int k_slices, int64_t slice_stride,
+                                                                 const float* __restrict__ part, const float* __restrict__ bias,
+                                                                 float w_unscale, float* __restrict__ C, __half* __restrict__ C_h1,
+                                                                 __half* __restrict__ C_h2, int* __restrict__ overflow) {
+    const int64_t total = M * (int64_t)(ldc / 4);
+    for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t row = e / (ldc / 4);
+        const int n = (int)(e % (ldc / 4)) * 4;
+        if (n >= N) continue;
+        const int64_t off = row * ldc + n;
+        float4 acc = *reinterpret_cast<const float4*>(part + off);
+        for (int sl = 1; sl < k_slices; ++sl) {
+            const float4 p = *reinterpret_cast<const float4*>(part + sl * slice_stride + off);
+            acc.x += p.x; acc.y += p.y; acc.z += p.z; acc.w += p.w;
+        }
+        float v[4] = {acc.x, acc.y, acc.z, acc.w};
+        int ov = 0;
+        for (int u = 0; u < 4; ++u) {
+            if (n + u >= N) continue;
+            float x = v[u] * w_unscale + (bias ? bias[n + u] : 0.f);
+            if (GELU) x = gelu_erf_u(x);
+            if (C) C[off + u] = x;
+            if (C_h1) { __half a, b; split_half(x, a, b, &ov); C_h1[off + u] = a; C_h2[off + u] = b; }
+        }
+        if (ov) atomicExch(overflow, 1);
+    }
+}
+
+}  // namespace sealb200

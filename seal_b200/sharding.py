@@ -6,7 +6,7 @@ fixed-size hypothesis records are gathered once to rank 0 — the only collectiv
 
 The records of a rank live in ONE contiguous byte buffer (`RecordLayout`): the decode kernels write
 scores / lengths / tokens / validity / SA ranges straight into it on the device, and that buffer is what
-the collective moves — one `dist.gather` (NCCL on the B200s, device to device over NVLink; gloo on CPU
+the collective moves — one `dist.gather` (NCCL on the GPUs, device to device over NVLink; gloo on CPU
 tensors in the tests), no packing pass, no host bounce.  This module is numpy/torch only.
 """
 from typing import Callable, Dict, List, Optional

@@ -167,12 +167,14 @@ def test_fm_index_generate_vs_reference_code_fixture(case):
     print(f"reference-code fixture {kw}: worst |dscore| = {worst:.3e}")
 
 
-def test_fm_index_generate_many_rows_tiny():
-    """40 queries x 8 beams = 320 live rows: more than one 128-row GEMM tile, so the default GEMM (CTA pairs,
-    gemm_mode 5) runs its cta_group::2 kernel inside the decode loop (odd number of row tiles: the last
-    pair has an empty second CTA)."""
+@pytest.mark.parametrize("gemm_mode", [3, 5])
+def test_fm_index_generate_many_rows_tiny(gemm_mode, monkeypatch):
+    """40 queries x 8 beams = 320 live rows: more than one 128-row GEMM tile, so the persistent GEMM (gemm_mode 3,
+    the default) and the 2-CTA cluster GEMM (gemm_mode 5) run inside the decode loop (odd number of row tiles: the
+    last cluster has an empty second CTA)."""
     from oracle.decode_oracle import fm_index_generate_oracle
     from seal_b200.beam_search import fm_index_generate
+    monkeypatch.setenv("SEALB200_GEMM", str(gemm_mode))
     docs, ora, idx, model = tiny_setup()
     rng = np.random.default_rng(21)
     ids, am = make_inputs(rng, Q=40, S=14, vocab=2000)

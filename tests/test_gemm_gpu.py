@@ -1,5 +1,5 @@
-"""GPU: the GEMM back-ends of the BART path -- 3xFP16 (one CTA per tile, CTA pairs) and the 3xTF32 range-safe fallback,
-all tcgen05 -- against a float64 reference of the same op (C = A W^T + b, optional exact GELU): they must stay within a
+"""GPU: the GEMM back-ends of the BART path -- 3xFP16 (one CTA per tile, 2-CTA clusters) and the 3xTF32 range-safe
+fallback, all wgmma -- against a float64 reference of the same op (C = A W^T + b, optional exact GELU): they must stay within a
 few fp32 ulps of it (that is what the 1e-4 beam-score parity rests on)."""
 import ctypes as C
 import math
@@ -34,8 +34,8 @@ SHAPES = [(5, 128, 128, False), (77, 384, 128, False), (300, 1024, 1024, False),
           (513, 1024, 4096, False), (200, 1003, 1024, False), (6, 50265, 1024, False)]
 
 
-# gemm_mode 5 (CTA pairs, cta_group::2) takes over once a problem fills the machine; these shapes do (odd and
-# even numbers of 128-row tiles, ragged N, K = 4096, GELU epilogue), the small SHAPES run its split-K fallback
+# gemm_mode 5 (2-CTA clusters sharing the W tile) takes over once a problem fills the machine; these shapes do (odd
+# and even numbers of 128-row tiles, ragged N, K = 4096, GELU epilogue), the small SHAPES run its split-K fallback
 SHAPES_PAIR = [(2600, 1024, 1024, False), (1300, 4096, 1024, True), (2400, 1003, 4096, False), (700, 50265, 1024, False),
                (1024, 3072, 1024, False)]
 
