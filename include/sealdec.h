@@ -147,6 +147,31 @@ int sealdec_generate_dx(sealbart_t* model, const sealfm_t* fm, const uint32_t* o
                         float* out_scores_d, int32_t* out_len_d, int32_t* out_tokens_d,
                         uint8_t* out_valid_d, uint64_t* out_lo_d, uint64_t* out_hi_d,
                         int32_t* error_flag_d, int64_t src_tokens_hint);
+/* ---- diverse beam groups (fm_index_generate's diverse_bs_groups / diverse_bs_penalty, seal/beam_search.py:447-532) ----
+ * With num_beam_groups = G > 1 the decode follows transformers 4.13's group_beam_search: the beams of a query form G
+ * groups of num_beams / G, chosen one group after the other at every step; the index mask is an ordinary logits
+ * processor there, so recorded scores are the constrained ones (tie-filled picks record -inf), and a positive
+ * diversity_penalty subtracts penalty * count(v) from group g's log-probability of token v, count(v) = how often the
+ * groups before g chose v at this step (HammingDiversityLogitsProcessor).  The record count and layout are those of
+ * one group: sealdec_hyps_per_query per query, each step's 2*num_beams records group by group, in rank order.
+ * The _ex entry points take this struct; NULL, or {1, 0}, is the single-group decode of the functions above, which
+ * call them that way.  1 <= num_beam_groups <= num_beams with num_beams % num_beam_groups == 0, else SEALFM_EINVAL. */
+typedef struct {
+    int32_t num_beam_groups;         /* G, 1 = one group                                             */
+    float   diversity_penalty;       /* <= 0: no Hamming penalty (only used with G > 1); finite      */
+} sealdec_groups_t;
+
+int sealdec_generate_ex(sealbart_t* model, const sealfm_t* fm, const uint32_t* occurring_mask_host,
+                        const sealdec_params_t* p, const int64_t* input_ids, const int64_t* attention_mask,
+                        int64_t Q, int64_t S, float* out_scores, int32_t* out_len, int32_t* out_tokens,
+                        uint8_t* out_valid, uint64_t* out_lo, uint64_t* out_hi, const sealdec_groups_t* groups);
+int sealdec_generate_dx_ex(sealbart_t* model, const sealfm_t* fm, const uint32_t* occurring_mask_d,
+                           const sealdec_params_t* p, const int64_t* input_ids_d,
+                           const int64_t* attention_mask_d, int64_t Q, int64_t S, sealfm_stream_t stream,
+                           float* out_scores_d, int32_t* out_len_d, int32_t* out_tokens_d,
+                           uint8_t* out_valid_d, uint64_t* out_lo_d, uint64_t* out_hi_d,
+                           int32_t* error_flag_d, int64_t src_tokens_hint, const sealdec_groups_t* groups);
+
 /* Options: "cuda_graph" (-1 auto, 0 off, 1 on), "gemm_mode" (switch between the 3xFP16 modes 3/5 and 2 = 3xTF32;
  * the TF32 operand copies are made on first use).  Stats: "last_used_graph", "overflow_fallbacks", "gemm_mode",
  * "cached_graphs" (-1 for an unknown name). */

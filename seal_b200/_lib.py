@@ -90,6 +90,10 @@ class DecParams(C.Structure):             # sealdec_params_t
                 ("force_decoding_from", C.POINTER(C.c_int64)), ("shift", C.c_int32)]
 
 
+class GroupParams(C.Structure):           # sealdec_groups_t
+    _fields_ = [("num_beam_groups", C.c_int32), ("diversity_penalty", C.c_float)]
+
+
 _DEC_SIGS = {
     "sealdec_apply_index_mask_d": (i32, [vp, vp, C.POINTER(ProcessorCfg), vp, C.c_int64, C.c_int64, vp, vp, vp,
                                          C.c_int64, C.c_int64]),
@@ -104,6 +108,10 @@ _DEC_SIGS = {
                                  vp, vp, vp]),
     "sealdec_generate_dx": (i32, [vp, vp, vp, C.POINTER(DecParams), vp, vp, C.c_int64, C.c_int64, vp, vp, vp, vp, vp,
                                   vp, vp, vp, C.c_int64]),
+    "sealdec_generate_ex": (i32, [vp, vp, vp, C.POINTER(DecParams), vp, vp, C.c_int64, C.c_int64, vp, vp, vp, vp, vp, vp,
+                                  C.POINTER(GroupParams)]),
+    "sealdec_generate_dx_ex": (i32, [vp, vp, vp, C.POINTER(DecParams), vp, vp, C.c_int64, C.c_int64, vp, vp, vp, vp, vp,
+                                     vp, vp, vp, C.c_int64, C.POINTER(GroupParams)]),
     "sealbart_set_option": (i32, [vp, cp, C.c_int64]),
     "sealbart_get_stat": (C.c_int64, [vp, cp]),
     "sealdec_teacher_forced": (i32, [vp, vp, vp, C.c_int64, C.c_int64, vp, vp, C.c_int64, C.c_int64, C.c_float, vp,

@@ -3,11 +3,12 @@
 * ``IndexBasedLogitsProcessor`` — same constructor, attributes and HF ``LogitsProcessor`` protocol
   (``__call__(input_ids, scores) -> scores + mask``, beam_search.py:33-140); the FM-index work and
   the mask run as CUDA kernels on the tensors' device, no ``.tolist()`` / H2D round trips.
-* ``fm_index_generate`` — same signature and return value (beam_search.py:391-557), one beam group, no
-  sampling: encoder, every decoder step, log-softmax, processors, FM-index constraint, top-k and
-  BeamSearchScorerWithMemory all run inside libsealb200.so.  ``keep_history=True`` is the path SEALSearcher
-  uses; ``keep_history=False`` (transformers' stock BeamSearchScorer, the signature's default) and
-  ``transformers_output=True`` run the same kernels and replay the stock scorer over the per-step records.
+* ``fm_index_generate`` — same signature and return value (beam_search.py:391-557), no sampling: encoder,
+  every decoder step, log-softmax, processors, FM-index constraint, top-k and BeamSearchScorerWithMemory all
+  run inside libsealb200.so.  ``keep_history=True`` is the path SEALSearcher uses, also with diverse beam
+  groups (``diverse_bs_groups`` / ``diverse_bs_penalty``); ``keep_history=False`` (transformers' stock
+  BeamSearchScorer, the signature's default) and ``transformers_output=True`` run the same kernels and replay
+  the stock scorer over the per-step records (one beam group only).
 * ``SealBartEngine`` — device copy of an HF ``BartForConditionalGeneration``'s weights.
 
 No CPU path: CPU tensors are rejected.
@@ -20,7 +21,7 @@ from typing import List, Optional
 
 import numpy as np
 
-from ._lib import lib, check, vp, ProcessorCfg, BartConfig, DecParams
+from ._lib import lib, check, vp, ProcessorCfg, BartConfig, DecParams, GroupParams
 from .index import FMIndex, SHIFT
 
 stopword_token_ids = [10, 41, 660, 5, 1941, 20, 7, 6]      # beam_search.py:22-31
@@ -194,11 +195,36 @@ def _make_params(cfg, num_beams, min_length, max_length, length_penalty, eos_tok
     return p
 
 
+def _check_diverse_groups(num_beams, diverse_bs_groups, diverse_bs_penalty):
+    """The argument checks fm_index_generate's diverse-beam path meets before any decoding (seal/beam_search.py:447-454,
+    :597-601): transformers 4.13's HammingDiversityLogitsProcessor constructor when the penalty applies, then
+    BeamSearchScorerWithMemory's group check.  Same exception type and message."""
+    if diverse_bs_groups > 1 and diverse_bs_penalty > 0.0:
+        if not isinstance(diverse_bs_penalty, float):
+            raise ValueError("`diversity_penalty` should be a float strictly larger than 0.")
+        if not isinstance(num_beams, int) or num_beams < 2:
+            raise ValueError("`num_beams` should be an integer strictly larger than 1.")
+        if diverse_bs_groups > num_beams:
+            raise ValueError("`beam_groups` has to be smaller or equal to `num_beams`.")
+    if (not isinstance(diverse_bs_groups, int) or diverse_bs_groups > num_beams or num_beams % diverse_bs_groups != 0
+            or diverse_bs_groups < 1):
+        raise ValueError(
+            f"`num_beam_groups` has to be an integer smaller or equal than `num_beams` and `num_beams` "
+            f"has to be divisible by `num_beam_groups`, but is {diverse_bs_groups} with `num_beams` being {num_beams}.")
+
+
+def _group_params(num_beam_groups, diversity_penalty):
+    # a penalty <= 0 means no Hamming processor (seal/beam_search.py:447)
+    return GroupParams(int(num_beam_groups), float(diversity_penalty) if diversity_penalty > 0.0 else 0.0)
+
+
 def generate_records(model, index, input_ids, attention_mask, min_length=3, max_length=25, length_penalty=1.0,
                      num_beams=3, eos_token_id=None, force_decoding_from=None, always_allow_eos=False,
-                     disable_fm_index=False, stop_at_count=0, forced_bos_token_id="config", want_ranges=True):
-    """The C-ABI call with HOST buffers (sealdec_generate): returns the packed hypothesis records
-    (scores [Q,H] f32, lens [Q,H] i32, tokens [Q,H,T] i32, valid [Q,H] u8, lo/hi [Q,H] u64)."""
+                     disable_fm_index=False, stop_at_count=0, forced_bos_token_id="config", want_ranges=True,
+                     num_beam_groups=1, diversity_penalty=0.0):
+    """The C-ABI call with HOST buffers (sealdec_generate_ex): returns the packed hypothesis records
+    (scores [Q,H] f32, lens [Q,H] i32, tokens [Q,H,T] i32, valid [Q,H] u8, lo/hi [Q,H] u64).
+    num_beam_groups > 1: diverse beam groups (include/sealdec.h sealdec_groups_t), records group by group per step."""
     eng = _engine_for(model)
     cfg = eng.config
     if forced_bos_token_id == "config":
@@ -224,9 +250,11 @@ def generate_records(model, index, input_ids, attention_mask, min_length=3, max_
         fm_h = index._dev()
         occ = _occurring_mask(index, int(cfg.vocab_size))
         occ_ptr = occ.ctypes.data
-    check(lib.sealdec_generate(eng._h, fm_h, occ_ptr, C.byref(p), ids.ctypes.data, am.ctypes.data, Q, S,
-                               scores.ctypes.data, lens.ctypes.data, toks.ctypes.data, valid.ctypes.data,
-                               lo.ctypes.data if want_ranges else None, hi.ctypes.data if want_ranges else None))
+    grp = _group_params(num_beam_groups, diversity_penalty)
+    check(lib.sealdec_generate_ex(eng._h, fm_h, occ_ptr, C.byref(p), ids.ctypes.data, am.ctypes.data, Q, S,
+                                  scores.ctypes.data, lens.ctypes.data, toks.ctypes.data, valid.ctypes.data,
+                                  lo.ctypes.data if want_ranges else None, hi.ctypes.data if want_ranges else None,
+                                  C.byref(grp)))
     return {"scores": scores, "lens": lens, "tokens": toks, "valid": valid, "lo": lo, "hi": hi}
 
 
@@ -271,12 +299,13 @@ def _side_stream(device):
 def generate_records_device(model, index, input_ids_d, attention_mask_d, min_length=3, max_length=25, length_penalty=1.0,
                             num_beams=3, eos_token_id=None, force_decoding_from=None, always_allow_eos=False,
                             disable_fm_index=False, stop_at_count=0, forced_bos_token_id="config", out=None,
-                            src_tokens=-1, stream=None):
+                            src_tokens=-1, stream=None, num_beam_groups=1, diversity_penalty=0.0):
     """sealdec_generate_dx on DEVICE tensors, asynchronous: input_ids / attention_mask are int64 CUDA tensors
     [Q, S]; the records land in `out` (a DeviceRecords, created if None) on `stream` (default: the current stream if
     it is not the legacy default stream, else a per-device side stream that first waits for the current one).
     `src_tokens`: number of non-zero mask entries if the caller knows it (right-padded masks) — then the call never
-    touches the host; -1 = unknown.  Errors are flags inside the buffer (`out.host()["errors"]`, include/sealdec.h)."""
+    touches the host; -1 = unknown.  Errors are flags inside the buffer (`out.host()["errors"]`, include/sealdec.h).
+    `num_beam_groups` / `diversity_penalty`: diverse beam groups, as in generate_records."""
     torch = _torch()
     from .sharding import RecordLayout
     eng = _engine_for(model)
@@ -311,11 +340,13 @@ def generate_records_device(model, index, input_ids_d, attention_mask_d, min_len
             stream = cur if cur.cuda_stream != 0 else _side_stream(dev)
         if stream.cuda_stream != cur.cuda_stream:
             stream.wait_stream(cur)
+        grp = _group_params(num_beam_groups, diversity_penalty)
         with torch.cuda.stream(stream):
             out.set_filled(Q)
-            check(lib.sealdec_generate_dx(eng._h, fm_h, occ_ptr, C.byref(p), ids.data_ptr(), am.data_ptr(), Q, S,
-                                          stream.cuda_stream, out.ptr("scores"), out.ptr("lens"), out.ptr("tokens"),
-                                          out.ptr("valid"), out.ptr("lo"), out.ptr("hi"), out.err_ptr, int(src_tokens)))
+            check(lib.sealdec_generate_dx_ex(eng._h, fm_h, occ_ptr, C.byref(p), ids.data_ptr(), am.data_ptr(), Q, S,
+                                             stream.cuda_stream, out.ptr("scores"), out.ptr("lens"), out.ptr("tokens"),
+                                             out.ptr("valid"), out.ptr("lo"), out.ptr("hi"), out.err_ptr, int(src_tokens),
+                                             C.byref(grp)))
         for t in (ids, am, out.buf):
             t.record_stream(stream)
         if stream.cuda_stream != cur.cuda_stream:
@@ -326,7 +357,8 @@ def generate_records_device(model, index, input_ids_d, attention_mask_d, min_len
 def sharded_generate_records(model, index, input_ids, attention_mask, group=None, dst=0, **kw):
     """N-GPU generate: this rank decodes its contiguous block of the batch (host arrays in, as SEALSearcher holds
     them), the records stay on the device and ONE NCCL gather brings every rank's buffer to `dst`
-    (SURVEY.md section 8e).  Returns the full-batch record arrays on `dst`, None elsewhere."""
+    (SURVEY.md section 8e).  Returns the full-batch record arrays on `dst`, None elsewhere.  `kw` are
+    generate_records_device's arguments, num_beam_groups / diversity_penalty included (same record layout)."""
     torch = _torch()
     from .sharding import sharded_generate
     eng = _engine_for(model)
@@ -472,14 +504,19 @@ def fm_index_generate(model, index: FMIndex, input_ids, attention_mask, min_leng
                       stop_at_count: int = 0, topk: int = 0, transformers_output: bool = False, **kwargs):
     """beam_search.py:391-557.  `model` is an HF BartForConditionalGeneration (its weights are
     mirrored on the GPU once and cached) or a SealBartEngine."""
-    if diverse_bs_groups != 1 or sample or topk:
-        raise NotImplementedError("diverse beam groups / sampling / top-k warping are outside the constrained-decoding hot path")
+    if sample or topk:
+        raise NotImplementedError("sampling / top-k warping are outside the constrained-decoding hot path")
+    _check_diverse_groups(num_beams, diverse_bs_groups, diverse_bs_penalty)
+    if diverse_bs_groups > 1 and not keep_history:
+        raise NotImplementedError("diverse_bs_groups > 1 with keep_history=False (transformers' stock grouped BeamSearchScorer) "
+                                  "is not implemented; keep_history=True, the path SEALSearcher uses, is")
     forced_bos = kwargs.pop("forced_bos_token_id", "config")                     # :415-418
     torch = _torch()
     if keep_history:
         rec = generate_records(model, index, input_ids, attention_mask, min_length, max_length, length_penalty,
                                num_beams, eos_token_id, force_decoding_from, always_allow_eos, disable_fm_index,
-                               stop_at_count, forced_bos, want_ranges=False)
+                               stop_at_count, forced_bos, want_ranges=False, num_beam_groups=diverse_bs_groups,
+                               diversity_penalty=diverse_bs_penalty)
         if transformers_output:
             # BeamSearchScorerWithMemory.finalize returns an UNINITIALISED [Q*num_beams, 3] tensor as `sequences`
             # (:727); zeros of that shape here

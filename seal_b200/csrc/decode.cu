@@ -399,12 +399,14 @@ __global__ void prep_enc_packed_kernel(int64_t n, int S, const int64_t* __restri
     if (s2 < src_off[q + 1] - src_off[q]) { const int64_t dst = src_off[q] + s2; tok[dst] = (int32_t)ids[i]; pos[dst] = s2; }
 }
 
-__global__ void init_state_kernel(int64_t R, int B, int T, int start_tok, int pad, uint64_t lo0, uint64_t hi0,
+// gs = beams per group: the first beam of every group starts at 0, the others at -1e9 (seal/beam_search.py:214-216;
+// with diverse beam groups 4.13's group_beam_search sets beam_scores[:, ::gs] = 0)
+__global__ void init_state_kernel(int64_t R, int gs, int T, int start_tok, int pad, uint64_t lo0, uint64_t hi0,
                                   float* __restrict__ scores, int32_t* __restrict__ tokens, uint64_t* __restrict__ lo,
                                   uint64_t* __restrict__ hi, uint64_t* __restrict__ pw, int32_t* __restrict__ anc) {
     const int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     if (r >= R) return;
-    scores[r] = (r % B) == 0 ? 0.f : -1e9f;                 // seal/beam_search.py:214-216
+    scores[r] = (r % gs) == 0 ? 0.f : -1e9f;
     for (int t = 0; t < T; ++t) { tokens[r * T + t] = t == 0 ? start_tok : pad; anc[r * T + t] = (int32_t)r; }
     lo[r] = lo0; hi[r] = hi0; pw[r] = hi0 - lo0;
 }
@@ -780,7 +782,7 @@ int64_t sealdec_hyps_per_query(const sealdec_params_t* p) {
 namespace {
 
 struct GenArgs {
-    const sealfm_t* fm; const uint32_t* occ_d; const sealdec_params_t* p;
+    const sealfm_t* fm; const uint32_t* occ_d; const sealdec_params_t* p; sealdec_groups_t grp;
     const int64_t* ids_d; const int64_t* mask_d; int64_t Q, S;
     float* o_score; int32_t* o_len; int32_t* o_tok; uint8_t* o_valid; uint64_t* o_lo; uint64_t* o_hi; int32_t* err_d;
 };
@@ -813,7 +815,8 @@ void generate_enqueue(Ctx& cx, const Dims& D, const GenArgs& a, const FmView& vi
     uint64_t* pw[2] = {m->st_pw.as<uint64_t>(), m->st_pw.as<uint64_t>() + R};
     int32_t* an[2] = {m->st_anc.as<int32_t>(), m->st_anc.as<int32_t>() + R * T};
     uint32_t* mk[2] = {m->st_mask.as<uint32_t>(), m->st_mask.as<uint32_t>() + (size_t)R * D.W};
-    init_state_kernel<<<(unsigned)((R + 255) / 256), 256, 0, cx.s>>>(R, B, T, p->decoder_start_token_id, p->pad_token_id,
+    const int G = a.grp.num_beam_groups, gs = B / G;
+    init_state_kernel<<<(unsigned)((R + 255) / 256), 256, 0, cx.s>>>(R, gs, T, p->decoder_start_token_id, p->pad_token_id,
                                                                     lo0, hi0, sc[0], tk[0], lo[0], hi[0], pw[0], an[0]);
     CUDA_CHECK(cudaGetLastError()); m->launches++;
 
@@ -825,6 +828,7 @@ void generate_enqueue(Ctx& cx, const Dims& D, const GenArgs& a, const FmView& vi
     c.stop_at_count = p->stop_at_count; c.always_allow_eos = p->always_allow_eos; c.disable_fm_index = p->disable_fm_index;
     c.remove_invalid_values = p->remove_invalid_values; c.shift = p->shift; c.T = T; c.mask_words = D.W;
     c.hyps_per_query = sealdec_hyps_per_query(p);
+    c.num_groups = G; c.diversity_penalty = a.grp.diversity_penalty;
     using RowsFirst = SelSharedT<8192>; using RowsLater = SelSharedT<4096>;
     CUDA_CHECK(cudaFuncSetAttribute(topk_rows_kernel<512, 8192>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RowsFirst)));
     CUDA_CHECK(cudaFuncSetAttribute(topk_rows_kernel<256, 4096>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RowsLater)));
@@ -865,8 +869,14 @@ void generate_enqueue(Ctx& cx, const Dims& D, const GenArgs& a, const FmView& vi
         st.occurring_mask = a.occ_d; st.logits = m->logits.as<float>();
         st.hyp_score = a.o_score; st.hyp_len = a.o_len; st.hyp_tokens = a.o_tok; st.hyp_valid = a.o_valid;
         st.hyp_lo = a.o_lo; st.hyp_hi = a.o_hi; st.error_flag = a.err_d;
-        // first step: beams 1.. carry -1e9 and are pruned exactly inside one CTA per query; afterwards one CTA per row
-        if (cur_len == 1) {
+        // first step: beams 1.. carry -1e9 and are pruned exactly inside one CTA per query; afterwards one CTA per row.
+        // Diverse beam groups at the first step: lists of row 0 (every group leader) and row 1 (every other beam) only,
+        // see select_merge_kernel.
+        if (cur_len == 1 && G > 1) {
+            const int lists = gs > 1 ? 2 : 1;
+            launch_k(topk_rows_kernel<512, 8192>, (unsigned)(Q * lists), 512, sizeof(RowsFirst), cx.s, c, st, rs, lists, 1);
+            launch_k(select_merge_kernel, (unsigned)Q, kMergeThreads, 0, cx.s, view, c, st, rs, lists);
+        } else if (cur_len == 1) {
             launch_k(topk_rows_kernel<512, 8192>, (unsigned)Q, 512, sizeof(RowsFirst), cx.s, c, st, rs, 1, B);
             launch_k(select_merge_kernel, (unsigned)Q, kMergeThreads, 0, cx.s, view, c, st, rs, 1);
         } else {
@@ -896,6 +906,19 @@ template <typename T> void key_put(std::vector<uint8_t>& k, const T& v) {
     k.insert(k.end(), b, b + sizeof(T));
 }
 
+// NULL = one group.  1 <= G <= num_beams, num_beams % G == 0 (BeamSearchScorerWithMemory, seal/beam_search.py:597-601);
+// the penalty only exists with G > 1 and > 0 (seal/beam_search.py:447-454), it is 0 otherwise.
+sealdec_groups_t checked_groups(const sealdec_groups_t* g, int num_beams) {
+    sealdec_groups_t r{1, 0.f};
+    if (!g) return r;
+    if (g->num_beam_groups < 1 || g->num_beam_groups > num_beams || num_beams % g->num_beam_groups != 0)
+        throw ApiError(SEALFM_EINVAL, "num_beam_groups must divide num_beams and be in [1, num_beams]");
+    if (!std::isfinite(g->diversity_penalty)) throw ApiError(SEALFM_EINVAL, "diversity_penalty must be finite");
+    r.num_beam_groups = g->num_beam_groups;
+    if (r.num_beam_groups > 1 && g->diversity_penalty > 0.f) r.diversity_penalty = g->diversity_penalty;
+    return r;
+}
+
 void drop_graphs(sealbart* m) {
     for (auto& g : m->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
     m->graphs.clear();
@@ -906,15 +929,16 @@ void drop_graphs(sealbart* m) {
 
 extern "C" {
 
-int sealdec_generate_dx(sealbart_t* m, const sealfm_t* fm, const uint32_t* occ_d, const sealdec_params_t* p,
-                        const int64_t* ids_d, const int64_t* mask_d, int64_t Q, int64_t S, sealfm_stream_t stream,
-                        float* o_score, int32_t* o_len, int32_t* o_tok, uint8_t* o_valid, uint64_t* o_lo,
-                        uint64_t* o_hi, int32_t* err_d, int64_t src_tokens_hint) {
+int sealdec_generate_dx_ex(sealbart_t* m, const sealfm_t* fm, const uint32_t* occ_d, const sealdec_params_t* p,
+                           const int64_t* ids_d, const int64_t* mask_d, int64_t Q, int64_t S, sealfm_stream_t stream,
+                           float* o_score, int32_t* o_len, int32_t* o_tok, uint8_t* o_valid, uint64_t* o_lo,
+                           uint64_t* o_hi, int32_t* err_d, int64_t src_tokens_hint, const sealdec_groups_t* groups) {
     return guarded([&] {
         check_model(m);
         if (!p || !ids_d || !mask_d || !o_score || !o_len || !o_tok || !o_valid || !err_d) throw ApiError(SEALFM_EINVAL, "null argument");
         const int B = p->num_beams, K = 2 * B, T = p->max_length;
         if (B < 1 || B > kSelMaxBeams || K > kSelMaxK) throw ApiError(SEALFM_EINVAL, "num_beams must be in [1,32]");
+        const sealdec_groups_t grp = checked_groups(groups, B);
         if (T < 2 || T > kMaxLen) throw ApiError(SEALFM_EINVAL, "max_length must be in [2,128]");
         if (Q <= 0 || S <= 0) throw ApiError(SEALFM_EINVAL, "empty batch");
         if (S > m->cfg.max_positions) throw ApiError(SEALFM_EINVAL, "source longer than max_positions");
@@ -940,7 +964,7 @@ int sealdec_generate_dx(sealbart_t* m, const sealfm_t* fm, const uint32_t* occ_d
         const Dims D = make_dims(m, Q, S, B, T);
         ensure_workspace(m, D);
         if (!p->disable_fm_index) m->st_wide.ensure(expand_scratch_bytes(view.L, (uint64_t)D.R));   // wide-row work list + BFS frontiers
-        const GenArgs a{fm, occ_d, p, ids_d, mask_d, Q, S, o_score, o_len, o_tok, o_valid, o_lo, o_hi, err_d};
+        const GenArgs a{fm, occ_d, p, grp, ids_d, mask_d, Q, S, o_score, o_len, o_tok, o_valid, o_lo, o_hi, err_d};
 
         // ---- CUDA graph of the whole call: a batch-20 generate is ~1 900 short kernels, i.e. launch-latency-bound.
         // Shapes, parameters and buffer addresses are the key; the first call of a key runs eagerly (it sizes every
@@ -963,6 +987,7 @@ int sealdec_generate_dx(sealbart_t* m, const sealfm_t* fm, const uint32_t* occ_d
         key_put(key, m->cfg.gemm_mode); key_put(key, cx.s);
         sealdec_params_t pc = *p; pc.force_decoding_from = nullptr; key_put(key, pc);
         for (int i = 0; i < p->n_force_decoding_from; ++i) key_put(key, p->force_decoding_from[i]);
+        key_put(key, grp.num_beam_groups); key_put(key, grp.diversity_penalty);
         key_put(key, view.blocks); key_put(key, view.csym); key_put(key, view.node_tab); key_put(key, view.m);
         key_put(key, occ_d); key_put(key, ids_d); key_put(key, mask_d); key_put(key, o_score); key_put(key, o_len);
         key_put(key, o_tok); key_put(key, o_valid); key_put(key, o_lo); key_put(key, o_hi); key_put(key, err_d);
@@ -1018,6 +1043,14 @@ int sealdec_generate_dx(sealbart_t* m, const sealfm_t* fm, const uint32_t* occ_d
         CUDA_CHECK(cudaGraphLaunch(exec, cx.s));
         m->last_used_graph = 1;
     });
+}
+
+int sealdec_generate_dx(sealbart_t* m, const sealfm_t* fm, const uint32_t* occ_d, const sealdec_params_t* p,
+                        const int64_t* ids_d, const int64_t* mask_d, int64_t Q, int64_t S, sealfm_stream_t stream,
+                        float* o_score, int32_t* o_len, int32_t* o_tok, uint8_t* o_valid, uint64_t* o_lo,
+                        uint64_t* o_hi, int32_t* err_d, int64_t src_tokens_hint) {
+    return sealdec_generate_dx_ex(m, fm, occ_d, p, ids_d, mask_d, Q, S, stream, o_score, o_len, o_tok, o_valid, o_lo, o_hi,
+                                  err_d, src_tokens_hint, nullptr);
 }
 
 int sealdec_generate_d(sealbart_t* m, const sealfm_t* fm, const uint32_t* occ_d, const sealdec_params_t* p,
@@ -1104,9 +1137,16 @@ int sealdec_profile_gemm(sealbart_t* m, int enable, double* total_us, int64_t* l
 int sealdec_generate(sealbart_t* m, const sealfm_t* fm, const uint32_t* occ_host, const sealdec_params_t* p,
                      const int64_t* ids, const int64_t* mask, int64_t Q, int64_t S, float* o_score, int32_t* o_len,
                      int32_t* o_tok, uint8_t* o_valid, uint64_t* o_lo, uint64_t* o_hi) {
+    return sealdec_generate_ex(m, fm, occ_host, p, ids, mask, Q, S, o_score, o_len, o_tok, o_valid, o_lo, o_hi, nullptr);
+}
+
+int sealdec_generate_ex(sealbart_t* m, const sealfm_t* fm, const uint32_t* occ_host, const sealdec_params_t* p,
+                        const int64_t* ids, const int64_t* mask, int64_t Q, int64_t S, float* o_score, int32_t* o_len,
+                        int32_t* o_tok, uint8_t* o_valid, uint64_t* o_lo, uint64_t* o_hi, const sealdec_groups_t* groups) {
     return guarded([&] {
         check_model(m);
         if (!p || !ids || !mask || Q <= 0 || S <= 0) throw ApiError(SEALFM_EINVAL, "null argument / empty batch");
+        checked_groups(groups, p->num_beams);
         const int64_t H = sealdec_hyps_per_query(p), T = p->max_length;
         const int W = (m->cfg.vocab_size + 31) / 32;
         // the caller's buffers are host memory: the real-token count costs nothing to know here, so the encoder
@@ -1128,10 +1168,10 @@ int sealdec_generate(sealbart_t* m, const sealfm_t* fm, const uint32_t* occ_host
         if (occ_host) CUDA_CHECK(cudaMemcpyAsync(m->in_occ.p, occ_host, (size_t)W * 4, cudaMemcpyHostToDevice, s));
         int32_t errs[4] = {0, 0, 0, 0};
         for (int attempt = 0; attempt < 2; ++attempt) {
-            int rc = sealdec_generate_dx(m, fm, occ_host ? m->in_occ.as<uint32_t>() : nullptr, p, m->in_ids.as<int64_t>(),
-                                         m->in_mask.as<int64_t>(), Q, S, s, m->hy_score.as<float>(), m->hy_len.as<int32_t>(),
-                                         m->hy_tok.as<int32_t>(), m->hy_valid.as<uint8_t>(), o_lo ? m->hy_lo.as<uint64_t>() : nullptr,
-                                         o_hi ? m->hy_hi.as<uint64_t>() : nullptr, m->err.as<int32_t>(), hint);
+            int rc = sealdec_generate_dx_ex(m, fm, occ_host ? m->in_occ.as<uint32_t>() : nullptr, p, m->in_ids.as<int64_t>(),
+                                            m->in_mask.as<int64_t>(), Q, S, s, m->hy_score.as<float>(), m->hy_len.as<int32_t>(),
+                                            m->hy_tok.as<int32_t>(), m->hy_valid.as<uint8_t>(), o_lo ? m->hy_lo.as<uint64_t>() : nullptr,
+                                            o_hi ? m->hy_hi.as<uint64_t>() : nullptr, m->err.as<int32_t>(), hint, groups);
             if (rc) throw ApiError(rc, last_error());
             CUDA_CHECK(cudaMemcpyAsync(errs, m->err.p, 16, cudaMemcpyDeviceToHost, s));
             CUDA_CHECK(cudaStreamSynchronize(s));
@@ -1141,10 +1181,10 @@ int sealdec_generate(sealbart_t* m, const sealfm_t* fm, const uint32_t* occ_host
             const int mode = m->cfg.gemm_mode;
             { const int r0 = sealbart_set_option(m, "gemm_mode", 2); if (r0) throw ApiError(r0, last_error()); }
             m->overflow_fallbacks++;
-            rc = sealdec_generate_dx(m, fm, occ_host ? m->in_occ.as<uint32_t>() : nullptr, p, m->in_ids.as<int64_t>(),
-                                     m->in_mask.as<int64_t>(), Q, S, s, m->hy_score.as<float>(), m->hy_len.as<int32_t>(),
-                                     m->hy_tok.as<int32_t>(), m->hy_valid.as<uint8_t>(), o_lo ? m->hy_lo.as<uint64_t>() : nullptr,
-                                     o_hi ? m->hy_hi.as<uint64_t>() : nullptr, m->err.as<int32_t>(), hint);
+            rc = sealdec_generate_dx_ex(m, fm, occ_host ? m->in_occ.as<uint32_t>() : nullptr, p, m->in_ids.as<int64_t>(),
+                                        m->in_mask.as<int64_t>(), Q, S, s, m->hy_score.as<float>(), m->hy_len.as<int32_t>(),
+                                        m->hy_tok.as<int32_t>(), m->hy_valid.as<uint8_t>(), o_lo ? m->hy_lo.as<uint64_t>() : nullptr,
+                                        o_hi ? m->hy_hi.as<uint64_t>() : nullptr, m->err.as<int32_t>(), hint, groups);
             const int rc2 = sealbart_set_option(m, "gemm_mode", mode);
             if (rc) throw ApiError(rc, last_error());
             if (rc2) throw ApiError(rc2, last_error());

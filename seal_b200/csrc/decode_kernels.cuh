@@ -34,6 +34,8 @@ struct StepCfg {
                                        //    so the model was not run and `logits` must not be read
     int64_t hyps_per_query;
     int32_t hyp_base;                  // index of this step's first hypothesis record
+    int32_t num_groups;                // diverse beam groups G (1: constrained_beam_search; > 1: group_beam_search)
+    float diversity_penalty;           // Hamming diversity penalty, 0 = no HammingDiversityLogitsProcessor
 };
 
 struct StepState {
@@ -151,24 +153,25 @@ __device__ void sel_merge(SH& S, int K) {
 // Per-row scratch between the two kernels of a step.
 struct RowScratch {
     float* row_max; float* row_logsum; uint8_t* row_rule;     // [R]  log-softmax statistics / index rule of every row
-    float* cand_val; int32_t* cand_idx; int32_t* cand_cnt;    // [Q * groups][K] sorted best candidates per row group, [Q * groups]
+    float* cand_val; int32_t* cand_idx; int32_t* cand_cnt;    // [Q * lists][K] sorted best candidates per candidate list, [Q * lists]
 };
 
-// ---- step kernel 1 of 2: row statistics + the best K constrained candidates of a GROUP of beams ---------------------
-// grid = Q * groups CTAs; group g of query q covers beams [g * rows_per_cta, ...).  After the first step a group is ONE
-// row (groups = num_beams): 15 000 CTAs stream the 3 GB of logits in parallel (a CTA per whole query -- 15 rows,
+// ---- step kernel 1 of 2: row statistics + the best K constrained candidates of a run of beams -----------------------
+// grid = Q * lists CTAs; list g of query q covers beams [g * rows_per_cta, ...).  After the first step a list is ONE
+// row (lists = num_beams): 15 000 CTAs stream the 3 GB of logits in parallel (a CTA per whole query -- 15 rows,
 // 3 MB -- stayed far from the byte floor and kept only 20 SMs busy at batch 20).  At the first step a
-// group is the whole query (groups = 1): beams 1.. carry -1e9 and are pruned exactly against the running K-th best.
+// list is the whole query (lists = 1): beams 1.. carry -1e9 and are pruned exactly against the running K-th best.
 // Full-vocabulary log-softmax (seal/beam_search.py:251), HF processors (:255), FM-index mask (:260-262), top-2B of
-// the constrained scores restricted to the group (:302-307) -- exact: the query's top-K is the top-K of its groups' top-Ks.
+// the constrained scores restricted to the list's rows (:302-307) -- exact: the query's top-K is the top-K of its lists' top-Ks.
+// Diverse beam groups (num_groups > 1) always use one row per list: see select_merge_kernel for why that is exact.
 template <int THREADS, int BUF>
-__global__ void __launch_bounds__(THREADS, THREADS >= 512 ? 2 : 4) topk_rows_kernel(StepCfg c, StepState st, RowScratch rs, int groups, int rows_per_cta) {
+__global__ void __launch_bounds__(THREADS, THREADS >= 512 ? 2 : 4) topk_rows_kernel(StepCfg c, StepState st, RowScratch rs, int lists, int rows_per_cta) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     using SH = SelSharedT<BUF>;
     SH& S = *reinterpret_cast<SH*>(smem_raw);
     const int B = c.num_beams, K = c.K, V = c.V;
-    const int64_t qi = blockIdx.x / groups;
-    const int g = blockIdx.x - (int)(qi * groups);
+    const int64_t qi = blockIdx.x / lists;
+    const int g = blockIdx.x - (int)(qi * lists);
     const int64_t r0 = qi * B;
     const int tid = threadIdx.x;
     if (tid == 0) { S.ccount = 0; S.tcount = 0; S.overflow = 0; S.thr = -INFINITY; S.thr_idx = 0x7fffffff; }
@@ -309,7 +312,7 @@ __global__ void __launch_bounds__(THREADS, THREADS >= 512 ? 2 : 4) topk_rows_ker
     }
     sel_merge(S, K);
     static_assert(BUF >= THREADS * 16, "a sub-round stages up to 8 candidates per thread on top of a half-full buffer");
-    const int64_t gidx = qi * groups + g;
+    const int64_t gidx = qi * lists + g;
     for (int k = tid; k < S.tcount; k += THREADS) { rs.cand_val[gidx * K + k] = S.tval[k]; rs.cand_idx[gidx * K + k] = S.tidx[k]; }
     if (tid == 0) rs.cand_cnt[gidx] = S.tcount;
 }
@@ -325,156 +328,225 @@ struct MergeShared {
     float rv[kMergeThreads / 32]; int ri[kMergeThreads / 32]; int rslot[kMergeThreads / 32];
     int nbeam_src[kSelMaxBeams];          // candidate index feeding each new beam
     int n_noneos;
+    int new_tok[kSelMaxBeams];            // token of every new beam of this step so far (4.13's `current_tokens`)
+    int pen_tok[kSelMaxBeams]; int pen_cnt[kSelMaxBeams]; int n_pen;   // (token, count) of the earlier groups' new beams
 };
 
-// ---- step kernel 2 of 2, one CTA per query: merge the groups' candidate lists into the query's top-2B (:302-307),
-// -inf fill-ins (SURVEY.md H4), BeamSearchScorerWithMemory.process (:614-703), hypothesis records, and the LF step
-// (incremental get_range) of every record and new beam.  The successor sets of the new beams (next step's masks)
-// are expanded by the FM-index kernels right after (fm_kernels.cu launch_expand_masks), over all rows of the batch.
-__global__ void __launch_bounds__(kMergeThreads) select_merge_kernel(FmView fm, StepCfg c, StepState st, RowScratch rs, int groups) {
+// ---- step kernel 2 of 2, one CTA per query: merge the candidate lists into the top-2B (:302-307), -inf fill-ins
+// (SURVEY.md H4), BeamSearchScorerWithMemory.process (:614-703), hypothesis records, and the LF step (incremental
+// get_range) of every record and new beam.  The successor sets of the new beams (next step's masks) are expanded by the
+// FM-index kernels right after (fm_kernels.cu launch_expand_masks), over all rows of the batch.
+//
+// Diverse beam groups (c.num_groups = G > 1, transformers 4.13 group_beam_search as fm_index_generate calls it,
+// seal/beam_search.py:447-469,523-532): the groups of gs = B / G beams are handled in order, each like a query of its
+// own -- top-2gs over its [gs * V] view, process with group_size = gs, 2gs records, gs new beams -- except that
+//   * the index mask is an ordinary logits processor there, so the recorded and carried scores are the CONSTRAINED
+//     ones: a tie-filled pick scores -inf (and drops out of the reference's output, :555);
+//   * HammingDiversityLogitsProcessor runs between the HF processors and the index mask: group g's score of token v is
+//     (p - penalty * count(v)) + beam_score, count(v) = how often v is the new token of a beam of groups < g.
+// Exactness of the per-row lists (topk_rows_kernel, K = 2B per row): the penalty lowers only tokens earlier groups
+// chose, at most (G-1) * gs distinct ones, so a candidate of the group's penalised top-2gs is among its row's
+// unpenalised top 2gs + (G-1)gs = B + gs <= 2B.  (A list over several rows would need (G-1)gs more per row.)
+// At the first step every group leader is the same row (same logits, start token, mask and score 0), and so is every
+// other beam (score -1e9): topk_rows_kernel lists rows 0 and 1 only (lists = 2, or 1 if gs = 1), and here a leader
+// takes row 0's list and statistics, a non-leader row 1's -- exactly the per-row lists of all rows, relabelled.
+__global__ void __launch_bounds__(kMergeThreads) select_merge_kernel(FmView fm, StepCfg c, StepState st, RowScratch rs, int lists) {
     __shared__ MergeShared S;
     const int B = c.num_beams, K = c.K, V = c.V;
+    const int G = c.num_groups, gs = B / G, Kg = 2 * gs;
+    const bool grouped = G > 1;
     const int64_t qi = blockIdx.x;
     const int64_t r0 = qi * B;
     const int tid = threadIdx.x;
     const int lane = tid & 31, warp = tid >> 5;
-    // gather the sorted lists of this query's groups
-    int n = 0;
-    for (int g = 0; g < groups; ++g) {
-        const int cnt = rs.cand_cnt[qi * groups + g];
-        for (int k = tid; k < cnt; k += kMergeThreads) { S.cval[n + k] = rs.cand_val[(qi * groups + g) * K + k]; S.cidx[n + k] = rs.cand_idx[(qi * groups + g) * K + k]; }
-        n += cnt;
-    }
-    __syncthreads();
-    const int want = n < K ? n : K;
-    for (int round = 0; round < want; ++round) {
-        float bv = -INFINITY; int bi = 0x7fffffff; int bs = -1;
-        for (int i = tid; i < n; i += kMergeThreads) {
-            const int id = S.cidx[i];
-            if (id < 0) continue;
-            const float v = S.cval[i];
-            if (bs < 0 || cand_better(v, id, bv, bi)) { bv = v; bi = id; bs = i; }
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-            const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-            const int os = __shfl_xor_sync(0xffffffffu, bs, o);
-            if (os >= 0 && (bs < 0 || cand_better(ov, oi, bv, bi))) { bv = ov; bi = oi; bs = os; }
-        }
-        if (lane == 0) { S.rv[warp] = bv; S.ri[warp] = bi; S.rslot[warp] = bs; }
-        __syncthreads();
+    // grouped path: which candidate list / row statistics stand for row b of group [b0, b0 + gs)
+    auto src_row = [&](int b, int b0) -> int { return lists == B ? b : (b == b0 ? 0 : 1); };
+    auto row_logprob = [&](int64_t r, int64_t stat_r, int v) -> float {
+        float p = c.logits_ignored ? 0.f : (st.logits[(c.logits_shared ? qi : r) * c.ld + v] - rs.row_max[stat_r]) - rs.row_logsum[stat_r];
+        return apply_processors(c, v, p);
+    };
+    for (int g = 0; g < G; ++g) {
+        const int b0 = g * gs;
+        // ---- (token, count) table of the new tokens of groups < g (HammingDiversityLogitsProcessor) ----------------
         if (tid == 0) {
-            float v = S.rv[0]; int id = S.ri[0]; int sl = S.rslot[0];
-            for (int w = 1; w < kMergeThreads / 32; ++w)
-                if (S.rslot[w] >= 0 && (sl < 0 || cand_better(S.rv[w], S.ri[w], v, id))) { v = S.rv[w]; id = S.ri[w]; sl = S.rslot[w]; }
-            S.tval[round] = v; S.tidx[round] = id;
-            S.cidx[sl] = -1;
+            int np = 0;
+            if (c.diversity_penalty > 0.f)
+                for (int j = 0; j < b0; ++j) {
+                    const int t = S.new_tok[j];
+                    if (t < 0) continue;
+                    int i = 0;
+                    while (i < np && S.pen_tok[i] != t) ++i;
+                    if (i == np) { S.pen_tok[np] = t; S.pen_cnt[np] = 0; ++np; }
+                    S.pen_cnt[i] += 1;
+                }
+            S.n_pen = np;
         }
         __syncthreads();
-    }
-    if (tid < kSelMaxK) S.tvalid[tid] = tid < want ? 1 : 0;
-    __syncthreads();
-
-    // ---- fewer than K finite constrained candidates: fill with masked ones (SURVEY.md §H4) -------
-    // torch.topk's choice among -inf ties is unspecified; ours: lowest flat index first.
-    if (tid == 0 && want < K) {                                  // `want` is the same register value in every thread
-        int have = want;
-        for (int flat = 0; have < K && flat < B * V; ++flat) {
-            const int b = flat / V, v = flat - b * V;
-            const int64_t r = r0 + b;
-            float p = c.logits_ignored ? 0.f : (st.logits[(c.logits_shared ? qi : r) * c.ld + v] - rs.row_max[r]) - rs.row_logsum[r];
-            p = apply_processors(c, v, p);
-            const float s = p + st.beam_scores_in[r];
-            // was it a finite constrained candidate (then it is already in the list)?
-            bool allowed;
-            if (c.disable_fm_index) allowed = true;
-            else if (c.forced_bos_token_id >= 0 && c.cur_len == 1) allowed = v == c.forced_bos_token_id;
-            else {
-                const uint32_t* mrow = c.first_step_shared_mask ? st.occurring_mask : st.mask_in + r * c.mask_words;
-                const int rule = rs.row_rule[r];
-                allowed = rule == 1 ? v == c.eos_token_id : rule == 2 ? v == c.pad_token_id : ((mrow[v >> 5] >> (v & 31)) & 1);
-                if (c.always_allow_eos && v == c.eos_token_id) allowed = true;
+        // ---- gather the candidate lists of the group's rows ----------------------------------------------------------
+        int n = 0;
+        if (!grouped) {
+            for (int l = 0; l < lists; ++l) {
+                const int cnt = rs.cand_cnt[qi * lists + l];
+                for (int k = tid; k < cnt; k += kMergeThreads) { S.cval[n + k] = rs.cand_val[(qi * lists + l) * K + k]; S.cidx[n + k] = rs.cand_idx[(qi * lists + l) * K + k]; }
+                n += cnt;
             }
-            if (allowed && s > -INFINITY) continue;
-            S.tval[have] = s; S.tidx[have] = flat; S.tvalid[have] = 0; ++have;
-        }
-    }
-    __syncthreads();
-
-    // ---- BeamSearchScorerWithMemory.process (seal/beam_search.py:642-695) -----------------------
-    if (tid == 0) {
-        int nb = 0;
-        for (int k = 0; k < K; ++k) {
-            const int tok = S.tidx[k] % V;
-            if (tok != c.eos_token_id && nb < B) S.nbeam_src[nb++] = k;     // :673-681
-        }
-        S.n_noneos = nb;
-        if (nb < B) atomicExch(st.error_flag, 1);                           // :687-690 ValueError
-    }
-    __syncthreads();
-    const int new_len = c.cur_len + 1;
-    if (tid < K) {
-        const int k = tid;
-        const int flat = S.tidx[k];
-        const int pb = flat / V, tok = flat - pb * V;                        // :309-310
-        const int64_t pr = r0 + pb;
-        const int64_t h = qi * c.hyps_per_query + c.hyp_base + k;
-        st.hyp_score[h] = S.tval[k];                                         // :662-668
-        st.hyp_len[h] = new_len;
-        st.hyp_valid[h] = S.tvalid[k];
-        int32_t* ht = st.hyp_tokens + h * c.T;
-        const int32_t* pt = st.tokens_in + pr * c.T;
-        for (int i = 0; i < c.cur_len; ++i) ht[i] = pt[i];
-        ht[c.cur_len] = tok;
-        for (int i = new_len; i < c.T; ++i) ht[i] = c.pad_token_id;
-        if (st.hyp_lo) {
-            uint64_t l = 0, r = 0;
-            if (!c.disable_fm_index && S.tvalid[k] && !(c.forced_bos_token_id >= 0 && c.cur_len == 1)) {
-                uint64_t rr;
-                lf_step(fm, (uint64_t)tok + c.shift, st.lo_in[pr], st.hi_in[pr] - 1, l, rr);
-                r = rr + 1;
-            }
-            st.hyp_lo[h] = l; st.hyp_hi[h] = r;
-        }
-    }
-    // ---- next beams: state of row j comes from candidate nbeam_src[j] (threads K .. K+B-1: other warps than the
-    // record writers where possible) -------------------------------------------------------------------------------
-    const int jt = tid - (K + B <= kMergeThreads ? K : 0);
-    if (jt >= 0 && jt < B) {
-        const int j = jt;
-        const int64_t nr = r0 + j;
-        if (j < S.n_noneos) {
-            const int k = S.nbeam_src[j];
-            const int flat = S.tidx[k];
-            const int pb = flat / V, tok = flat - pb * V;
-            const int64_t pr = r0 + pb;
-            st.beam_scores_out[nr] = S.tval[k];
-            const int32_t* pt = st.tokens_in + pr * c.T;
-            int32_t* nt = st.tokens_out + nr * c.T;
-            for (int i = 0; i < c.cur_len; ++i) nt[i] = pt[i];
-            nt[c.cur_len] = tok;
-            for (int i = new_len; i < c.T; ++i) nt[i] = c.pad_token_id;
-            const int32_t* pa = st.anc_in + pr * c.T;
-            int32_t* na = st.anc_out + nr * c.T;
-            for (int i = 0; i + 1 < c.cur_len; ++i) na[i] = pa[i];
-            na[c.cur_len - 1] = (int32_t)pr;                                // KV of position cur_len-1 lives in the parent's slot
-            uint64_t l = 0, rr = 0;
-            if (c.forced_bos_token_id >= 0 && c.cur_len == 1) {
-                // the forced BOS is not part of the FM-index query (the reference drops it, :71)
-                l = st.lo_in[pr]; rr = st.hi_in[pr];
-            } else if (!c.disable_fm_index) {
-                // incremental get_range: one backward_search_step on the parent's range
-                // (seal/index.py:102-111 recomputed from scratch by the reference, :96-101)
-                lf_step(fm, (uint64_t)tok + c.shift, st.lo_in[pr], st.hi_in[pr] - 1, l, rr);
-                rr += 1;
-            }
-            st.lo_out[nr] = l; st.hi_out[nr] = rr;
-            st.pw_out[nr] = (c.forced_bos_token_id >= 0 && c.cur_len == 1) ? st.pw_in[pr] : st.hi_in[pr] - st.lo_in[pr];
         } else {
-            st.beam_scores_out[nr] = 0.f;
-            st.lo_out[nr] = 0; st.hi_out[nr] = 0; st.pw_out[nr] = 0;
+            const int np = S.n_pen;
+            for (int b = b0; b < b0 + gs; ++b) {
+                const int64_t li = qi * lists + src_row(b, b0);
+                const int64_t r = r0 + b, stat_r = r0 + src_row(b, b0);
+                const int cnt = rs.cand_cnt[li];
+                for (int k = tid; k < cnt; k += kMergeThreads) {
+                    const int f = rs.cand_idx[li * K + k];
+                    const int v = f - (f / V) * V;
+                    float s = rs.cand_val[li * K + k];
+                    int count = 0;
+                    for (int i = 0; i < np; ++i) count += S.pen_tok[i] == v ? S.pen_cnt[i] : 0;
+                    if (count) {
+                        // recomputed in the reference's order: (p - penalty * count) + beam_score, no contraction
+                        const float p = __fsub_rn(row_logprob(r, stat_r, v), __fmul_rn(c.diversity_penalty, (float)count));
+                        s = __fadd_rn(p, st.beam_scores_in[r]);
+                    }
+                    S.cval[n + k] = s; S.cidx[n + k] = b * V + v;
+                }
+                n += cnt;
+            }
         }
+        __syncthreads();
+        // ---- top-Kg, score descending then lower flat index -----------------------------------------------------------
+        const int want = n < Kg ? n : Kg;
+        for (int round = 0; round < want; ++round) {
+            float bv = -INFINITY; int bi = 0x7fffffff; int bs = -1;
+            for (int i = tid; i < n; i += kMergeThreads) {
+                const int id = S.cidx[i];
+                if (id < 0) continue;
+                const float v = S.cval[i];
+                if (bs < 0 || cand_better(v, id, bv, bi)) { bv = v; bi = id; bs = i; }
+            }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+                const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+                const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+                const int os = __shfl_xor_sync(0xffffffffu, bs, o);
+                if (os >= 0 && (bs < 0 || cand_better(ov, oi, bv, bi))) { bv = ov; bi = oi; bs = os; }
+            }
+            if (lane == 0) { S.rv[warp] = bv; S.ri[warp] = bi; S.rslot[warp] = bs; }
+            __syncthreads();
+            if (tid == 0) {
+                float v = S.rv[0]; int id = S.ri[0]; int sl = S.rslot[0];
+                for (int w = 1; w < kMergeThreads / 32; ++w)
+                    if (S.rslot[w] >= 0 && (sl < 0 || cand_better(S.rv[w], S.ri[w], v, id))) { v = S.rv[w]; id = S.ri[w]; sl = S.rslot[w]; }
+                S.tval[round] = v; S.tidx[round] = id;
+                S.cidx[sl] = -1;
+            }
+            __syncthreads();
+        }
+        if (tid < kSelMaxK) S.tvalid[tid] = tid < want ? 1 : 0;
+        __syncthreads();
+
+        // ---- fewer than Kg finite constrained candidates: fill with masked ones (SURVEY.md §H4) -------
+        // torch.topk's choice among -inf ties is unspecified; ours: lowest flat index first.  The single-group path
+        // records the unconstrained score of a fill-in (:258,:304-307), the grouped path the constrained one, -inf.
+        if (tid == 0 && want < Kg) {                                 // `want` is the same register value in every thread
+            int have = want;
+            for (int flat = b0 * V; have < Kg && flat < (b0 + gs) * V; ++flat) {
+                const int b = flat / V, v = flat - b * V;
+                const int64_t r = r0 + b;
+                const int64_t stat_r = grouped ? r0 + src_row(b, b0) : r;
+                const float s = row_logprob(r, stat_r, v) + st.beam_scores_in[r];
+                // was it a finite constrained candidate (then it is already in the list)?
+                bool allowed;
+                if (c.disable_fm_index) allowed = true;
+                else if (c.forced_bos_token_id >= 0 && c.cur_len == 1) allowed = v == c.forced_bos_token_id;
+                else {
+                    const uint32_t* mrow = c.first_step_shared_mask ? st.occurring_mask : st.mask_in + r * c.mask_words;
+                    const int rule = rs.row_rule[stat_r];
+                    allowed = rule == 1 ? v == c.eos_token_id : rule == 2 ? v == c.pad_token_id : ((mrow[v >> 5] >> (v & 31)) & 1);
+                    if (c.always_allow_eos && v == c.eos_token_id) allowed = true;
+                }
+                if (allowed && s > -INFINITY) continue;
+                S.tval[have] = grouped ? -INFINITY : s; S.tidx[have] = flat; S.tvalid[have] = 0; ++have;
+            }
+        }
+        __syncthreads();
+
+        // ---- BeamSearchScorerWithMemory.process (seal/beam_search.py:642-695), group_size = gs -----------------------
+        if (tid == 0) {
+            int nb = 0;
+            for (int k = 0; k < Kg; ++k) {
+                const int tok = S.tidx[k] % V;
+                if (tok != c.eos_token_id && nb < gs) S.nbeam_src[nb++] = k;     // :673-681
+            }
+            S.n_noneos = nb;
+            if (nb < gs) atomicExch(st.error_flag, 1);                          // :687-690 ValueError
+        }
+        __syncthreads();
+        const int new_len = c.cur_len + 1;
+        if (tid < Kg) {
+            const int k = tid;
+            const int flat = S.tidx[k];
+            const int pb = flat / V, tok = flat - pb * V;                        // :309-310
+            const int64_t pr = r0 + pb;
+            const int64_t h = qi * c.hyps_per_query + c.hyp_base + 2 * b0 + k;  // group-major, rank order
+            st.hyp_score[h] = S.tval[k];                                         // :662-668
+            st.hyp_len[h] = new_len;
+            st.hyp_valid[h] = S.tvalid[k];
+            int32_t* ht = st.hyp_tokens + h * c.T;
+            const int32_t* pt = st.tokens_in + pr * c.T;
+            for (int i = 0; i < c.cur_len; ++i) ht[i] = pt[i];
+            ht[c.cur_len] = tok;
+            for (int i = new_len; i < c.T; ++i) ht[i] = c.pad_token_id;
+            if (st.hyp_lo) {
+                uint64_t l = 0, r = 0;
+                if (!c.disable_fm_index && S.tvalid[k] && !(c.forced_bos_token_id >= 0 && c.cur_len == 1)) {
+                    uint64_t rr;
+                    lf_step(fm, (uint64_t)tok + c.shift, st.lo_in[pr], st.hi_in[pr] - 1, l, rr);
+                    r = rr + 1;
+                }
+                st.hyp_lo[h] = l; st.hyp_hi[h] = r;
+            }
+        }
+        // ---- next beams: state of row b0 + j comes from candidate nbeam_src[j] (threads Kg .. Kg+gs-1: other warps
+        // than the record writers where possible) ---------------------------------------------------------------------
+        const int jt = tid - (Kg + gs <= kMergeThreads ? Kg : 0);
+        if (jt >= 0 && jt < gs) {
+            const int j = jt;
+            const int64_t nr = r0 + b0 + j;
+            if (j < S.n_noneos) {
+                const int k = S.nbeam_src[j];
+                const int flat = S.tidx[k];
+                const int pb = flat / V, tok = flat - pb * V;
+                const int64_t pr = r0 + pb;
+                S.new_tok[b0 + j] = tok;
+                st.beam_scores_out[nr] = S.tval[k];
+                const int32_t* pt = st.tokens_in + pr * c.T;
+                int32_t* nt = st.tokens_out + nr * c.T;
+                for (int i = 0; i < c.cur_len; ++i) nt[i] = pt[i];
+                nt[c.cur_len] = tok;
+                for (int i = new_len; i < c.T; ++i) nt[i] = c.pad_token_id;
+                const int32_t* pa = st.anc_in + pr * c.T;
+                int32_t* na = st.anc_out + nr * c.T;
+                for (int i = 0; i + 1 < c.cur_len; ++i) na[i] = pa[i];
+                na[c.cur_len - 1] = (int32_t)pr;                                // KV of position cur_len-1 lives in the parent's slot
+                uint64_t l = 0, rr = 0;
+                if (c.forced_bos_token_id >= 0 && c.cur_len == 1) {
+                    // the forced BOS is not part of the FM-index query (the reference drops it, :71)
+                    l = st.lo_in[pr]; rr = st.hi_in[pr];
+                } else if (!c.disable_fm_index) {
+                    // incremental get_range: one backward_search_step on the parent's range
+                    // (seal/index.py:102-111 recomputed from scratch by the reference, :96-101)
+                    lf_step(fm, (uint64_t)tok + c.shift, st.lo_in[pr], st.hi_in[pr] - 1, l, rr);
+                    rr += 1;
+                }
+                st.lo_out[nr] = l; st.hi_out[nr] = rr;
+                st.pw_out[nr] = (c.forced_bos_token_id >= 0 && c.cur_len == 1) ? st.pw_in[pr] : st.hi_in[pr] - st.lo_in[pr];
+            } else {
+                S.new_tok[b0 + j] = -1;
+                st.beam_scores_out[nr] = 0.f;
+                st.lo_out[nr] = 0; st.hi_out[nr] = 0; st.pw_out[nr] = 0;
+            }
+        }
+        __syncthreads();                                                         // S is reused by the next group
     }
 }
 
