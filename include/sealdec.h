@@ -173,8 +173,12 @@ int sealdec_generate_dx_ex(sealbart_t* model, const sealfm_t* fm, const uint32_t
                            int32_t* error_flag_d, int64_t src_tokens_hint, const sealdec_groups_t* groups);
 
 /* Options: "cuda_graph" (-1 auto, 0 off, 1 on), "gemm_mode" (switch between the 3xFP16 modes 3/5 and 2 = 3xTF32;
- * the TF32 operand copies are made on first use).  Stats: "last_used_graph", "overflow_fallbacks", "gemm_mode",
- * "cached_graphs" (-1 for an unknown name). */
+ * the TF32 operand copies are made on first use), "fused_head" (-1 = $SEALB200_FUSED_HEAD, default on; 0 = the
+ * lm_head stores every logit and the select kernel streams them for the log-softmax statistics; 1 = where the select
+ * kernels read only the row's allowed tokens, the lm_head emits per-tile statistics and stores only those logits),
+ * "poison_logits" (testing: 1 fills the logits buffer with NaN before every such lm_head).  Stats: "last_used_graph",
+ * "overflow_fallbacks", "gemm_mode", "cached_graphs", "fused_head_steps" (decode steps of the last generate run
+ * eagerly that used the statistics epilogue) (-1 for an unknown name). */
 int     sealbart_set_option(sealbart_t* model, const char* name, int64_t value);
 int64_t sealbart_get_stat(const sealbart_t* model, const char* name);
 
@@ -201,6 +205,17 @@ int sealdec_debug_step_logits(sealbart_t* model, const int64_t* input_ids, const
  * device time per call (CUDA events, includes the activation split). */
 int sealdec_debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A, const float* W,
                        const float* bias, float* C, int32_t gelu, int32_t iters, double* avg_us);
+/* the same with the tile order (mode 3 without split-K; other paths ignore band) and the store as variables
+ * (tools/head_bench.py): band -1 = the order the decoder
+ * uses, 0 = no bands (m fastest over all rows when N > M), > 0 = bands of that many 128-row tiles; store 0 = the
+ * epilogue writes nothing (C may be NULL, and is not written).  Modes 3 / 5 split A into halves once, outside the
+ * timed calls, as the decoder's producers do. */
+int sealdec_debug_gemm_ex(int mode, int64_t M, int32_t N, int32_t K, const float* A, const float* W,
+                          const float* bias, float* C, int32_t gelu, int32_t iters, double* avg_us, int32_t band,
+                          int32_t store);
+/* average device time of the decoder's per-row statistics + top-2*beam kernel over R rows of V pseudo-random logits
+ * (a later step of constrained beam search, per_row allowed tokens per row) */
+int sealdec_debug_topk_rows(int64_t R, int32_t V, int32_t num_beams, int32_t per_row, int32_t iters, double* avg_us);
 /* in-kernel timeline of CTA 0 of the mode-3/4 GEMM kernel (development aid): out20 (may be NULL) receives
  * the stamps of the last traced launch -- SM cycles at 0 entry, 1 prologue done, 2 first operands landed,
  * 3 last MMA issued, 4 last chunk complete, 5 tile stored, 6 exit; 7/8 globaltimer ns at entry / exit --

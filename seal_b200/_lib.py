@@ -119,6 +119,9 @@ _DEC_SIGS = {
     "sealdec_debug_step_logits": (i32, [vp, vp, vp, C.c_int64, C.c_int64, C.c_int32, vp, C.c_int64, vp]),
     "sealdec_debug_gemm": (i32, [i32, C.c_int64, C.c_int32, C.c_int32, vp, vp, vp, vp, C.c_int32, C.c_int32,
                                  C.POINTER(C.c_double)]),
+    "sealdec_debug_gemm_ex": (i32, [i32, C.c_int64, C.c_int32, C.c_int32, vp, vp, vp, vp, C.c_int32, C.c_int32,
+                                    C.POINTER(C.c_double), C.c_int32, C.c_int32]),
+    "sealdec_debug_topk_rows": (i32, [C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_double)]),
     "sealdec_debug_gemm_trace": (i32, [i32, C.POINTER(C.c_int64)]),
     "sealev_first_stage": (i32, [C.c_int64, vp, vp, vp, vp, C.c_int64, vp, vp, vp, i32, i32, C.c_double, C.c_double, C.c_int64, vp, vp]),
     "sealev_score_docs": (i32, [C.c_int64, vp, vp, vp, vp, C.c_int64, C.c_int64, vp, vp, vp, C.c_int64, i32, i32, i32, i32,

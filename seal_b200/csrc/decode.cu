@@ -75,12 +75,17 @@ struct sealbart {
     Buf ex_hi, ex_lo, eattn_hi, eattn_lo, effn_hi, effn_lo, dx_hi, dx_lo, dattn_hi, dattn_lo, dffn_hi, dffn_lo;   // activation splits (halves or TF32)
     Buf st_scores, st_tokens, st_lo, st_hi, st_pw, st_anc, st_mask;
     Buf st_rowmax, st_rowls, st_rule, st_cval, st_cidx, st_ccnt, st_wide;     // scratch between the kernels of a step
+    Buf st_hstat;                     // [R][V / 128] lm_head tile statistics (HeadEpi)
     Buf hy_score, hy_len, hy_tok, hy_valid, hy_lo, hy_hi, err, dbg_ids, force_syms, a_hi, a_lo, splitk;
     std::vector<void*> split_allocs;
     int64_t launches = 0;
     int* ovf = nullptr;               // where the producers raise "fp16 range exceeded" (set by every entry point)
     double phase_us[5] = {0, 0, 0, 0, 0};
     bool profile_gemm = false;
+    int fused_head = -1;              // -1 $SEALB200_FUSED_HEAD (default on), 0 dense lm_head logits, 1 statistics epilogue
+    bool poison_logits = false;
+    int fused_head_steps = 0;         // steps of the last enqueued generate whose lm_head used the statistics epilogue       // testing: the logits buffer is filled with NaN before every statistics-epilogue head
+    int gemm_band = -1;               // sealdec_debug_gemm_ex: -1 tile order chosen by gemm_impl, 0 no bands, > 0 band size
     std::vector<std::pair<cudaEvent_t, cudaEvent_t>> gemm_events;
     double gemm_flops = 0;
     std::vector<cudaEvent_t> events;
@@ -167,7 +172,8 @@ void build_slots(sealbart* m) {
 // ---- launch helpers ----------------------------------------------------------------------------
 // pending: a split-K GEMM whose slices are still unsummed -- its consumer (add+LN on small batches, the attention kernels)
 // folds the finish pass in; defer_rows = how many rows that consumer accepts (0: the GEMM must finish itself)
-struct Ctx { sealbart* m; cudaStream_t s; SplitSrc pending{}; int64_t defer_rows = 0; };
+// head: the lm_head GEMM may use the statistics epilogue (HeadEpi); head_fused reports that it did
+struct Ctx { sealbart* m; cudaStream_t s; SplitSrc pending{}; int64_t defer_rows = 0; HeadEpi head{}; bool head_fused = false; };
 
 // ---- TMA descriptors ------------------------------------------------------------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -219,11 +225,11 @@ SplitOut split_of(const Act& a, int* overflow) {
     return so;
 }
 
-template <typename T, bool GELU, int CL>
+template <typename T, bool GELU, int CL, bool HEAD = false>
 void gemm_launch(cudaStream_t s, int ctas, const CUtensorMap& ahi, const CUtensorMap& alo, const CUtensorMap& whi, const CUtensorMap& wlo,
-                 int64_t M, int N, int K, const float* bias, float w_unscale, float* C, T* C1, T* C2, int ldc, int n_fastest, int* ovf,
-                 int k_slices, int64_t slice_stride) {
-    auto kern = wgmma_gemm_x3_kernel<T, GELU, CL>;
+                 int64_t M, int N, int K, const float* bias, float w_unscale, float* C, T* C1, T* C2, int ldc, int n_fastest, int m_band,
+                 int* ovf, int k_slices, int64_t slice_stride, const HeadEpi& he = HeadEpi{}) {
+    auto kern = wgmma_gemm_x3_kernel<T, GELU, CL, HEAD>;
     CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, G_SMEM));
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -231,8 +237,8 @@ void gemm_launch(cudaStream_t s, int ctas, const CUtensorMap& ahi, const CUtenso
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3((unsigned)ctas); cfg.blockDim = dim3(GTHREADS); cfg.dynamicSmemBytes = G_SMEM; cfg.stream = s;
     cfg.attrs = attr; cfg.numAttrs = 1;
-    CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, ahi, alo, whi, wlo, (int)M, N, K, bias, w_unscale, C, C1, C2, ldc, n_fastest, ovf,
-                                  k_slices, slice_stride));
+    CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, ahi, alo, whi, wlo, (int)M, N, K, bias, w_unscale, C, C1, C2, ldc, n_fastest, m_band, ovf,
+                                  k_slices, slice_stride, he));
 }
 
 // C = A W^T + b (+GELU) on the tensor cores: gemm_mode 3 / 5 = 3xFP16 (one CTA per tile / clusters of 2 sharing W), 2 = 3xTF32 (fp32
@@ -286,8 +292,8 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
             if (!l.maps2_ready) { make_map(&l.map2_hi, l.w_h1, N, K, K, GN / 2, true); make_map(&l.map2_lo, l.w_h2, N, K, K, GN / 2, true); l.maps2_ready = true; }
             const int groups = (int)((M + 2 * GM - 1) / (2 * GM)) * ((N + GN - 1) / GN);
             const int ctas = 2 * std::min(groups, sm_count() / 2);
-            if (gelu) gemm_launch<__half, true, 2>(cx.s, ctas, ma1, ma2, l.map2_hi, l.map2_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, ovf, 1, 0);
-            else gemm_launch<__half, false, 2>(cx.s, ctas, ma1, ma2, l.map2_hi, l.map2_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, ovf, 1, 0);
+            if (gelu) gemm_launch<__half, true, 2>(cx.s, ctas, ma1, ma2, l.map2_hi, l.map2_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, 0, ovf, 1, 0);
+            else gemm_launch<__half, false, 2>(cx.s, ctas, ma1, ma2, l.map2_hi, l.map2_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, 0, ovf, 1, 0);
             m->launches++;
             return;
         }
@@ -296,7 +302,7 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
             m->splitk.ensure((size_t)k_slices * slice_stride * 4);
             float* part = m->splitk.as<float>();
             const int ctas2 = std::min(tiles * k_slices, sm_count());
-            gemm_launch<__half, false, 1>(cx.s, ctas2, ma1, ma2, l.map_hi, l.map_lo, M, N, K, nullptr, 1.0f, part, nullptr, nullptr, ldc, n_fastest, ovf,
+            gemm_launch<__half, false, 1>(cx.s, ctas2, ma1, ma2, l.map_hi, l.map_lo, M, N, K, nullptr, 1.0f, part, nullptr, nullptr, ldc, n_fastest, 0, ovf,
                                           k_slices, slice_stride);
             m->launches++;
             if (M <= cx.defer_rows && !gelu && !C.h1 && !C.hi && ldc == N && l.b) {     // summed by the consumer kernel
@@ -309,9 +315,19 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
             CUDA_CHECK(cudaGetLastError()); m->launches++;
             return;
         }
+        // m fastest with more A than a band holds (the lm_head at thousands of rows): bands of m tiles whose A halves
+        // take <= 8 MB of the 50 MB L2, so A is read from HBM once and W once per band (wgmma_gemm.cuh, tile_coords).
+        // 8 MB (16 tiles at K = 1 024) measured fastest of 4 / 8 / 16 / 32 MB bands for the lm_head at 15 000 rows
+        // (tools/head_bench.py); the band shares the L2 with the streaming W tiles and the logits stores.
+        const int64_t a_tile_bytes = (int64_t)GM * K * 4, band_bytes = 8ll << 20;
+        int band = (!n_fastest && M * K * 4 > band_bytes) ? (int)std::max<int64_t>(1, band_bytes / a_tile_bytes) : 0;
+        if (m->gemm_band >= 0) band = m->gemm_band;
         const int ctas = std::min(tiles, sm_count());
-        if (gelu) gemm_launch<__half, true, 1>(cx.s, ctas, ma1, ma2, l.map_hi, l.map_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, ovf, 1, 0);
-        else gemm_launch<__half, false, 1>(cx.s, ctas, ma1, ma2, l.map_hi, l.map_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, ovf, 1, 0);
+        if (cx.head.stats && !gelu) {
+            gemm_launch<__half, false, 1, true>(cx.s, ctas, ma1, ma2, l.map_hi, l.map_lo, M, N, K, l.b, l.w_unscale, C.x, nullptr, nullptr, ldc, n_fastest, band, ovf, 1, 0, cx.head);
+            cx.head_fused = true;
+        } else if (gelu) gemm_launch<__half, true, 1>(cx.s, ctas, ma1, ma2, l.map_hi, l.map_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, band, ovf, 1, 0);
+        else gemm_launch<__half, false, 1>(cx.s, ctas, ma1, ma2, l.map_hi, l.map_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, band, ovf, 1, 0);
         m->launches++;
         return;
     }
@@ -326,8 +342,8 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
         make_map(&mah, ahi, M, K, K, GM); make_map(&mal, alo, M, K, K, GM);
         if (!l.maps_ready) { make_map(&l.map_hi, l.w_hi, N, K, K, GN); make_map(&l.map_lo, l.w_lo, N, K, K, GN); l.maps_ready = true; }
         const int ctas = std::min(tiles, sm_count());
-        if (gelu) gemm_launch<float, true, 1>(cx.s, ctas, mah, mal, l.map_hi, l.map_lo, M, N, K, l.b, 1.0f, C.x, C.hi, C.lo, ldc, n_fastest, m->ovf, 1, 0);
-        else gemm_launch<float, false, 1>(cx.s, ctas, mah, mal, l.map_hi, l.map_lo, M, N, K, l.b, 1.0f, C.x, C.hi, C.lo, ldc, n_fastest, m->ovf, 1, 0);
+        if (gelu) gemm_launch<float, true, 1>(cx.s, ctas, mah, mal, l.map_hi, l.map_lo, M, N, K, l.b, 1.0f, C.x, C.hi, C.lo, ldc, n_fastest, 0, m->ovf, 1, 0);
+        else gemm_launch<float, false, 1>(cx.s, ctas, mah, mal, l.map_hi, l.map_lo, M, N, K, l.b, 1.0f, C.x, C.hi, C.lo, ldc, n_fastest, 0, m->ovf, 1, 0);
         m->launches++;
         return;
     }
@@ -438,6 +454,7 @@ void ensure_workspace(sealbart* m, const Dims& D) {
     m->st_lo.ensure(2 * D.R * 8); m->st_hi.ensure(2 * D.R * 8); m->st_pw.ensure(2 * D.R * 8);
     m->st_anc.ensure(2 * D.R * D.T * 4); m->st_mask.ensure((size_t)2 * D.R * D.W * 4);
     m->st_rowmax.ensure(D.R * 4); m->st_rowls.ensure(D.R * 4); m->st_rule.ensure(D.R);
+    m->st_hstat.ensure((size_t)D.R * ((D.V + GN - 1) / GN) * 8);
     m->st_cval.ensure((size_t)D.R * 2 * D.B * 4); m->st_cidx.ensure((size_t)D.R * 2 * D.B * 4); m->st_ccnt.ensure(D.R * 4);
     {
         m->ex_hi.ensure(Tk * D.d * 4); m->ex_lo.ensure(Tk * D.d * 4);
@@ -528,7 +545,7 @@ void encoder_forward(Ctx& cx, const Dims& D, const int64_t* ids_d, const int64_t
 // row's logits for all of the query's beams (StepCfg::logits_shared); the k / v of position 0 are written to the
 // cache entries of all B beams.  1/T of the decoder + lm_head work disappears (~8 % of a 9-step generate).
 void decoder_step(Ctx& cx, const Dims& D, const int32_t* tokens, int cur_len, const int32_t* anc, bool want_logits,
-                  cudaEvent_t ev_layers_done, bool compact = false) {
+                  cudaEvent_t ev_layers_done, bool compact = false, const HeadEpi& head = HeadEpi{}) {
     sealbart* m = cx.m;
     const int d = D.d; const int64_t Rc = D.R; const int64_t Tk = D.Q * D.S;
     if (compact && (cur_len != 1 || D.grp_start)) throw ApiError(SEALFM_EINVAL, "internal: compact step only at position 0 of a generate");
@@ -613,7 +630,9 @@ void decoder_step(Ctx& cx, const Dims& D, const int32_t* tokens, int cur_len, co
         add_ln(cx, R, d, x.x, tmp.x, L.ln_final, x);
     }
     if (ev_layers_done) CUDA_CHECK(cudaEventRecord(ev_layers_done, cx.s));
+    cx.head = head;                 // only the lm_head may take the statistics epilogue
     if (want_logits) gemm(cx, R, D.V, d, x, d, m->head, Act{m->logits.as<float>()}, D.ld, false);
+    cx.head = HeadEpi{};
 }
 
 void check_model(const sealbart* m) {
@@ -688,7 +707,7 @@ void sealbart_free(sealbart_t* m) {
     if (m->lm_head_given) cudaFree(m->lm_head);
     for (Buf* b : {&m->enc_tok, &m->enc_mask, &m->src_off, &m->ex, &m->eqkv, &m->eattn, &m->etmp, &m->effn, &m->ckv, &m->dx, &m->dqkv,
                    &m->dattn, &m->dtmp, &m->dcq, &m->dffn, &m->logits, &m->kc, &m->vc, &m->st_scores, &m->st_tokens,
-                   &m->st_lo, &m->st_hi, &m->st_pw, &m->st_anc, &m->st_mask, &m->st_rowmax, &m->st_rowls, &m->st_rule, &m->st_cval,
+                   &m->st_lo, &m->st_hi, &m->st_pw, &m->st_anc, &m->st_mask, &m->st_rowmax, &m->st_hstat, &m->st_rowls, &m->st_rule, &m->st_cval,
                    &m->st_cidx, &m->st_ccnt, &m->st_wide, &m->hy_score, &m->hy_len, &m->hy_tok,
                    &m->hy_valid, &m->hy_lo, &m->hy_hi, &m->err, &m->dbg_ids, &m->force_syms, &m->a_hi, &m->a_lo, &m->ex_hi, &m->ex_lo,
                    &m->eattn_hi, &m->eattn_lo, &m->effn_hi, &m->effn_lo, &m->dx_hi, &m->dx_lo, &m->dattn_hi, &m->dattn_lo,
@@ -789,6 +808,11 @@ struct GenArgs {
 
 // Enqueues one whole generate (encoder, every decode step, records) on cx.s.  No host synchronisation unless
 // src_hint == -1.  `timing` = bracket the phases with CUDA events (not possible while the stream is being captured).
+bool fused_head_on(const sealbart* m) {
+    static const bool env_on = [] { const char* e = std::getenv("SEALB200_FUSED_HEAD"); return !e || std::atoi(e) != 0; }();
+    return m->fused_head >= 0 ? m->fused_head != 0 : env_on;
+}
+
 void generate_enqueue(Ctx& cx, const Dims& D, const GenArgs& a, const FmView& view, uint64_t lo0, uint64_t hi0,
                       int64_t src_hint, bool timing) {
     sealbart* m = cx.m;
@@ -804,6 +828,7 @@ void generate_enqueue(Ctx& cx, const Dims& D, const GenArgs& a, const FmView& vi
         return e;
     };
     CUDA_CHECK(cudaMemsetAsync(a.err_d, 0, 16, cx.s));
+    m->fused_head_steps = 0;
     mark();
     encoder_forward(cx, D, a.ids_d, a.mask_d, src_hint, a.err_d + 2);
     mark();
@@ -849,13 +874,32 @@ void generate_enqueue(Ctx& cx, const Dims& D, const GenArgs& a, const FmView& vi
                                 !(p->forced_bos_token_id >= 0 && cur_len == 1);
         const bool dead = skip_dead && forced_all;
         cudaEvent_t b = timing ? new_event(m) : nullptr;
-        if (!dead) decoder_step(cx, D, tk[cur], cur_len, an[cur], true, b, compact);
+        // Statistics epilogue of the lm_head (HeadEpi): the select kernels then read this step's logits only at the
+        // row's read set.  topk_rows_kernel reads lp[v] for v in row_bits() and select_merge_kernel (G > 1) for the
+        // candidates it re-scores.  With the FM index on, past the first (shared-mask) step and with one group,
+        // row_bits() is the row's mask_in bits, or eos (rule 1), or pad (rule 2), plus eos with always_allow_eos --
+        // within mask bits + {eos, pad}; apply_processors only overwrites values.  select_merge_kernel's -inf fill-ins
+        // (fewer than K = 2B finite candidates, want < K) read the unconstrained score of the lowest flat indices of the
+        // query that are not finite candidates: fewer than K + want < 2K <= 128 flat indices from the query's first
+        // row, i.e. columns 0..127 of that row (V >= 128) -- the first n tile, which HeadEpi stores in full for every
+        // row.  Every other case stays dense:
+        // the compact first step, disable_fm_index, forced BOS (eff_len 1 reads the occurring mask), G > 1, the
+        // other GEMM modes.
+        const int eff_len = cur_len - (p->forced_bos_token_id >= 0 ? 1 : 0);
+        HeadEpi he{};
+        if (fused_head_on(m) && !dead && !compact && !p->disable_fm_index && eff_len > 1 && G == 1 && m->cfg.gemm_mode == 3) {
+            he = HeadEpi{m->st_hstat.as<float2>(), mk[cur], (int)D.W, p->eos_token_id, p->pad_token_id};
+            if (m->poison_logits) CUDA_CHECK(cudaMemsetAsync(m->logits.p, 0xFF, (size_t)D.R * D.ld * 4, cx.s));
+        }
+        cx.head_fused = false;
+        if (!dead) decoder_step(cx, D, tk[cur], cur_len, an[cur], true, b, compact, he);
         else if (b) CUDA_CHECK(cudaEventRecord(b, cx.s));
         mark();
         c.cur_len = cur_len;
         c.logits_shared = (compact && !dead) ? 1 : 0;
         c.logits_ignored = dead ? 1 : 0;
-        const int eff_len = cur_len - (p->forced_bos_token_id >= 0 ? 1 : 0);
+        c.head_tiles = cx.head_fused ? (D.V + GN - 1) / GN : 0;
+        m->fused_head_steps += cx.head_fused ? 1 : 0;
         c.first_step_shared_mask = (!p->disable_fm_index && eff_len == 1) ? 1 : 0;
         c.expand_next = (cur_len + 1 < T) ? 1 : 0;
         c.hyp_base = step * K;
@@ -866,7 +910,7 @@ void generate_enqueue(Ctx& cx, const Dims& D, const GenArgs& a, const FmView& vi
         st.pw_in = pw[cur]; st.pw_out = pw[cur ^ 1];
         st.anc_in = an[cur]; st.anc_out = an[cur ^ 1];
         st.mask_in = mk[cur]; st.mask_out = mk[cur ^ 1];
-        st.occurring_mask = a.occ_d; st.logits = m->logits.as<float>();
+        st.occurring_mask = a.occ_d; st.logits = m->logits.as<float>(); st.head_stats = m->st_hstat.as<float2>();
         st.hyp_score = a.o_score; st.hyp_len = a.o_len; st.hyp_tokens = a.o_tok; st.hyp_valid = a.o_valid;
         st.hyp_lo = a.o_lo; st.hyp_hi = a.o_hi; st.error_flag = a.err_d;
         // first step: beams 1.. carry -1e9 and are pruned exactly inside one CTA per query; afterwards one CTA per row.
@@ -988,6 +1032,7 @@ int sealdec_generate_dx_ex(sealbart_t* m, const sealfm_t* fm, const uint32_t* oc
         sealdec_params_t pc = *p; pc.force_decoding_from = nullptr; key_put(key, pc);
         for (int i = 0; i < p->n_force_decoding_from; ++i) key_put(key, p->force_decoding_from[i]);
         key_put(key, grp.num_beam_groups); key_put(key, grp.diversity_penalty);
+        key_put(key, fused_head_on(m)); key_put(key, m->poison_logits);
         key_put(key, view.blocks); key_put(key, view.csym); key_put(key, view.node_tab); key_put(key, view.m);
         key_put(key, occ_d); key_put(key, ids_d); key_put(key, mask_d); key_put(key, o_score); key_put(key, o_len);
         key_put(key, o_tok); key_put(key, o_valid); key_put(key, o_lo); key_put(key, o_hi); key_put(key, err_d);
@@ -1074,6 +1119,11 @@ int sealbart_set_option(sealbart_t* m, const char* name, int64_t value) {
             for_each_lin(m, [](Lin& l) { l.maps_ready = false; l.maps2_ready = false; });
             drop_graphs(m);
         }
+        else if (n == "fused_head") {
+            if (value < -1 || value > 1) throw ApiError(SEALFM_EINVAL, "fused_head: -1 environment, 0 off, 1 on");
+            m->fused_head = (int)value;
+        }
+        else if (n == "poison_logits") m->poison_logits = value != 0;
         else throw ApiError(SEALFM_EINVAL, "unknown option: " + n);
     });
 }
@@ -1085,6 +1135,7 @@ int64_t sealbart_get_stat(const sealbart_t* m, const char* name) {
     if (n == "overflow_fallbacks") return m->overflow_fallbacks;
     if (n == "gemm_mode") return m->cfg.gemm_mode;
     if (n == "cached_graphs") return (int64_t)m->graphs.size();
+    if (n == "fused_head_steps") return m->fused_head_steps;
     return -1;
 }
 
@@ -1299,10 +1350,15 @@ int sealdec_teacher_forced(sealbart_t* m, const int64_t* ids, const int64_t* mas
     });
 }
 
-int sealdec_debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A, const float* W, const float* bias, float* C,
-                       int32_t gelu, int32_t iters, double* avg_us) {
+}  // extern "C"
+
+namespace {
+
+// presplit: the activations are split into halves once, outside the timed calls (as the decoder's producers do)
+int debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A, const float* W, const float* bias, float* C,
+               int32_t gelu, int32_t iters, double* avg_us, int32_t band, int32_t store, bool presplit) {
     return guarded([&] {
-        if (!A || !W || !C || M <= 0 || N <= 0 || K <= 0) throw ApiError(SEALFM_EINVAL, "bad argument");
+        if (!A || !W || (store && !C) || M <= 0 || N <= 0 || K <= 0 || band < -1) throw ApiError(SEALFM_EINVAL, "bad argument");
         int count = 0;
         if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) { cudaGetLastError(); throw ApiError(SEALFM_ENODEVICE, "no CUDA device available"); }
         if (mode != 2 && mode != 3 && mode != 5) throw ApiError(SEALFM_EINVAL, "gemm_mode must be 2, 3 or 5");
@@ -1332,20 +1388,98 @@ int sealdec_debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A
             split_half_kernel<<<sm_count() * 8, 256>>>((int64_t)N * K, l.w, std::ldexp(1.0f, sexp), l.w_h1, l.w_h2, fake.err.as<int>() + 1);
             CUDA_CHECK(cudaGetLastError());
         }
+        fake.gemm_band = band;
+        Act a{dA.as<float>()};
+        Buf ah1, ah2;
+        struct RelA { Buf *x, *y; ~RelA() { x->release(); y->release(); } } rela{&ah1, &ah2};
+        if (presplit && mode >= 3) {
+            ah1.ensure((size_t)M * K * 2); ah2.ensure((size_t)M * K * 2);
+            a.h1 = ah1.as<__half>(); a.h2 = ah2.as<__half>();
+            split_half_kernel<<<sm_count() * 8, 256>>>((int64_t)M * K, a.x, 1.0f, a.h1, a.h2, fake.ovf);
+            CUDA_CHECK(cudaGetLastError());
+        }
+        const Act c{store ? dC.as<float>() : nullptr};
         Ctx cx{&fake, nullptr};
-        gemm(cx, M, N, K, Act{dA.as<float>()}, K, l, Act{dC.as<float>()}, ldc, gelu != 0);
+        gemm(cx, M, N, K, a, K, l, c, ldc, gelu != 0);
         CUDA_CHECK(cudaDeviceSynchronize());
         if (iters > 0 && avg_us) {
             cudaEvent_t e0, e1; CUDA_CHECK(cudaEventCreate(&e0)); CUDA_CHECK(cudaEventCreate(&e1));
             CUDA_CHECK(cudaEventRecord(e0, nullptr));
-            for (int i = 0; i < iters; ++i) gemm(cx, M, N, K, Act{dA.as<float>()}, K, l, Act{dC.as<float>()}, ldc, gelu != 0);
+            for (int i = 0; i < iters; ++i) gemm(cx, M, N, K, a, K, l, c, ldc, gelu != 0);
             CUDA_CHECK(cudaEventRecord(e1, nullptr));
             CUDA_CHECK(cudaEventSynchronize(e1));
             float ms = 0; CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
             *avg_us = (double)ms * 1e3 / iters;
             cudaEventDestroy(e0); cudaEventDestroy(e1);
         }
-        CUDA_CHECK(cudaMemcpy2D(C, (size_t)N * 4, dC.p, (size_t)ldc * 4, (size_t)N * 4, M, cudaMemcpyDeviceToHost));
+        if (store) CUDA_CHECK(cudaMemcpy2D(C, (size_t)N * 4, dC.p, (size_t)ldc * 4, (size_t)N * 4, M, cudaMemcpyDeviceToHost));
+    });
+}
+
+// deterministic pseudo-random logits in [-8, 8) and `per_row` allowed tokens per row
+__global__ void debug_fill_rows_kernel(int64_t R, int V, int ld, int W, int per_row, float* __restrict__ logits, uint32_t* __restrict__ mask) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < R * ld; i += (int64_t)gridDim.x * blockDim.x) {
+        uint32_t h = (uint32_t)i * 2654435761u; h ^= h >> 15; h *= 2246822519u; h ^= h >> 13;
+        logits[i] = (float)(h >> 8) * (16.f / 16777216.f) - 8.f;
+        if (i < R * per_row) {
+            const int64_t r = i / per_row;
+            const int v = (int)((uint64_t)(i % per_row + 1) * 7919u * (uint64_t)(r + 1) % (uint64_t)V);
+            atomicOr(&mask[r * W + (v >> 5)], 1u << (v & 31));
+        }
+    }
+}
+
+}  // namespace
+
+extern "C" {
+
+int sealdec_debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A, const float* W, const float* bias, float* C,
+                       int32_t gelu, int32_t iters, double* avg_us) {
+    return debug_gemm(mode, M, N, K, A, W, bias, C, gelu, iters, avg_us, -1, 1, false);
+}
+
+int sealdec_debug_gemm_ex(int mode, int64_t M, int32_t N, int32_t K, const float* A, const float* W, const float* bias, float* C,
+                          int32_t gelu, int32_t iters, double* avg_us, int32_t band, int32_t store) {
+    return debug_gemm(mode, M, N, K, A, W, bias, C, gelu, iters, avg_us, band, store, true);
+}
+
+int sealdec_debug_topk_rows(int64_t R, int32_t V, int32_t num_beams, int32_t per_row, int32_t iters, double* avg_us) {
+    return guarded([&] {
+        if (R <= 0 || V <= 0 || num_beams < 1 || num_beams > kSelMaxBeams || R % num_beams || per_row < 0 || iters <= 0 || !avg_us)
+            throw ApiError(SEALFM_EINVAL, "bad argument");
+        int count = 0;
+        if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) { cudaGetLastError(); throw ApiError(SEALFM_ENODEVICE, "no CUDA device available"); }
+        const int ld = (V + 3) / 4 * 4, W = (V + 31) / 32, B = num_beams, K = 2 * B, T = 3;
+        Buf lg, mk, sc, tk, pw, rmax, rls, rule, cval, cidx, ccnt;
+        struct Rel { std::vector<Buf*> v; ~Rel() { for (auto b : v) b->release(); } } rel{{&lg, &mk, &sc, &tk, &pw, &rmax, &rls, &rule, &cval, &cidx, &ccnt}};
+        lg.ensure((size_t)R * ld * 4); mk.ensure((size_t)R * W * 4); sc.ensure((size_t)R * 4); tk.ensure((size_t)R * T * 4);
+        pw.ensure((size_t)R * 8); rmax.ensure((size_t)R * 4); rls.ensure((size_t)R * 4); rule.ensure((size_t)R);
+        cval.ensure((size_t)R * K * 4); cidx.ensure((size_t)R * K * 4); ccnt.ensure((size_t)R * 4);
+        CUDA_CHECK(cudaMemset(mk.p, 0, (size_t)R * W * 4)); CUDA_CHECK(cudaMemset(sc.p, 0, (size_t)R * 4));
+        CUDA_CHECK(cudaMemset(tk.p, 0, (size_t)R * T * 4)); CUDA_CHECK(cudaMemset(pw.p, 0, (size_t)R * 8));
+        debug_fill_rows_kernel<<<sm_count() * 8, 256>>>(R, V, ld, W, per_row, lg.as<float>(), mk.as<uint32_t>());
+        CUDA_CHECK(cudaGetLastError());
+        // a later step (cur_len 2) of plain constrained beam search: every row is its own candidate list
+        StepCfg c{};
+        c.num_beams = B; c.K = K; c.V = V; c.ld = ld; c.cur_len = 2; c.min_length = 0; c.max_length = T;
+        c.eos_token_id = 2; c.pad_token_id = 1; c.model_eos_token_id = 2; c.forced_eos_token_id = -1; c.forced_bos_token_id = -1;
+        c.T = T; c.mask_words = W; c.expand_next = 1; c.num_groups = 1;
+        StepState st{};
+        st.beam_scores_in = sc.as<float>(); st.tokens_in = tk.as<int32_t>(); st.pw_in = pw.as<uint64_t>();
+        st.mask_in = mk.as<uint32_t>(); st.logits = lg.as<float>();
+        RowScratch rs{rmax.as<float>(), rls.as<float>(), rule.as<uint8_t>(), cval.as<float>(), cidx.as<int32_t>(), ccnt.as<int32_t>()};
+        using RowsLater = SelSharedT<4096>;
+        CUDA_CHECK(cudaFuncSetAttribute(topk_rows_kernel<256, 4096>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RowsLater)));
+        launch_k(topk_rows_kernel<256, 4096>, (unsigned)R, 256, sizeof(RowsLater), nullptr, c, st, rs, B, 1);
+        CUDA_CHECK(cudaDeviceSynchronize());
+        cudaEvent_t e0, e1; CUDA_CHECK(cudaEventCreate(&e0)); CUDA_CHECK(cudaEventCreate(&e1));
+        CUDA_CHECK(cudaEventRecord(e0, nullptr));
+        for (int i = 0; i < iters; ++i) launch_k(topk_rows_kernel<256, 4096>, (unsigned)R, 256, sizeof(RowsLater), nullptr, c, st, rs, B, 1);
+        CUDA_CHECK(cudaEventRecord(e1, nullptr));
+        CUDA_CHECK(cudaEventSynchronize(e1));
+        float ms = 0; CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
+        *avg_us = (double)ms * 1e3 / iters;
+        cudaEventDestroy(e0); cudaEventDestroy(e1);
     });
 }
 

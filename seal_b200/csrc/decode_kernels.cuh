@@ -36,6 +36,8 @@ struct StepCfg {
     int32_t hyp_base;                  // index of this step's first hypothesis record
     int32_t num_groups;                // diverse beam groups G (1: constrained_beam_search; > 1: group_beam_search)
     float diversity_penalty;           // Hamming diversity penalty, 0 = no HammingDiversityLogitsProcessor
+    int32_t head_tiles;                // > 0: the lm_head wrote per-(row, n tile) statistics (head_stats, HeadEpi) and the
+                                       //    logits only at the row's read set; 0: dense logits, statistics streamed here
 };
 
 struct StepState {
@@ -49,6 +51,7 @@ struct StepState {
     const uint32_t* mask_in;      uint32_t* mask_out;         // [R][mask_words] allowed-token bitmasks
     const uint32_t* occurring_mask;                           // [mask_words]
     const float* logits;                                      // [R][ld]
+    const float2* head_stats;                                 // [R][head_tiles] (max, sum exp(x - max)) per lm_head tile
     // hypothesis records
     float* hyp_score; int32_t* hyp_len; int32_t* hyp_tokens; uint8_t* hyp_valid; uint64_t* hyp_lo; uint64_t* hyp_hi;
     int32_t* error_flag;
@@ -190,6 +193,14 @@ __global__ void __launch_bounds__(THREADS, THREADS >= 512 ? 2 : 4) topk_rows_ker
         float mx = -INFINITY, se = 0.f;
         if (c.logits_ignored) { mx = 0.f; se = 1.f; }           // log-softmax statistics are never used (uniform branch)
         else {
+        if (c.head_tiles > 0) {                                  // the lm_head's partials, a fixed order per thread
+            const float2* ps = st.head_stats + r * c.head_tiles;
+            for (int i = tid; i < c.head_tiles; i += THREADS) {
+                const float2 p = ps[i];
+                if (p.x > mx) { se = se * expf(mx - p.x) + p.y; mx = p.x; }
+                else if (p.x > -INFINITY) se += p.y * expf(p.x - mx);
+            }
+        } else {
         // four 16-byte loads in flight per thread, one running-max update per 16 values
         constexpr int kStride = THREADS * 4;
         int v = tid * 4;
@@ -222,6 +233,7 @@ __global__ void __launch_bounds__(THREADS, THREADS >= 512 ? 2 : 4) topk_rows_ker
             const float m4 = fmaxf(fmaxf(x0, x1), fmaxf(x2, x3));
             if (m4 > mx) { se *= expf(mx - m4); mx = m4; }          // mx = -inf: se is 0, expf(-inf) = 0
             if (mx > -INFINITY) se += expf(x0 - mx) + expf(x1 - mx) + expf(x2 - mx) + expf(x3 - mx);
+        }
         }
         {
             const float bm = block_reduce_max(mx, S.red);

@@ -217,21 +217,45 @@ __device__ __forceinline__ void store_pair(float* C, float* S1, float* S2, int64
     }
 }
 
+// Tile group (mg, n_tile) of work index `tile`.  n_fastest: row-major over (m group, n tile).  Otherwise the m groups
+// are walked in bands of `band` groups (0: one band of all of them), band after band; inside a band the walk is
+// n-major with m fastest, so the concurrent CTAs share W tiles and the band's A rows are re-read from L2, not HBM.
+// Producer and consumers of a CTA must agree on this mapping.
+__device__ __forceinline__ void tile_coords(int tile, int n_fastest, int band, int m_groups, int n_tiles, int& mg, int& n_tile) {
+    if (n_fastest) { mg = tile / n_tiles; n_tile = tile % n_tiles; return; }
+    if (band <= 0 || band > m_groups) band = m_groups;
+    const int b0 = tile / (band * n_tiles) * band;                       // first m group of the band
+    const int rows = min(band, m_groups - b0);
+    const int r = tile - b0 * n_tiles;
+    n_tile = r / rows; mg = b0 + r % rows;
+}
+
+// lm_head epilogue of a constrained-decode step (HEAD = true, 3xFP16, CL = 1, no split-K).  Per (row, n tile) it writes
+// the partial log-softmax statistics (max, sum exp(x - max)) over the tile's columns n < N to stats[row * n_tiles +
+// n_tile], which topk_rows_kernel combines in place of streaming the row, and it stores x only at the columns the select
+// kernels read (the read set): the row's bits of `mask` ([M][mask_words]), eos and pad (topk_rows_kernel, row_bits),
+// and the whole first n tile, columns 0..127 (select_merge_kernel's -inf fill-ins, see generate_enqueue).
+struct HeadEpi {
+    float2* stats = nullptr; const uint32_t* mask = nullptr; int mask_words = 0; int eos = -1, pad = -1;
+};
+
 // T = __half (3xFP16) or float (3xTF32); CL = CTAs per cluster sharing the W tile (1 or 2).
 // Persistent: work unit u = blockIdx.x / CL walks units u, u + gridDim.x / CL, ...  A unit is (tile group, K slice);
-// a tile group is CL vertically adjacent 128 x 128 tiles.  Tile order is chosen by the host so that the LARGER operand
-// is streamed from HBM once: n fastest when the activations dominate (concurrent CTAs then share A tiles and all of W
-// stays in L2), m fastest when the weights dominate (lm_head).
+// a tile group is CL vertically adjacent 128 x 128 tiles.  Tile order is chosen by the host (tile_coords): n fastest
+// when the activations dominate (concurrent CTAs then share A tiles and all of W stays in L2), m fastest when the
+// weights dominate (lm_head).  With m fastest each n column re-reads all of A, which streams from HBM once per column
+// when A is larger than the L2 (lm_head at 15 000 rows: 61 MB of A halves, 393 columns); m_band > 0 then bounds the
+// A rows in flight to a band that stays in L2, so A is read from HBM once and W once per band.
 // Split-K (CL = 1 only; skinny M, where a handful of tiles would leave most SMs idle): slice s accumulates k-blocks
 // [s*num_k, (s+1)*num_k) and stores its raw fp32 partial tile at C + s*slice_stride (the caller passes bias = nullptr,
 // w_unscale = 1, no split outputs; gemm_splitk_finish_kernel or the consumer kernel sums the slices in a fixed order).
-template <typename T, bool GELU, int CL>
+template <typename T, bool GELU, int CL, bool HEAD = false>
 __global__ void __launch_bounds__(GTHREADS, 1)
 wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                      const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo,
                      int M, int N, int K, const float* __restrict__ bias, float w_unscale, float* __restrict__ C,
-                     T* __restrict__ C_s1, T* __restrict__ C_s2, int ldc, int n_fastest, int* __restrict__ overflow,
-                     int k_slices, int64_t slice_stride) {
+                     T* __restrict__ C_s1, T* __restrict__ C_s2, int ldc, int n_fastest, int m_band, int* __restrict__ overflow,
+                     int k_slices, int64_t slice_stride, HeadEpi he) {
     using E = GemmElem<T>;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;          // SWIZZLE_128B wants 1024 B alignment
@@ -260,7 +284,8 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
             uint32_t it = 0;                                               // k-blocks issued so far (all units)
             for (int u = unit0; u < total; u += n_units) {
                 const int tile = u / k_slices, kb0 = (u % k_slices) * num_k;
-                const int mg = n_fastest ? tile / n_tiles : tile % m_groups, n_tile = n_fastest ? tile % n_tiles : tile / m_groups;
+                int mg, n_tile;
+                tile_coords(tile, n_fastest, m_band, m_groups, n_tiles, mg, n_tile);
                 const int row_a = (mg * CL + (int)rank) * GM;
                 for (int kb = 0; kb < num_k; ++kb, ++it) {
                     const int s = it % GSTAGES;
@@ -336,11 +361,49 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
             if (first && t == 0 && wg == 1) gemm_trace(4);
             // accumulator layout of m64n128: warp w holds rows 16w + lane/4 (+8); register 4j + {0,1} / {2,3} holds
             // columns 8j + 2 (lane % 4) + {0, 1} of the first / second of those rows
-            const int mg = n_fastest ? tile / n_tiles : tile % m_groups, n_tile = n_fastest ? tile % n_tiles : tile / m_groups;
+            int mg, n_tile;
+            tile_coords(tile, n_fastest, m_band, m_groups, n_tiles, mg, n_tile);
             const int row0 = (mg * CL + (int)rank) * GM + (wg - 1) * 64 + warp * 16 + (lane >> 2);
             const int col0 = n_tile * GN + 2 * (lane & 3);
             float* Cs = C ? C + (int64_t)(u % k_slices) * slice_stride : nullptr;
             int ov = 0;
+            if constexpr (HEAD) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int row = row0 + 8 * h;
+                    auto xv = [&](int j, int e) {
+                        const int n = col0 + 8 * j + e;
+                        return n < N ? acc[4 * j + 2 * h + e] * w_unscale + (bias ? bias[n] : 0.f) : -INFINITY;
+                    };
+                    // the 4 lanes of a quad hold the row's 128 columns: reduce across them (all lanes take part)
+                    float mx = -INFINITY;
+#pragma unroll
+                    for (int j = 0; j < 16; ++j) mx = fmaxf(mx, fmaxf(xv(j, 0), xv(j, 1)));
+                    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+                    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+                    float se = 0.f;
+                    if (mx > -INFINITY) {
+#pragma unroll
+                        for (int j = 0; j < 16; ++j) se += expf(xv(j, 0) - mx) + expf(xv(j, 1) - mx);
+                    }
+                    se += __shfl_xor_sync(0xffffffffu, se, 1);
+                    se += __shfl_xor_sync(0xffffffffu, se, 2);
+                    if (row >= M) continue;
+                    if ((lane & 3) == 0) he.stats[(int64_t)row * n_tiles + n_tile] = make_float2(mx, se);
+                    const uint32_t* mrow = he.mask + (int64_t)row * he.mask_words;
+                    uint32_t w[4];
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) w[i] = n_tile * 4 + i < he.mask_words ? mrow[n_tile * 4 + i] : 0u;
+#pragma unroll
+                    for (int j = 0; j < 16; ++j) {
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int n = col0 + 8 * j + e, bit = 8 * (j & 3) + 2 * (lane & 3) + e;
+                            if (n < N && (n_tile == 0 || ((w[j >> 2] >> bit) & 1u) || n == he.eos || n == he.pad)) Cs[(int64_t)row * ldc + n] = xv(j, e);
+                        }
+                    }
+                }
+            } else
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int row = row0 + 8 * h;
