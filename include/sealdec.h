@@ -107,6 +107,9 @@ int64_t sealdec_hyps_per_query(const sealdec_params_t* p);
  *                                    finalize records carry 2
  *   out_lo/out_hi uint64 [Q][H]      SA range [lo,hi) of the hypothesis' tokens[1:] (0,0 if invalid
  *                                    or FM index disabled); may be NULL
+ * Every source must attend to at least one position: a row of attention_mask that is all zero is rejected with
+ * SEALFM_EINVAL (here, by sealdec_teacher_forced and by the debug entry points); the device-buffer entry points
+ * below do not check it, and their results for such a source are undefined.
  * H = sealdec_hyps_per_query(p).  Returns SEALFM_EINVAL("beam") if some query had fewer than
  * num_beams non-EOS candidates (the reference raises ValueError, :687-690).  If an activation leaves the fp16
  * range of the default GEMM mode the pass is repeated with the 3xTF32 kernels (sealbart_get_stat "overflow_fallbacks"). */
@@ -178,7 +181,17 @@ int sealdec_generate_dx_ex(sealbart_t* model, const sealfm_t* fm, const uint32_t
  * kernels read only the row's allowed tokens, the lm_head emits per-tile statistics and stores only those logits),
  * "poison_logits" (testing: 1 fills the logits buffer with NaN before every such lm_head).  Stats: "last_used_graph",
  * "overflow_fallbacks", "gemm_mode", "cached_graphs", "fused_head_steps" (decode steps of the last generate run
- * eagerly that used the statistics epilogue) (-1 for an unknown name). */
+ * eagerly that used the statistics epilogue), "last_paths" (-1 for an unknown name).
+ * "last_paths" is the OR, over the last generate / teacher-forced / debug-step call (a CUDA-graph replay reports
+ * the call it was captured from), of one bit per kernel branch of the BART forward:
+ *   0 encoder on the real tokens only (packed)         1 encoder on the padded rows (mask per key)
+ *   2 decoder self-attention, beams of a query together (dec_self_attn_query_kernel)
+ *   3 ... one row per CTA, <= 12 keys                  4 ... <= 32 keys                5 ... > 32 keys
+ *   6 cross-attention, source <= 32 positions          7 cross-attention, longer sources
+ *   8 add + LayerNorm, one CTA per row (<= 2048 rows)  9 add + LayerNorm, one warp per row
+ *  10 split-K GEMM summed by its consumer kernel      11 split-K GEMM + finish pass
+ *  12 3xFP16 GEMM on whole tiles                      13 3xFP16 GEMM on 2-CTA clusters (gemm_mode 5)
+ *  14 3xTF32 GEMM (gemm_mode 2) */
 int     sealbart_set_option(sealbart_t* model, const char* name, int64_t value);
 int64_t sealbart_get_stat(const sealbart_t* model, const char* name);
 
@@ -200,6 +213,15 @@ int sealdec_teacher_forced(sealbart_t* model, const int64_t* input_ids, const in
 int sealdec_debug_step_logits(sealbart_t* model, const int64_t* input_ids, const int64_t* attention_mask,
                               int64_t Q, int64_t S, int32_t num_beams, const int64_t* decoder_input_ids,
                               int64_t t, float* out_logits);
+/* The same with the beam ancestry and the encoder's packing as inputs:
+ *   ancestry int32 [R][t] host, or NULL for every row its own ancestor: row r reads the decoder cache of position s
+ *            from row ancestry[r][s] (in [0, R)), as a generate does after beams were reordered; entries at
+ *            position t-1 are not read.  The caller keeps it consistent (equal decoder_input_ids[:s+1]).
+ *   src_tokens_hint as in sealdec_generate_dx: -1 pack right-padded masks, -2 never pack, >= 1 the count of
+ *            non-zero mask entries of right-padded masks (checked here). */
+int sealdec_debug_step_logits_ex(sealbart_t* model, const int64_t* input_ids, const int64_t* attention_mask,
+                                 int64_t Q, int64_t S, int32_t num_beams, const int64_t* decoder_input_ids,
+                                 int64_t t, const int32_t* ancestry, int64_t src_tokens_hint, float* out_logits);
 /* Stand-alone GEMM C[M,N] = A[M,K] W[N,K]^T + bias (+GELU) through the model's GEMM kernels
  * (mode 2 = 3xTF32, 3 = 3xFP16, 5 = 3xFP16 on CTA pairs), host pointers; if iters > 0 also reports the average
  * device time per call (CUDA events, includes the activation split). */

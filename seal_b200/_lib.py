@@ -117,6 +117,8 @@ _DEC_SIGS = {
     "sealdec_teacher_forced": (i32, [vp, vp, vp, C.c_int64, C.c_int64, vp, vp, C.c_int64, C.c_int64, C.c_float, vp,
                                      C.c_int64, vp]),
     "sealdec_debug_step_logits": (i32, [vp, vp, vp, C.c_int64, C.c_int64, C.c_int32, vp, C.c_int64, vp]),
+    "sealdec_debug_step_logits_ex": (i32, [vp, vp, vp, C.c_int64, C.c_int64, C.c_int32, vp, C.c_int64, vp, C.c_int64,
+                                           vp]),
     "sealdec_debug_gemm": (i32, [i32, C.c_int64, C.c_int32, C.c_int32, vp, vp, vp, vp, C.c_int32, C.c_int32,
                                  C.POINTER(C.c_double)]),
     "sealdec_debug_gemm_ex": (i32, [i32, C.c_int64, C.c_int32, C.c_int32, vp, vp, vp, vp, C.c_int32, C.c_int32,

@@ -141,18 +141,32 @@ class SealBartEngine:
     def device_bytes(self):
         return int(lib.sealbart_device_bytes(self._h))
 
-    def debug_step_logits(self, input_ids, attention_mask, num_beams, decoder_input_ids):
-        """Teacher-forced logits of the last decoder position for explicit decoder inputs [R,t]."""
+    def debug_step_logits(self, input_ids, attention_mask, num_beams, decoder_input_ids, anc=None, src_tokens=-1):
+        """Teacher-forced logits of the last decoder position for explicit decoder inputs [R,t].
+        anc: optional int32 [R,t] beam ancestry (row r reads the decoder cache of position s from row anc[r,s]);
+        src_tokens: -1 pack right-padded sources, -2 never pack (include/sealdec.h sealdec_debug_step_logits_ex)."""
         ids = np.ascontiguousarray(np.asarray(input_ids, dtype=np.int64))
         am = np.ascontiguousarray(np.asarray(attention_mask, dtype=np.int64))
         dec = np.ascontiguousarray(np.asarray(decoder_input_ids, dtype=np.int64))
         Q, S = ids.shape
         R, t = dec.shape
         assert R == Q * num_beams
+        a = None
+        if anc is not None:
+            a = np.ascontiguousarray(np.asarray(anc, dtype=np.int32))
+            assert a.shape == (R, t)
         out = np.empty((R, int(self.config.vocab_size)), dtype=np.float32)
-        check(lib.sealdec_debug_step_logits(self._h, ids.ctypes.data, am.ctypes.data, Q, S, num_beams,
-                                            dec.ctypes.data, t, out.ctypes.data))
+        check(lib.sealdec_debug_step_logits_ex(self._h, ids.ctypes.data, am.ctypes.data, Q, S, num_beams,
+                                               dec.ctypes.data, t, a.ctypes.data if a is not None else None,
+                                               int(src_tokens), out.ctypes.data))
         return out
+
+    def stat(self, name):
+        """sealbart_get_stat (include/sealdec.h), e.g. "last_paths"."""
+        return int(lib.sealbart_get_stat(self._h, name.encode()))
+
+    def set_option(self, name, value):
+        check(lib.sealbart_set_option(self._h, name.encode(), int(value)))
 
     def last_phase_us(self):
         a = (C.c_double * 5)()

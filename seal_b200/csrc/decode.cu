@@ -79,7 +79,8 @@ struct sealbart {
     Buf hy_score, hy_len, hy_tok, hy_valid, hy_lo, hy_hi, err, dbg_ids, force_syms, a_hi, a_lo, splitk;
     std::vector<void*> split_allocs;
     int64_t launches = 0;
-    int* ovf = nullptr;               // where the producers raise "fp16 range exceeded" (set by every entry point)
+    uint32_t last_paths = 0;          // OR of the kPath* bits of every kernel branch the last model call took
+    int* ovf = nullptr;              // where the producers raise "fp16 range exceeded" (set by every entry point)
     double phase_us[5] = {0, 0, 0, 0, 0};
     bool profile_gemm = false;
     int fused_head = -1;              // -1 $SEALB200_FUSED_HEAD (default on), 0 dense lm_head logits, 1 statistics epilogue
@@ -92,7 +93,7 @@ struct sealbart {
     // host-buffer entry point: persistent device staging of the inputs (stable addresses -> CUDA graph reuse)
     Buf in_ids, in_mask, in_occ;
     // CUDA graphs of whole generate calls (small batches are launch-latency-bound: ~1 900 kernels per generate)
-    struct GraphEntry { std::vector<uint8_t> key; uint64_t epoch = 0; cudaGraphExec_t exec = nullptr; int64_t launches = 0; uint64_t stamp = 0; };
+    struct GraphEntry { std::vector<uint8_t> key; uint64_t epoch = 0; cudaGraphExec_t exec = nullptr; int64_t launches = 0; uint32_t paths = 0; uint64_t stamp = 0; };
     std::vector<GraphEntry> graphs;
     std::vector<std::vector<uint8_t>> seen_keys;     // shapes run once already (their buffers are sized): capture next time
     uint64_t graph_stamp = 0;
@@ -204,6 +205,17 @@ void make_map(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t K, uint
 
 constexpr int64_t kAddLnRowMax = 2048;      // up to this many rows add+LN runs one CTA per row
 
+// sealbart_get_stat(model, "last_paths"): one bit per kernel branch of the BART forward (include/sealdec.h), set on
+// the host next to the launch it names
+enum : uint32_t {
+    kPathEncPacked = 1u << 0, kPathEncUnpacked = 1u << 1,
+    kPathSelfQuery = 1u << 2, kPathSelfRounds3 = 1u << 3, kPathSelfRounds8 = 1u << 4, kPathSelfLong = 1u << 5,
+    kPathCrossSmall = 1u << 6, kPathCrossGrouped = 1u << 7,
+    kPathAddLnRow = 1u << 8, kPathAddLnWarp = 1u << 9,
+    kPathSplitKDeferred = 1u << 10, kPathSplitKFinish = 1u << 11, kPathGemmFullTile = 1u << 12, kPathGemmCluster = 1u << 13,
+    kPathGemmTf32 = 1u << 14,
+};
+
 void split_into(cudaStream_t s, const float* x, float* hi, float* lo, uint64_t numel) {
     const int64_t n4 = (int64_t)(numel / 4);
     const int blocks = (int)std::min<int64_t>((n4 + 255) / 256, (int64_t)sm_count() * 8);
@@ -294,7 +306,7 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
             const int ctas = 2 * std::min(groups, sm_count() / 2);
             if (gelu) gemm_launch<__half, true, 2>(cx.s, ctas, ma1, ma2, l.map2_hi, l.map2_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, 0, ovf, 1, 0);
             else gemm_launch<__half, false, 2>(cx.s, ctas, ma1, ma2, l.map2_hi, l.map2_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, 0, ovf, 1, 0);
-            m->launches++;
+            m->launches++; m->last_paths |= kPathGemmCluster;
             return;
         }
         if (k_slices > 1) {
@@ -307,12 +319,13 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
             m->launches++;
             if (M <= cx.defer_rows && !gelu && !C.h1 && !C.hi && ldc == N && l.b) {     // summed by the consumer kernel
                 cx.pending = SplitSrc{part, k_slices, slice_stride, l.b, l.w_unscale};
+                m->last_paths |= kPathSplitKDeferred;
                 return;
             }
             const int fblocks = (int)std::min<int64_t>((M * (ldc / 4) + 255) / 256, (int64_t)sm_count() * 8);
             if (gelu) launch_k(gemm_splitk_finish_kernel<true>, fblocks, 256, 0, cx.s, M, N, ldc, k_slices, slice_stride, part, l.b, l.w_unscale, C.x, C.h1, C.h2, ovf);
             else launch_k(gemm_splitk_finish_kernel<false>, fblocks, 256, 0, cx.s, M, N, ldc, k_slices, slice_stride, part, l.b, l.w_unscale, C.x, C.h1, C.h2, ovf);
-            CUDA_CHECK(cudaGetLastError()); m->launches++;
+            CUDA_CHECK(cudaGetLastError()); m->launches++; m->last_paths |= kPathSplitKFinish;
             return;
         }
         // m fastest with more A than a band holds (the lm_head at thousands of rows): bands of m tiles whose A halves
@@ -328,7 +341,7 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
             cx.head_fused = true;
         } else if (gelu) gemm_launch<__half, true, 1>(cx.s, ctas, ma1, ma2, l.map_hi, l.map_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, band, ovf, 1, 0);
         else gemm_launch<__half, false, 1>(cx.s, ctas, ma1, ma2, l.map_hi, l.map_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, band, ovf, 1, 0);
-        m->launches++;
+        m->launches++; m->last_paths |= kPathGemmFullTile;
         return;
     }
     if (m->cfg.gemm_mode == 2 && K % UK == 0 && lda == K && l.w_hi) {
@@ -344,7 +357,7 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
         const int ctas = std::min(tiles, sm_count());
         if (gelu) gemm_launch<float, true, 1>(cx.s, ctas, mah, mal, l.map_hi, l.map_lo, M, N, K, l.b, 1.0f, C.x, C.hi, C.lo, ldc, n_fastest, 0, m->ovf, 1, 0);
         else gemm_launch<float, false, 1>(cx.s, ctas, mah, mal, l.map_hi, l.map_lo, M, N, K, l.b, 1.0f, C.x, C.hi, C.lo, ldc, n_fastest, 0, m->ovf, 1, 0);
-        m->launches++;
+        m->launches++; m->last_paths |= kPathGemmTf32;
         return;
     }
     throw ApiError(SEALFM_EINVAL, "GEMM: K must be a multiple of 64 (3xFP16) / 32 (3xTF32) with contiguous operands");
@@ -359,6 +372,7 @@ void add_ln(Ctx& cx, int64_t rows, int d, const float* a, const float* b, const 
     else
         launch_k(add_ln_kernel, (unsigned)((rows + 3) / 4), 128, 0, cx.s, rows, d, a, b, (const float*)ln.g, (const float*)ln.b, out.x, split_of(out, cx.m->ovf));
     cx.m->launches++;
+    cx.m->last_paths |= rows <= kAddLnRowMax ? kPathAddLnRow : kPathAddLnWarp;
 }
 
 __global__ void prep_enc_kernel(int64_t n, int S, const int64_t* __restrict__ ids, const int64_t* __restrict__ mask,
@@ -499,6 +513,7 @@ void encoder_forward(Ctx& cx, const Dims& D, const int64_t* ids_d, const int64_t
     if (m->enc_packed) prep_enc_packed_kernel<<<(unsigned)((Tk + 255) / 256), 256, 0, cx.s>>>(Tk, (int)D.S, ids_d, src_off, tok, pos);
     else prep_enc_kernel<<<(unsigned)((Tk + 255) / 256), 256, 0, cx.s>>>(Tk, (int)D.S, ids_d, mask_d, tok, m32, pos);
     CUDA_CHECK(cudaGetLastError()); m->launches++;
+    m->last_paths |= m->enc_packed ? kPathEncPacked : kPathEncUnpacked;
     const int64_t Te = rows_enc;                    // encoder rows actually computed
     const int gm = m->cfg.gemm_mode;
     auto mk = [&](float* plain, Buf& bh, Buf& bl, bool keep_plain) {
@@ -600,6 +615,7 @@ void decoder_step(Ctx& cx, const Dims& D, const int32_t* tokens, int cur_len, co
         else
             launch_k(dec_self_attn_long_kernel, (unsigned)R, sa_threads, 0, cx.s, Rc, d, heads, pos, D.T, (const float*)qkv.x, kc, vc, anc, attn.x, split_of(attn, ovf));
         m->launches++;
+        m->last_paths |= use_saq ? kPathSelfQuery : pos + 1 <= 12 ? kPathSelfRounds3 : pos + 1 <= 32 ? kPathSelfRounds8 : kPathSelfLong;
         cx.defer_rows = kAddLnRowMax;
         gemm(cx, R, d, d, attn, d, L.o, tmp, d, false);
         cx.defer_rows = 0;
@@ -619,6 +635,7 @@ void decoder_step(Ctx& cx, const Dims& D, const int32_t* tokens, int cur_len, co
             launch_k(cross_attn_kernel, dim3((unsigned)groups, heads), kGAttnWarps * 32, 0, cx.s, groups, d, heads, compact ? 1 : D.B, (int)D.S, (const float*)cq.x,
                        ckv_l, m32, D.grp_query, D.grp_start, attn.x, split_of(attn, ovf), soff_x);
         m->launches++;
+        m->last_paths |= D.S <= kXKeys ? kPathCrossSmall : kPathCrossGrouped;
         cx.defer_rows = kAddLnRowMax;
         gemm(cx, R, d, d, attn, d, L.co, tmp, d, false);
         cx.defer_rows = 0;
@@ -969,6 +986,18 @@ void drop_graphs(sealbart* m) {
     m->seen_keys.clear();
 }
 
+// A source whose attention mask is all zero has nothing to attend to: the softmax denominator of the encoder and
+// cross-attention kernels stays zero (HF instead spreads the weight over the masked keys and gives finite logits).
+// SEAL never builds one; the host-buffer
+// entry points reject it, the device-buffer ones document it as a precondition.
+void check_sources(const int64_t* mask, int64_t Q, int64_t S) {
+    for (int64_t q = 0; q < Q; ++q) {
+        bool any = false;
+        for (int64_t s2 = 0; s2 < S && !any; ++s2) any = mask[q * S + s2] != 0;
+        if (!any) throw ApiError(SEALFM_EINVAL, "source " + std::to_string(q) + " has an all-zero attention mask");
+    }
+}
+
 }  // namespace
 
 extern "C" {
@@ -1003,6 +1032,7 @@ int sealdec_generate_dx_ex(sealbart_t* m, const sealfm_t* fm, const uint32_t* oc
         }
         Ctx cx{m, (cudaStream_t)stream};
         m->launches = 0;
+        m->last_paths = 0;
         m->ovf = err_d + 1;
         m->last_used_graph = 0;
         const Dims D = make_dims(m, Q, S, B, T);
@@ -1040,7 +1070,7 @@ int sealdec_generate_dx_ex(sealbart_t* m, const sealfm_t* fm, const uint32_t* oc
         for (auto& g : m->graphs)
             if (g.key == key) {
                 CUDA_CHECK(cudaGraphLaunch(g.exec, cx.s));
-                g.stamp = ++m->graph_stamp; m->launches = g.launches; m->last_used_graph = 1;
+                g.stamp = ++m->graph_stamp; m->launches = g.launches; m->last_paths = g.paths; m->last_used_graph = 1;
                 return;
             }
         bool seen = false;
@@ -1073,7 +1103,7 @@ int sealdec_generate_dx_ex(sealbart_t* m, const sealfm_t* fm, const uint32_t* oc
             // only recorded, nothing ran): run it the ordinary way, and stop trying on this model
             cudaGetLastError();
             if (g_ws_epoch == epoch0) m->graph_policy = 0;
-            m->launches = 0;
+            m->launches = 0; m->last_paths = 0;
             generate_enqueue(cx, D, a, view, lo0, hi0, eff_hint, true);
             return;
         }
@@ -1083,7 +1113,7 @@ int sealdec_generate_dx_ex(sealbart_t* m, const sealfm_t* fm, const uint32_t* oc
             cudaGraphExecDestroy(m->graphs[victim].exec);
             m->graphs.erase(m->graphs.begin() + victim);
         }
-        sealbart::GraphEntry ge; ge.key = std::move(key); ge.epoch = g_ws_epoch; ge.exec = exec; ge.launches = m->launches; ge.stamp = ++m->graph_stamp;
+        sealbart::GraphEntry ge; ge.key = std::move(key); ge.epoch = g_ws_epoch; ge.exec = exec; ge.launches = m->launches; ge.paths = m->last_paths; ge.stamp = ++m->graph_stamp;
         m->graphs.push_back(std::move(ge));
         CUDA_CHECK(cudaGraphLaunch(exec, cx.s));
         m->last_used_graph = 1;
@@ -1136,6 +1166,7 @@ int64_t sealbart_get_stat(const sealbart_t* m, const char* name) {
     if (n == "gemm_mode") return m->cfg.gemm_mode;
     if (n == "cached_graphs") return (int64_t)m->graphs.size();
     if (n == "fused_head_steps") return m->fused_head_steps;
+    if (n == "last_paths") return m->last_paths;
     return -1;
 }
 
@@ -1198,6 +1229,7 @@ int sealdec_generate_ex(sealbart_t* m, const sealfm_t* fm, const uint32_t* occ_h
         check_model(m);
         if (!p || !ids || !mask || Q <= 0 || S <= 0) throw ApiError(SEALFM_EINVAL, "null argument / empty batch");
         checked_groups(groups, p->num_beams);
+        check_sources(mask, Q, S);
         const int64_t H = sealdec_hyps_per_query(p), T = p->max_length;
         const int W = (m->cfg.vocab_size + 31) / 32;
         // the caller's buffers are host memory: the real-token count costs nothing to know here, so the encoder
@@ -1257,11 +1289,33 @@ int sealdec_generate_ex(sealbart_t* m, const sealfm_t* fm, const uint32_t* occ_h
 
 int sealdec_debug_step_logits(sealbart_t* m, const int64_t* ids, const int64_t* mask, int64_t Q, int64_t S, int32_t B,
                               const int64_t* dec_ids, int64_t t, float* out_logits) {
+    return sealdec_debug_step_logits_ex(m, ids, mask, Q, S, B, dec_ids, t, nullptr, -1, out_logits);
+}
+
+int sealdec_debug_step_logits_ex(sealbart_t* m, const int64_t* ids, const int64_t* mask, int64_t Q, int64_t S, int32_t B,
+                                 const int64_t* dec_ids, int64_t t, const int32_t* anc, int64_t src_tokens_hint,
+                                 float* out_logits) {
     return guarded([&] {
         check_model(m);
-        if (!ids || !mask || !dec_ids || !out_logits || t < 1 || t > kMaxLen) throw ApiError(SEALFM_EINVAL, "bad argument");
+        if (!ids || !mask || !dec_ids || !out_logits || t < 1 || t > kMaxLen || Q <= 0 || S <= 0 || B < 1)
+            throw ApiError(SEALFM_EINVAL, "bad argument");
+        if (S > m->cfg.max_positions) throw ApiError(SEALFM_EINVAL, "source longer than max_positions");
+        check_sources(mask, Q, S);
+        if (src_tokens_hint != -1 && src_tokens_hint != -2) {
+            // a count is only valid for right-padded masks; checked here, where the mask is host memory
+            int64_t n = 0; bool prefix = true;
+            for (int64_t q = 0; q < Q; ++q) {
+                int64_t len = 0;
+                for (int64_t s2 = 0; s2 < S; ++s2) { const bool on = mask[q * S + s2] != 0; if (on && s2 != len) prefix = false; len += on; }
+                n += len;
+            }
+            if (!prefix || n != src_tokens_hint) throw ApiError(SEALFM_EINVAL, "src_tokens_hint does not match a right-padded mask");
+        }
         const int T = (int)t;
         const Dims D = make_dims(m, Q, S, B, T);
+        if (anc)
+            for (int64_t i = 0; i < D.R * T; ++i)
+                if (anc[i] < 0 || anc[i] >= D.R) throw ApiError(SEALFM_EINVAL, "ancestor row out of range");
         ensure_workspace(m, D);
         m->ovf = m->err.as<int>() + 1;
         Buf d_ids, d_mask;
@@ -1273,10 +1327,12 @@ int sealdec_debug_step_logits(sealbart_t* m, const int64_t* ids, const int64_t* 
         CUDA_CHECK(cudaMemcpyAsync(m->dbg_ids.p, dec_ids, D.R * t * 8, cudaMemcpyHostToDevice, s));
         Ctx cx{m, s};
         m->launches = 0;
-        encoder_forward(cx, D, d_ids.as<int64_t>(), d_mask.as<int64_t>());
+        m->last_paths = 0;
+        encoder_forward(cx, D, d_ids.as<int64_t>(), d_mask.as<int64_t>(), src_tokens_hint);
         int32_t* tk = m->st_tokens.as<int32_t>(); int32_t* an = m->st_anc.as<int32_t>();
         ids_to_tokens_kernel<<<(unsigned)((D.R + 255) / 256), 256, 0, s>>>(D.R, T, T, m->dbg_ids.as<int64_t>(), tk, an);
         CUDA_CHECK(cudaGetLastError());
+        if (anc) CUDA_CHECK(cudaMemcpyAsync(an, anc, (size_t)D.R * T * 4, cudaMemcpyHostToDevice, s));   // replaces the identity
         for (int cur_len = 1; cur_len <= T; ++cur_len) decoder_step(cx, D, tk, cur_len, an, cur_len == T, nullptr);
         CUDA_CHECK(cudaMemcpy2DAsync(out_logits, (size_t)D.V * 4, m->logits.p, (size_t)D.ld * 4, (size_t)D.V * 4, D.R,
                                      cudaMemcpyDeviceToHost, s));
@@ -1292,6 +1348,7 @@ int sealdec_teacher_forced(sealbart_t* m, const int64_t* ids, const int64_t* mas
         if (!ids || !mask || !dec_ids || !row_query || N <= 0 || T < 1 || T > kMaxLen || Q <= 0 || S <= 0)
             throw ApiError(SEALFM_EINVAL, "bad argument");
         if (S > m->cfg.max_positions) throw ApiError(SEALFM_EINVAL, "source longer than max_positions");
+        check_sources(mask, Q, S);
         for (int64_t r = 0; r < N; ++r) {
             if (row_query[r] < 0 || row_query[r] >= Q || (r && row_query[r] < row_query[r - 1]))
                 throw ApiError(SEALFM_EINVAL, "row_query must be sorted and within [0, Q)");
@@ -1309,6 +1366,7 @@ int sealdec_teacher_forced(sealbart_t* m, const int64_t* ids, const int64_t* mas
         CUDA_CHECK(cudaMemcpyAsync(d_mask.p, mask, Q * S * 8, cudaMemcpyHostToDevice, s));
         Ctx cx{m, s};
         m->launches = 0;
+        m->last_paths = 0;
         encoder_forward(cx, D, d_ids.as<int64_t>(), d_mask.as<int64_t>());
         d_dec.ensure(D.R * T * 8); d_gq.ensure((D.R + 1) * 4); d_gs.ensure((D.R + 2) * 4);
         if (T > 1) d_out.ensure(D.R * (T - 1) * 4);

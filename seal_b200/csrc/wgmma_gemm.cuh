@@ -5,9 +5,14 @@
 // which keeps the fp32-level accuracy the 1e-4 beam-score parity needs (a single TF32/FP16 pass does not).
 // Two operand splits:
 //   3xFP16 (gemm_mode 3 / 5): x = h1 + h2, h1 = rn_half(x), h2 = rn_half(x - h1).  fp16 products are exact in the
-//     fp32 accumulator, so the accuracy class is that of 3xTF32 at half the operand bytes and twice the tensor rate.
-//     Activations are used unscaled (|x| must stay below 65504; the producers saturate and raise a sticky flag
-//     otherwise); each weight matrix is pre-multiplied by a power of two 2^s so that max|W| ~ 2^14 and the epilogue
+//     fp32 accumulator, so the accuracy class is that of 3xTF32 at half the operand bytes and twice the tensor rate --
+//     for activations of magnitude at least 2^-3.  Activations are used unscaled (|x| must stay below 65504; the
+//     producers saturate and raise a sticky flag otherwise).  |x - h1| <= 2^-11 |x|, so below about 2^-3 the low half
+//     h2 is an fp16 subnormal (spacing 2^-24) and below 2^-14 h1 is too: each such activation carries an absolute
+//     error of up to 2^-25 (relative 2^-19 at 2^-6, 2^-11 at 2^-14), and below 2^-25 it flushes to zero.  Element
+//     (i, j) is then good to about
+//     sum_k |w_jk| * max(2^-22 |a_ik|, 2^-25), not 2^-22 sum_k |a_ik w_jk| (tests/test_gemm_range_gpu.py); at the
+//     BART activation scales that floor is far below the forward's rounding.  Each weight matrix is pre-multiplied by a power of two 2^s so that max|W| ~ 2^14 and the epilogue
 //     multiplies the accumulator by 2^-s (exact).
 //   3xTF32 (gemm_mode 2, fp32 range): hi = x with the 13 low mantissa bits cleared, lo = x - hi (exact).
 //
