@@ -235,6 +235,43 @@ int sealdec_debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A
 int sealdec_debug_gemm_ex(int mode, int64_t M, int32_t N, int32_t K, const float* A, const float* W,
                           const float* bias, float* C, int32_t gelu, int32_t iters, double* avg_us, int32_t band,
                           int32_t store);
+/* The lm_head GEMM of a decode step with the statistics epilogue requested (gemm_mode 3, through the same GEMM
+ * dispatch as the decoder; tests/test_select_step_gpu.py): C[M,N] = A W^T + bias with the row masks
+ * mask uint32 [M][ceil(N/32)] and eos / pad defining each row's read set.  Host pointers.  With Mpad = M rounded up
+ * to 128 rows, C is float32 [Mpad][N] and stats float32 [Mpad][ceil(N/128)][2] = per (row, 128-column tile)
+ * (max, sum exp(x - max)); both are filled with NaN on the device before the call, so whatever the GEMM does not
+ * write comes back as NaN.  *fused = 1 if the statistics epilogue ran (then C holds only the read set: the whole
+ * first tile, the mask bits, eos and pad); 0 if the shape took the split-K path, which stores C densely and no
+ * statistics, as the decoder then does. */
+int sealdec_debug_head(int64_t M, int32_t N, int32_t K, const float* A, const float* W, const float* bias,
+                       const uint32_t* mask, int32_t eos, int32_t pad, float* C, float* stats, int32_t* fused);
+/* One decode step's selection (log-softmax statistics, processors, index mask, top-2*beam, the scorer bookkeeping,
+ * the records and the LF step) on caller-supplied inputs, through the same kernel dispatch as the generate entry
+ * points.  Host pointers; B = p->num_beams, T = p->max_length, R = Q*B, W = ceil(V/32), G from `groups` (NULL = 1).
+ * Configurations a generate never produces are rejected with SEALFM_EINVAL (B > 32, cur_len outside
+ * [1, max_length-1], logits_shared away from cur_len 1, logits_ignored away from the forced-EOS step, head statistics
+ * on a step where the lm_head would not write them, ...).
+ * Inputs:  logits float32 [logits_shared ? Q : R][V] (NULL with logits_ignored; padded to the generate's stride with
+ *          NaN), head_stats float32 [R][ceil(V/128)][2] from the lm_head epilogue or NULL (statistics streamed from
+ *          the logits), masks uint32 [R][W] (may be NULL where not read), occurring_mask uint32 [W] (the first
+ *          step's mask), beam_scores float32 [R], tokens and ancestry int32 [R][T], lo, hi, pw uint64 [R]; fm is
+ *          needed unless p->disable_fm_index.
+ * Outputs: row_max, row_logsum float32 [R], row_rule uint8 [R]; the candidate lists cand_val float32 / cand_idx
+ *          int32 [R][2B] and cand_cnt int32 [R], of which the first Q * (*lists) are the step's lists; the next beams
+ *          beam_scores_out [R], tokens_out / ancestry_out [R][T], lo_out, hi_out, pw_out [R]; the step's records
+ *          rec_score, rec_len, rec_tokens [Q][2B][T], rec_valid, rec_lo, rec_hi, [Q][2B] each; error_flag int32 [1]
+ *          (fewer than num_beams non-EOS candidates).  Every output and scratch buffer is filled with NaN / all-ones
+ *          bits on the device first, so an element the step does not write comes back that way. */
+int sealdec_debug_select_step(const sealfm_t* fm, const sealdec_params_t* p, const sealdec_groups_t* groups, int64_t Q,
+                              int32_t V, int32_t cur_len, int32_t logits_shared, int32_t logits_ignored,
+                              const float* logits, const float* head_stats, const uint32_t* masks,
+                              const uint32_t* occurring_mask, const float* beam_scores, const int32_t* tokens,
+                              const int32_t* ancestry, const uint64_t* lo, const uint64_t* hi, const uint64_t* pw,
+                              float* row_max, float* row_logsum, uint8_t* row_rule, float* cand_val, int32_t* cand_idx,
+                              int32_t* cand_cnt, int32_t* lists, float* beam_scores_out, int32_t* tokens_out,
+                              int32_t* ancestry_out, uint64_t* lo_out, uint64_t* hi_out, uint64_t* pw_out,
+                              float* rec_score, int32_t* rec_len, int32_t* rec_tokens, uint8_t* rec_valid,
+                              uint64_t* rec_lo, uint64_t* rec_hi, int32_t* error_flag);
 /* average device time of the decoder's per-row statistics + top-2*beam kernel over R rows of V pseudo-random logits
  * (a later step of constrained beam search, per_row allowed tokens per row) */
 int sealdec_debug_topk_rows(int64_t R, int32_t V, int32_t num_beams, int32_t per_row, int32_t iters, double* avg_us);

@@ -830,6 +830,32 @@ bool fused_head_on(const sealbart* m) {
     return m->fused_head >= 0 ? m->fused_head != 0 : env_on;
 }
 
+void set_select_smem() {
+    CUDA_CHECK(cudaFuncSetAttribute(topk_rows_kernel<512, 8192>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SelSharedT<8192>)));
+    CUDA_CHECK(cudaFuncSetAttribute(topk_rows_kernel<256, 4096>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SelSharedT<4096>)));
+}
+
+// One decode step's selection on Q queries: topk_rows_kernel, then select_merge_kernel (set_select_smem() first).
+// Returns `lists`, the candidate lists per query.  The first step (cur_len 1): beams 1.. carry -1e9 and are pruned
+// exactly inside one CTA per query; afterwards one CTA per row.  Diverse beam groups at the first step: lists of row 0
+// (every group leader) and row 1 (every other beam) only, see select_merge_kernel.
+int launch_select_step(cudaStream_t s, const FmView& view, const StepCfg& c, const StepState& st, const RowScratch& rs, int64_t Q) {
+    const int B = c.num_beams, gs = B / c.num_groups;
+    int lists;
+    if (c.cur_len == 1 && c.num_groups > 1) {
+        lists = gs > 1 ? 2 : 1;
+        launch_k(topk_rows_kernel<512, 8192>, (unsigned)(Q * lists), 512, sizeof(SelSharedT<8192>), s, c, st, rs, lists, 1);
+    } else if (c.cur_len == 1) {
+        lists = 1;
+        launch_k(topk_rows_kernel<512, 8192>, (unsigned)Q, 512, sizeof(SelSharedT<8192>), s, c, st, rs, 1, B);
+    } else {
+        lists = B;
+        launch_k(topk_rows_kernel<256, 4096>, (unsigned)(Q * B), 256, sizeof(SelSharedT<4096>), s, c, st, rs, B, 1);
+    }
+    launch_k(select_merge_kernel, (unsigned)Q, kMergeThreads, 0, s, view, c, st, rs, lists);
+    return lists;
+}
+
 void generate_enqueue(Ctx& cx, const Dims& D, const GenArgs& a, const FmView& view, uint64_t lo0, uint64_t hi0,
                       int64_t src_hint, bool timing) {
     sealbart* m = cx.m;
@@ -871,9 +897,7 @@ void generate_enqueue(Ctx& cx, const Dims& D, const GenArgs& a, const FmView& vi
     c.remove_invalid_values = p->remove_invalid_values; c.shift = p->shift; c.T = T; c.mask_words = D.W;
     c.hyps_per_query = sealdec_hyps_per_query(p);
     c.num_groups = G; c.diversity_penalty = a.grp.diversity_penalty;
-    using RowsFirst = SelSharedT<8192>; using RowsLater = SelSharedT<4096>;
-    CUDA_CHECK(cudaFuncSetAttribute(topk_rows_kernel<512, 8192>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RowsFirst)));
-    CUDA_CHECK(cudaFuncSetAttribute(topk_rows_kernel<256, 4096>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RowsLater)));
+    set_select_smem();
     RowScratch rs{m->st_rowmax.as<float>(), m->st_rowls.as<float>(), m->st_rule.as<uint8_t>(),
                   m->st_cval.as<float>(), m->st_cidx.as<int32_t>(), m->st_ccnt.as<int32_t>()};
     int cur = 0;
@@ -930,20 +954,7 @@ void generate_enqueue(Ctx& cx, const Dims& D, const GenArgs& a, const FmView& vi
         st.occurring_mask = a.occ_d; st.logits = m->logits.as<float>(); st.head_stats = m->st_hstat.as<float2>();
         st.hyp_score = a.o_score; st.hyp_len = a.o_len; st.hyp_tokens = a.o_tok; st.hyp_valid = a.o_valid;
         st.hyp_lo = a.o_lo; st.hyp_hi = a.o_hi; st.error_flag = a.err_d;
-        // first step: beams 1.. carry -1e9 and are pruned exactly inside one CTA per query; afterwards one CTA per row.
-        // Diverse beam groups at the first step: lists of row 0 (every group leader) and row 1 (every other beam) only,
-        // see select_merge_kernel.
-        if (cur_len == 1 && G > 1) {
-            const int lists = gs > 1 ? 2 : 1;
-            launch_k(topk_rows_kernel<512, 8192>, (unsigned)(Q * lists), 512, sizeof(RowsFirst), cx.s, c, st, rs, lists, 1);
-            launch_k(select_merge_kernel, (unsigned)Q, kMergeThreads, 0, cx.s, view, c, st, rs, lists);
-        } else if (cur_len == 1) {
-            launch_k(topk_rows_kernel<512, 8192>, (unsigned)Q, 512, sizeof(RowsFirst), cx.s, c, st, rs, 1, B);
-            launch_k(select_merge_kernel, (unsigned)Q, kMergeThreads, 0, cx.s, view, c, st, rs, 1);
-        } else {
-            launch_k(topk_rows_kernel<256, 4096>, (unsigned)R, 256, sizeof(RowsLater), cx.s, c, st, rs, B, 1);
-            launch_k(select_merge_kernel, (unsigned)Q, kMergeThreads, 0, cx.s, view, c, st, rs, B);
-        }
+        launch_select_step(cx.s, view, c, st, rs, Q);
         m->launches += 2;
         if (c.expand_next && !p->disable_fm_index) {           // successor sets of the new beams -> next step's masks (:107)
             launch_expand_masks(view, cx.s, (uint64_t)R, lo[cur ^ 1], hi[cur ^ 1], mk[cur ^ 1], (uint32_t)D.W, (uint32_t)D.V,
@@ -1412,11 +1423,18 @@ int sealdec_teacher_forced(sealbart_t* m, const int64_t* ids, const int64_t* mas
 
 namespace {
 
+// The lm_head statistics epilogue of sealdec_debug_head: the row masks [M][ceil(N/32)] (host), eos / pad, and where
+// the statistics [Mpad][ceil(N/128)] go (host; Mpad = M rounded up to 128 rows) and whether the epilogue ran.
+struct DebugHead { const uint32_t* mask; int eos, pad; float* stats; int32_t* fused; };
+
 // presplit: the activations are split into halves once, outside the timed calls (as the decoder's producers do)
 int debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A, const float* W, const float* bias, float* C,
-               int32_t gelu, int32_t iters, double* avg_us, int32_t band, int32_t store, bool presplit) {
+               int32_t gelu, int32_t iters, double* avg_us, int32_t band, int32_t store, bool presplit,
+               const DebugHead* head = nullptr) {
     return guarded([&] {
         if (!A || !W || (store && !C) || M <= 0 || N <= 0 || K <= 0 || band < -1) throw ApiError(SEALFM_EINVAL, "bad argument");
+        if (head && (mode != 3 || !store || gelu || iters > 0 || !head->mask || !head->stats || !head->fused))
+            throw ApiError(SEALFM_EINVAL, "bad argument");
         int count = 0;
         if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) { cudaGetLastError(); throw ApiError(SEALFM_ENODEVICE, "no CUDA device available"); }
         if (mode != 2 && mode != 3 && mode != 5) throw ApiError(SEALFM_EINVAL, "gemm_mode must be 2, 3 or 5");
@@ -1458,8 +1476,28 @@ int debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A, const 
         }
         const Act c{store ? dC.as<float>() : nullptr};
         Ctx cx{&fake, nullptr};
-        gemm(cx, M, N, K, a, K, l, c, ldc, gelu != 0);
+        Buf dmask, dstats;
+        struct RelH { Buf *x, *y; ~RelH() { x->release(); y->release(); } } relh{&dmask, &dstats};
+        const int64_t m_pad = (M + GM - 1) / GM * GM;
+        const int n_tiles = (N + GN - 1) / GN, mask_words = (N + 31) / 32;
+        if (head) {
+            // every output the epilogue may skip starts poisoned: C is NaN, the statistics all-ones bits (NaN)
+            dC.release(); dC.ensure((size_t)m_pad * ldc * 4);
+            CUDA_CHECK(cudaMemset(dC.p, 0xFF, (size_t)m_pad * ldc * 4));
+            dstats.ensure((size_t)m_pad * n_tiles * 8);
+            CUDA_CHECK(cudaMemset(dstats.p, 0xFF, (size_t)m_pad * n_tiles * 8));
+            dmask.ensure((size_t)M * mask_words * 4);
+            CUDA_CHECK(cudaMemcpy(dmask.p, head->mask, (size_t)M * mask_words * 4, cudaMemcpyHostToDevice));
+            cx.head = HeadEpi{dstats.as<float2>(), dmask.as<uint32_t>(), mask_words, head->eos, head->pad};
+        }
+        gemm(cx, M, N, K, a, K, l, head ? Act{dC.as<float>()} : c, ldc, gelu != 0);
         CUDA_CHECK(cudaDeviceSynchronize());
+        if (head) {
+            *head->fused = cx.head_fused ? 1 : 0;
+            CUDA_CHECK(cudaMemcpy2D(C, (size_t)N * 4, dC.p, (size_t)ldc * 4, (size_t)N * 4, m_pad, cudaMemcpyDeviceToHost));
+            CUDA_CHECK(cudaMemcpy(head->stats, dstats.p, (size_t)m_pad * n_tiles * 8, cudaMemcpyDeviceToHost));
+            return;
+        }
         if (iters > 0 && avg_us) {
             cudaEvent_t e0, e1; CUDA_CHECK(cudaEventCreate(&e0)); CUDA_CHECK(cudaEventCreate(&e1));
             CUDA_CHECK(cudaEventRecord(e0, nullptr));
@@ -1499,6 +1537,135 @@ int sealdec_debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A
 int sealdec_debug_gemm_ex(int mode, int64_t M, int32_t N, int32_t K, const float* A, const float* W, const float* bias, float* C,
                           int32_t gelu, int32_t iters, double* avg_us, int32_t band, int32_t store) {
     return debug_gemm(mode, M, N, K, A, W, bias, C, gelu, iters, avg_us, band, store, true);
+}
+
+int sealdec_debug_head(int64_t M, int32_t N, int32_t K, const float* A, const float* W, const float* bias,
+                       const uint32_t* mask, int32_t eos, int32_t pad, float* C, float* stats, int32_t* fused) {
+    const DebugHead h{mask, eos, pad, stats, fused};
+    return debug_gemm(3, M, N, K, A, W, bias, C, 0, 0, nullptr, -1, 1, true, &h);
+}
+
+int sealdec_debug_select_step(const sealfm_t* fm, const sealdec_params_t* p, const sealdec_groups_t* groups, int64_t Q,
+                              int32_t V, int32_t cur_len, int32_t logits_shared, int32_t logits_ignored,
+                              const float* logits, const float* head_stats, const uint32_t* masks,
+                              const uint32_t* occurring_mask, const float* beam_scores, const int32_t* tokens,
+                              const int32_t* ancestry, const uint64_t* lo, const uint64_t* hi, const uint64_t* pw,
+                              float* row_max, float* row_logsum, uint8_t* row_rule, float* cand_val, int32_t* cand_idx,
+                              int32_t* cand_cnt, int32_t* lists, float* beam_scores_out, int32_t* tokens_out,
+                              int32_t* ancestry_out, uint64_t* lo_out, uint64_t* hi_out, uint64_t* pw_out,
+                              float* rec_score, int32_t* rec_len, int32_t* rec_tokens, uint8_t* rec_valid,
+                              uint64_t* rec_lo, uint64_t* rec_hi, int32_t* error_flag) {
+    return guarded([&] {
+        if (!p || !beam_scores || !tokens || !ancestry || !lo || !hi || !pw || !row_max || !row_logsum || !row_rule ||
+            !cand_val || !cand_idx || !cand_cnt || !lists || !beam_scores_out || !tokens_out || !ancestry_out || !lo_out ||
+            !hi_out || !pw_out || !rec_score || !rec_len || !rec_tokens || !rec_valid || !rec_lo || !rec_hi || !error_flag)
+            throw ApiError(SEALFM_EINVAL, "null argument");
+        // only configurations a generate produces (generate_enqueue)
+        const int B = p->num_beams, K = 2 * B, T = p->max_length;
+        if (B < 1 || B > kSelMaxBeams || K > kSelMaxK) throw ApiError(SEALFM_EINVAL, "num_beams must be in [1,32]");
+        const sealdec_groups_t grp = checked_groups(groups, B);
+        if (T < 2 || T > kMaxLen) throw ApiError(SEALFM_EINVAL, "max_length must be in [2,128]");
+        if (cur_len < 1 || cur_len > T - 1) throw ApiError(SEALFM_EINVAL, "cur_len must be in [1, max_length - 1]");
+        if (Q <= 0 || V <= 0 || (int64_t)B * V > INT32_MAX) throw ApiError(SEALFM_EINVAL, "bad Q / V");
+        if (p->eos_token_id < 0 || p->eos_token_id >= V || p->pad_token_id < 0 || p->pad_token_id >= V ||
+            p->model_eos_token_id >= V || p->forced_eos_token_id >= V || p->forced_bos_token_id >= V)
+            throw ApiError(SEALFM_EINVAL, "token ids must be below V");
+        const bool fb_step = p->forced_bos_token_id >= 0 && cur_len == 1;
+        const int eff_len = cur_len - (p->forced_bos_token_id >= 0 ? 1 : 0);
+        const bool fm_on = !p->disable_fm_index;
+        const bool shared_mask = fm_on && eff_len == 1;
+        if (logits_ignored && !(p->forced_eos_token_id >= 0 && cur_len == T - 1 && !fb_step))
+            throw ApiError(SEALFM_EINVAL, "logits_ignored: only on the forced-EOS step");
+        if (logits_shared && (cur_len != 1 || logits_ignored)) throw ApiError(SEALFM_EINVAL, "logits_shared: only at cur_len 1");
+        if (!logits_ignored && !logits) throw ApiError(SEALFM_EINVAL, "logits missing");
+        if (head_stats && !(fm_on && eff_len > 1 && grp.num_beam_groups == 1 && V >= GN && !logits_ignored && !logits_shared))
+            throw ApiError(SEALFM_EINVAL, "head statistics: only after the first step, with the FM index on, one group and V >= 128");
+        if (fm_on && !fb_step && !shared_mask && !masks) throw ApiError(SEALFM_EINVAL, "masks missing");
+        if (shared_mask && !occurring_mask) throw ApiError(SEALFM_EINVAL, "occurring mask missing");
+        FmView view{};
+        if (fm_on) {
+            if (!fm || sealfm_device(fm) < 0) throw ApiError(SEALFM_ENODEVICE, "FM index not on a device");
+            CUDA_CHECK(cudaSetDevice(sealfm_device(fm)));
+            view = sealfm_view(fm);
+        } else {
+            int count = 0;
+            if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) { cudaGetLastError(); throw ApiError(SEALFM_ENODEVICE, "no CUDA device available"); }
+        }
+        const int64_t R = Q * B;
+        for (int64_t r = 0; r < R; ++r) {
+            if (lo[r] > hi[r] || (fm_on && hi[r] > view.m + 1)) throw ApiError(SEALFM_EINVAL, "SA range out of the index");
+            for (int i = 0; i < T; ++i)
+                if (ancestry[r * T + i] < 0 || ancestry[r * T + i] >= R) throw ApiError(SEALFM_EINVAL, "ancestor row out of range");
+        }
+        const int ld = (V + 3) / 4 * 4, W = (V + 31) / 32, tiles = (V + GN - 1) / GN;
+        const int64_t lrows = logits_shared ? Q : R;
+
+        std::vector<Buf> b(29);
+        struct Rel { std::vector<Buf>& v; ~Rel() { for (auto& x : v) x.release(); } } rel{b};
+        auto up = [&](Buf& d, const void* h, size_t bytes) {
+            d.ensure(bytes);
+            if (h) CUDA_CHECK(cudaMemcpy(d.p, h, bytes, cudaMemcpyHostToDevice));
+            else CUDA_CHECK(cudaMemset(d.p, 0, bytes));
+        };
+        // outputs and scratch start as NaN / all-ones bits: a value read before it is written, or never written, shows
+        auto poisoned = [&](Buf& d, size_t bytes) { d.ensure(bytes); CUDA_CHECK(cudaMemset(d.p, 0xFF, bytes)); };
+        Buf &d_lg = b[0], &d_hs = b[1], &d_mk = b[2], &d_occ = b[3], &d_sc = b[4], &d_tk = b[5], &d_an = b[6], &d_lo = b[7],
+            &d_hi = b[8], &d_pw = b[9], &d_rmax = b[10], &d_rls = b[11], &d_rule = b[12], &d_cval = b[13], &d_cidx = b[14],
+            &d_ccnt = b[15], &d_sco = b[16], &d_tko = b[17], &d_ano = b[18], &d_loo = b[19], &d_hio = b[20], &d_pwo = b[21],
+            &d_hsc = b[22], &d_hlen = b[23], &d_htk = b[24], &d_hval = b[25], &d_hlo = b[26], &d_hhi = b[27], &d_err = b[28];
+        poisoned(d_lg, (size_t)lrows * ld * 4);                 // the padding columns ld - V stay NaN
+        if (!logits_ignored)
+            CUDA_CHECK(cudaMemcpy2D(d_lg.p, (size_t)ld * 4, logits, (size_t)V * 4, (size_t)V * 4, lrows, cudaMemcpyHostToDevice));
+        if (head_stats) up(d_hs, head_stats, (size_t)R * tiles * 8);
+        up(d_mk, masks, (size_t)R * W * 4);
+        up(d_occ, occurring_mask, (size_t)W * 4);
+        up(d_sc, beam_scores, R * 4); up(d_tk, tokens, (size_t)R * T * 4); up(d_an, ancestry, (size_t)R * T * 4);
+        up(d_lo, lo, R * 8); up(d_hi, hi, R * 8); up(d_pw, pw, R * 8);
+        poisoned(d_rmax, R * 4); poisoned(d_rls, R * 4); poisoned(d_rule, R);
+        poisoned(d_cval, (size_t)R * K * 4); poisoned(d_cidx, (size_t)R * K * 4); poisoned(d_ccnt, R * 4);
+        poisoned(d_sco, R * 4); poisoned(d_tko, (size_t)R * T * 4); poisoned(d_ano, (size_t)R * T * 4);
+        poisoned(d_loo, R * 8); poisoned(d_hio, R * 8); poisoned(d_pwo, R * 8);
+        poisoned(d_hsc, (size_t)Q * K * 4); poisoned(d_hlen, (size_t)Q * K * 4); poisoned(d_htk, (size_t)Q * K * T * 4);
+        poisoned(d_hval, (size_t)Q * K); poisoned(d_hlo, (size_t)Q * K * 8); poisoned(d_hhi, (size_t)Q * K * 8);
+        d_err.ensure(16); CUDA_CHECK(cudaMemset(d_err.p, 0, 16));
+
+        StepCfg c{};
+        c.num_beams = B; c.K = K; c.V = V; c.ld = ld; c.cur_len = cur_len;
+        c.min_length = p->min_length; c.max_length = p->max_length;
+        c.eos_token_id = p->eos_token_id; c.pad_token_id = p->pad_token_id; c.model_eos_token_id = p->model_eos_token_id;
+        c.forced_eos_token_id = p->forced_eos_token_id; c.forced_bos_token_id = p->forced_bos_token_id;
+        c.stop_at_count = p->stop_at_count; c.always_allow_eos = p->always_allow_eos; c.disable_fm_index = p->disable_fm_index;
+        c.remove_invalid_values = p->remove_invalid_values; c.shift = p->shift; c.T = T; c.mask_words = W;
+        c.first_step_shared_mask = shared_mask ? 1 : 0; c.expand_next = cur_len + 1 < T ? 1 : 0;
+        c.logits_shared = logits_shared ? 1 : 0; c.logits_ignored = logits_ignored ? 1 : 0;
+        c.hyps_per_query = K; c.hyp_base = 0;                  // the step's 2B records of each query
+        c.num_groups = grp.num_beam_groups; c.diversity_penalty = grp.diversity_penalty;
+        c.head_tiles = head_stats ? tiles : 0;
+        StepState st{};
+        st.beam_scores_in = d_sc.as<float>(); st.beam_scores_out = d_sco.as<float>();
+        st.tokens_in = d_tk.as<int32_t>(); st.tokens_out = d_tko.as<int32_t>();
+        st.lo_in = d_lo.as<uint64_t>(); st.lo_out = d_loo.as<uint64_t>(); st.hi_in = d_hi.as<uint64_t>(); st.hi_out = d_hio.as<uint64_t>();
+        st.pw_in = d_pw.as<uint64_t>(); st.pw_out = d_pwo.as<uint64_t>();
+        st.anc_in = d_an.as<int32_t>(); st.anc_out = d_ano.as<int32_t>();
+        st.mask_in = d_mk.as<uint32_t>(); st.occurring_mask = d_occ.as<uint32_t>();
+        st.logits = d_lg.as<float>(); st.head_stats = head_stats ? d_hs.as<float2>() : nullptr;
+        st.hyp_score = d_hsc.as<float>(); st.hyp_len = d_hlen.as<int32_t>(); st.hyp_tokens = d_htk.as<int32_t>();
+        st.hyp_valid = d_hval.as<uint8_t>(); st.hyp_lo = d_hlo.as<uint64_t>(); st.hyp_hi = d_hhi.as<uint64_t>();
+        st.error_flag = d_err.as<int32_t>();
+        RowScratch rs{d_rmax.as<float>(), d_rls.as<float>(), d_rule.as<uint8_t>(), d_cval.as<float>(), d_cidx.as<int32_t>(),
+                      d_ccnt.as<int32_t>()};
+        set_select_smem();
+        *lists = launch_select_step(nullptr, view, c, st, rs, Q);
+        CUDA_CHECK(cudaDeviceSynchronize());
+        auto down = [&](void* h, const Buf& d, size_t bytes) { CUDA_CHECK(cudaMemcpy(h, d.p, bytes, cudaMemcpyDeviceToHost)); };
+        down(row_max, d_rmax, R * 4); down(row_logsum, d_rls, R * 4); down(row_rule, d_rule, R);
+        down(cand_val, d_cval, (size_t)R * K * 4); down(cand_idx, d_cidx, (size_t)R * K * 4); down(cand_cnt, d_ccnt, R * 4);
+        down(beam_scores_out, d_sco, R * 4); down(tokens_out, d_tko, (size_t)R * T * 4); down(ancestry_out, d_ano, (size_t)R * T * 4);
+        down(lo_out, d_loo, R * 8); down(hi_out, d_hio, R * 8); down(pw_out, d_pwo, R * 8);
+        down(rec_score, d_hsc, (size_t)Q * K * 4); down(rec_len, d_hlen, (size_t)Q * K * 4); down(rec_tokens, d_htk, (size_t)Q * K * T * 4);
+        down(rec_valid, d_hval, (size_t)Q * K); down(rec_lo, d_hlo, (size_t)Q * K * 8); down(rec_hi, d_hhi, (size_t)Q * K * 8);
+        down(error_flag, d_err, 4);
+    });
 }
 
 int sealdec_debug_topk_rows(int64_t R, int32_t V, int32_t num_beams, int32_t per_row, int32_t iters, double* avg_us) {
