@@ -179,7 +179,11 @@ int sealdec_generate_dx_ex(sealbart_t* model, const sealfm_t* fm, const uint32_t
  * the TF32 operand copies are made on first use), "fused_head" (-1 = $SEALB200_FUSED_HEAD, default on; 0 = the
  * lm_head stores every logit and the select kernel streams them for the log-softmax statistics; 1 = where the select
  * kernels read only the row's allowed tokens, the lm_head emits per-tile statistics and stores only those logits),
- * "poison_logits" (testing: 1 fills the logits buffer with NaN before every such lm_head).  Stats: "last_used_graph",
+ * "poison_logits" (testing: 1 fills the logits buffer with NaN before every such lm_head), "query_slices" (-1 =
+ * $SEALB200_QUERY_SLICES, default on; 1 = after the first decode step a generate whose two halves of the batch have
+ * more than 2 048 rows (queries x beams) each runs the two halves on two streams -- the caller's and one the model
+ * owns, forked and joined with events on the caller's stream, so a CUDA graph captures both -- with bit-identical
+ * records; never while GEMM profiling is on).  Stats: "last_used_graph",
  * "overflow_fallbacks", "gemm_mode", "cached_graphs", "fused_head_steps" (decode steps of the last generate run
  * eagerly that used the statistics epilogue), "last_paths" (-1 for an unknown name).
  * "last_paths" is the OR, over the last generate / teacher-forced / debug-step call (a CUDA-graph replay reports
@@ -191,7 +195,7 @@ int sealdec_generate_dx_ex(sealbart_t* model, const sealfm_t* fm, const uint32_t
  *   8 add + LayerNorm, one CTA per row (<= 2048 rows)  9 add + LayerNorm, one warp per row
  *  10 split-K GEMM summed by its consumer kernel      11 split-K GEMM + finish pass
  *  12 3xFP16 GEMM on whole tiles                      13 3xFP16 GEMM on 2-CTA clusters (gemm_mode 5)
- *  14 3xTF32 GEMM (gemm_mode 2) */
+ *  14 3xTF32 GEMM (gemm_mode 2)                      15 generate run as two query slices ("query_slices") */
 int     sealbart_set_option(sealbart_t* model, const char* name, int64_t value);
 int64_t sealbart_get_stat(const sealbart_t* model, const char* name);
 
@@ -288,7 +292,9 @@ int64_t sealdec_last_launch_count(const sealbart_t* model);
  * then clears the record. */
 int sealdec_profile_gemm(sealbart_t* model, int enable, double* total_us, int64_t* launches, double* flops);
 /* microseconds spent (CUDA events) in the last generate, split by phase:
- * 0 encoder, 1 decoder layers, 2 lm_head, 3 select+expand (FM index), 4 total */
+ * 0 encoder, 1 decoder layers, 2 lm_head, 3 select+expand (FM index), 4 total.  0 and 4 are taken on the caller's
+ * stream; when the generate ran as two query slices, 1..3 of every step after the first are those of the first
+ * slice (the second runs beside it on another stream). */
 int sealdec_last_phase_us(const sealbart_t* model, double out5[5]);
 
 #ifdef __cplusplus

@@ -102,6 +102,12 @@ struct sealbart {
     bool tf32_ready = false;          // 3xTF32 weight splits exist (gemm_mode 2 fallback after an fp16 range overflow)
     int64_t overflow_fallbacks = 0;
     cudaStream_t stream = nullptr;    // the host-buffer entry point's own (non-blocking) stream
+    // query slices (generate_enqueue): the second slice runs on slice_stream, forked from and joined back into the
+    // caller's stream with two events, and has GEMM / mask-expansion scratch of its own
+    int query_slices = -1;            // -1 $SEALB200_QUERY_SLICES (default on), 0 off, 1 on
+    cudaStream_t slice_stream = nullptr;
+    cudaEvent_t slice_fork = nullptr, slice_join = nullptr;
+    Buf a_hi1, a_lo1, splitk1, st_wide1;
 };
 
 namespace {
@@ -174,7 +180,8 @@ void build_slots(sealbart* m) {
 // pending: a split-K GEMM whose slices are still unsummed -- its consumer (add+LN on small batches, the attention kernels)
 // folds the finish pass in; defer_rows = how many rows that consumer accepts (0: the GEMM must finish itself)
 // head: the lm_head GEMM may use the statistics epilogue (HeadEpi); head_fused reports that it did
-struct Ctx { sealbart* m; cudaStream_t s; SplitSrc pending{}; int64_t defer_rows = 0; HeadEpi head{}; bool head_fused = false; };
+// slice: 1 = the second query slice of a generate, which has its own GEMM scratch (a_hi1, a_lo1, splitk1)
+struct Ctx { sealbart* m; cudaStream_t s; SplitSrc pending{}; int64_t defer_rows = 0; HeadEpi head{}; bool head_fused = false; int slice = 0; };
 
 // ---- TMA descriptors ------------------------------------------------------------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -213,7 +220,7 @@ enum : uint32_t {
     kPathCrossSmall = 1u << 6, kPathCrossGrouped = 1u << 7,
     kPathAddLnRow = 1u << 8, kPathAddLnWarp = 1u << 9,
     kPathSplitKDeferred = 1u << 10, kPathSplitKFinish = 1u << 11, kPathGemmFullTile = 1u << 12, kPathGemmCluster = 1u << 13,
-    kPathGemmTf32 = 1u << 14,
+    kPathGemmTf32 = 1u << 14, kPathQuerySlices = 1u << 15,
 };
 
 void split_into(cudaStream_t s, const float* x, float* hi, float* lo, uint64_t numel) {
@@ -273,17 +280,20 @@ void gemm(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, const
 void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, const Act& C, int ldc, bool gelu) {
     if (M == 0) return;
     sealbart* m = cx.m;
+    Buf& a_hi = cx.slice ? m->a_hi1 : m->a_hi;
+    Buf& a_lo = cx.slice ? m->a_lo1 : m->a_lo;
+    Buf& splitk = cx.slice ? m->splitk1 : m->splitk;
     const int tiles = (int)(((N + GN - 1) / GN) * ((M + GM - 1) / GM));
     const int n_fastest = ((int64_t)M >= (int64_t)N) ? 1 : 0;     // stream the larger operand once
     if (m->cfg.gemm_mode >= 3 && K % UK16 == 0 && lda == K && l.w_h1) {
         // 3xFP16; operands pre-split into halves by the producers
         const __half* a1 = A.h1; const __half* a2 = A.h2;
         if (!a1) {
-            m->a_hi.ensure((size_t)M * K * 2); m->a_lo.ensure((size_t)M * K * 2);
+            a_hi.ensure((size_t)M * K * 2); a_lo.ensure((size_t)M * K * 2);
             const int blocks = (int)std::min<int64_t>(((int64_t)M * K + 255) / 256, (int64_t)sm_count() * 8);
-            split_half_kernel<<<blocks, 256, 0, cx.s>>>((int64_t)M * K, A.x, 1.0f, m->a_hi.as<__half>(), m->a_lo.as<__half>(), m->ovf);
+            split_half_kernel<<<blocks, 256, 0, cx.s>>>((int64_t)M * K, A.x, 1.0f, a_hi.as<__half>(), a_lo.as<__half>(), m->ovf);
             CUDA_CHECK(cudaGetLastError()); m->launches++;
-            a1 = m->a_hi.as<__half>(); a2 = m->a_lo.as<__half>();
+            a1 = a_hi.as<__half>(); a2 = a_lo.as<__half>();
         }
         CUtensorMap ma1, ma2;
         make_map(&ma1, a1, M, K, K, GM, true); make_map(&ma2, a2, M, K, K, GM, true);
@@ -311,8 +321,8 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
         }
         if (k_slices > 1) {
             const int64_t slice_stride = (int64_t)M * ldc;
-            m->splitk.ensure((size_t)k_slices * slice_stride * 4);
-            float* part = m->splitk.as<float>();
+            splitk.ensure((size_t)k_slices * slice_stride * 4);
+            float* part = splitk.as<float>();
             const int ctas2 = std::min(tiles * k_slices, sm_count());
             gemm_launch<__half, false, 1>(cx.s, ctas2, ma1, ma2, l.map_hi, l.map_lo, M, N, K, nullptr, 1.0f, part, nullptr, nullptr, ldc, n_fastest, 0, ovf,
                                           k_slices, slice_stride);
@@ -347,9 +357,9 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
     if (m->cfg.gemm_mode == 2 && K % UK == 0 && lda == K && l.w_hi) {
         const float* ahi = A.hi; const float* alo = A.lo;
         if (!ahi) {
-            m->a_hi.ensure((size_t)M * K * 4); m->a_lo.ensure((size_t)M * K * 4);
-            split_into(cx.s, A.x, m->a_hi.as<float>(), m->a_lo.as<float>(), (uint64_t)M * K); m->launches++;
-            ahi = m->a_hi.as<float>(); alo = m->a_lo.as<float>();
+            a_hi.ensure((size_t)M * K * 4); a_lo.ensure((size_t)M * K * 4);
+            split_into(cx.s, A.x, a_hi.as<float>(), a_lo.as<float>(), (uint64_t)M * K); m->launches++;
+            ahi = a_hi.as<float>(); alo = a_lo.as<float>();
         }
         CUtensorMap mah, mal;
         make_map(&mah, ahi, M, K, K, GM); make_map(&mal, alo, M, K, K, GM);
@@ -451,6 +461,10 @@ __global__ void ids_to_tokens_kernel(int64_t R, int t, int T, const int64_t* __r
 struct Dims {
     int64_t Q, S, R; int B, T, d, f, V, ld, W;
     int64_t G = 0; const int32_t* grp_query = nullptr; const int32_t* grp_start = nullptr;   // ragged row groups (re-scoring)
+    // A query slice (generate_enqueue): queries [q0, q0 + Q) of a batch of Qb queries and Rb rows.  Its rows start at
+    // r0 = q0 * B in every row-indexed buffer; the KV cache keeps the batch's row stride Rb, its ancestor indices are
+    // relative to r0.  Qb = Rb = 0: not a slice.
+    int64_t q0 = 0, r0 = 0, Qb = 0, Rb = 0;
 };
 
 void ensure_workspace(sealbart* m, const Dims& D) {
@@ -562,36 +576,41 @@ void encoder_forward(Ctx& cx, const Dims& D, const int64_t* ids_d, const int64_t
 void decoder_step(Ctx& cx, const Dims& D, const int32_t* tokens, int cur_len, const int32_t* anc, bool want_logits,
                   cudaEvent_t ev_layers_done, bool compact = false, const HeadEpi& head = HeadEpi{}) {
     sealbart* m = cx.m;
-    const int d = D.d; const int64_t Rc = D.R; const int64_t Tk = D.Q * D.S;
-    if (compact && (cur_len != 1 || D.grp_start)) throw ApiError(SEALFM_EINVAL, "internal: compact step only at position 0 of a generate");
+    const int d = D.d; const int64_t Rc = D.Rb ? D.Rb : D.R; const int64_t Tk = (D.Qb ? D.Qb : D.Q) * D.S;
+    if (compact && (cur_len != 1 || D.grp_start || D.Qb)) throw ApiError(SEALFM_EINVAL, "internal: compact step only at position 0 of a generate");
     const int64_t R = compact ? D.Q : D.R;          // rows processed
     const int row_mul = compact ? D.B : 1;
     const int pos = cur_len - 1;
     const int gm = m->cfg.gemm_mode;
-    auto mk = [&](float* plain, Buf& bh, Buf& bl, bool keep_plain) {
+    // rows r0 .. r0 + R of the activation buffers ([rows][width])
+    auto mk = [&](float* plain, Buf& bh, Buf& bl, bool keep_plain, int width) {
+        const int64_t o = D.r0 * width;
         Act a;
-        if (keep_plain) a.x = plain;
-        if (gm == 2) { a.hi = bh.as<float>(); a.lo = bl.as<float>(); }
-        if (gm >= 3) { a.h1 = bh.as<__half>(); a.h2 = bl.as<__half>(); }
+        if (keep_plain) a.x = plain + o;
+        if (gm == 2) { a.hi = bh.as<float>() + o; a.lo = bl.as<float>() + o; }
+        if (gm >= 3) { a.h1 = bh.as<__half>() + o; a.h2 = bl.as<__half>() + o; }
         return a;
     };
     int* ovf = m->ovf;
-    const Act x = mk(m->dx.as<float>(), m->dx_hi, m->dx_lo, true);
-    const Act qkv{m->dqkv.as<float>()};
-    const Act attn = mk(m->dattn.as<float>(), m->dattn_hi, m->dattn_lo, false);
-    const Act tmp{m->dtmp.as<float>()};
-    const Act cq{m->dcq.as<float>()};
-    const Act ffn = mk(m->dffn.as<float>(), m->dffn_hi, m->dffn_lo, false);
+    const Act x = mk(m->dx.as<float>(), m->dx_hi, m->dx_lo, true, d);
+    const Act qkv{m->dqkv.as<float>() + D.r0 * 3 * d};
+    const Act attn = mk(m->dattn.as<float>(), m->dattn_hi, m->dattn_lo, false, d);
+    const Act tmp{m->dtmp.as<float>() + D.r0 * d};
+    const Act cq{m->dcq.as<float>() + D.r0 * d};
+    const Act ffn = mk(m->dffn.as<float>(), m->dffn_hi, m->dffn_lo, false, D.f);
     const float scale = m->cfg.scale_embedding ? sqrtf((float)d) : 1.0f;
     launch_k(embed_ln_kernel, (unsigned)((R + 3) / 4), 128, 0, cx.s, R, d, tokens + pos, (int64_t)(D.T * row_mul), (const int32_t*)nullptr, pos,
                (const float*)m->shared, scale, (const float*)m->dec_pos, (const float*)m->dec_ln_emb.g, (const float*)m->dec_ln_emb.b, x.x, split_of(x, ovf));
     m->launches++;
     const int heads = m->cfg.heads;
-    const int32_t* m32 = m->enc_mask.as<int32_t>();
+    // encoder side of queries q0 ..: packed, src_off holds absolute ckv rows; unpacked, query q's rows are q * S
+    const int32_t* m32 = m->enc_mask.as<int32_t>() + D.q0 * D.S;
+    const int32_t* soff_x = m->enc_packed ? m->src_off.as<int32_t>() + D.q0 : nullptr;
+    const int64_t ckv_q0 = m->enc_packed ? 0 : D.q0 * D.S * 2 * d;
     for (int l = 0; l < m->cfg.decoder_layers; ++l) {
         DecLayerW& L = m->dec[l];
-        float* kc = m->kc.as<float>() + (size_t)l * D.T * Rc * d;
-        float* vc = m->vc.as<float>() + (size_t)l * D.T * Rc * d;
+        float* kc = m->kc.as<float>() + (size_t)l * D.T * Rc * d + D.r0 * d;
+        float* vc = m->vc.as<float>() + (size_t)l * D.T * Rc * d + D.r0 * d;
         // the beams of a query together, distinct ancestors staged once (not at the compact first step, where a row
         // stands for all beams, nor for ragged re-scoring groups)
         static const bool sa_query = [] { const char* e = std::getenv("SEALB200_SELF_ATTN_QUERY"); return !e || std::atoi(e) != 0; }();
@@ -626,8 +645,7 @@ void decoder_step(Ctx& cx, const Dims& D, const int32_t* tokens, int cur_len, co
         const SplitSrc cq_src = cx.pending;
         cx.pending = SplitSrc{};
         const int64_t groups = D.grp_start ? D.G : D.Q;
-        const float* ckv_l = m->ckv.as<float>() + (size_t)l * Tk * 2 * d;
-        const int32_t* soff_x = m->enc_packed ? m->src_off.as<int32_t>() : nullptr;
+        const float* ckv_l = m->ckv.as<float>() + (size_t)l * Tk * 2 * d + ckv_q0;
         if (D.S <= kXKeys)
             launch_k(cross_attn_small_kernel, dim3((unsigned)groups, heads), 128, 0, cx.s, groups, d, heads, compact ? 1 : D.B, (int)D.S, (const float*)cq.x,
                        ckv_l, m32, D.grp_query, D.grp_start, attn.x, split_of(attn, ovf), soff_x, cq_src);
@@ -648,7 +666,7 @@ void decoder_step(Ctx& cx, const Dims& D, const int32_t* tokens, int cur_len, co
     }
     if (ev_layers_done) CUDA_CHECK(cudaEventRecord(ev_layers_done, cx.s));
     cx.head = head;                 // only the lm_head may take the statistics epilogue
-    if (want_logits) gemm(cx, R, D.V, d, x, d, m->head, Act{m->logits.as<float>()}, D.ld, false);
+    if (want_logits) gemm(cx, R, D.V, d, x, d, m->head, Act{m->logits.as<float>() + D.r0 * D.ld}, D.ld, false);
     cx.head = HeadEpi{};
 }
 
@@ -728,8 +746,11 @@ void sealbart_free(sealbart_t* m) {
                    &m->st_cidx, &m->st_ccnt, &m->st_wide, &m->hy_score, &m->hy_len, &m->hy_tok,
                    &m->hy_valid, &m->hy_lo, &m->hy_hi, &m->err, &m->dbg_ids, &m->force_syms, &m->a_hi, &m->a_lo, &m->ex_hi, &m->ex_lo,
                    &m->eattn_hi, &m->eattn_lo, &m->effn_hi, &m->effn_lo, &m->dx_hi, &m->dx_lo, &m->dattn_hi, &m->dattn_lo,
-                   &m->dffn_hi, &m->dffn_lo, &m->splitk})
+                   &m->dffn_hi, &m->dffn_lo, &m->splitk, &m->a_hi1, &m->a_lo1, &m->splitk1, &m->st_wide1})
         b->release();
+    if (m->slice_fork) cudaEventDestroy(m->slice_fork);
+    if (m->slice_join) cudaEventDestroy(m->slice_join);
+    if (m->slice_stream) cudaStreamDestroy(m->slice_stream);
     for (auto e : m->events) cudaEventDestroy(e);
     for (auto& g : m->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
     for (Buf* b : {&m->in_ids, &m->in_mask, &m->in_occ}) b->release();
@@ -830,6 +851,11 @@ bool fused_head_on(const sealbart* m) {
     return m->fused_head >= 0 ? m->fused_head != 0 : env_on;
 }
 
+bool query_slices_on(const sealbart* m) {
+    static const bool env_on = [] { const char* e = std::getenv("SEALB200_QUERY_SLICES"); return !e || std::atoi(e) != 0; }();
+    return m->query_slices >= 0 ? m->query_slices != 0 : env_on;
+}
+
 void set_select_smem() {
     CUDA_CHECK(cudaFuncSetAttribute(topk_rows_kernel<512, 8192>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SelSharedT<8192>)));
     CUDA_CHECK(cudaFuncSetAttribute(topk_rows_kernel<256, 4096>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SelSharedT<4096>)));
@@ -898,23 +924,44 @@ void generate_enqueue(Ctx& cx, const Dims& D, const GenArgs& a, const FmView& vi
     c.hyps_per_query = sealdec_hyps_per_query(p);
     c.num_groups = G; c.diversity_penalty = a.grp.diversity_penalty;
     set_select_smem();
-    RowScratch rs{m->st_rowmax.as<float>(), m->st_rowls.as<float>(), m->st_rule.as<uint8_t>(),
-                  m->st_cval.as<float>(), m->st_cidx.as<int32_t>(), m->st_ccnt.as<int32_t>()};
-    int cur = 0;
-    for (int step = 0; step + 1 < T; ++step) {
-        const int cur_len = step + 1;
-        mark();
-        static const bool compact_first = [] { const char* e = std::getenv("SEALB200_COMPACT_FIRST"); return !e || std::atoi(e) != 0; }();
-        const bool compact = compact_first && cur_len == 1;
+    // Query slices.  The rows of a decode step are independent, so after the first step (compact: one row per query,
+    // run on the whole batch) queries [0, Q0) and [Q0, Q), Q0 = ceil(Q / 2), run the rest of the decode -- decoder
+    // layers, lm_head, selection, mask expansion -- on two streams: the caller's and m->slice_stream.  One
+    // slice's attention and add+LN kernels then run beside the other slice's GEMM CTAs (wgmma_gemm_x3_kernel leaves
+    // registers and shared memory on the SM for them), and each slice's last GEMM wave is filled by the other's work.
+    // A kernel computes every row the same way on a slice as on the whole batch once a slice has more than kAddLnRowMax
+    // rows (add+LN takes the warp-per-row kernel either way) and no GEMM of a slice is skinny enough for split-K (more
+    // than sm_count / 2 tiles at the narrowest N; bart-large from 2 049 rows on): the lm_head's banded tile order only
+    // reorders independent tiles -- the records are bit-identical with slicing on or off.  Off while profile_gemm
+    // brackets every GEMM with events: overlapping GEMMs would make their summed durations meaningless.
+    const int64_t Q0 = (Q + 1) / 2, R1 = (Q - Q0) * B;       // R1: rows of the smaller slice
+    const int64_t min_tiles = (R1 + GM - 1) / GM * ((std::min(D.d, D.V) + GN - 1) / GN);
+    const bool sliced = query_slices_on(m) && !m->profile_gemm && R1 > kAddLnRowMax && 2 * min_tiles > sm_count();
+    auto slice_dims = [&](int64_t q0, int64_t nq) {
+        Dims S = D;
+        S.Q = nq; S.R = nq * B; S.q0 = q0; S.r0 = q0 * B; S.Qb = D.Q; S.Rb = D.R;
+        return S;
+    };
+    const int H = (int)c.hyps_per_query, head_tiles = (D.V + GN - 1) / GN;
+    static const bool compact_first = [] { const char* e = std::getenv("SEALB200_COMPACT_FIRST"); return !e || std::atoi(e) != 0; }();
+    static const bool skip_dead = [] { const char* e = std::getenv("SEALB200_SKIP_DEAD_STEP"); return !e || std::atoi(e) != 0; }();
+    auto is_dead = [&](int cur_len) {
         // Dead step: when ForcedEOSTokenLogitsProcessor fires (cur_len == max_length - 1, HF semantics restated
         // in apply_processors) it overwrites EVERY processed score with a constant, so neither the recorded
         // hypotheses nor the (already final) beams depend on the model output of this step -- the reference
         // computes it and discards it.  Nothing later reads this position's k / v either.
-        static const bool skip_dead = [] { const char* e = std::getenv("SEALB200_SKIP_DEAD_STEP"); return !e || std::atoi(e) != 0; }();
         const bool forced_all = p->forced_eos_token_id >= 0 && cur_len == p->max_length - 1 && cur_len + 1 == T &&
                                 !(p->forced_bos_token_id >= 0 && cur_len == 1);
-        const bool dead = skip_dead && forced_all;
-        cudaEvent_t b = timing ? new_event(m) : nullptr;
+        return skip_dead && forced_all;
+    };
+    // The model forward of step `step` on the rows of PD (the whole batch or a slice); `timed` parts record the phase
+    // events (sealdec_last_phase_us).  Returns whether the lm_head took the statistics epilogue.
+    auto model_part = [&](Ctx& pc, const Dims& PD, int step, bool timed) {
+        const int cur = step & 1, cur_len = step + 1;
+        const bool compact = compact_first && cur_len == 1;
+        const bool dead = is_dead(cur_len);
+        if (timing && timed) CUDA_CHECK(cudaEventRecord(new_event(m), pc.s));
+        cudaEvent_t b = (timing && timed) ? new_event(m) : nullptr;
         // Statistics epilogue of the lm_head (HeadEpi): the select kernels then read this step's logits only at the
         // row's read set.  topk_rows_kernel reads lp[v] for v in row_bits() and select_merge_kernel (G > 1) for the
         // candidates it re-scores.  With the FM index on, past the first (shared-mask) step and with one group,
@@ -929,48 +976,99 @@ void generate_enqueue(Ctx& cx, const Dims& D, const GenArgs& a, const FmView& vi
         const int eff_len = cur_len - (p->forced_bos_token_id >= 0 ? 1 : 0);
         HeadEpi he{};
         if (fused_head_on(m) && !dead && !compact && !p->disable_fm_index && eff_len > 1 && G == 1 && m->cfg.gemm_mode == 3) {
-            he = HeadEpi{m->st_hstat.as<float2>(), mk[cur], (int)D.W, p->eos_token_id, p->pad_token_id};
-            if (m->poison_logits) CUDA_CHECK(cudaMemsetAsync(m->logits.p, 0xFF, (size_t)D.R * D.ld * 4, cx.s));
+            he = HeadEpi{m->st_hstat.as<float2>() + PD.r0 * head_tiles, mk[cur] + PD.r0 * D.W, (int)D.W, p->eos_token_id, p->pad_token_id};
+            if (m->poison_logits) CUDA_CHECK(cudaMemsetAsync(m->logits.as<float>() + PD.r0 * D.ld, 0xFF, (size_t)PD.R * D.ld * 4, pc.s));
         }
-        cx.head_fused = false;
-        if (!dead) decoder_step(cx, D, tk[cur], cur_len, an[cur], true, b, compact, he);
-        else if (b) CUDA_CHECK(cudaEventRecord(b, cx.s));
-        mark();
-        c.cur_len = cur_len;
-        c.logits_shared = (compact && !dead) ? 1 : 0;
-        c.logits_ignored = dead ? 1 : 0;
-        c.head_tiles = cx.head_fused ? (D.V + GN - 1) / GN : 0;
-        m->fused_head_steps += cx.head_fused ? 1 : 0;
-        c.first_step_shared_mask = (!p->disable_fm_index && eff_len == 1) ? 1 : 0;
-        c.expand_next = (cur_len + 1 < T) ? 1 : 0;
-        c.hyp_base = step * K;
+        pc.head_fused = false;
+        if (!dead) decoder_step(pc, PD, tk[cur] + PD.r0 * T, cur_len, an[cur] + PD.r0 * T, true, b, compact, he);
+        else if (b) CUDA_CHECK(cudaEventRecord(b, pc.s));
+        if (timing && timed) CUDA_CHECK(cudaEventRecord(new_event(m), pc.s));
+        if (timed) m->fused_head_steps += pc.head_fused ? 1 : 0;
+        return pc.head_fused;
+    };
+    // The selection of step `step` on the rows of PD, from the logits model_part left (head_fused: statistics epilogue).
+    auto select_part = [&](Ctx& pc, const Dims& PD, unsigned long long* wide, int step, bool head_fused, bool timed) {
+        const int cur = step & 1, cur_len = step + 1;
+        const bool compact = compact_first && cur_len == 1;
+        const bool dead = is_dead(cur_len);
+        const int64_t r0 = PD.r0, q0 = PD.q0;
+        const int eff_len = cur_len - (p->forced_bos_token_id >= 0 ? 1 : 0);
+        StepCfg cs = c;
+        cs.cur_len = cur_len;
+        cs.logits_shared = (compact && !dead) ? 1 : 0;
+        cs.logits_ignored = dead ? 1 : 0;
+        cs.head_tiles = head_fused ? head_tiles : 0;
+        cs.first_step_shared_mask = (!p->disable_fm_index && eff_len == 1) ? 1 : 0;
+        cs.expand_next = (cur_len + 1 < T) ? 1 : 0;
+        cs.hyp_base = step * K;
         StepState st{};
-        st.beam_scores_in = sc[cur]; st.beam_scores_out = sc[cur ^ 1];
-        st.tokens_in = tk[cur]; st.tokens_out = tk[cur ^ 1];
-        st.lo_in = lo[cur]; st.lo_out = lo[cur ^ 1]; st.hi_in = hi[cur]; st.hi_out = hi[cur ^ 1];
-        st.pw_in = pw[cur]; st.pw_out = pw[cur ^ 1];
-        st.anc_in = an[cur]; st.anc_out = an[cur ^ 1];
-        st.mask_in = mk[cur]; st.mask_out = mk[cur ^ 1];
-        st.occurring_mask = a.occ_d; st.logits = m->logits.as<float>(); st.head_stats = m->st_hstat.as<float2>();
-        st.hyp_score = a.o_score; st.hyp_len = a.o_len; st.hyp_tokens = a.o_tok; st.hyp_valid = a.o_valid;
-        st.hyp_lo = a.o_lo; st.hyp_hi = a.o_hi; st.error_flag = a.err_d;
-        launch_select_step(cx.s, view, c, st, rs, Q);
+        st.beam_scores_in = sc[cur] + r0; st.beam_scores_out = sc[cur ^ 1] + r0;
+        st.tokens_in = tk[cur] + r0 * T; st.tokens_out = tk[cur ^ 1] + r0 * T;
+        st.lo_in = lo[cur] + r0; st.lo_out = lo[cur ^ 1] + r0; st.hi_in = hi[cur] + r0; st.hi_out = hi[cur ^ 1] + r0;
+        st.pw_in = pw[cur] + r0; st.pw_out = pw[cur ^ 1] + r0;
+        st.anc_in = an[cur] + r0 * T; st.anc_out = an[cur ^ 1] + r0 * T;
+        st.mask_in = mk[cur] + r0 * D.W; st.mask_out = mk[cur ^ 1] + r0 * D.W;
+        // the compact first step wrote one logits row per query (of the whole batch)
+        st.occurring_mask = a.occ_d; st.logits = m->logits.as<float>() + (cs.logits_shared ? q0 : r0) * D.ld;
+        st.head_stats = m->st_hstat.as<float2>() + r0 * head_tiles;
+        st.hyp_score = a.o_score + q0 * H; st.hyp_len = a.o_len + q0 * H; st.hyp_tokens = a.o_tok + q0 * H * T;
+        st.hyp_valid = a.o_valid + q0 * H; st.hyp_lo = a.o_lo ? a.o_lo + q0 * H : nullptr; st.hyp_hi = a.o_hi ? a.o_hi + q0 * H : nullptr;
+        st.error_flag = a.err_d;
+        const RowScratch rs{m->st_rowmax.as<float>() + r0, m->st_rowls.as<float>() + r0, m->st_rule.as<uint8_t>() + r0,
+                            m->st_cval.as<float>() + r0 * K, m->st_cidx.as<int32_t>() + r0 * K, m->st_ccnt.as<int32_t>() + r0};
+        launch_select_step(pc.s, view, cs, st, rs, PD.Q);
         m->launches += 2;
-        if (c.expand_next && !p->disable_fm_index) {           // successor sets of the new beams -> next step's masks (:107)
-            launch_expand_masks(view, cx.s, (uint64_t)R, lo[cur ^ 1], hi[cur ^ 1], mk[cur ^ 1], (uint32_t)D.W, (uint32_t)D.V,
-                                (uint32_t)p->shift, m->st_wide.as<unsigned long long>());
+        if (cs.expand_next && !p->disable_fm_index) {          // successor sets of the new beams -> next step's masks (:107)
+            launch_expand_masks(view, pc.s, (uint64_t)PD.R, lo[cur ^ 1] + r0, hi[cur ^ 1] + r0, mk[cur ^ 1] + r0 * D.W, (uint32_t)D.W,
+                                (uint32_t)D.V, (uint32_t)p->shift, wide);
             m->launches += 2;
         }
-        mark();
-        cur ^= 1;
+        if (timing && timed) CUDA_CHECK(cudaEventRecord(new_event(m), pc.s));
+    };
+    auto finalize_part = [&](Ctx& pc, const Dims& PD) {
+        const int cur = (T - 1) & 1;
+        const int64_t r0 = PD.r0, q0 = PD.q0;
+        StepCfg cs = c;
+        cs.cur_len = T; cs.hyp_base = (T - 1) * K;
+        StepState st{};
+        st.hyp_score = a.o_score + q0 * H; st.hyp_len = a.o_len + q0 * H; st.hyp_tokens = a.o_tok + q0 * H * T;
+        st.hyp_valid = a.o_valid + q0 * H; st.hyp_lo = a.o_lo ? a.o_lo + q0 * H : nullptr; st.hyp_hi = a.o_hi ? a.o_hi + q0 * H : nullptr;
+        finalize_kernel<<<(unsigned)((PD.R + 255) / 256), 256, 0, pc.s>>>(PD.Q, cs, sc[cur] + r0, tk[cur] + r0 * T, lo[cur] + r0, hi[cur] + r0, st);
+        CUDA_CHECK(cudaGetLastError()); m->launches++;
+    };
+    if (!sliced) {
+        for (int step = 0; step + 1 < T; ++step) {
+            const bool fused = model_part(cx, D, step, true);
+            select_part(cx, D, m->st_wide.as<unsigned long long>(), step, fused, true);
+        }
+        finalize_part(cx, D);
+    } else {
+        // slice 0 on the caller's stream (it records the per-step phase events), slice 1 on slice_stream; the steps of
+        // the two are enqueued alternately so that both streams always have work queued
+        m->last_paths |= kPathQuerySlices;
+        const Dims PD[2] = {slice_dims(0, Q0), slice_dims(Q0, Q - Q0)};
+        unsigned long long* wide[2] = {m->st_wide.as<unsigned long long>(), m->st_wide1.as<unsigned long long>()};
+        // The first step selects per slice, so that every ancestor index is slice-relative from the start, but both
+        // slices do so before the fork: the compact step's logits rows (one per query of the whole batch) lie inside
+        // slice 0's rows, which its next lm_head overwrites.
+        const bool fused0 = model_part(cx, D, 0, true);
+        for (int i = 0; i < 2; ++i) select_part(cx, PD[i], wide[i], 0, fused0, i == 0);
+        CUDA_CHECK(cudaEventRecord(m->slice_fork, cx.s));
+        CUDA_CHECK(cudaStreamWaitEvent(m->slice_stream, m->slice_fork, 0));
+        Ctx pcx[2] = {Ctx{m, cx.s}, Ctx{m, m->slice_stream}};
+        pcx[1].slice = 1;
+        for (int step = 1; step + 1 < T; ++step)
+            for (int i = 0; i < 2; ++i) {
+                const bool fused = model_part(pcx[i], PD[i], step, i == 0);
+                select_part(pcx[i], PD[i], wide[i], step, fused, i == 0);
+            }
+        for (int i = 0; i < 2; ++i) finalize_part(pcx[i], PD[i]);
+        CUDA_CHECK(cudaEventRecord(m->slice_join, m->slice_stream));
+        CUDA_CHECK(cudaStreamWaitEvent(cx.s, m->slice_join, 0));
     }
-    c.cur_len = T; c.hyp_base = (T - 1) * K;
-    StepState st{};
-    st.hyp_score = a.o_score; st.hyp_len = a.o_len; st.hyp_tokens = a.o_tok; st.hyp_valid = a.o_valid; st.hyp_lo = a.o_lo; st.hyp_hi = a.o_hi;
-    finalize_kernel<<<(unsigned)((R + 255) / 256), 256, 0, cx.s>>>(Q, c, sc[cur], tk[cur], lo[cur], hi[cur], st);
-    CUDA_CHECK(cudaGetLastError()); m->launches++;
     mark();
-    // events in creation order: ev0, ev_enc, then per step a, b, c, d, then end (sealdec_last_phase_us)
+    // events in creation order: ev0, ev_enc, then per step a, b, c, d, then end (sealdec_last_phase_us); with query
+    // slices a..d of every step after the first come from slice 0
 }
 
 template <typename T> void key_put(std::vector<uint8_t>& k, const T& v) {
@@ -1049,6 +1147,12 @@ int sealdec_generate_dx_ex(sealbart_t* m, const sealfm_t* fm, const uint32_t* oc
         const Dims D = make_dims(m, Q, S, B, T);
         ensure_workspace(m, D);
         if (!p->disable_fm_index) m->st_wide.ensure(expand_scratch_bytes(view.L, (uint64_t)D.R));   // wide-row work list + BFS frontiers
+        if (query_slices_on(m)) {                              // generate_enqueue may run the batch as two query slices
+            if (!m->slice_stream) CUDA_CHECK(cudaStreamCreateWithFlags(&m->slice_stream, cudaStreamNonBlocking));
+            if (!m->slice_fork) CUDA_CHECK(cudaEventCreateWithFlags(&m->slice_fork, cudaEventDisableTiming));
+            if (!m->slice_join) CUDA_CHECK(cudaEventCreateWithFlags(&m->slice_join, cudaEventDisableTiming));
+            if (!p->disable_fm_index) m->st_wide1.ensure(expand_scratch_bytes(view.L, (uint64_t)(Q / 2) * B));
+        }
         const GenArgs a{fm, occ_d, p, grp, ids_d, mask_d, Q, S, o_score, o_len, o_tok, o_valid, o_lo, o_hi, err_d};
 
         // ---- CUDA graph of the whole call: a batch-20 generate is ~1 900 short kernels, i.e. launch-latency-bound.
@@ -1073,7 +1177,7 @@ int sealdec_generate_dx_ex(sealbart_t* m, const sealfm_t* fm, const uint32_t* oc
         sealdec_params_t pc = *p; pc.force_decoding_from = nullptr; key_put(key, pc);
         for (int i = 0; i < p->n_force_decoding_from; ++i) key_put(key, p->force_decoding_from[i]);
         key_put(key, grp.num_beam_groups); key_put(key, grp.diversity_penalty);
-        key_put(key, fused_head_on(m)); key_put(key, m->poison_logits);
+        key_put(key, fused_head_on(m)); key_put(key, m->poison_logits); key_put(key, query_slices_on(m));
         key_put(key, view.blocks); key_put(key, view.csym); key_put(key, view.node_tab); key_put(key, view.m);
         key_put(key, occ_d); key_put(key, ids_d); key_put(key, mask_d); key_put(key, o_score); key_put(key, o_len);
         key_put(key, o_tok); key_put(key, o_valid); key_put(key, o_lo); key_put(key, o_hi); key_put(key, err_d);
@@ -1165,6 +1269,10 @@ int sealbart_set_option(sealbart_t* m, const char* name, int64_t value) {
             m->fused_head = (int)value;
         }
         else if (n == "poison_logits") m->poison_logits = value != 0;
+        else if (n == "query_slices") {
+            if (value < -1 || value > 1) throw ApiError(SEALFM_EINVAL, "query_slices: -1 environment, 0 off, 1 on");
+            m->query_slices = (int)value;
+        }
         else throw ApiError(SEALFM_EINVAL, "unknown option: " + n);
     });
 }

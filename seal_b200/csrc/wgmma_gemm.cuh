@@ -254,8 +254,14 @@ struct HeadEpi {
 // Split-K (CL = 1 only; skinny M, where a handful of tiles would leave most SMs idle): slice s accumulates k-blocks
 // [s*num_k, (s+1)*num_k) and stores its raw fp32 partial tile at C + s*slice_stride (the caller passes bias = nullptr,
 // w_unscale = 1, no split outputs; gemm_splitk_finish_kernel or the consumer kernel sums the slices in a fixed order).
+// Registers: the CTA launches at 128 per thread (49 152 of the SM's 65 536), then the producer warpgroup, whose one live
+// thread only issues TMA, gives its share back (40) and the consumer warpgroups take 168 each (128 x 40 + 256 x 168 <=
+// 384 x 128).  The 16 384 registers left over (and the ~33 KB of shared memory) let small memory-bound kernels of another
+// stream -- add+LN, cross attention -- run beside a GEMM CTA on the same SM.
+constexpr int G_REGS = 128, G_REGS_PRODUCER = 40, G_REGS_CONSUMER = 168;
+static_assert(128 * G_REGS_PRODUCER + 256 * G_REGS_CONSUMER <= GTHREADS * G_REGS, "setmaxnreg budget");
 template <typename T, bool GELU, int CL, bool HEAD = false>
-__global__ void __launch_bounds__(GTHREADS, 1)
+__global__ void __maxnreg__(G_REGS)                   // (excludes __launch_bounds__; launched with GTHREADS threads)
 wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                      const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo,
                      int M, int N, int K, const float* __restrict__ bias, float w_unscale, float* __restrict__ C,
@@ -285,6 +291,7 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
     if (threadIdx.x == 0) gemm_trace(1);
 
     if (wg == 0) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(G_REGS_PRODUCER));
         if (threadIdx.x == 0) {
             uint32_t it = 0;                                               // k-blocks issued so far (all units)
             for (int u = unit0; u < total; u += n_units) {
@@ -313,6 +320,7 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
             }
         }
     } else {
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(G_REGS_CONSUMER));
         const int t = threadIdx.x - 128 * wg, warp = t >> 5, lane = t & 31;
         const uint32_t a_off = (uint32_t)(wg - 1) * 64 * 128;               // this warpgroup's 64 rows of the A tile
         uint32_t empty_peer[CL];
