@@ -184,16 +184,18 @@ __global__ void __launch_bounds__(kWideThreads) expand_rows_wide_kernel(FmView v
 }
 
 // Unordered (symbol, count) pairs + presence bitmap -> ascending-symbol pairs: the position of a symbol is the number
-// of present symbols below it.  One CTA per range: block scan of the bitmap's popcounts, then a scatter.
+// of present symbols below it.  One CTA per range: block scan of the bitmap's popcounts, then a scatter.  The scan goes
+// to `prefix`, global scratch of the bitmap's size (2^L / 8 bytes per range: beyond shared memory from L = 19 on).
 __global__ void __launch_bounds__(256) order_pairs_kernel(uint32_t present_words, const uint32_t* __restrict__ present,
                                                           const unsigned int* __restrict__ counters,
                                                           const uint64_t* __restrict__ list, const uint64_t* __restrict__ list_off,
+                                                          uint32_t* __restrict__ prefix,
                                                           uint64_t* __restrict__ out, uint64_t* __restrict__ out_len) {
-    extern __shared__ uint32_t pre[];                           // exclusive prefix of popcounts, present_words entries
     __shared__ uint32_t warp_tot[8];
     __shared__ uint32_t carry;
     const uint64_t r = blockIdx.x;
     const uint32_t* bm = present + r * (uint64_t)present_words;
+    uint32_t* pre = prefix + r * (uint64_t)present_words;      // exclusive prefix of popcounts, present_words entries
     const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     if (threadIdx.x == 0) carry = 0;
     __syncthreads();
@@ -418,9 +420,10 @@ void release_device(sealfm_t* h) {
 }  // namespace
 
 namespace sealb200 {
-// CTAs of the wide kernel: four per SM, fewer when their global frontiers (2^(L-1) entries each) would pass 1 GB
+// CTAs of the wide kernel: four per SM, fewer when their global frontiers (global_frontier_bytes(L) each) would pass
+// 1 GiB in all, and at least one (528 at L = 16 on 132 SMs; 3 at L = 24, whose frontiers take 320 MiB each)
 static int wide_ctas_for(uint64_t R, uint32_t L) {
-    const uint64_t by_mem = std::max<uint64_t>((uint64_t)sm_count() / 2, ((uint64_t)1 << 30) / global_frontier_bytes(L));
+    const uint64_t by_mem = std::max<uint64_t>(1, ((uint64_t)1 << 30) / global_frontier_bytes(L));
     return (int)std::max<uint64_t>(1, std::min<uint64_t>(R, std::min<uint64_t>((uint64_t)sm_count() * 4, by_mem)));
 }
 // device scratch launch_expand_masks needs for R ranges on a tree of height L: the wide-row work list, then one global
@@ -654,12 +657,15 @@ int sealfm_distinct_count_multi(const sealfm_t* h, uint64_t n, const uint64_t* l
         std::vector<uint64_t> lens(n, 0), tmp;
         out_offsets[0] = 0;
         const uint64_t kChunkPairs = 1ULL << 24;                // u64 of list scratch per pass (2 x 128 MB at most)
+        // presence bitmaps per pass (2^L / 8 bytes per range, and as much again for their prefix): 4 096 ranges up to
+        // L = 18, 64 at L = 24
+        const uint64_t kChunkBitmapBytes = 1ULL << 27;
         const int ns = (int)narrow_smem(L);
         CUDA_CHECK(cudaFuncSetAttribute(expand_rows_kernel<PairRows>, cudaFuncAttributeMaxDynamicSharedMemorySize, ns));
         uint64_t written = 0;
         for (uint64_t c0 = 0; c0 < n;) {
             uint64_t c1 = c0 + 1;
-            while (c1 < n && ub[c1 + 1] - ub[c0] <= kChunkPairs && c1 - c0 < 4096) ++c1;
+            while (c1 < n && ub[c1 + 1] - ub[c0] <= kChunkPairs && c1 - c0 < 4096 && (c1 + 1 - c0) * words * 4 <= kChunkBitmapBytes) ++c1;
             const uint64_t cn = c1 - c0, pairs = ub[c1] - ub[c0];
             std::vector<uint64_t> off(cn + 1);
             for (uint64_t i = 0; i <= cn; ++i) off[i] = ub[c0 + i] - ub[c0];
@@ -667,7 +673,7 @@ int sealfm_distinct_count_multi(const sealfm_t* h, uint64_t n, const uint64_t* l
             const size_t wide_bytes = ((cn + 2 + 1) / 2 * 2) * 8;
             const size_t zero_bytes = cnt_bytes + present_bytes + wide_bytes;
             const size_t bfs_bytes = (size_t)wide_ctas_for(cn, L) * global_frontier_bytes(L);
-            Stage st(h, (2 * cn + cn + 1 + 2 * pairs + cn) * 8 + zero_bytes + bfs_bytes + 512, true);
+            Stage st(h, (2 * cn + cn + 1 + 2 * pairs + cn) * 8 + zero_bytes + present_bytes + bfs_bytes + 512, true);
             const uint64_t* dlo = (const uint64_t*)st.put(lows + c0, cn * 8);
             const uint64_t* dhi = (const uint64_t*)st.put(highs + c0, cn * 8);
             const uint64_t* doff = (const uint64_t*)st.put(off.data(), (cn + 1) * 8);
@@ -684,7 +690,8 @@ int sealfm_distinct_count_multi(const sealfm_t* h, uint64_t n, const uint64_t* l
             unsigned char* dbfs = (unsigned char*)st.reserve(bfs_bytes);
             expand_rows_wide_kernel<PairRows><<<wide_ctas_for(cn, L), kWideThreads, 0, st.stream()>>>(h->view, dlo, dhi, rows, dwide, dbfs);
             CUDA_CHECK(cudaGetLastError());
-            order_pairs_kernel<<<(unsigned)cn, 256, words * 4, st.stream()>>>(words, dpresent, dcnt, dlist, doff, dout, dlen);
+            uint32_t* dprefix = (uint32_t*)st.reserve(present_bytes);
+            order_pairs_kernel<<<(unsigned)cn, 256, 0, st.stream()>>>(words, dpresent, dcnt, dlist, doff, dprefix, dout, dlen);
             CUDA_CHECK(cudaGetLastError());
             st.get(lens.data() + c0, dlen, cn * 8);
             if (out) { tmp.resize(pairs); st.get(tmp.data(), dout, pairs * 8); }
