@@ -107,9 +107,10 @@ int64_t sealdec_hyps_per_query(const sealdec_params_t* p);
  *                                    finalize records carry 2
  *   out_lo/out_hi uint64 [Q][H]      SA range [lo,hi) of the hypothesis' tokens[1:] (0,0 if invalid
  *                                    or FM index disabled); may be NULL
- * Every source must attend to at least one position: a row of attention_mask that is all zero is rejected with
- * SEALFM_EINVAL (here, by sealdec_teacher_forced and by the debug entry points); the device-buffer entry points
- * below do not check it, and their results for such a source are undefined.
+ * Every source must attend to at least one position, and every token id must lie in [0, vocab_size): an
+ * attention_mask row that is all zero or an id outside that range is rejected with SEALFM_EINVAL (here, by
+ * sealdec_teacher_forced and by the debug entry points); the device-buffer entry points below do not check either,
+ * and their results for such a source are undefined.
  * H = sealdec_hyps_per_query(p).  Returns SEALFM_EINVAL("beam") if some query had fewer than
  * num_beams non-EOS candidates (the reference raises ValueError, :687-690).  If an activation leaves the fp16
  * range of the default GEMM mode the pass is repeated with the 3xTF32 kernels (sealbart_get_stat "overflow_fallbacks"). */
@@ -205,7 +206,13 @@ int64_t sealbart_get_stat(const sealbart_t* model, const char* name);
  * scored against encoder input row_query[r] (sorted ascending).  HOST pointers.
  *   out_logprob [N][T-1]: log_softmax(logits_p / temperature)[dec_ids[r][p+1]] for p = 0..T-2
  *                         (full-vocabulary normalisation; the caller masks padding and sums, :131-135)
- *   out_full    [N][V]  : if non-NULL, the whole log-prob vector of position out_full_pos (:167-172) */
+ *   out_full    [N][V]  : if non-NULL, the whole log-prob vector of position out_full_pos (:167-172)
+ * Rows are decoded in passes of 4096; T <= 128.  Returns SEALFM_EINVAL, before anything runs, for an all-zero
+ * attention_mask row, a token id of input_ids or dec_ids outside [0, vocab_size) (the reference raises IndexError),
+ * row_query unsorted or outside [0, Q), and out_full with out_full_pos outside [0, T).  It also returns SEALFM_EINVAL
+ * ("fp16 range exceeded") when an activation of the encoder or the decoder left the fp16 range of the 3xFP16 GEMM
+ * modes: unlike sealdec_generate there is no automatic re-run, the outputs are not to be used, and the caller may
+ * switch to gemm_mode 2 (3xTF32) and call again. */
 int sealdec_teacher_forced(sealbart_t* model, const int64_t* input_ids, const int64_t* attention_mask,
                            int64_t Q, int64_t S, const int64_t* dec_ids, const int32_t* row_query,
                            int64_t N, int64_t T, float temperature, float* out_logprob,
@@ -276,6 +283,17 @@ int sealdec_debug_select_step(const sealfm_t* fm, const sealdec_params_t* p, con
                               int32_t* ancestry_out, uint64_t* lo_out, uint64_t* hi_out, uint64_t* pw_out,
                               float* rec_score, int32_t* rec_len, int32_t* rec_tokens, uint8_t* rec_valid,
                               uint64_t* rec_lo, uint64_t* rec_hi, int32_t* error_flag);
+/* The teacher-forced log-prob kernel of sealdec_teacher_forced on caller-supplied logits, through the same launch.
+ * Host pointers: logits float32 [R][ld] (ld >= V; columns V .. ld-1 are not read), targets int64 read at
+ * r * tgt_stride, out float32 [(R-1)*out_stride + 1] with out[r * out_stride] = log_softmax(logits[r][:V] /
+ * temperature)[target] (fp32 division, as the reference; exactly 0 for a target outside [0, V)), full float32
+ * [(R-1)*full_ld + V] with the whole log-prob row at full[r * full_ld].  out or full may be NULL, not both.  Both are
+ * filled with NaN on the device first, so an element the kernel does not write comes back as NaN.  Arguments the
+ * teacher-forced path never passes (ld < V, temperature <= 0 or not finite, strides < 1, full_ld < V) give
+ * SEALFM_EINVAL. */
+int sealdec_debug_target_logprob(int64_t R, int32_t V, int64_t ld, const float* logits, const int64_t* targets,
+                                 int64_t tgt_stride, float temperature, float* out, int64_t out_stride, float* full,
+                                 int64_t full_ld);
 /* average device time of the decoder's per-row statistics + top-2*beam kernel over R rows of V pseudo-random logits
  * (a later step of constrained beam search, per_row allowed tokens per row) */
 int sealdec_debug_topk_rows(int64_t R, int32_t V, int32_t num_beams, int32_t per_row, int32_t iters, double* avg_us);

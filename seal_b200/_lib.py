@@ -126,6 +126,8 @@ _DEC_SIGS = {
     "sealdec_debug_head": (i32, [C.c_int64, C.c_int32, C.c_int32, vp, vp, vp, vp, C.c_int32, C.c_int32, vp, vp, vp]),
     "sealdec_debug_select_step": (i32, [vp, C.POINTER(DecParams), C.POINTER(GroupParams), C.c_int64, C.c_int32, C.c_int32,
                                         C.c_int32, C.c_int32] + [vp] * 30),
+    "sealdec_debug_target_logprob": (i32, [C.c_int64, C.c_int32, C.c_int64, vp, vp, C.c_int64, C.c_float, vp, C.c_int64,
+                                           vp, C.c_int64]),
     "sealdec_debug_topk_rows":(i32, [C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_double)]),
     "sealdec_debug_gemm_trace": (i32, [i32, C.POINTER(C.c_int64)]),
     "sealev_first_stage": (i32, [C.c_int64, vp, vp, vp, vp, C.c_int64, vp, vp, vp, i32, i32, C.c_double, C.c_double, C.c_int64, vp, vp]),

@@ -1098,13 +1098,31 @@ void drop_graphs(sealbart* m) {
 // A source whose attention mask is all zero has nothing to attend to: the softmax denominator of the encoder and
 // cross-attention kernels stays zero (HF instead spreads the weight over the masked keys and gives finite logits).
 // SEAL never builds one; the host-buffer
-// entry points reject it, the device-buffer ones document it as a precondition.
-void check_sources(const int64_t* mask, int64_t Q, int64_t S) {
+// entry points reject it, the device-buffer ones document it as a precondition.  The same holds for token ids
+// outside [0, V): the embedding kernels index the table with them unchecked (the reference raises IndexError).
+void check_token_ids(const int64_t* ids, int64_t n, int V, const char* what) {
+    for (int64_t i = 0; i < n; ++i)
+        if (ids[i] < 0 || ids[i] >= V)
+            throw ApiError(SEALFM_EINVAL, std::string(what) + " token id " + std::to_string(ids[i]) + " outside [0, vocab_size)");
+}
+
+void check_sources(const int64_t* ids, const int64_t* mask, int64_t Q, int64_t S, int V) {
     for (int64_t q = 0; q < Q; ++q) {
         bool any = false;
         for (int64_t s2 = 0; s2 < S && !any; ++s2) any = mask[q * S + s2] != 0;
         if (!any) throw ApiError(SEALFM_EINVAL, "source " + std::to_string(q) + " has an all-zero attention mask");
     }
+    check_token_ids(ids, Q * S, V, "source");
+}
+
+// out[r * out_stride] = log_softmax(logits[r] / temperature)[targets[r * tgt_stride]] (0 for a target outside
+// [0, V)) and / or the whole row into full[r * full_ld ..]: sealdec_teacher_forced and sealdec_debug_target_logprob
+void launch_target_logprob(cudaStream_t s, int64_t R, int V, int64_t ld, const float* logits, const int64_t* targets,
+                           int64_t tgt_stride, float temperature, float* out, int64_t out_stride, float* full,
+                           int64_t full_ld) {
+    target_logprob_kernel<<<(unsigned)R, 256, 0, s>>>(R, V, ld, logits, targets, tgt_stride, temperature, out, out_stride,
+                                                      full, full_ld);
+    CUDA_CHECK(cudaGetLastError());
 }
 
 }  // namespace
@@ -1348,7 +1366,7 @@ int sealdec_generate_ex(sealbart_t* m, const sealfm_t* fm, const uint32_t* occ_h
         check_model(m);
         if (!p || !ids || !mask || Q <= 0 || S <= 0) throw ApiError(SEALFM_EINVAL, "null argument / empty batch");
         checked_groups(groups, p->num_beams);
-        check_sources(mask, Q, S);
+        check_sources(ids, mask, Q, S, m->cfg.vocab_size);
         const int64_t H = sealdec_hyps_per_query(p), T = p->max_length;
         const int W = (m->cfg.vocab_size + 31) / 32;
         // the caller's buffers are host memory: the real-token count costs nothing to know here, so the encoder
@@ -1419,7 +1437,7 @@ int sealdec_debug_step_logits_ex(sealbart_t* m, const int64_t* ids, const int64_
         if (!ids || !mask || !dec_ids || !out_logits || t < 1 || t > kMaxLen || Q <= 0 || S <= 0 || B < 1)
             throw ApiError(SEALFM_EINVAL, "bad argument");
         if (S > m->cfg.max_positions) throw ApiError(SEALFM_EINVAL, "source longer than max_positions");
-        check_sources(mask, Q, S);
+        check_sources(ids, mask, Q, S, m->cfg.vocab_size);
         if (src_tokens_hint != -1 && src_tokens_hint != -2) {
             // a count is only valid for right-padded masks; checked here, where the mask is host memory
             int64_t n = 0; bool prefix = true;
@@ -1432,6 +1450,7 @@ int sealdec_debug_step_logits_ex(sealbart_t* m, const int64_t* ids, const int64_
         }
         const int T = (int)t;
         const Dims D = make_dims(m, Q, S, B, T);
+        check_token_ids(dec_ids, D.R * T, m->cfg.vocab_size, "decoder");
         if (anc)
             for (int64_t i = 0; i < D.R * T; ++i)
                 if (anc[i] < 0 || anc[i] >= D.R) throw ApiError(SEALFM_EINVAL, "ancestor row out of range");
@@ -1467,7 +1486,9 @@ int sealdec_teacher_forced(sealbart_t* m, const int64_t* ids, const int64_t* mas
         if (!ids || !mask || !dec_ids || !row_query || N <= 0 || T < 1 || T > kMaxLen || Q <= 0 || S <= 0)
             throw ApiError(SEALFM_EINVAL, "bad argument");
         if (S > m->cfg.max_positions) throw ApiError(SEALFM_EINVAL, "source longer than max_positions");
-        check_sources(mask, Q, S);
+        if (out_full && (out_full_pos < 0 || out_full_pos >= T)) throw ApiError(SEALFM_EINVAL, "out_full_pos must be in [0, T)");
+        check_sources(ids, mask, Q, S, m->cfg.vocab_size);
+        check_token_ids(dec_ids, N * T, m->cfg.vocab_size, "decoder");
         for (int64_t r = 0; r < N; ++r) {
             if (row_query[r] < 0 || row_query[r] >= Q || (r && row_query[r] < row_query[r - 1]))
                 throw ApiError(SEALFM_EINVAL, "row_query must be sorted and within [0, Q)");
@@ -1478,6 +1499,7 @@ int sealdec_teacher_forced(sealbart_t* m, const int64_t* ids, const int64_t* mas
         ensure_workspace(m, D);
         m->ovf = m->err.as<int>() + 1;
         cudaStream_t s = nullptr;
+        CUDA_CHECK(cudaMemsetAsync(m->ovf, 0, 4, s));          // before the encoder: its producers raise it too
         Buf d_ids, d_mask, d_dec, d_gq, d_gs, d_out, d_full;
         struct Rel { std::vector<Buf*> v; ~Rel() { for (auto b : v) b->release(); } } rel{{&d_ids, &d_mask, &d_dec, &d_gq, &d_gs, &d_out, &d_full}};
         d_ids.ensure(Q * S * 8); d_mask.ensure(Q * S * 8);
@@ -1490,7 +1512,6 @@ int sealdec_teacher_forced(sealbart_t* m, const int64_t* ids, const int64_t* mas
         d_dec.ensure(D.R * T * 8); d_gq.ensure((D.R + 1) * 4); d_gs.ensure((D.R + 2) * 4);
         if (T > 1) d_out.ensure(D.R * (T - 1) * 4);
         if (out_full) d_full.ensure((size_t)D.R * D.V * 4);
-        CUDA_CHECK(cudaMemsetAsync(m->err.as<int>() + 1, 0, 4, s));
         for (int64_t r0 = 0; r0 < N; r0 += kChunk) {
             const int64_t rows = std::min(kChunk, N - r0);
             std::vector<int32_t> gq, gs;
@@ -1509,11 +1530,10 @@ int sealdec_teacher_forced(sealbart_t* m, const int64_t* ids, const int64_t* mas
                 const bool need = (p + 1 < T) || (out_full && p == out_full_pos);
                 if (!need) continue;                           // the last position only feeds the full-vector output
                 decoder_step(cx, C, tk, p + 1, an, true, nullptr);
-                target_logprob_kernel<<<(unsigned)rows, 256, 0, s>>>(
-                    rows, C.V, C.ld, m->logits.as<float>(), d_dec.as<int64_t>() + (p + 1 < T ? p + 1 : 0), T, temperature,
-                    (p + 1 < T) ? d_out.as<float>() + p : nullptr, T - 1,
-                    (out_full && p == out_full_pos) ? d_full.as<float>() : nullptr, C.V);
-                CUDA_CHECK(cudaGetLastError()); m->launches++;
+                launch_target_logprob(s, rows, C.V, C.ld, m->logits.as<float>(), d_dec.as<int64_t>() + (p + 1 < T ? p + 1 : 0), T,
+                                      temperature, (p + 1 < T) ? d_out.as<float>() + p : nullptr, T - 1,
+                                      (out_full && p == out_full_pos) ? d_full.as<float>() : nullptr, C.V);
+                m->launches++;
             }
             if (T > 1 && out_logprob)
                 CUDA_CHECK(cudaMemcpyAsync(out_logprob + r0 * (T - 1), d_out.p, rows * (T - 1) * 4, cudaMemcpyDeviceToHost, s));
@@ -1813,6 +1833,40 @@ int sealdec_debug_topk_rows(int64_t R, int32_t V, int32_t num_beams, int32_t per
         float ms = 0; CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
         *avg_us = (double)ms * 1e3 / iters;
         cudaEventDestroy(e0); cudaEventDestroy(e1);
+    });
+}
+
+int sealdec_debug_target_logprob(int64_t R, int32_t V, int64_t ld, const float* logits, const int64_t* targets,
+                                 int64_t tgt_stride, float temperature, float* out, int64_t out_stride, float* full,
+                                 int64_t full_ld) {
+    return guarded([&] {
+        // only what sealdec_teacher_forced passes: ld >= V, a positive finite temperature, at least one output
+        if (R <= 0 || V <= 0 || ld < V || !logits || (!out && !full)) throw ApiError(SEALFM_EINVAL, "bad argument");
+        if (!(temperature > 0.f) || !std::isfinite(temperature)) throw ApiError(SEALFM_EINVAL, "temperature must be positive and finite");
+        if (out && (!targets || tgt_stride < 1 || out_stride < 1)) throw ApiError(SEALFM_EINVAL, "bad target / output stride");
+        if (full && full_ld < V) throw ApiError(SEALFM_EINVAL, "full_ld must be >= V");
+        if ((uint64_t)R > INT32_MAX) throw ApiError(SEALFM_EINVAL, "too many rows");
+        int count = 0;
+        if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) { cudaGetLastError(); throw ApiError(SEALFM_ENODEVICE, "no CUDA device available"); }
+        Buf d_lg, d_tg, d_out, d_full;
+        struct Rel { std::vector<Buf*> v; ~Rel() { for (auto b : v) b->release(); } } rel{{&d_lg, &d_tg, &d_out, &d_full}};
+        const size_t n_out = out ? (size_t)(R - 1) * out_stride + 1 : 0;
+        const size_t n_tg = out ? (size_t)(R - 1) * tgt_stride + 1 : 0;
+        const size_t n_full = full ? (size_t)(R - 1) * full_ld + V : 0;
+        d_lg.ensure((size_t)R * ld * 4);
+        CUDA_CHECK(cudaMemcpy(d_lg.p, logits, (size_t)R * ld * 4, cudaMemcpyHostToDevice));
+        // the outputs start as NaN: an element the kernel does not write comes back that way
+        if (out) {
+            d_tg.ensure(n_tg * 8); d_out.ensure(n_out * 4);
+            CUDA_CHECK(cudaMemcpy(d_tg.p, targets, n_tg * 8, cudaMemcpyHostToDevice));
+            CUDA_CHECK(cudaMemset(d_out.p, 0xFF, n_out * 4));
+        }
+        if (full) { d_full.ensure(n_full * 4); CUDA_CHECK(cudaMemset(d_full.p, 0xFF, n_full * 4)); }
+        launch_target_logprob(nullptr, R, V, ld, d_lg.as<float>(), out ? d_tg.as<int64_t>() : nullptr, tgt_stride, temperature,
+                              out ? d_out.as<float>() : nullptr, out_stride, full ? d_full.as<float>() : nullptr, full_ld);
+        CUDA_CHECK(cudaDeviceSynchronize());
+        if (out) CUDA_CHECK(cudaMemcpy(out, d_out.p, n_out * 4, cudaMemcpyDeviceToHost));
+        if (full) CUDA_CHECK(cudaMemcpy(full, d_full.p, n_full * 4, cudaMemcpyDeviceToHost));
     });
 }
 

@@ -643,9 +643,11 @@ __global__ void __launch_bounds__(256) target_logprob_kernel(int64_t R, int V, i
         const float x = lp[v] / temperature;              // the reference divides the logits (seal/keys.py:167)
         if (x > mx) { se *= expf(mx - x); mx = x; }
         if (mx > -INFINITY) se += expf(x - mx);
+        else if (isnan(x)) se = x;                        // a NaN ahead of the thread's first finite entry
     }
     const float bm = block_reduce_max(mx, red);
-    const float scaled = (mx > -INFINITY) ? se * expf(mx - bm) : 0.f;
+    // se is 0 while mx = -inf unless a NaN was seen: it then makes the whole row NaN, as torch's log_softmax does
+    const float scaled = (mx > -INFINITY) ? se * expf(mx - bm) : se;
     const float tot = block_reduce_sum(scaled, red);
     const float logsum = logf(tot);
     if (out && threadIdx.x == 0) {
