@@ -90,7 +90,18 @@ typedef struct {
     int32_t n_force_decoding_from;
     const int64_t* force_decoding_from;   /* host pointer */
     int32_t shift;                   /* 10 */
+    int32_t top_k;                   /* 0 = off; > 0: TopKLogitsWarper(top_k) on every step's raw logits, see below */
 } sealdec_params_t;
+/* top_k (constrained_beam_search's topk, seal/beam_search.py:163-164,249-253): before the log-softmax, every logit below
+ * tau, the min(top_k, V)-th largest of its fp32 row, becomes -inf (ties at tau are kept, -0.0 == +0.0, -inf entries count
+ * as values).  The row max is unchanged; the log-softmax denominator sums exp(x - max) over x >= tau only, and a -inf
+ * fill-in pick (a masked candidate, SURVEY.md H4) records -inf when its logit is below tau.  The forcing steps (forced
+ * BOS, forced EOS) overwrite every score and are unaffected.  top_k >= V is no warp at all and takes the top_k = 0 path
+ * (bit-identical records).  A top_k > 0 step stores the lm_head's logits densely (no statistics epilogue) and runs one
+ * more kernel per step whose logits are read.  SEALFM_EINVAL for top_k < 0, for top_k > 0 with num_beam_groups > 1
+ * (group_beam_search has no warper) and for top_k > 0 with vocab_size > 53 248 (the row is staged in shared memory;
+ * bart-large's 50 265 fits).  The member sits in the struct's former tail padding: a caller that zero-initialises the
+ * struct keeps the previous behaviour. */
 
 /* Number of hypothesis records per query that sealdec_generate writes:
  * (max_length-1) * 2*num_beams + num_beams   (process :662-668 every step + finalize :717-725). */
@@ -256,12 +267,12 @@ int sealdec_debug_gemm_ex(int mode, int64_t M, int32_t N, int32_t K, const float
  * statistics, as the decoder then does. */
 int sealdec_debug_head(int64_t M, int32_t N, int32_t K, const float* A, const float* W, const float* bias,
                        const uint32_t* mask, int32_t eos, int32_t pad, float* C, float* stats, int32_t* fused);
-/* One decode step's selection (log-softmax statistics, processors, index mask, top-2*beam, the scorer bookkeeping,
+/* One decode step's selection (log-softmax statistics or the top-k warp of p->top_k, processors, index mask, top-2*beam, the scorer bookkeeping,
  * the records and the LF step) on caller-supplied inputs, through the same kernel dispatch as the generate entry
  * points.  Host pointers; B = p->num_beams, T = p->max_length, R = Q*B, W = ceil(V/32), G from `groups` (NULL = 1).
  * Configurations a generate never produces are rejected with SEALFM_EINVAL (B > 32, cur_len outside
  * [1, max_length-1], logits_shared away from cur_len 1, logits_ignored away from the forced-EOS step, head statistics
- * on a step where the lm_head would not write them, ...).
+ * on a step where the lm_head would not write them or with p->top_k > 0, ...).
  * Inputs:  logits float32 [logits_shared ? Q : R][V] (NULL with logits_ignored; padded to the generate's stride with
  *          NaN), head_stats float32 [R][ceil(V/128)][2] from the lm_head epilogue or NULL (statistics streamed from
  *          the logits), masks uint32 [R][W] (may be NULL where not read), occurring_mask uint32 [W] (the first
@@ -294,6 +305,12 @@ int sealdec_debug_select_step(const sealfm_t* fm, const sealdec_params_t* p, con
 int sealdec_debug_target_logprob(int64_t R, int32_t V, int64_t ld, const float* logits, const int64_t* targets,
                                  int64_t tgt_stride, float temperature, float* out, int64_t out_stride, float* full,
                                  int64_t full_ld);
+/* The top-k warp's threshold kernel of the generate (one CTA per row) on caller-supplied rows, through the same launch.
+ * Host pointers: logits float32 [R][ld] (ld >= V; columns V .. ld-1 are not read), V <= 53 248, top_k >= 1 (values above
+ * V select the smallest value).  Per row: out_thr = tau, the min(top_k, V)-th largest value (-0.0 returned as +0.0),
+ * out_max = the row max, out_logsum = log(sum over x >= tau of exp(x - max)). */
+int sealdec_debug_topk_threshold(int64_t R, int32_t V, int64_t ld, const float* logits, int32_t top_k, float* out_thr,
+                                 float* out_max, float* out_logsum);
 /* average device time of the decoder's per-row statistics + top-2*beam kernel over R rows of V pseudo-random logits
  * (a later step of constrained beam search, per_row allowed tokens per row) */
 int sealdec_debug_topk_rows(int64_t R, int32_t V, int32_t num_beams, int32_t per_row, int32_t iters, double* avg_us);

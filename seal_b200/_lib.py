@@ -87,7 +87,7 @@ class DecParams(C.Structure):             # sealdec_params_t
                 ("forced_eos_token_id", C.c_int32), ("forced_bos_token_id", C.c_int32),
                 ("stop_at_count", C.c_int32), ("always_allow_eos", C.c_int32), ("disable_fm_index", C.c_int32),
                 ("remove_invalid_values", C.c_int32), ("n_force_decoding_from", C.c_int32),
-                ("force_decoding_from", C.POINTER(C.c_int64)), ("shift", C.c_int32)]
+                ("force_decoding_from", C.POINTER(C.c_int64)), ("shift", C.c_int32), ("top_k", C.c_int32)]
 
 
 class GroupParams(C.Structure):           # sealdec_groups_t
@@ -128,6 +128,7 @@ _DEC_SIGS = {
                                         C.c_int32, C.c_int32] + [vp] * 30),
     "sealdec_debug_target_logprob": (i32, [C.c_int64, C.c_int32, C.c_int64, vp, vp, C.c_int64, C.c_float, vp, C.c_int64,
                                            vp, C.c_int64]),
+    "sealdec_debug_topk_threshold": (i32, [C.c_int64, C.c_int32, C.c_int64, vp, C.c_int32, vp, vp, vp]),
     "sealdec_debug_topk_rows":(i32, [C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_double)]),
     "sealdec_debug_gemm_trace": (i32, [i32, C.POINTER(C.c_int64)]),
     "sealev_first_stage": (i32, [C.c_int64, vp, vp, vp, vp, C.c_int64, vp, vp, vp, i32, i32, C.c_double, C.c_double, C.c_int64, vp, vp]),

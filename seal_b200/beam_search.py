@@ -4,8 +4,8 @@
   (``__call__(input_ids, scores) -> scores + mask``, beam_search.py:33-140); the FM-index work and
   the mask run as CUDA kernels on the tensors' device, no ``.tolist()`` / H2D round trips.
 * ``fm_index_generate`` — same signature and return value (beam_search.py:391-557), no sampling: encoder,
-  every decoder step, log-softmax, processors, FM-index constraint, top-k and BeamSearchScorerWithMemory all
-  run inside libsealb200.so.  ``keep_history=True`` is the path SEALSearcher uses, also with diverse beam
+  every decoder step, the top-k logits warp (``topk``), log-softmax, processors, FM-index constraint, top-k and
+  BeamSearchScorerWithMemory all run inside libsealb200.so.  ``keep_history=True`` is the path SEALSearcher uses, also with diverse beam
   groups (``diverse_bs_groups`` / ``diverse_bs_penalty``); ``keep_history=False`` (transformers' stock
   BeamSearchScorer, the signature's default) and ``transformers_output=True`` run the same kernels and replay
   the stock scorer over the per-step records (one beam group only).
@@ -197,14 +197,15 @@ def _engine_for(model):
 
 
 def _make_params(cfg, num_beams, min_length, max_length, length_penalty, eos_token_id, force_decoding_from,
-                 always_allow_eos, disable_fm_index, stop_at_count, forced_bos_token_id):
+                 always_allow_eos, disable_fm_index, stop_at_count, forced_bos_token_id, top_k=0):
     force = list(force_decoding_from or [])
     farr = (C.c_int64 * max(len(force), 1))(*force)
     none = lambda x: -1 if x is None else int(x)
     p = DecParams(int(num_beams), int(min_length if min_length is not None else -1), int(max_length),
                   float(length_penalty), int(eos_token_id), int(cfg.pad_token_id), int(cfg.decoder_start_token_id),
                   none(cfg.eos_token_id), none(getattr(cfg, "forced_eos_token_id", None)), none(forced_bos_token_id),
-                  int(stop_at_count), int(bool(always_allow_eos)), int(bool(disable_fm_index)), 1, len(force), farr, SHIFT)
+                  int(stop_at_count), int(bool(always_allow_eos)), int(bool(disable_fm_index)), 1, len(force), farr, SHIFT,
+                  int(top_k))
     p._keepalive = farr
     return p
 
@@ -227,6 +228,21 @@ def _check_diverse_groups(num_beams, diverse_bs_groups, diverse_bs_penalty):
             f"has to be divisible by `num_beam_groups`, but is {diverse_bs_groups} with `num_beams` being {num_beams}.")
 
 
+def _check_topk(topk, diverse_bs_groups):
+    """fm_index_generate's `topk` as the kernels take it (include/sealdec.h sealdec_params_t.top_k), checked the way the
+    reference meets it before its first step (seal/beam_search.py:163-164, :249-250): a falsy value is off (None too,
+    where the reference would raise a TypeError at `topk > 0`); a positive value goes through transformers'
+    TopKLogitsWarper constructor (`True` is the int 1); a negative one leaves `topk_warper` unbound.  Diverse beam groups
+    run group_beam_search, which never sees topk (:523-532): then it is neither checked nor used."""
+    if diverse_bs_groups > 1 or not topk:
+        return 0
+    if topk > 0:
+        if not isinstance(topk, int):
+            raise ValueError(f"`top_k` has to be a strictly positive integer, but is {topk}")
+        return int(topk)
+    raise UnboundLocalError("cannot access local variable 'topk_warper' where it is not associated with a value")
+
+
 def _group_params(num_beam_groups, diversity_penalty):
     # a penalty <= 0 means no Hamming processor (seal/beam_search.py:447)
     return GroupParams(int(num_beam_groups), float(diversity_penalty) if diversity_penalty > 0.0 else 0.0)
@@ -235,10 +251,11 @@ def _group_params(num_beam_groups, diversity_penalty):
 def generate_records(model, index, input_ids, attention_mask, min_length=3, max_length=25, length_penalty=1.0,
                      num_beams=3, eos_token_id=None, force_decoding_from=None, always_allow_eos=False,
                      disable_fm_index=False, stop_at_count=0, forced_bos_token_id="config", want_ranges=True,
-                     num_beam_groups=1, diversity_penalty=0.0):
+                     num_beam_groups=1, diversity_penalty=0.0, top_k=0):
     """The C-ABI call with HOST buffers (sealdec_generate_ex): returns the packed hypothesis records
     (scores [Q,H] f32, lens [Q,H] i32, tokens [Q,H,T] i32, valid [Q,H] u8, lo/hi [Q,H] u64).
-    num_beam_groups > 1: diverse beam groups (include/sealdec.h sealdec_groups_t), records group by group per step."""
+    num_beam_groups > 1: diverse beam groups (include/sealdec.h sealdec_groups_t), records group by group per step.
+    top_k > 0: the top-k logits warp on every step (sealdec_params_t.top_k; one group only)."""
     eng = _engine_for(model)
     cfg = eng.config
     if forced_bos_token_id == "config":
@@ -249,7 +266,7 @@ def generate_records(model, index, input_ids, attention_mask, min_length=3, max_
     am = np.ascontiguousarray(np.asarray(attention_mask.cpu() if hasattr(attention_mask, "cpu") else attention_mask, dtype=np.int64))
     Q, S = ids.shape
     p = _make_params(cfg, num_beams, min_length, max_length, length_penalty, eos_token_id, force_decoding_from,
-                     always_allow_eos, disable_fm_index, stop_at_count, forced_bos_token_id)
+                     always_allow_eos, disable_fm_index, stop_at_count, forced_bos_token_id, top_k)
     H = int(lib.sealdec_hyps_per_query(C.byref(p)))
     T = int(max_length)
     scores = np.empty((Q, H), dtype=np.float32); lens = np.empty((Q, H), dtype=np.int32)
@@ -313,13 +330,13 @@ def _side_stream(device):
 def generate_records_device(model, index, input_ids_d, attention_mask_d, min_length=3, max_length=25, length_penalty=1.0,
                             num_beams=3, eos_token_id=None, force_decoding_from=None, always_allow_eos=False,
                             disable_fm_index=False, stop_at_count=0, forced_bos_token_id="config", out=None,
-                            src_tokens=-1, stream=None, num_beam_groups=1, diversity_penalty=0.0):
+                            src_tokens=-1, stream=None, num_beam_groups=1, diversity_penalty=0.0, top_k=0):
     """sealdec_generate_dx on DEVICE tensors, asynchronous: input_ids / attention_mask are int64 CUDA tensors
     [Q, S]; the records land in `out` (a DeviceRecords, created if None) on `stream` (default: the current stream if
     it is not the legacy default stream, else a per-device side stream that first waits for the current one).
     `src_tokens`: number of non-zero mask entries if the caller knows it (right-padded masks) — then the call never
     touches the host; -1 = unknown.  Errors are flags inside the buffer (`out.host()["errors"]`, include/sealdec.h).
-    `num_beam_groups` / `diversity_penalty`: diverse beam groups, as in generate_records."""
+    `num_beam_groups` / `diversity_penalty` / `top_k`: diverse beam groups and the top-k warp, as in generate_records."""
     torch = _torch()
     from .sharding import RecordLayout
     eng = _engine_for(model)
@@ -333,7 +350,7 @@ def generate_records_device(model, index, input_ids_d, attention_mask_d, min_len
     ids = input_ids_d.contiguous(); am = attention_mask_d.contiguous()
     Q, S = ids.shape
     p = _make_params(cfg, num_beams, min_length, max_length, length_penalty, eos_token_id, force_decoding_from,
-                     always_allow_eos, disable_fm_index, stop_at_count, forced_bos_token_id)
+                     always_allow_eos, disable_fm_index, stop_at_count, forced_bos_token_id, top_k)
     H = int(lib.sealdec_hyps_per_query(C.byref(p)))
     dev = ids.device
     if out is None:
@@ -372,7 +389,7 @@ def sharded_generate_records(model, index, input_ids, attention_mask, group=None
     """N-GPU generate: this rank decodes its contiguous block of the batch (host arrays in, as SEALSearcher holds
     them), the records stay on the device and ONE NCCL gather brings every rank's buffer to `dst`
     (SURVEY.md section 8e).  Returns the full-batch record arrays on `dst`, None elsewhere.  `kw` are
-    generate_records_device's arguments, num_beam_groups / diversity_penalty included (same record layout)."""
+    generate_records_device's arguments, num_beam_groups / diversity_penalty / top_k included (same record layout)."""
     torch = _torch()
     from .sharding import sharded_generate
     eng = _engine_for(model)
@@ -518,9 +535,10 @@ def fm_index_generate(model, index: FMIndex, input_ids, attention_mask, min_leng
                       stop_at_count: int = 0, topk: int = 0, transformers_output: bool = False, **kwargs):
     """beam_search.py:391-557.  `model` is an HF BartForConditionalGeneration (its weights are
     mirrored on the GPU once and cached) or a SealBartEngine."""
-    if sample or topk:
-        raise NotImplementedError("sampling / top-k warping are outside the constrained-decoding hot path")
+    if sample:
+        raise NotImplementedError("sampling is outside the constrained-decoding hot path")
     _check_diverse_groups(num_beams, diverse_bs_groups, diverse_bs_penalty)
+    top_k = _check_topk(topk, diverse_bs_groups)
     if diverse_bs_groups > 1 and not keep_history:
         raise NotImplementedError("diverse_bs_groups > 1 with keep_history=False (transformers' stock grouped BeamSearchScorer) "
                                   "is not implemented; keep_history=True, the path SEALSearcher uses, is")
@@ -530,7 +548,7 @@ def fm_index_generate(model, index: FMIndex, input_ids, attention_mask, min_leng
         rec = generate_records(model, index, input_ids, attention_mask, min_length, max_length, length_penalty,
                                num_beams, eos_token_id, force_decoding_from, always_allow_eos, disable_fm_index,
                                stop_at_count, forced_bos, want_ranges=False, num_beam_groups=diverse_bs_groups,
-                               diversity_penalty=diverse_bs_penalty)
+                               diversity_penalty=diverse_bs_penalty, top_k=top_k)
         if transformers_output:
             # BeamSearchScorerWithMemory.finalize returns an UNINITIALISED [Q*num_beams, 3] tensor as `sequences`
             # (:727); zeros of that shape here
@@ -546,14 +564,14 @@ def fm_index_generate(model, index: FMIndex, input_ids, attention_mask, min_leng
     am_np = np.ascontiguousarray(np.asarray(attention_mask.cpu() if hasattr(attention_mask, "cpu") else attention_mask, dtype=np.int64))
     out = generate_records_device(eng, index, torch.from_numpy(ids_np).to(dev), torch.from_numpy(am_np).to(dev), min_length,
                                   max_length, length_penalty, num_beams, eos_token_id, force_decoding_from, always_allow_eos,
-                                  disable_fm_index, stop_at_count, forced_bos, src_tokens=-2)
+                                  disable_fm_index, stop_at_count, forced_bos, src_tokens=-2, top_k=top_k)
     rec = out.host()
     if rec["errors"][1] and eng.gemm_mode >= 3:        # fp16 range exceeded: redo with the 3xTF32 kernels (sealdec.h)
         check(lib.sealbart_set_option(eng._h, b"gemm_mode", 2))
         try:
             rec = generate_records_device(eng, index, torch.from_numpy(ids_np).to(dev), torch.from_numpy(am_np).to(dev), min_length,
                                           max_length, length_penalty, num_beams, eos_token_id, force_decoding_from, always_allow_eos,
-                                          disable_fm_index, stop_at_count, forced_bos, src_tokens=-2).host()
+                                          disable_fm_index, stop_at_count, forced_bos, src_tokens=-2, top_k=top_k).host()
         finally:
             check(lib.sealbart_set_option(eng._h, b"gemm_mode", eng.gemm_mode))
     # the device's "fewer than num_beams non-EOS candidates" flag also fires for queries the stock scorer had already

@@ -76,6 +76,7 @@ struct sealbart {
     Buf st_scores, st_tokens, st_lo, st_hi, st_pw, st_anc, st_mask;
     Buf st_rowmax, st_rowls, st_rule, st_cval, st_cidx, st_ccnt, st_wide;     // scratch between the kernels of a step
     Buf st_hstat;                     // [R][V / 128] lm_head tile statistics (HeadEpi)
+    Buf st_thr;                       // [R][3] top-k warp statistics of each logits row (topk_threshold_kernel)
     Buf hy_score, hy_len, hy_tok, hy_valid, hy_lo, hy_hi, err, dbg_ids, force_syms, a_hi, a_lo, splitk;
     std::vector<void*> split_allocs;
     int64_t launches = 0;
@@ -483,6 +484,7 @@ void ensure_workspace(sealbart* m, const Dims& D) {
     m->st_anc.ensure(2 * D.R * D.T * 4); m->st_mask.ensure((size_t)2 * D.R * D.W * 4);
     m->st_rowmax.ensure(D.R * 4); m->st_rowls.ensure(D.R * 4); m->st_rule.ensure(D.R);
     m->st_hstat.ensure((size_t)D.R * ((D.V + GN - 1) / GN) * 8);
+    m->st_thr.ensure((size_t)D.R * 3 * 4);
     m->st_cval.ensure((size_t)D.R * 2 * D.B * 4); m->st_cidx.ensure((size_t)D.R * 2 * D.B * 4); m->st_ccnt.ensure(D.R * 4);
     {
         m->ex_hi.ensure(Tk * D.d * 4); m->ex_lo.ensure(Tk * D.d * 4);
@@ -742,7 +744,7 @@ void sealbart_free(sealbart_t* m) {
     if (m->lm_head_given) cudaFree(m->lm_head);
     for (Buf* b : {&m->enc_tok, &m->enc_mask, &m->src_off, &m->ex, &m->eqkv, &m->eattn, &m->etmp, &m->effn, &m->ckv, &m->dx, &m->dqkv,
                    &m->dattn, &m->dtmp, &m->dcq, &m->dffn, &m->logits, &m->kc, &m->vc, &m->st_scores, &m->st_tokens,
-                   &m->st_lo, &m->st_hi, &m->st_pw, &m->st_anc, &m->st_mask, &m->st_rowmax, &m->st_hstat, &m->st_rowls, &m->st_rule, &m->st_cval,
+                   &m->st_lo, &m->st_hi, &m->st_pw, &m->st_anc, &m->st_mask, &m->st_rowmax, &m->st_hstat, &m->st_thr, &m->st_rowls, &m->st_rule, &m->st_cval,
                    &m->st_cidx, &m->st_ccnt, &m->st_wide, &m->hy_score, &m->hy_len, &m->hy_tok,
                    &m->hy_valid, &m->hy_lo, &m->hy_hi, &m->err, &m->dbg_ids, &m->force_syms, &m->a_hi, &m->a_lo, &m->ex_hi, &m->ex_lo,
                    &m->eattn_hi, &m->eattn_lo, &m->effn_hi, &m->effn_lo, &m->dx_hi, &m->dx_lo, &m->dattn_hi, &m->dattn_lo,
@@ -859,15 +861,24 @@ bool query_slices_on(const sealbart* m) {
 void set_select_smem() {
     CUDA_CHECK(cudaFuncSetAttribute(topk_rows_kernel<512, 8192>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SelSharedT<8192>)));
     CUDA_CHECK(cudaFuncSetAttribute(topk_rows_kernel<256, 4096>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SelSharedT<4096>)));
+    CUDA_CHECK(cudaFuncSetAttribute(topk_threshold_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTopkMaxVocab * 4));
 }
 
-// One decode step's selection on Q queries: topk_rows_kernel, then select_merge_kernel (set_select_smem() first).
-// Returns `lists`, the candidate lists per query.  The first step (cur_len 1): beams 1.. carry -1e9 and are pruned
+// (max, log sum exp over x >= tau, tau) of `rows` logits rows of V <= kTopkMaxVocab values at stride ld into row_thr[rows][3]
+// (set_select_smem() first): the generate's top-k steps and sealdec_debug_topk_threshold
+void launch_topk_threshold(cudaStream_t s, int64_t rows, int V, int64_t ld, const float* logits, int top_k, float* row_thr) {
+    launch_k(topk_threshold_kernel, (unsigned)rows, kTopkThreads, (size_t)V * 4, s, V, ld, logits, top_k, row_thr);
+}
+
+// One decode step's selection on Q queries: topk_threshold_kernel on a top-k step (topk_warp_step), topk_rows_kernel, then
+// select_merge_kernel (set_select_smem() first).  Returns `lists`, the candidate lists per query.  The first step (cur_len 1): beams 1.. carry -1e9 and are pruned
 // exactly inside one CTA per query; afterwards one CTA per row.  Diverse beam groups at the first step: lists of row 0
 // (every group leader) and row 1 (every other beam) only, see select_merge_kernel.
 int launch_select_step(cudaStream_t s, const FmView& view, const StepCfg& c, const StepState& st, const RowScratch& rs, int64_t Q) {
     const int B = c.num_beams, gs = B / c.num_groups;
     int lists;
+    if (topk_warp_step(c))
+        launch_topk_threshold(s, c.logits_shared ? Q : Q * B, c.V, c.ld, st.logits, c.top_k, rs.row_thr);
     if (c.cur_len == 1 && c.num_groups > 1) {
         lists = gs > 1 ? 2 : 1;
         launch_k(topk_rows_kernel<512, 8192>, (unsigned)(Q * lists), 512, sizeof(SelSharedT<8192>), s, c, st, rs, lists, 1);
@@ -923,6 +934,7 @@ void generate_enqueue(Ctx& cx, const Dims& D, const GenArgs& a, const FmView& vi
     c.remove_invalid_values = p->remove_invalid_values; c.shift = p->shift; c.T = T; c.mask_words = D.W;
     c.hyps_per_query = sealdec_hyps_per_query(p);
     c.num_groups = G; c.diversity_penalty = a.grp.diversity_penalty;
+    c.top_k = p->top_k < D.V ? p->top_k : 0;                 // top_k >= V keeps every logit: the top_k = 0 path
     set_select_smem();
     // Query slices.  The rows of a decode step are independent, so after the first step (compact: one row per query,
     // run on the whole batch) queries [0, Q0) and [Q0, Q), Q0 = ceil(Q / 2), run the rest of the decode -- decoder
@@ -971,11 +983,12 @@ void generate_enqueue(Ctx& cx, const Dims& D, const GenArgs& a, const FmView& vi
         // query that are not finite candidates: fewer than K + want < 2K <= 128 flat indices from the query's first
         // row, i.e. columns 0..127 of that row (V >= 128) -- the first n tile, which HeadEpi stores in full for every
         // row.  Every other case stays dense:
-        // the compact first step, disable_fm_index, forced BOS (eff_len 1 reads the occurring mask), G > 1, the
-        // other GEMM modes.
+        // the compact first step, disable_fm_index, forced BOS (eff_len 1 reads the occurring mask), G > 1, the top-k
+        // warp (its threshold needs every logit of the row), the other GEMM modes.
         const int eff_len = cur_len - (p->forced_bos_token_id >= 0 ? 1 : 0);
         HeadEpi he{};
-        if (fused_head_on(m) && !dead && !compact && !p->disable_fm_index && eff_len > 1 && G == 1 && m->cfg.gemm_mode == 3) {
+        if (fused_head_on(m) && !dead && !compact && !p->disable_fm_index && eff_len > 1 && G == 1 && c.top_k == 0 &&
+            m->cfg.gemm_mode == 3) {
             he = HeadEpi{m->st_hstat.as<float2>() + PD.r0 * head_tiles, mk[cur] + PD.r0 * D.W, (int)D.W, p->eos_token_id, p->pad_token_id};
             if (m->poison_logits) CUDA_CHECK(cudaMemsetAsync(m->logits.as<float>() + PD.r0 * D.ld, 0xFF, (size_t)PD.R * D.ld * 4, pc.s));
         }
@@ -1015,9 +1028,10 @@ void generate_enqueue(Ctx& cx, const Dims& D, const GenArgs& a, const FmView& vi
         st.hyp_valid = a.o_valid + q0 * H; st.hyp_lo = a.o_lo ? a.o_lo + q0 * H : nullptr; st.hyp_hi = a.o_hi ? a.o_hi + q0 * H : nullptr;
         st.error_flag = a.err_d;
         const RowScratch rs{m->st_rowmax.as<float>() + r0, m->st_rowls.as<float>() + r0, m->st_rule.as<uint8_t>() + r0,
-                            m->st_cval.as<float>() + r0 * K, m->st_cidx.as<int32_t>() + r0 * K, m->st_ccnt.as<int32_t>() + r0};
+                            m->st_cval.as<float>() + r0 * K, m->st_cidx.as<int32_t>() + r0 * K, m->st_ccnt.as<int32_t>() + r0,
+                            m->st_thr.as<float>() + (cs.logits_shared ? q0 : r0) * 3};
         launch_select_step(pc.s, view, cs, st, rs, PD.Q);
-        m->launches += 2;
+        m->launches += topk_warp_step(cs) ? 3 : 2;
         if (cs.expand_next && !p->disable_fm_index) {          // successor sets of the new beams -> next step's masks (:107)
             launch_expand_masks(view, pc.s, (uint64_t)PD.R, lo[cur ^ 1] + r0, hi[cur ^ 1] + r0, mk[cur ^ 1] + r0 * D.W, (uint32_t)D.W,
                                 (uint32_t)D.V, (uint32_t)p->shift, wide);
@@ -1089,6 +1103,15 @@ sealdec_groups_t checked_groups(const sealdec_groups_t* g, int num_beams) {
     return r;
 }
 
+// top_k: 0 = off, > 0 TopKLogitsWarper(top_k) on every step's logits -- only on the single-group path (group_beam_search
+// has no warper, seal/beam_search.py:523-532) and for rows that fit topk_threshold_kernel's shared memory.
+void check_top_k(int32_t top_k, const sealdec_groups_t& grp, int V) {
+    if (top_k < 0) throw ApiError(SEALFM_EINVAL, "top_k must be >= 0 (0 = off)");
+    if (top_k > 0 && grp.num_beam_groups > 1) throw ApiError(SEALFM_EINVAL, "top_k > 0 needs num_beam_groups == 1");
+    if (top_k > 0 && V > kTopkMaxVocab)
+        throw ApiError(SEALFM_EINVAL, "top_k > 0 needs vocab_size <= " + std::to_string(kTopkMaxVocab));
+}
+
 void drop_graphs(sealbart* m) {
     for (auto& g : m->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
     m->graphs.clear();
@@ -1139,6 +1162,7 @@ int sealdec_generate_dx_ex(sealbart_t* m, const sealfm_t* fm, const uint32_t* oc
         const int B = p->num_beams, K = 2 * B, T = p->max_length;
         if (B < 1 || B > kSelMaxBeams || K > kSelMaxK) throw ApiError(SEALFM_EINVAL, "num_beams must be in [1,32]");
         const sealdec_groups_t grp = checked_groups(groups, B);
+        check_top_k(p->top_k, grp, m->cfg.vocab_size);
         if (T < 2 || T > kMaxLen) throw ApiError(SEALFM_EINVAL, "max_length must be in [2,128]");
         if (Q <= 0 || S <= 0) throw ApiError(SEALFM_EINVAL, "empty batch");
         if (S > m->cfg.max_positions) throw ApiError(SEALFM_EINVAL, "source longer than max_positions");
@@ -1708,6 +1732,8 @@ int sealdec_debug_select_step(const sealfm_t* fm, const sealdec_params_t* p, con
         if (!logits_ignored && !logits) throw ApiError(SEALFM_EINVAL, "logits missing");
         if (head_stats && !(fm_on && eff_len > 1 && grp.num_beam_groups == 1 && V >= GN && !logits_ignored && !logits_shared))
             throw ApiError(SEALFM_EINVAL, "head statistics: only after the first step, with the FM index on, one group and V >= 128");
+        check_top_k(p->top_k, grp, V);
+        if (head_stats && p->top_k > 0) throw ApiError(SEALFM_EINVAL, "head statistics: not with top_k > 0 (dense logits)");
         if (fm_on && !fb_step && !shared_mask && !masks) throw ApiError(SEALFM_EINVAL, "masks missing");
         if (shared_mask && !occurring_mask) throw ApiError(SEALFM_EINVAL, "occurring mask missing");
         FmView view{};
@@ -1728,7 +1754,7 @@ int sealdec_debug_select_step(const sealfm_t* fm, const sealdec_params_t* p, con
         const int ld = (V + 3) / 4 * 4, W = (V + 31) / 32, tiles = (V + GN - 1) / GN;
         const int64_t lrows = logits_shared ? Q : R;
 
-        std::vector<Buf> b(29);
+        std::vector<Buf> b(30);
         struct Rel { std::vector<Buf>& v; ~Rel() { for (auto& x : v) x.release(); } } rel{b};
         auto up = [&](Buf& d, const void* h, size_t bytes) {
             d.ensure(bytes);
@@ -1740,7 +1766,8 @@ int sealdec_debug_select_step(const sealfm_t* fm, const sealdec_params_t* p, con
         Buf &d_lg = b[0], &d_hs = b[1], &d_mk = b[2], &d_occ = b[3], &d_sc = b[4], &d_tk = b[5], &d_an = b[6], &d_lo = b[7],
             &d_hi = b[8], &d_pw = b[9], &d_rmax = b[10], &d_rls = b[11], &d_rule = b[12], &d_cval = b[13], &d_cidx = b[14],
             &d_ccnt = b[15], &d_sco = b[16], &d_tko = b[17], &d_ano = b[18], &d_loo = b[19], &d_hio = b[20], &d_pwo = b[21],
-            &d_hsc = b[22], &d_hlen = b[23], &d_htk = b[24], &d_hval = b[25], &d_hlo = b[26], &d_hhi = b[27], &d_err = b[28];
+            &d_hsc = b[22], &d_hlen = b[23], &d_htk = b[24], &d_hval = b[25], &d_hlo = b[26], &d_hhi = b[27], &d_err = b[28],
+            &d_thr = b[29];
         poisoned(d_lg, (size_t)lrows * ld * 4);                 // the padding columns ld - V stay NaN
         if (!logits_ignored)
             CUDA_CHECK(cudaMemcpy2D(d_lg.p, (size_t)ld * 4, logits, (size_t)V * 4, (size_t)V * 4, lrows, cudaMemcpyHostToDevice));
@@ -1749,7 +1776,7 @@ int sealdec_debug_select_step(const sealfm_t* fm, const sealdec_params_t* p, con
         up(d_occ, occurring_mask, (size_t)W * 4);
         up(d_sc, beam_scores, R * 4); up(d_tk, tokens, (size_t)R * T * 4); up(d_an, ancestry, (size_t)R * T * 4);
         up(d_lo, lo, R * 8); up(d_hi, hi, R * 8); up(d_pw, pw, R * 8);
-        poisoned(d_rmax, R * 4); poisoned(d_rls, R * 4); poisoned(d_rule, R);
+        poisoned(d_rmax, R * 4); poisoned(d_rls, R * 4); poisoned(d_rule, R); poisoned(d_thr, (size_t)R * 3 * 4);
         poisoned(d_cval, (size_t)R * K * 4); poisoned(d_cidx, (size_t)R * K * 4); poisoned(d_ccnt, R * 4);
         poisoned(d_sco, R * 4); poisoned(d_tko, (size_t)R * T * 4); poisoned(d_ano, (size_t)R * T * 4);
         poisoned(d_loo, R * 8); poisoned(d_hio, R * 8); poisoned(d_pwo, R * 8);
@@ -1769,6 +1796,7 @@ int sealdec_debug_select_step(const sealfm_t* fm, const sealdec_params_t* p, con
         c.hyps_per_query = K; c.hyp_base = 0;                  // the step's 2B records of each query
         c.num_groups = grp.num_beam_groups; c.diversity_penalty = grp.diversity_penalty;
         c.head_tiles = head_stats ? tiles : 0;
+        c.top_k = p->top_k < V ? p->top_k : 0;
         StepState st{};
         st.beam_scores_in = d_sc.as<float>(); st.beam_scores_out = d_sco.as<float>();
         st.tokens_in = d_tk.as<int32_t>(); st.tokens_out = d_tko.as<int32_t>();
@@ -1781,7 +1809,7 @@ int sealdec_debug_select_step(const sealfm_t* fm, const sealdec_params_t* p, con
         st.hyp_valid = d_hval.as<uint8_t>(); st.hyp_lo = d_hlo.as<uint64_t>(); st.hyp_hi = d_hhi.as<uint64_t>();
         st.error_flag = d_err.as<int32_t>();
         RowScratch rs{d_rmax.as<float>(), d_rls.as<float>(), d_rule.as<uint8_t>(), d_cval.as<float>(), d_cidx.as<int32_t>(),
-                      d_ccnt.as<int32_t>()};
+                      d_ccnt.as<int32_t>(), d_thr.as<float>()};
         set_select_smem();
         *lists = launch_select_step(nullptr, view, c, st, rs, Q);
         CUDA_CHECK(cudaDeviceSynchronize());
@@ -1820,7 +1848,8 @@ int sealdec_debug_topk_rows(int64_t R, int32_t V, int32_t num_beams, int32_t per
         StepState st{};
         st.beam_scores_in = sc.as<float>(); st.tokens_in = tk.as<int32_t>(); st.pw_in = pw.as<uint64_t>();
         st.mask_in = mk.as<uint32_t>(); st.logits = lg.as<float>();
-        RowScratch rs{rmax.as<float>(), rls.as<float>(), rule.as<uint8_t>(), cval.as<float>(), cidx.as<int32_t>(), ccnt.as<int32_t>()};
+        RowScratch rs{rmax.as<float>(), rls.as<float>(), rule.as<uint8_t>(), cval.as<float>(), cidx.as<int32_t>(), ccnt.as<int32_t>(),
+                      nullptr};
         using RowsLater = SelSharedT<4096>;
         CUDA_CHECK(cudaFuncSetAttribute(topk_rows_kernel<256, 4096>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RowsLater)));
         launch_k(topk_rows_kernel<256, 4096>, (unsigned)R, 256, sizeof(RowsLater), nullptr, c, st, rs, B, 1);
@@ -1833,6 +1862,28 @@ int sealdec_debug_topk_rows(int64_t R, int32_t V, int32_t num_beams, int32_t per
         float ms = 0; CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
         *avg_us = (double)ms * 1e3 / iters;
         cudaEventDestroy(e0); cudaEventDestroy(e1);
+    });
+}
+
+int sealdec_debug_topk_threshold(int64_t R, int32_t V, int64_t ld, const float* logits, int32_t top_k, float* out_thr,
+                                 float* out_max, float* out_logsum) {
+    return guarded([&] {
+        if (R <= 0 || V <= 0 || ld < V || !logits || top_k < 1 || !out_thr || !out_max || !out_logsum || (uint64_t)R > INT32_MAX)
+            throw ApiError(SEALFM_EINVAL, "bad argument");
+        if (V > kTopkMaxVocab) throw ApiError(SEALFM_EINVAL, "V must be <= " + std::to_string(kTopkMaxVocab));
+        int count = 0;
+        if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) { cudaGetLastError(); throw ApiError(SEALFM_ENODEVICE, "no CUDA device available"); }
+        Buf d_lg, d_thr;
+        struct Rel { std::vector<Buf*> v; ~Rel() { for (auto b : v) b->release(); } } rel{{&d_lg, &d_thr}};
+        d_lg.ensure((size_t)R * ld * 4); d_thr.ensure((size_t)R * 3 * 4);
+        CUDA_CHECK(cudaMemcpy(d_lg.p, logits, (size_t)R * ld * 4, cudaMemcpyHostToDevice));
+        CUDA_CHECK(cudaMemset(d_thr.p, 0xFF, (size_t)R * 3 * 4));
+        set_select_smem();
+        launch_topk_threshold(nullptr, R, V, ld, d_lg.as<float>(), top_k, d_thr.as<float>());
+        CUDA_CHECK(cudaDeviceSynchronize());
+        std::vector<float> h((size_t)R * 3);
+        CUDA_CHECK(cudaMemcpy(h.data(), d_thr.p, h.size() * 4, cudaMemcpyDeviceToHost));
+        for (int64_t r = 0; r < R; ++r) { out_max[r] = h[r * 3]; out_logsum[r] = h[r * 3 + 1]; out_thr[r] = h[r * 3 + 2]; }
     });
 }
 

@@ -38,7 +38,14 @@ struct StepCfg {
     float diversity_penalty;           // Hamming diversity penalty, 0 = no HammingDiversityLogitsProcessor
     int32_t head_tiles;                // > 0: the lm_head wrote per-(row, n tile) statistics (head_stats, HeadEpi) and the
                                        //    logits only at the row's read set; 0: dense logits, statistics streamed here
+    int32_t top_k;                     // TopKLogitsWarper on the raw logits, 1 <= top_k < V; 0 = off (also for top_k >= V)
 };
+
+// Whether this step's logits go through the top-k warp: the forcing steps (forced BOS at cur_len 1, the forced-EOS step
+// whose logits are ignored) overwrite every score in apply_processors, so the warp cannot change them and is skipped.
+__host__ __device__ __forceinline__ bool topk_warp_step(const StepCfg& c) {
+    return c.top_k > 0 && !c.logits_ignored && !(c.forced_bos_token_id >= 0 && c.cur_len == 1);
+}
 
 struct StepState {
     // per row (R = Q*num_beams), double-buffered by the caller
@@ -157,7 +164,142 @@ __device__ void sel_merge(SH& S, int K) {
 struct RowScratch {
     float* row_max; float* row_logsum; uint8_t* row_rule;     // [R]  log-softmax statistics / index rule of every row
     float* cand_val; int32_t* cand_idx; int32_t* cand_cnt;    // [Q * lists][K] sorted best candidates per candidate list, [Q * lists]
+    float* row_thr;                                           // [logits rows][3] (max, log sum exp over x >= tau, tau) of the
+                                                              // top-k warp (topk_threshold_kernel); read on topk_warp_step only
 };
+
+// ---- top-k warp (transformers' TopKLogitsWarper before log_softmax, seal/beam_search.py:249-253) ----------------------
+// One CTA per logits row: tau = the k-th largest value of the fp32 row (ties at tau kept, -inf entries count as values),
+// the exact row max, and log(sum over x >= tau of exp(x - max)).  The row is staged once in shared memory as
+// order-preserving uint32 keys (-0.0 canonicalised to +0.0, so that the two compare equal as floats do); the max is the
+// largest key, tau comes out of an MSB-first radix select over 4 digits of 8 bits that counts ties, and the sum is taken
+// over the staged keys in a fixed order (per thread strided, then the warp tree, then the warps in order).
+constexpr int kTopkThreads = 512;
+constexpr int kTopkWarps = kTopkThreads / 32;
+constexpr int kTopkMaxVocab = 53248;   // V * 4 bytes of keys + the static arrays below fit the 227 KB a CTA can opt into
+
+__device__ __forceinline__ uint32_t float_key(float x) {
+    uint32_t u = __float_as_uint(x);
+    if (u == 0x80000000u) u = 0u;                                 // -0.0 == +0.0
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float key_float(uint32_t k) {
+    return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+
+// hist[d] += the number of lanes of this warp with digit d; every lane of the warp calls it, d = 256: no count
+__device__ __forceinline__ void warp_hist_add(uint32_t* hist, uint32_t d) {
+    const unsigned same = __match_any_sync(0xffffffffu, d);
+    if (d < 256u && (threadIdx.x & 31) == (unsigned)(__ffs(same) - 1)) atomicAdd(&hist[d], (uint32_t)__popc(same));
+}
+
+__global__ void __launch_bounds__(kTopkThreads, 1) topk_threshold_kernel(int V, int64_t ld, const float* __restrict__ logits,
+                                                                         int top_k, float* __restrict__ row_thr) {
+    extern __shared__ __align__(16) uint32_t keys[];
+    __shared__ uint32_t hist[kTopkWarps][256];
+    __shared__ uint32_t s_max[kTopkWarps];
+    __shared__ float red[32];
+    __shared__ uint32_t s_prefix, s_rem;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const float* lp = logits + (int64_t)blockIdx.x * ld;
+    const int k = top_k < 1 ? 1 : (top_k > V ? V : top_k);
+    for (int i = tid; i < kTopkWarps * 256; i += kTopkThreads) (&hist[0][0])[i] = 0u;
+    if (tid == 0) { s_prefix = 0u; s_rem = (uint32_t)k; }
+    __syncthreads();
+    // Stage the keys, taking the max and the histogram of the top digit in the same pass.  Every loop below runs the
+    // same number of iterations in all lanes of a warp (warp_hist_add is a warp-wide operation).
+    uint32_t mk = 0u;
+    auto stage = [&](int v, float x, bool in) {
+        uint32_t d = 256u;
+        if (in) {
+            const uint32_t key = float_key(x);
+            keys[v] = key;
+            mk = key > mk ? key : mk;
+            d = key >> 24;
+        }
+        warp_hist_add(hist[warp], d);
+    };
+    int v0 = 0;
+    if ((ld & 3) == 0 && (reinterpret_cast<uintptr_t>(logits) & 15) == 0) {
+        const int V4 = V >> 2;
+        for (int i0 = 0; i0 < V4; i0 += kTopkThreads) {
+            const int i = i0 + tid;
+            const bool in = i < V4;
+            float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (in) x = reinterpret_cast<const float4*>(lp)[i];
+            const float xs[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll
+            for (int j = 0; j < 4; ++j) stage(4 * i + j, xs[j], in);
+        }
+        v0 = V4 * 4;
+    }
+    for (int b = v0; b < V; b += kTopkThreads) stage(b + tid, b + tid < V ? lp[b + tid] : 0.f, b + tid < V);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { const uint32_t t = __shfl_xor_sync(0xffffffffu, mk, o); mk = t > mk ? t : mk; }
+    if (lane == 0) s_max[warp] = mk;
+    __syncthreads();
+    uint32_t max_key = s_max[0];
+    for (int w = 1; w < kTopkWarps; ++w) max_key = s_max[w] > max_key ? s_max[w] : max_key;
+    // Radix select, most significant digit first: with rem = the rank still wanted among the keys matching the prefix,
+    // take the digit d where (keys above d) < rem <= (keys above d) + (keys with digit d), and continue with rem minus the
+    // keys above d.  Ties at tau are counted, so after the last digit the prefix is the k-th largest key.
+    for (int pass = 0; pass < 4; ++pass) {
+        const int shift = 24 - 8 * pass;
+        if (pass > 0) {
+            const uint32_t prefix = s_prefix;
+            const uint32_t hmask = 0xffffffffu << (shift + 8);
+            for (int b = 0; b < V; b += kTopkThreads) {
+                const int v = b + tid;
+                uint32_t d = 256u;
+                if (v < V) {
+                    const uint32_t key = keys[v];
+                    if ((key & hmask) == prefix) d = (key >> shift) & 0xffu;
+                }
+                warp_hist_add(hist[warp], d);
+            }
+            __syncthreads();
+        }
+        if (warp == 0) {
+            // lane l owns digits 255 - 8l down to 248 - 8l; counts summed over the warp histograms
+            uint32_t cnt[8], tot = 0;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int d = 255 - 8 * lane - j;
+                uint32_t c = 0;
+                for (int w = 0; w < kTopkWarps; ++w) c += hist[w][d];
+                cnt[j] = c; tot += c;
+            }
+            uint32_t incl = tot;                                 // inclusive prefix over the lanes (higher digits first)
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
+            const uint32_t rem = s_rem, excl = incl - tot;
+            __syncwarp();                                        // every lane has read s_rem before one lane writes it
+            if (excl < rem && rem <= incl) {
+                uint32_t above = excl;
+                int j = 0;
+                while (above + cnt[j] < rem) { above += cnt[j]; ++j; }
+                s_prefix |= (uint32_t)(255 - 8 * lane - j) << shift;
+                s_rem = rem - above;
+            }
+        }
+        __syncthreads();
+        for (int i = tid; i < kTopkWarps * 256; i += kTopkThreads) (&hist[0][0])[i] = 0u;
+        __syncthreads();
+    }
+    const uint32_t tau_key = s_prefix;
+    const float mx = key_float(max_key);
+    float se = 0.f;
+    if (mx > -INFINITY)
+        for (int v = tid; v < V; v += kTopkThreads) {
+            const uint32_t key = keys[v];
+            if (key >= tau_key) se += expf(key_float(key) - mx);
+        }
+    se = block_reduce_sum(se, red);
+    if (tid == 0) {
+        float* o = row_thr + (int64_t)blockIdx.x * 3;
+        o[0] = mx; o[1] = logf(se); o[2] = key_float(tau_key);
+    }
+}
 
 // ---- step kernel 1 of 2: row statistics + the best K constrained candidates of a run of beams -----------------------
 // grid = Q * lists CTAs; list g of query q covers beams [g * rows_per_cta, ...).  After the first step a list is ONE
@@ -191,8 +333,13 @@ __global__ void __launch_bounds__(THREADS, THREADS >= 512 ? 2 : 4) topk_rows_ker
         // ---- full-vocabulary log-softmax statistics (seal/beam_search.py:251), ONE streaming pass:
         // per-thread running (max, sum exp(x - max)), merged across the block.
         float mx = -INFINITY, se = 0.f;
+        float tau = -INFINITY;                                   // top-k warp: logits below tau score -inf
+        const bool warp_k = topk_warp_step(c);
         if (c.logits_ignored) { mx = 0.f; se = 1.f; }           // log-softmax statistics are never used (uniform branch)
-        else {
+        else if (warp_k) {                                       // statistics of the warped row (topk_threshold_kernel)
+            const float* t3 = rs.row_thr + (c.logits_shared ? qi : r) * 3;
+            mx = t3[0]; tau = t3[2];
+        } else {
         if (c.head_tiles > 0) {                                  // the lm_head's partials, a fixed order per thread
             const float2* ps = st.head_stats + r * c.head_tiles;
             for (int i = tid; i < c.head_tiles; i += THREADS) {
@@ -242,7 +389,7 @@ __global__ void __launch_bounds__(THREADS, THREADS >= 512 ? 2 : 4) topk_rows_ker
             mx = bm;
         }
         }
-        const float logsum = logf(se);
+        const float logsum = warp_k ? rs.row_thr[(c.logits_shared ? qi : r) * 3 + 1] : logf(se);
         // ---- which tokens does the index allow on this row (seal/beam_search.py:87-135) ----------
         const int32_t* trow = st.tokens_in + r * c.T;
         const int last = trow[c.cur_len - 1];
@@ -277,6 +424,7 @@ __global__ void __launch_bounds__(THREADS, THREADS >= 512 ? 2 : 4) topk_rows_ker
         };
         auto consider = [&](int v, bool guarded) {
             float p = c.logits_ignored ? 0.f : (lp[v] - mx) - logsum;
+            if (warp_k && lp[v] < tau) p = -INFINITY;
             p = apply_processors(c, v, p);
             const float s = p + bs;
             const int flat = b * V + v;
@@ -373,8 +521,11 @@ __global__ void __launch_bounds__(kMergeThreads) select_merge_kernel(FmView fm, 
     const int lane = tid & 31, warp = tid >> 5;
     // grouped path: which candidate list / row statistics stand for row b of group [b0, b0 + gs)
     auto src_row = [&](int b, int b0) -> int { return lists == B ? b : (b == b0 ? 0 : 1); };
+    const bool warp_k = topk_warp_step(c);
     auto row_logprob = [&](int64_t r, int64_t stat_r, int v) -> float {
-        float p = c.logits_ignored ? 0.f : (st.logits[(c.logits_shared ? qi : r) * c.ld + v] - rs.row_max[stat_r]) - rs.row_logsum[stat_r];
+        const int64_t lr = c.logits_shared ? qi : r;
+        float p = c.logits_ignored ? 0.f : (st.logits[lr * c.ld + v] - rs.row_max[stat_r]) - rs.row_logsum[stat_r];
+        if (warp_k && st.logits[lr * c.ld + v] < rs.row_thr[lr * 3 + 2]) p = -INFINITY;    // top-k warp (single group only)
         return apply_processors(c, v, p);
     };
     for (int g = 0; g < G; ++g) {
