@@ -6,7 +6,8 @@
  *   - constrained_beam_search's step                seal/beam_search.py:219-345
  *   - BeamSearchScorerWithMemory.process/finalize   seal/beam_search.py:614-735
  *   - the BART-large forward the reference gets from transformers 4.13 (call sites
- *     seal/beam_search.py:231-238,481-483; model = BartForConditionalGeneration)
+ *     seal/beam_search.py:231-238,481-483; model = BartForConditionalGeneration), or the T5 forward
+ *     (T5ForConditionalGeneration, SEALSearcher's 't5' backbone) behind the same handle (sealt5_create)
  * Plain pointers and sizes only.  Status codes and sealfm_last_error() as in sealfm.h.
  * Everything runs on the GPU; there is no CPU path.
  */
@@ -69,6 +70,45 @@ int  sealbart_set_tensor(sealbart_t* m, const char* key, const float* host, uint
  * given, derives fused/pre-split copies. */
 int  sealbart_finalize(sealbart_t* m);
 uint64_t sealbart_device_bytes(const sealbart_t* m);
+
+/* ---- T5 weights ------------------------------------------------------------------------------- */
+
+typedef struct {
+    int32_t vocab_size;                      /* 32128 for the released t5 checkpoints                          */
+    int32_t d_model;                         /* multiple of 128, <= 1024 (t5-small 512, t5-base 768, t5-large 1024) */
+    int32_t num_layers;                      /* encoder blocks                                                 */
+    int32_t num_decoder_layers;              /* decoder blocks (may differ from num_layers)                    */
+    int32_t num_heads;                       /* num_heads * 64 == d_model                                      */
+    int32_t d_kv;                            /* must be 64 (t5-3b / t5-11b use 128: not covered)               */
+    int32_t d_ff;                            /* multiple of 64                                                 */
+    int32_t ffn_kind;                        /* 0 = relu (DenseReluDense.wi / wo); 1 = gated-gelu (wi_0, wi_1, wo; gelu_new, the tanh form) */
+    int32_t relative_attention_num_buckets;  /* 32; in [4, 1024]                                               */
+    int32_t relative_attention_max_distance; /* 128; > num_buckets / 2                                         */
+    float   layer_norm_epsilon;              /* 1e-6                                                           */
+    int32_t scale_decoder_outputs;           /* 1: the last decoder state is multiplied by d_model^-0.5 before the lm_head */
+    int32_t gemm_mode;                       /* as sealbart_config_t                                           */
+} sealt5_config_t;
+
+/* Creates a T5 model behind the same opaque handle: sealbart_set_tensor / sealbart_finalize / sealbart_free and every
+ * entry point below take it and behave as documented for BART.  A shape the kernels do not cover is rejected with
+ * SEALFM_EINVAL before any allocation (d_kv != 64, num_heads * 64 != d_model, d_model not a multiple of 128 or above
+ * 1024, d_ff % 64 != 0, an unknown ffn_kind, a bucket count / max distance outside the ranges above).
+ * sealbart_set_tensor takes HF T5ForConditionalGeneration state_dict keys: "shared.weight" (aliases
+ * "encoder.embed_tokens.weight", "decoder.embed_tokens.weight"), "encoder.block.{i}.layer.0.SelfAttention.{q,k,v,o}.weight",
+ * "encoder.block.{i}.layer.{0,1}.layer_norm.weight", "encoder.block.{i}.layer.1.DenseReluDense.{wi | wi_0, wi_1, wo}.weight",
+ * "decoder.block.{i}.layer.0.SelfAttention.*", "decoder.block.{i}.layer.1.EncDecAttention.{q,k,v,o}.weight",
+ * "decoder.block.{i}.layer.{0,1,2}.layer_norm.weight", "decoder.block.{i}.layer.2.DenseReluDense.*",
+ * "{encoder,decoder}.block.0.layer.0.SelfAttention.relative_attention_bias.weight" (the only bias tables: every layer
+ * reuses layer 0's, as in HF), "{encoder,decoder}.final_layer_norm.weight" and "lm_head.weight" (tied to shared.weight if
+ * not given).  Every other key -- the keys of the other ffn_kind included -- is SEALFM_EINVAL.
+ * Sources are limited to 1024 positions (T5 has no position table; the encoder's bucket table covers distances
+ * -1023 .. 1023): a longer source is rejected where BART's max_positions is enforced.  Relative position buckets are
+ * computed on the host once per model, in the float32 arithmetic of transformers' _relative_position_bucket. */
+int  sealt5_create(const sealt5_config_t* cfg, int device, sealbart_t** out);
+/* The host bucket table (no device needed): bidirectional (encoder) out[2n-1], out[i] = bucket of key - query = i - (n-1);
+ * unidirectional (decoder) out[n], out[i] = bucket of key - query = -i.  SEALFM_EINVAL for n < 1 or bucket settings
+ * sealt5_create rejects. */
+int  sealt5_relative_buckets(int32_t num_buckets, int32_t max_distance, int32_t bidirectional, int32_t n, int32_t* out);
 
 /* ---- fused generate --------------------------------------------------------------------------- */
 
@@ -207,7 +247,12 @@ int sealdec_generate_dx_ex(sealbart_t* model, const sealfm_t* fm, const uint32_t
  *   8 add + LayerNorm, one CTA per row (<= 2048 rows)  9 add + LayerNorm, one warp per row
  *  10 split-K GEMM summed by its consumer kernel      11 split-K GEMM + finish pass
  *  12 3xFP16 GEMM on whole tiles                      13 3xFP16 GEMM on 2-CTA clusters (gemm_mode 5)
- *  14 3xTF32 GEMM (gemm_mode 2)                      15 generate run as two query slices ("query_slices") */
+ *  14 3xTF32 GEMM (gemm_mode 2)                      15 generate run as two query slices ("query_slices")
+ * and of the T5 forward (a T5 call also sets 6, 7, 10 .. 15 as above; 0 / 1 name its encoder packing):
+ *  16 T5 encoder self-attention with the relative position bias
+ *  17 T5 decoder self-attention with the relative position bias (one warp per row and head, any position)
+ *  18 embedding / add + RMSNorm (one CTA per row; folds a pending split-K GEMM)
+ *  19 ReLU feed-forward (ReLU GEMM epilogue)          20 gated-gelu feed-forward (gelu_new(wi_0 x) * wi_1 x kernel) */
 int     sealbart_set_option(sealbart_t* model, const char* name, int64_t value);
 int64_t sealbart_get_stat(const sealbart_t* model, const char* name);
 

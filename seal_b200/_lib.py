@@ -80,6 +80,14 @@ class BartConfig(C.Structure):            # sealbart_config_t
                 ("max_positions", C.c_int32), ("scale_embedding", C.c_int32), ("gemm_mode", C.c_int32)]
 
 
+class T5Config(C.Structure):              # sealt5_config_t
+    _fields_ = [("vocab_size", C.c_int32), ("d_model", C.c_int32), ("num_layers", C.c_int32),
+                ("num_decoder_layers", C.c_int32), ("num_heads", C.c_int32), ("d_kv", C.c_int32), ("d_ff", C.c_int32),
+                ("ffn_kind", C.c_int32), ("relative_attention_num_buckets", C.c_int32),
+                ("relative_attention_max_distance", C.c_int32), ("layer_norm_epsilon", C.c_float),
+                ("scale_decoder_outputs", C.c_int32), ("gemm_mode", C.c_int32)]
+
+
 class DecParams(C.Structure):             # sealdec_params_t
     _fields_ = [("num_beams", C.c_int32), ("min_length", C.c_int32), ("max_length", C.c_int32),
                 ("length_penalty", C.c_float), ("eos_token_id", C.c_int32), ("pad_token_id", C.c_int32),
@@ -99,6 +107,8 @@ _DEC_SIGS = {
                                          C.c_int64, C.c_int64]),
     "sealbart_create": (i32, [C.POINTER(BartConfig), i32, C.POINTER(vp)]),
     "sealbart_free": (None, [vp]),
+    "sealt5_create": (i32, [C.POINTER(T5Config), i32, C.POINTER(vp)]),
+    "sealt5_relative_buckets": (i32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp]),
     "sealbart_set_tensor": (i32, [vp, cp, vp, u64]),
     "sealbart_finalize": (i32, [vp]),
     "sealbart_device_bytes": (u64, [vp]),

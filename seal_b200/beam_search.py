@@ -21,7 +21,7 @@ from typing import List, Optional
 
 import numpy as np
 
-from ._lib import lib, check, vp, ProcessorCfg, BartConfig, DecParams, GroupParams
+from ._lib import lib, check, vp, ProcessorCfg, BartConfig, DecParams, GroupParams, T5Config
 from .index import FMIndex, SHIFT
 
 stopword_token_ids = [10, 41, 660, 5, 1941, 20, 7, 6]      # beam_search.py:22-31
@@ -126,6 +126,8 @@ class SealBartEngine:
 
     @classmethod
     def from_hf(cls, model, device=None, gemm_mode=None):
+        if getattr(model.config, "model_type", None) == "t5":
+            return SealT5Engine.from_hf(model, device=device, gemm_mode=gemm_mode)
         torch = _torch()
         if device is None:
             p = next(model.parameters())
@@ -181,6 +183,95 @@ class SealBartEngine:
 
     def last_launch_count(self):
         return int(lib.sealdec_last_launch_count(self._h))
+
+
+T5_FFN_KINDS = {"relu": 0, "gated-gelu": 1}      # sealt5_config_t.ffn_kind
+
+
+class T5ConfigView:
+    """A T5 config as the decode reads it, resolved the way transformers 4.13 (the reference's pin) sees a T5
+    checkpoint: decoder_start_token_id from the config, else from the model's generation_config, else pad_token_id (0);
+    forced_bos_token_id / forced_eos_token_id None where the attribute is missing; the decoder output scale
+    d_model^-0.5 applied iff config.scale_decoder_outputs, or tie_word_embeddings where that attribute is missing.
+    Every other attribute is the HF config's."""
+
+    def __init__(self, config, generation_config=None):
+        self._hf = config
+        start = getattr(config, "decoder_start_token_id", None)
+        if start is None and generation_config is not None:
+            start = getattr(generation_config, "decoder_start_token_id", None)
+        if start is None:
+            start = config.pad_token_id
+        self.decoder_start_token_id = int(start)
+        self.forced_bos_token_id = getattr(config, "forced_bos_token_id", None)
+        self.forced_eos_token_id = getattr(config, "forced_eos_token_id", None)
+        self.bos_token_id = getattr(config, "bos_token_id", None)
+        scale = getattr(config, "scale_decoder_outputs", None)
+        self.scale_decoder_outputs = bool(config.tie_word_embeddings if scale is None else scale)
+
+    def __getattr__(self, name):
+        return getattr(self.__dict__["_hf"], name)
+
+
+def t5_native_config(config, gemm_mode):
+    """sealt5_config_t for an HF T5Config; ValueError for a shape or feed-forward the kernels do not cover (the same
+    limits sealt5_create enforces, include/sealdec.h), before anything touches the device."""
+    d, heads, d_kv, d_ff = int(config.d_model), int(config.num_heads), int(config.d_kv), int(config.d_ff)
+    proj = getattr(config, "feed_forward_proj", "relu")
+    if proj not in T5_FFN_KINDS:
+        raise ValueError(f"T5 feed_forward_proj {proj!r} is not implemented (supported: {sorted(T5_FFN_KINDS)})")
+    if d_kv != 64 or heads * 64 != d:
+        raise ValueError(f"T5 shape not covered: d_kv must be 64 and num_heads * 64 == d_model (d_kv={d_kv}, "
+                         f"num_heads={heads}, d_model={d})")
+    if d % 128 or d > 1024:
+        raise ValueError(f"T5 shape not covered: d_model must be a multiple of 128 and <= 1024 (d_model={d})")
+    if d_ff % 64:
+        raise ValueError(f"T5 shape not covered: d_ff must be a multiple of 64 (d_ff={d_ff})")
+    nb = int(config.relative_attention_num_buckets)
+    md = int(getattr(config, "relative_attention_max_distance", 128))
+    if not 4 <= nb <= 1024 or md <= nb // 2:
+        raise ValueError(f"T5 relative attention buckets not covered: num_buckets must be in [4, 1024] and "
+                         f"max_distance > num_buckets / 2 (num_buckets={nb}, max_distance={md})")
+    view = T5ConfigView(config)
+    n_dec = getattr(config, "num_decoder_layers", None)
+    return T5Config(int(config.vocab_size), d, int(config.num_layers), int(n_dec if n_dec is not None else config.num_layers),
+                    heads, d_kv, d_ff, T5_FFN_KINDS[proj], nb, md, float(config.layer_norm_epsilon),
+                    int(view.scale_decoder_outputs), int(gemm_mode))
+
+
+class SealT5Engine(SealBartEngine):
+    """Device-resident T5 weights + workspace behind the same handle (include/sealdec.h `sealt5_create`): every method
+    of SealBartEngine, and every entry point that takes an engine, works the same way.  `config` is a T5ConfigView."""
+
+    def __init__(self, state_dict, config, device=0, gemm_mode=None, generation_config=None):
+        if gemm_mode is None:
+            gemm_mode = int(os.environ.get("SEALB200_GEMM", "3"))
+        cfg = t5_native_config(config, gemm_mode)
+        self.gemm_mode = int(gemm_mode)
+        self.config = T5ConfigView(config, generation_config)
+        self.device = int(device)
+        h = vp()
+        check(lib.sealt5_create(C.byref(cfg), self.device, C.byref(h)))
+        self._h = h.value
+        shared = state_dict.get("shared.weight")
+        for k, v in state_dict.items():
+            if shared is not None and k in ("encoder.embed_tokens.weight", "decoder.embed_tokens.weight"):
+                continue                                    # tied aliases of shared.weight
+            if k == "lm_head.weight" and shared is not None and v.data_ptr() == shared.data_ptr():
+                continue                                    # tie_word_embeddings: the library ties it itself
+            a = np.ascontiguousarray(v.detach().to("cpu").float().numpy())
+            check(lib.sealbart_set_tensor(self._h, k.encode(), a.ctypes.data, a.size))
+        check(lib.sealbart_finalize(self._h))
+
+    @classmethod
+    def from_hf(cls, model, device=None, gemm_mode=None):
+        t5_native_config(model.config, 3 if gemm_mode is None else gemm_mode)      # ValueError before any device work
+        torch = _torch()
+        if device is None:
+            p = next(model.parameters())
+            device = p.device.index if p.is_cuda else torch.cuda.current_device()
+        return cls(model.state_dict(), model.config, device=device, gemm_mode=gemm_mode,
+                   generation_config=getattr(model, "generation_config", None))
 
 
 _ENGINES = weakref.WeakKeyDictionary()

@@ -1,10 +1,11 @@
 // Host orchestration + C ABI (include/sealdec.h) of the constrained beam-search decode:
-// BART weights, workspace, encoder pass, per-step decoder forward, fused select step.
+// BART and T5 weights, workspace, encoder pass, per-step decoder forward, fused select step.
 #include "../../include/sealdec.h"
 #include "bart_kernels.cuh"
 #include "common.cuh"
 #include "decode_kernels.cuh"
 #include "fm_handle.hpp"
+#include "t5_kernels.cuh"
 #include "wgmma_gemm.cuh"
 
 #include <cuda_runtime.h>
@@ -53,7 +54,14 @@ struct Buf {
 }  // namespace
 
 struct sealbart {
-    sealbart_config_t cfg{};
+    sealbart_config_t cfg{};          // a T5 handle fills it from its sealt5_config_t (max_positions = kT5MaxSource)
+    // architecture: 0 BART (sealbart_create), 1 T5 (sealt5_create).  For T5 the Lin biases stay zero, LNp::g holds the
+    // T5LayerNorm weights (EncLayerW: ln_attn = layer.0, ln_final = layer.1; DecLayerW: ln_self / ln_cross / ln_final =
+    // layer.0 / 1 / 2), enc_ln_emb / dec_ln_emb the final_layer_norm of each stack, and fc1 is wi or [wi_0; wi_1].
+    int arch = 0;
+    sealt5_config_t t5{};
+    float* t5_rel_enc = nullptr; float* t5_rel_dec = nullptr;          // layer-0 relative_attention_bias [buckets][heads]
+    int32_t* t5_bkt_enc = nullptr; int32_t* t5_bkt_dec = nullptr;      // bucket of distance k - q, see t5_bucket_tables
     int device = 0;
     float* shared = nullptr; float* enc_pos = nullptr; float* dec_pos = nullptr;
     float* lm_head = nullptr; float* final_bias = nullptr;
@@ -109,6 +117,7 @@ struct sealbart {
     cudaStream_t slice_stream = nullptr;
     cudaEvent_t slice_fork = nullptr, slice_join = nullptr;
     Buf a_hi1, a_lo1, splitk1, st_wide1;
+    Buf effn2, dffn2;                 // T5 gated-gelu: [rows][2 d_ff] output of the [wi_0; wi_1] GEMM
 };
 
 namespace {
@@ -133,6 +142,52 @@ void reg_lin(sealbart* m, const std::string& prefix, Lin& l, int row0, int rows)
 void reg_ln(sealbart* m, const std::string& prefix, LNp& l, int d) {
     reg(m, prefix + ".weight", l.g, d);
     reg(m, prefix + ".bias", l.b, d);
+}
+
+// HF T5ForConditionalGeneration state_dict keys.  No biases and no position tables; the bucket tables are not weights.
+void build_slots_t5(sealbart* m) {
+    const auto& c = m->cfg;
+    const int d = c.d_model, f = c.ffn_dim, V = c.vocab_size, nb = m->t5.relative_attention_num_buckets, H = c.heads;
+    const bool gated = m->t5.ffn_kind == 1;
+    m->shared = dalloc(m, (uint64_t)V * d); reg(m, "shared.weight", m->shared, (uint64_t)V * d);
+    m->final_bias = dalloc(m, V);                                          // zero: T5's lm_head has no bias
+    m->enc_ln_emb.g = dalloc(m, d); reg(m, "encoder.final_layer_norm.weight", m->enc_ln_emb.g, d);
+    m->dec_ln_emb.g = dalloc(m, d); reg(m, "decoder.final_layer_norm.weight", m->dec_ln_emb.g, d);
+    m->t5_rel_enc = dalloc(m, (uint64_t)nb * H);
+    reg(m, "encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight", m->t5_rel_enc, (uint64_t)nb * H);
+    m->t5_rel_dec = dalloc(m, (uint64_t)nb * H);
+    reg(m, "decoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight", m->t5_rel_dec, (uint64_t)nb * H);
+    auto reg_w = [&](const std::string& key, Lin& l, int row0, int rows) { reg(m, key + ".weight", l.w + (uint64_t)row0 * l.in, (uint64_t)rows * l.in); };
+    auto ffn = [&](const std::string& p, Lin& fc1, Lin& fc2) {
+        make_lin(m, fc1, gated ? 2 * f : f, d);
+        if (gated) { reg_w(p + "DenseReluDense.wi_0", fc1, 0, f); reg_w(p + "DenseReluDense.wi_1", fc1, f, f); }
+        else reg_w(p + "DenseReluDense.wi", fc1, 0, f);
+        make_lin(m, fc2, d, f); reg_w(p + "DenseReluDense.wo", fc2, 0, d);
+    };
+    auto attn = [&](const std::string& p, Lin& qkv, Lin& o) {
+        make_lin(m, qkv, 3 * d, d);
+        reg_w(p + "q", qkv, 0, d); reg_w(p + "k", qkv, d, d); reg_w(p + "v", qkv, 2 * d, d);
+        make_lin(m, o, d, d); reg_w(p + "o", o, 0, d);
+    };
+    auto norm = [&](const std::string& key, LNp& l) { l.g = dalloc(m, d); reg(m, key + ".layer_norm.weight", l.g, d); };
+    m->enc.resize(c.encoder_layers);
+    for (int i = 0; i < c.encoder_layers; ++i) {
+        EncLayerW& L = m->enc[i];
+        const std::string p = "encoder.block." + std::to_string(i) + ".layer.";
+        attn(p + "0.SelfAttention.", L.qkv, L.o); norm(p + "0", L.ln_attn);
+        ffn(p + "1.", L.fc1, L.fc2); norm(p + "1", L.ln_final);
+    }
+    m->dec.resize(c.decoder_layers);
+    for (int i = 0; i < c.decoder_layers; ++i) {
+        DecLayerW& L = m->dec[i];
+        const std::string p = "decoder.block." + std::to_string(i) + ".layer.";
+        attn(p + "0.SelfAttention.", L.qkv, L.o); norm(p + "0", L.ln_self);
+        make_lin(m, L.cq, d, d); reg_w(p + "1.EncDecAttention.q", L.cq, 0, d);
+        make_lin(m, L.ckv, 2 * d, d); reg_w(p + "1.EncDecAttention.k", L.ckv, 0, d); reg_w(p + "1.EncDecAttention.v", L.ckv, d, d);
+        make_lin(m, L.co, d, d); reg_w(p + "1.EncDecAttention.o", L.co, 0, d);
+        norm(p + "1", L.ln_cross);
+        ffn(p + "2.", L.fc1, L.fc2); norm(p + "2", L.ln_final);
+    }
 }
 
 void build_slots(sealbart* m) {
@@ -222,6 +277,7 @@ enum : uint32_t {
     kPathAddLnRow = 1u << 8, kPathAddLnWarp = 1u << 9,
     kPathSplitKDeferred = 1u << 10, kPathSplitKFinish = 1u << 11, kPathGemmFullTile = 1u << 12, kPathGemmCluster = 1u << 13,
     kPathGemmTf32 = 1u << 14, kPathQuerySlices = 1u << 15,
+    kPathT5EncAttn = 1u << 16, kPathT5DecAttn = 1u << 17, kPathT5Rms = 1u << 18, kPathT5Relu = 1u << 19, kPathT5Gate = 1u << 20,
 };
 
 void split_into(cudaStream_t s, const float* x, float* hi, float* lo, uint64_t numel) {
@@ -245,11 +301,11 @@ SplitOut split_of(const Act& a, int* overflow) {
     return so;
 }
 
-template <typename T, bool GELU, int CL, bool HEAD = false>
+template <typename T, int ACT, int CL, bool HEAD = false>
 void gemm_launch(cudaStream_t s, int ctas, const CUtensorMap& ahi, const CUtensorMap& alo, const CUtensorMap& whi, const CUtensorMap& wlo,
                  int64_t M, int N, int K, const float* bias, float w_unscale, float* C, T* C1, T* C2, int ldc, int n_fastest, int m_band,
                  int* ovf, int k_slices, int64_t slice_stride, const HeadEpi& he = HeadEpi{}) {
-    auto kern = wgmma_gemm_x3_kernel<T, GELU, CL, HEAD>;
+    auto kern = wgmma_gemm_x3_kernel<T, ACT, CL, HEAD>;
     CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, G_SMEM));
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -261,25 +317,27 @@ void gemm_launch(cudaStream_t s, int ctas, const CUtensorMap& ahi, const CUtenso
                                   k_slices, slice_stride, he));
 }
 
-// C = A W^T + b (+GELU) on the tensor cores: gemm_mode 3 / 5 = 3xFP16 (one CTA per tile / clusters of 2 sharing W), 2 = 3xTF32 (fp32
+// C = A W^T + b (+ the epilogue activation act: kActNone / kActGelu / kActRelu, wgmma_gemm.cuh) on the tensor cores: gemm_mode 3 / 5 = 3xFP16 (one CTA per tile / clusters of 2 sharing W), 2 = 3xTF32 (fp32
 // range: the fallback when an activation leaves the fp16 range).  Operands arrive pre-split from the producing kernel
 // (A.h1/A.h2 or A.hi/A.lo); they are split here only if the producer did not.
-void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, const Act& C, int ldc, bool gelu);
+void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, const Act& C, int ldc, int act);
 
-void gemm(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, const Act& C, int ldc, bool gelu) {
+void gemm(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, const Act& C, int ldc, int act) {
     sealbart* m = cx.m;
-    if (!m->profile_gemm || M == 0) { gemm_impl(cx, M, N, K, A, lda, l, C, ldc, gelu); return; }
+    if (!m->profile_gemm || M == 0) { gemm_impl(cx, M, N, K, A, lda, l, C, ldc, act); return; }
     cudaEvent_t a, b;
     CUDA_CHECK(cudaEventCreate(&a)); CUDA_CHECK(cudaEventCreate(&b));
     CUDA_CHECK(cudaEventRecord(a, cx.s));
-    gemm_impl(cx, M, N, K, A, lda, l, C, ldc, gelu);
+    gemm_impl(cx, M, N, K, A, lda, l, C, ldc, act);
     CUDA_CHECK(cudaEventRecord(b, cx.s));
     m->gemm_events.emplace_back(a, b);
     m->gemm_flops += 2.0 * (double)M * N * K;
 }
 
-void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, const Act& C, int ldc, bool gelu) {
+void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, const Act& C, int ldc, int act) {
     if (M == 0) return;
+    const bool gelu = act == kActGelu;
+    if (act == kActRelu) cx.m->last_paths |= kPathT5Relu;
     sealbart* m = cx.m;
     Buf& a_hi = cx.slice ? m->a_hi1 : m->a_hi;
     Buf& a_lo = cx.slice ? m->a_lo1 : m->a_lo;
@@ -315,8 +373,9 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
             if (!l.maps2_ready) { make_map(&l.map2_hi, l.w_h1, N, K, K, GN / 2, true); make_map(&l.map2_lo, l.w_h2, N, K, K, GN / 2, true); l.maps2_ready = true; }
             const int groups = (int)((M + 2 * GM - 1) / (2 * GM)) * ((N + GN - 1) / GN);
             const int ctas = 2 * std::min(groups, sm_count() / 2);
-            if (gelu) gemm_launch<__half, true, 2>(cx.s, ctas, ma1, ma2, l.map2_hi, l.map2_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, 0, ovf, 1, 0);
-            else gemm_launch<__half, false, 2>(cx.s, ctas, ma1, ma2, l.map2_hi, l.map2_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, 0, ovf, 1, 0);
+            if (gelu) gemm_launch<__half, kActGelu, 2>(cx.s, ctas, ma1, ma2, l.map2_hi, l.map2_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, 0, ovf, 1, 0);
+            else if (act == kActRelu) gemm_launch<__half, kActRelu, 2>(cx.s, ctas, ma1, ma2, l.map2_hi, l.map2_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, 0, ovf, 1, 0);
+            else gemm_launch<__half, kActNone, 2>(cx.s, ctas, ma1, ma2, l.map2_hi, l.map2_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, 0, ovf, 1, 0);
             m->launches++; m->last_paths |= kPathGemmCluster;
             return;
         }
@@ -325,17 +384,18 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
             splitk.ensure((size_t)k_slices * slice_stride * 4);
             float* part = splitk.as<float>();
             const int ctas2 = std::min(tiles * k_slices, sm_count());
-            gemm_launch<__half, false, 1>(cx.s, ctas2, ma1, ma2, l.map_hi, l.map_lo, M, N, K, nullptr, 1.0f, part, nullptr, nullptr, ldc, n_fastest, 0, ovf,
+            gemm_launch<__half, kActNone, 1>(cx.s, ctas2, ma1, ma2, l.map_hi, l.map_lo, M, N, K, nullptr, 1.0f, part, nullptr, nullptr, ldc, n_fastest, 0, ovf,
                                           k_slices, slice_stride);
             m->launches++;
-            if (M <= cx.defer_rows && !gelu && !C.h1 && !C.hi && ldc == N && l.b) {     // summed by the consumer kernel
+            if (M <= cx.defer_rows && act == kActNone && !C.h1 && !C.hi && ldc == N && l.b) {     // summed by the consumer kernel
                 cx.pending = SplitSrc{part, k_slices, slice_stride, l.b, l.w_unscale};
                 m->last_paths |= kPathSplitKDeferred;
                 return;
             }
             const int fblocks = (int)std::min<int64_t>((M * (ldc / 4) + 255) / 256, (int64_t)sm_count() * 8);
-            if (gelu) launch_k(gemm_splitk_finish_kernel<true>, fblocks, 256, 0, cx.s, M, N, ldc, k_slices, slice_stride, part, l.b, l.w_unscale, C.x, C.h1, C.h2, ovf);
-            else launch_k(gemm_splitk_finish_kernel<false>, fblocks, 256, 0, cx.s, M, N, ldc, k_slices, slice_stride, part, l.b, l.w_unscale, C.x, C.h1, C.h2, ovf);
+            if (gelu) launch_k(gemm_splitk_finish_kernel<kActGelu>, fblocks, 256, 0, cx.s, M, N, ldc, k_slices, slice_stride, part, l.b, l.w_unscale, C.x, C.h1, C.h2, ovf);
+            else if (act == kActRelu) launch_k(gemm_splitk_finish_kernel<kActRelu>, fblocks, 256, 0, cx.s, M, N, ldc, k_slices, slice_stride, part, l.b, l.w_unscale, C.x, C.h1, C.h2, ovf);
+            else launch_k(gemm_splitk_finish_kernel<kActNone>, fblocks, 256, 0, cx.s, M, N, ldc, k_slices, slice_stride, part, l.b, l.w_unscale, C.x, C.h1, C.h2, ovf);
             CUDA_CHECK(cudaGetLastError()); m->launches++; m->last_paths |= kPathSplitKFinish;
             return;
         }
@@ -347,11 +407,12 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
         int band = (!n_fastest && M * K * 4 > band_bytes) ? (int)std::max<int64_t>(1, band_bytes / a_tile_bytes) : 0;
         if (m->gemm_band >= 0) band = m->gemm_band;
         const int ctas = std::min(tiles, sm_count());
-        if (cx.head.stats && !gelu) {
-            gemm_launch<__half, false, 1, true>(cx.s, ctas, ma1, ma2, l.map_hi, l.map_lo, M, N, K, l.b, l.w_unscale, C.x, nullptr, nullptr, ldc, n_fastest, band, ovf, 1, 0, cx.head);
+        if (cx.head.stats && act == kActNone) {
+            gemm_launch<__half, kActNone, 1, true>(cx.s, ctas, ma1, ma2, l.map_hi, l.map_lo, M, N, K, l.b, l.w_unscale, C.x, nullptr, nullptr, ldc, n_fastest, band, ovf, 1, 0, cx.head);
             cx.head_fused = true;
-        } else if (gelu) gemm_launch<__half, true, 1>(cx.s, ctas, ma1, ma2, l.map_hi, l.map_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, band, ovf, 1, 0);
-        else gemm_launch<__half, false, 1>(cx.s, ctas, ma1, ma2, l.map_hi, l.map_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, band, ovf, 1, 0);
+        } else if (gelu) gemm_launch<__half, kActGelu, 1>(cx.s, ctas, ma1, ma2, l.map_hi, l.map_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, band, ovf, 1, 0);
+        else if (act == kActRelu) gemm_launch<__half, kActRelu, 1>(cx.s, ctas, ma1, ma2, l.map_hi, l.map_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, band, ovf, 1, 0);
+        else gemm_launch<__half, kActNone, 1>(cx.s, ctas, ma1, ma2, l.map_hi, l.map_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, band, ovf, 1, 0);
         m->launches++; m->last_paths |= kPathGemmFullTile;
         return;
     }
@@ -366,8 +427,9 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
         make_map(&mah, ahi, M, K, K, GM); make_map(&mal, alo, M, K, K, GM);
         if (!l.maps_ready) { make_map(&l.map_hi, l.w_hi, N, K, K, GN); make_map(&l.map_lo, l.w_lo, N, K, K, GN); l.maps_ready = true; }
         const int ctas = std::min(tiles, sm_count());
-        if (gelu) gemm_launch<float, true, 1>(cx.s, ctas, mah, mal, l.map_hi, l.map_lo, M, N, K, l.b, 1.0f, C.x, C.hi, C.lo, ldc, n_fastest, 0, m->ovf, 1, 0);
-        else gemm_launch<float, false, 1>(cx.s, ctas, mah, mal, l.map_hi, l.map_lo, M, N, K, l.b, 1.0f, C.x, C.hi, C.lo, ldc, n_fastest, 0, m->ovf, 1, 0);
+        if (gelu) gemm_launch<float, kActGelu, 1>(cx.s, ctas, mah, mal, l.map_hi, l.map_lo, M, N, K, l.b, 1.0f, C.x, C.hi, C.lo, ldc, n_fastest, 0, m->ovf, 1, 0);
+        else if (act == kActRelu) gemm_launch<float, kActRelu, 1>(cx.s, ctas, mah, mal, l.map_hi, l.map_lo, M, N, K, l.b, 1.0f, C.x, C.hi, C.lo, ldc, n_fastest, 0, m->ovf, 1, 0);
+        else gemm_launch<float, kActNone, 1>(cx.s, ctas, mah, mal, l.map_hi, l.map_lo, M, N, K, l.b, 1.0f, C.x, C.hi, C.lo, ldc, n_fastest, 0, m->ovf, 1, 0);
         m->launches++; m->last_paths |= kPathGemmTf32;
         return;
     }
@@ -486,6 +548,7 @@ void ensure_workspace(sealbart* m, const Dims& D) {
     m->st_hstat.ensure((size_t)D.R * ((D.V + GN - 1) / GN) * 8);
     m->st_thr.ensure((size_t)D.R * 3 * 4);
     m->st_cval.ensure((size_t)D.R * 2 * D.B * 4); m->st_cidx.ensure((size_t)D.R * 2 * D.B * 4); m->st_ccnt.ensure(D.R * 4);
+    if (m->arch == 1 && m->t5.ffn_kind == 1) { m->effn2.ensure(Tk * 2 * D.f * 4); m->dffn2.ensure(D.R * 2 * D.f * 4); }
     {
         m->ex_hi.ensure(Tk * D.d * 4); m->ex_lo.ensure(Tk * D.d * 4);
         m->eattn_hi.ensure(Tk * D.d * 4); m->eattn_lo.ensure(Tk * D.d * 4);
@@ -495,6 +558,145 @@ void ensure_workspace(sealbart* m, const Dims& D) {
         m->dffn_hi.ensure(D.R * D.f * 4); m->dffn_lo.ensure(D.R * D.f * 4);
     }
     m->err.ensure(16);
+}
+
+// ---- T5 forward --------------------------------------------------------------------------------------
+// Pre-norm layers: x (fp32, the residual stream) += sublayer(RMSNorm(x)).  The plain half of the Act x holds the
+// residual, its split half the normed operand of the next GEMM: every t5_rms launch adds the previous sublayer's output
+// (or gathers the embedding), stores the residual and writes RMSNorm(x) with the next sublayer's weight -- after the
+// last layer the stack's final_layer_norm (and, in the decoder, the d_model^-0.5 output scale).
+void t5_rms(Ctx& cx, int64_t rows, int d, const int32_t* tok, int64_t tok_stride, const Act& x, const float* b, const float* w,
+            float out_scale) {
+    const SplitSrc ps = cx.pending;
+    cx.pending = SplitSrc{};
+    launch_k(t5_rms_row_kernel, (unsigned)rows, 128, 0, cx.s, rows, d, tok, tok_stride, (const float*)cx.m->shared, x.x, b, ps, w,
+             cx.m->t5.layer_norm_epsilon, out_scale, split_of(x, cx.m->ovf));
+    cx.m->launches++;
+    cx.m->last_paths |= kPathT5Rms;
+}
+
+// wi (ReLU epilogue) or [wi_0; wi_1] + gate, then wo into tmp (split-K slices left to the next t5_rms)
+void t5_ffn(Ctx& cx, int64_t rows, int d, int f, const Act& x, Lin& fc1, Lin& fc2, const Act& ffn, float* ffn2, const Act& tmp) {
+    sealbart* m = cx.m;
+    if (m->t5.ffn_kind == 1) {
+        gemm(cx, rows, 2 * f, d, x, d, fc1, Act{ffn2}, 2 * f, kActNone);
+        const int blocks = (int)std::max<int64_t>(1, std::min<int64_t>((rows * (f / 4) + 255) / 256, (int64_t)sm_count() * 8));
+        launch_k(t5_gate_kernel, (unsigned)blocks, 256, 0, cx.s, rows, f, (const float*)ffn2, split_of(ffn, m->ovf));
+        m->launches++; m->last_paths |= kPathT5Gate;
+    } else
+        gemm(cx, rows, f, d, x, d, fc1, ffn, f, kActRelu);
+    cx.defer_rows = INT64_MAX;
+    gemm(cx, rows, d, f, ffn, f, fc2, tmp, d, kActNone);
+    cx.defer_rows = 0;
+}
+
+void t5_encoder_layers(Ctx& cx, const Dims& D, int64_t Te, const int32_t* tok, const int32_t* m32, const int32_t* soff) {
+    sealbart* m = cx.m;
+    const int d = D.d, gm = m->cfg.gemm_mode;
+    const int64_t Tk = D.Q * D.S;
+    auto mk = [&](float* plain, Buf& bh, Buf& bl) {
+        Act a; a.x = plain;
+        if (gm == 2) { a.hi = bh.as<float>(); a.lo = bl.as<float>(); }
+        if (gm >= 3) { a.h1 = bh.as<__half>(); a.h2 = bl.as<__half>(); }
+        return a;
+    };
+    const Act x = mk(m->ex.as<float>(), m->ex_hi, m->ex_lo);
+    const Act qkv{m->eqkv.as<float>()};
+    Act attn = mk(nullptr, m->eattn_hi, m->eattn_lo);
+    Act ffn = mk(nullptr, m->effn_hi, m->effn_lo);
+    const Act tmp{m->etmp.as<float>()};
+    const RelBias rb{m->t5_rel_enc, m->t5_bkt_enc, kT5MaxSource - 1, m->cfg.heads};
+    const int n = (int)m->enc.size();
+    t5_rms(cx, Te, d, tok, 1, x, nullptr, m->enc[0].ln_attn.g, 1.f);
+    for (int i = 0; i < n; ++i) {
+        EncLayerW& L = m->enc[i];
+        gemm(cx, Te, 3 * d, d, x, d, L.qkv, qkv, 3 * d, kActNone);
+        launch_k(t5_enc_self_attn_kernel<kGAttnWarps, kGAttnPasses>, dim3((unsigned)D.Q, m->cfg.heads), kGAttnWarps * 32, 0, cx.s, D.Q, d,
+                 (int)D.S, (const float*)qkv.x, m32, rb, split_of(attn, m->ovf), soff);
+        m->launches++; m->last_paths |= kPathT5EncAttn;
+        cx.defer_rows = INT64_MAX;
+        gemm(cx, Te, d, d, attn, d, L.o, tmp, d, kActNone);
+        cx.defer_rows = 0;
+        t5_rms(cx, Te, d, nullptr, 0, x, tmp.x, L.ln_final.g, 1.f);
+        t5_ffn(cx, Te, d, D.f, x, L.fc1, L.fc2, ffn, m->effn2.as<float>(), tmp);
+        t5_rms(cx, Te, d, nullptr, 0, x, tmp.x, i + 1 < n ? m->enc[i + 1].ln_attn.g : m->enc_ln_emb.g, 1.f);
+    }
+    // the cross-attention K / V of every decoder layer read the encoder's final_layer_norm output
+    for (int l = 0; l < m->cfg.decoder_layers; ++l)
+        gemm(cx, Te, 2 * d, d, x, d, m->dec[l].ckv, Act{m->ckv.as<float>() + (size_t)l * Tk * 2 * d}, 2 * d, kActNone);
+}
+
+// decoder_step for T5 (same contract, same buffers): the self-attention adds the relative position bias, the
+// cross-attention runs the BART kernels on the query projection pre-multiplied by 8 (their 0.125 undoes it exactly).
+void t5_decoder_step(Ctx& cx, const Dims& D, const int32_t* tokens, int cur_len, const int32_t* anc, bool want_logits,
+                     cudaEvent_t ev_layers_done, bool compact, const HeadEpi& head) {
+    sealbart* m = cx.m;
+    const int d = D.d; const int64_t Rc = D.Rb ? D.Rb : D.R; const int64_t Tk = (D.Qb ? D.Qb : D.Q) * D.S;
+    const int64_t R = compact ? D.Q : D.R;
+    const int row_mul = compact ? D.B : 1;
+    const int pos = cur_len - 1;
+    const int gm = m->cfg.gemm_mode;
+    auto mk = [&](float* plain, Buf& bh, Buf& bl, int width) {
+        const int64_t o = D.r0 * width;
+        Act a; a.x = plain ? plain + o : nullptr;
+        if (gm == 2) { a.hi = bh.as<float>() + o; a.lo = bl.as<float>() + o; }
+        if (gm >= 3) { a.h1 = bh.as<__half>() + o; a.h2 = bl.as<__half>() + o; }
+        return a;
+    };
+    int* ovf = m->ovf;
+    const Act x = mk(m->dx.as<float>(), m->dx_hi, m->dx_lo, d);
+    const Act qkv{m->dqkv.as<float>() + D.r0 * 3 * d};
+    const Act attn = mk(nullptr, m->dattn_hi, m->dattn_lo, d);
+    const Act tmp{m->dtmp.as<float>() + D.r0 * d};
+    const Act cq{m->dcq.as<float>() + D.r0 * d};
+    const Act ffn = mk(nullptr, m->dffn_hi, m->dffn_lo, D.f);
+    float* ffn2 = m->dffn2.as<float>() ? m->dffn2.as<float>() + D.r0 * 2 * D.f : nullptr;
+    const int heads = m->cfg.heads;
+    const RelBias rb{m->t5_rel_dec, m->t5_bkt_dec, kMaxLen - 1, heads};
+    const int32_t* m32 = m->enc_mask.as<int32_t>() + D.q0 * D.S;
+    const int32_t* soff_x = m->enc_packed ? m->src_off.as<int32_t>() + D.q0 : nullptr;
+    const int64_t ckv_q0 = m->enc_packed ? 0 : D.q0 * D.S * 2 * d;
+    const int n = (int)m->dec.size();
+    const float out_scale = m->t5.scale_decoder_outputs ? 1.0f / sqrtf((float)d) : 1.0f;
+    t5_rms(cx, R, d, tokens + pos, (int64_t)(D.T * row_mul), x, nullptr, m->dec[0].ln_self.g, 1.f);
+    for (int l = 0; l < n; ++l) {
+        DecLayerW& L = m->dec[l];
+        float* kc = m->kc.as<float>() + (size_t)l * D.T * Rc * d + D.r0 * d;
+        float* vc = m->vc.as<float>() + (size_t)l * D.T * Rc * d + D.r0 * d;
+        gemm(cx, R, 3 * d, d, x, d, L.qkv, qkv, 3 * d, kActNone);
+        launch_k(t5_dec_self_attn_kernel, (unsigned)R, 32 * std::min(heads, 16), 0, cx.s, Rc, d, heads, pos, D.T, (const float*)qkv.x, kc, vc,
+                 anc, rb, split_of(attn, ovf), row_mul, row_mul);
+        m->launches++; m->last_paths |= kPathT5DecAttn;
+        cx.defer_rows = INT64_MAX;
+        gemm(cx, R, d, d, attn, d, L.o, tmp, d, kActNone);
+        cx.defer_rows = 0;
+        t5_rms(cx, R, d, nullptr, 0, x, tmp.x, L.ln_cross.g, 1.f);
+        cx.defer_rows = (D.S <= kXKeys) ? INT64_MAX : 0;      // cross_attn_small_kernel sums a split-K cq itself
+        gemm(cx, R, d, d, x, d, L.cq, cq, d, kActNone);
+        cx.defer_rows = 0;
+        const SplitSrc cq_src = cx.pending;
+        cx.pending = SplitSrc{};
+        const int64_t groups = D.grp_start ? D.G : D.Q;
+        const float* ckv_l = m->ckv.as<float>() + (size_t)l * Tk * 2 * d + ckv_q0;
+        if (D.S <= kXKeys)
+            launch_k(cross_attn_small_kernel, dim3((unsigned)groups, heads), 128, 0, cx.s, groups, d, heads, compact ? 1 : D.B, (int)D.S, (const float*)cq.x,
+                     ckv_l, m32, D.grp_query, D.grp_start, (float*)nullptr, split_of(attn, ovf), soff_x, cq_src);
+        else
+            launch_k(cross_attn_kernel, dim3((unsigned)groups, heads), kGAttnWarps * 32, 0, cx.s, groups, d, heads, compact ? 1 : D.B, (int)D.S, (const float*)cq.x,
+                     ckv_l, m32, D.grp_query, D.grp_start, (float*)nullptr, split_of(attn, ovf), soff_x);
+        m->launches++;
+        m->last_paths |= D.S <= kXKeys ? kPathCrossSmall : kPathCrossGrouped;
+        cx.defer_rows = INT64_MAX;
+        gemm(cx, R, d, d, attn, d, L.co, tmp, d, kActNone);
+        cx.defer_rows = 0;
+        t5_rms(cx, R, d, nullptr, 0, x, tmp.x, L.ln_final.g, 1.f);
+        t5_ffn(cx, R, d, D.f, x, L.fc1, L.fc2, ffn, ffn2, tmp);
+        t5_rms(cx, R, d, nullptr, 0, x, tmp.x, l + 1 < n ? m->dec[l + 1].ln_self.g : m->dec_ln_emb.g, l + 1 < n ? 1.f : out_scale);
+    }
+    if (ev_layers_done) CUDA_CHECK(cudaEventRecord(ev_layers_done, cx.s));
+    cx.head = head;
+    if (want_logits) gemm(cx, R, D.V, d, x, d, m->head, Act{m->logits.as<float>() + D.r0 * D.ld}, D.ld, kActNone);
+    cx.head = HeadEpi{};
 }
 
 // src_tokens_hint: >= 0 the caller's count of real source tokens (right-padded masks): no host synchronisation, the
@@ -531,6 +733,7 @@ void encoder_forward(Ctx& cx, const Dims& D, const int64_t* ids_d, const int64_t
     CUDA_CHECK(cudaGetLastError()); m->launches++;
     m->last_paths |= m->enc_packed ? kPathEncPacked : kPathEncUnpacked;
     const int64_t Te = rows_enc;                    // encoder rows actually computed
+    if (m->arch == 1) { t5_encoder_layers(cx, D, Te, tok, m32, soff); return; }
     const int gm = m->cfg.gemm_mode;
     auto mk = [&](float* plain, Buf& bh, Buf& bl, bool keep_plain) {
         Act a;
@@ -580,6 +783,7 @@ void decoder_step(Ctx& cx, const Dims& D, const int32_t* tokens, int cur_len, co
     sealbart* m = cx.m;
     const int d = D.d; const int64_t Rc = D.Rb ? D.Rb : D.R; const int64_t Tk = (D.Qb ? D.Qb : D.Q) * D.S;
     if (compact && (cur_len != 1 || D.grp_start || D.Qb)) throw ApiError(SEALFM_EINVAL, "internal: compact step only at position 0 of a generate");
+    if (m->arch == 1) { t5_decoder_step(cx, D, tokens, cur_len, anc, want_logits, ev_layers_done, compact, head); return; }
     const int64_t R = compact ? D.Q : D.R;          // rows processed
     const int row_mul = compact ? D.B : 1;
     const int pos = cur_len - 1;
@@ -712,9 +916,89 @@ void ensure_tf32_splits(sealbart* m) {
     m->tf32_ready = true;
 }
 
+// HF's T5Attention._relative_position_bucket for one relative position (key - query), in its float32 arithmetic:
+// log(rel.float() / max_exact) in fp32, divided by math.log(max_distance / max_exact) (a Python float, rounded to fp32
+// where it meets the fp32 tensor), times (num_buckets - max_exact), truncated.  Computed here once per model: a device
+// logf may round differently from torch at the bucket boundaries.
+int32_t t5_bucket(int32_t rel, bool bidirectional, int num_buckets, int max_distance) {
+    int32_t ret = 0;
+    int nb = num_buckets;
+    if (bidirectional) {
+        nb /= 2;
+        if (rel > 0) ret += nb;
+        rel = rel < 0 ? -rel : rel;
+    } else
+        rel = rel < 0 ? -rel : 0;
+    const int max_exact = nb / 2;
+    if (rel < max_exact) return ret + rel;
+    const float den = (float)std::log((double)max_distance / (double)max_exact);
+    const float v = std::log((float)rel / (float)max_exact) / den * (float)(nb - max_exact);
+    const int64_t large = std::min<int64_t>((int64_t)max_exact + (int64_t)v, nb - 1);
+    return ret + (int32_t)large;
+}
+
+// [2 kT5MaxSource - 1] encoder buckets (entry i: distance i - (kT5MaxSource - 1), bidirectional) and [kMaxLen] decoder
+// buckets (entry i: distance i - (kMaxLen - 1) <= 0, unidirectional), uploaded once
+void t5_bucket_tables(sealbart* m) {
+    const int nb = m->t5.relative_attention_num_buckets, md = m->t5.relative_attention_max_distance;
+    std::vector<int32_t> enc(2 * kT5MaxSource - 1), dec(kMaxLen);
+    for (int i = 0; i < (int)enc.size(); ++i) enc[i] = t5_bucket(i - (kT5MaxSource - 1), true, nb, md);
+    for (int i = 0; i < (int)dec.size(); ++i) dec[i] = t5_bucket(i - (kMaxLen - 1), false, nb, md);
+    m->t5_bkt_enc = reinterpret_cast<int32_t*>(dalloc(m, enc.size()));
+    m->t5_bkt_dec = reinterpret_cast<int32_t*>(dalloc(m, dec.size()));
+    CUDA_CHECK(cudaMemcpy(m->t5_bkt_enc, enc.data(), enc.size() * 4, cudaMemcpyHostToDevice));
+    CUDA_CHECK(cudaMemcpy(m->t5_bkt_dec, dec.data(), dec.size() * 4, cudaMemcpyHostToDevice));
+}
+
+// sealt5_create's shape checks (before any allocation)
+void check_t5_config(const sealt5_config_t* c) {
+    if (c->d_kv != kHeadDim || c->num_heads * kHeadDim != c->d_model)
+        throw ApiError(SEALFM_EINVAL, "T5: d_kv must be 64 and num_heads * 64 == d_model");
+    if (c->d_model % 128 || c->d_model <= 0 || c->d_model > 1024) throw ApiError(SEALFM_EINVAL, "T5: d_model must be a multiple of 128, <= 1024");
+    if (c->d_ff <= 0 || c->d_ff % 64) throw ApiError(SEALFM_EINVAL, "T5: d_ff must be a positive multiple of 64");
+    if (c->vocab_size <= 0 || c->num_layers < 1 || c->num_decoder_layers < 1) throw ApiError(SEALFM_EINVAL, "T5: bad vocab_size / layer counts");
+    if (c->ffn_kind != 0 && c->ffn_kind != 1) throw ApiError(SEALFM_EINVAL, "T5: ffn_kind must be 0 (relu) or 1 (gated-gelu)");
+    if (c->relative_attention_num_buckets < 4 || c->relative_attention_num_buckets > 1024 ||
+        c->relative_attention_max_distance <= c->relative_attention_num_buckets / 2)
+        throw ApiError(SEALFM_EINVAL, "T5: relative_attention_num_buckets must be in [4, 1024] and relative_attention_max_distance > num_buckets / 2");
+    if (!(c->layer_norm_epsilon >= 0.f) || !std::isfinite(c->layer_norm_epsilon)) throw ApiError(SEALFM_EINVAL, "T5: bad layer_norm_epsilon");
+    if (c->gemm_mode != 2 && c->gemm_mode != 3 && c->gemm_mode != 5)
+        throw ApiError(SEALFM_EINVAL, "gemm_mode must be 3 (3xFP16, one CTA per tile, default), 5 (3xFP16 on 2-CTA clusters) or 2 (3xTF32)");
+}
+
 }  // namespace
 
 extern "C" {
+
+int sealt5_relative_buckets(int32_t num_buckets, int32_t max_distance, int32_t bidirectional, int32_t n, int32_t* out) {
+    return guarded([&] {
+        if (!out || n < 1 || num_buckets < 4 || num_buckets > 1024 || max_distance <= num_buckets / 2)
+            throw ApiError(SEALFM_EINVAL, "bad argument");
+        if (bidirectional) for (int i = 0; i < 2 * n - 1; ++i) out[i] = t5_bucket(i - (n - 1), true, num_buckets, max_distance);
+        else for (int i = 0; i < n; ++i) out[i] = t5_bucket(-i, false, num_buckets, max_distance);
+    });
+}
+
+int sealt5_create(const sealt5_config_t* cfg, int device, sealbart_t** out) {
+    return guarded([&] {
+        if (!cfg || !out) throw ApiError(SEALFM_EINVAL, "null argument");
+        check_t5_config(cfg);
+        int count = 0;
+        cudaError_t e = cudaGetDeviceCount(&count);
+        if (e != cudaSuccess || count == 0) { cudaGetLastError(); throw ApiError(SEALFM_ENODEVICE, "no CUDA device available"); }
+        if (device < 0 || device >= count) throw ApiError(SEALFM_EINVAL, "bad device id");
+        CUDA_CHECK(cudaSetDevice(device));
+        std::unique_ptr<sealbart> m(new sealbart());
+        m->arch = 1; m->t5 = *cfg; m->device = device;
+        m->cfg = sealbart_config_t{cfg->vocab_size, cfg->d_model, cfg->num_layers, cfg->num_decoder_layers, cfg->num_heads, cfg->d_ff,
+                                   kT5MaxSource, 0, cfg->gemm_mode};
+        struct Guard { sealbart* m; ~Guard() { if (m) sealbart_free(m); } } guard{m.get()};
+        build_slots_t5(m.get());
+        t5_bucket_tables(m.get());
+        guard.m = nullptr;
+        *out = m.release();
+    });
+}
 
 int sealbart_create(const sealbart_config_t* cfg, int device, sealbart_t** out) {
     return guarded([&] {
@@ -748,7 +1032,7 @@ void sealbart_free(sealbart_t* m) {
                    &m->st_cidx, &m->st_ccnt, &m->st_wide, &m->hy_score, &m->hy_len, &m->hy_tok,
                    &m->hy_valid, &m->hy_lo, &m->hy_hi, &m->err, &m->dbg_ids, &m->force_syms, &m->a_hi, &m->a_lo, &m->ex_hi, &m->ex_lo,
                    &m->eattn_hi, &m->eattn_lo, &m->effn_hi, &m->effn_lo, &m->dx_hi, &m->dx_lo, &m->dattn_hi, &m->dattn_lo,
-                   &m->dffn_hi, &m->dffn_lo, &m->splitk, &m->a_hi1, &m->a_lo1, &m->splitk1, &m->st_wide1})
+                   &m->dffn_hi, &m->dffn_lo, &m->splitk, &m->a_hi1, &m->a_lo1, &m->splitk1, &m->st_wide1, &m->effn2, &m->dffn2})
         b->release();
     if (m->slice_fork) cudaEventDestroy(m->slice_fork);
     if (m->slice_join) cudaEventDestroy(m->slice_join);
@@ -772,11 +1056,20 @@ int sealbart_set_tensor(sealbart_t* m, const char* key, const float* host, uint6
             CUDA_CHECK(cudaMemcpy(m->lm_head, host, want * 4, cudaMemcpyHostToDevice));
             return;
         }
-        if (k == "model.encoder.embed_tokens.weight" || k == "model.decoder.embed_tokens.weight") k = "model.shared.weight";
+        if (m->arch == 0 && (k == "model.encoder.embed_tokens.weight" || k == "model.decoder.embed_tokens.weight")) k = "model.shared.weight";
+        if (m->arch == 1 && (k == "encoder.embed_tokens.weight" || k == "decoder.embed_tokens.weight")) k = "shared.weight";
         auto it = m->slots.find(k);
         if (it == m->slots.end()) throw ApiError(SEALFM_EINVAL, "unknown state_dict key: " + k);
         if (it->second.numel != numel) throw ApiError(SEALFM_EINVAL, "wrong element count for " + k);
-        CUDA_CHECK(cudaMemcpy(it->second.dst, host, numel * 4, cudaMemcpyHostToDevice));
+        static const std::string kCrossQ = ".layer.1.EncDecAttention.q.weight";
+        if (m->arch == 1 && k.size() > kCrossQ.size() && k.compare(k.size() - kCrossQ.size(), kCrossQ.size(), kCrossQ) == 0) {
+            // T5 does not scale attention scores; the cross-attention kernels multiply by 0.125, so q is stored times 8
+            // (a power of two: (8q . k) * 0.125 == q . k exactly)
+            std::vector<float> q8(host, host + numel);
+            for (float& v : q8) v *= 8.f;
+            CUDA_CHECK(cudaMemcpy(it->second.dst, q8.data(), numel * 4, cudaMemcpyHostToDevice));
+        } else
+            CUDA_CHECK(cudaMemcpy(it->second.dst, host, numel * 4, cudaMemcpyHostToDevice));
         m->loaded.insert(k);
         m->finalized = false;
     });
@@ -787,7 +1080,7 @@ int sealbart_finalize(sealbart_t* m) {
         if (!m) throw ApiError(SEALFM_EINVAL, "null model");
         for (auto& kv : m->slots)
             if (!m->loaded.count(kv.first)) throw ApiError(SEALFM_EINVAL, "state_dict tensor missing: " + kv.first);
-        if (!m->lm_head_given) m->lm_head = m->shared;          // tied (seal/utils.py:48-49)
+        if (!m->lm_head_given) m->lm_head = m->shared;          // tied (seal/utils.py:48-49; T5: tie_word_embeddings)
         m->head.w = m->lm_head; m->head.b = m->final_bias; m->head.out = m->cfg.vocab_size; m->head.in = m->cfg.d_model;
         {
             CUDA_CHECK(cudaSetDevice(m->device));
@@ -1642,7 +1935,7 @@ int debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A, const 
             CUDA_CHECK(cudaMemcpy(dmask.p, head->mask, (size_t)M * mask_words * 4, cudaMemcpyHostToDevice));
             cx.head = HeadEpi{dstats.as<float2>(), dmask.as<uint32_t>(), mask_words, head->eos, head->pad};
         }
-        gemm(cx, M, N, K, a, K, l, head ? Act{dC.as<float>()} : c, ldc, gelu != 0);
+        gemm(cx, M, N, K, a, K, l, head ? Act{dC.as<float>()} : c, ldc, gelu ? kActGelu : kActNone);
         CUDA_CHECK(cudaDeviceSynchronize());
         if (head) {
             *head->fused = cx.head_fused ? 1 : 0;
@@ -1653,7 +1946,7 @@ int debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A, const 
         if (iters > 0 && avg_us) {
             cudaEvent_t e0, e1; CUDA_CHECK(cudaEventCreate(&e0)); CUDA_CHECK(cudaEventCreate(&e1));
             CUDA_CHECK(cudaEventRecord(e0, nullptr));
-            for (int i = 0; i < iters; ++i) gemm(cx, M, N, K, a, K, l, c, ldc, gelu != 0);
+            for (int i = 0; i < iters; ++i) gemm(cx, M, N, K, a, K, l, c, ldc, gelu ? kActGelu : kActNone);
             CUDA_CHECK(cudaEventRecord(e1, nullptr));
             CUDA_CHECK(cudaEventSynchronize(e1));
             float ms = 0; CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));

@@ -1,5 +1,5 @@
 // Hopper (sm_90a) GEMM for the BART encoder/decoder linears and the lm_head:
-//   C[M,N] = A[M,K] * W[N,K]^T + bias[N]   (optional exact GELU), fp32 in / fp32 out,
+//   C[M,N] = A[M,K] * W[N,K]^T + bias[N]   (optional exact GELU or ReLU), fp32 in / fp32 out,
 // computed on the tensor cores as an error-compensated 3-pass product
 //   A*W ~= A_lo*W_hi + A_hi*W_lo + A_hi*W_hi,
 // which keeps the fp32-level accuracy the 1e-4 beam-score parity needs (a single TF32/FP16 pass does not).
@@ -139,6 +139,12 @@ __device__ __forceinline__ void wgmma_128(float (&d)[64], uint64_t a, uint64_t b
 
 __device__ __forceinline__ float gelu_erf_u(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
 
+// Epilogue activation (template argument ACT): none, BART's exact-erf GELU, T5's ReLU (torch.relu: NaN stays NaN)
+constexpr int kActNone = 0, kActGelu = 1, kActRelu = 2;
+template <int ACT> __device__ __forceinline__ float epi_act(float x) {
+    return ACT == kActGelu ? gelu_erf_u(x) : ACT == kActRelu ? (x < 0.f ? 0.f : x) : x;
+}
+
 // x -> (hi, lo): hi keeps the TF32 bits (sign, exponent, 10 mantissa bits), lo = x - hi exactly.
 __global__ void __launch_bounds__(256) split_tf32_kernel(int64_t n4, const float4* __restrict__ x, float4* __restrict__ hi,
                                                          float4* __restrict__ lo) {
@@ -260,7 +266,7 @@ struct HeadEpi {
 // stream -- add+LN, cross attention -- run beside a GEMM CTA on the same SM.
 constexpr int G_REGS = 128, G_REGS_PRODUCER = 40, G_REGS_CONSUMER = 168;
 static_assert(128 * G_REGS_PRODUCER + 256 * G_REGS_CONSUMER <= GTHREADS * G_REGS, "setmaxnreg budget");
-template <typename T, bool GELU, int CL, bool HEAD = false>
+template <typename T, int ACT, int CL, bool HEAD = false>
 __global__ void __maxnreg__(G_REGS)                   // (excludes __launch_bounds__; launched with GTHREADS threads)
 wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                      const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo,
@@ -428,7 +434,7 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
                         const float x = acc[4 * j + 2 * h + e] * w_unscale + ((bias && n + e < N) ? bias[n + e] : 0.f);
-                        v[e] = GELU ? gelu_erf_u(x) : x;
+                        v[e] = epi_act<ACT>(x);
                     }
                     store_pair(Cs, C_s1, C_s2, (int64_t)row * ldc + n, n, N, v[0], v[1], ov);
                 }
@@ -445,7 +451,7 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
 
 // Finishes a split-K GEMM: out = act((sum_s part[s]) * w_unscale + bias), slices summed in index order
 // (deterministic), written as fp32 and/or as the half split the next GEMM consumes.
-template <bool GELU>
+template <int ACT>
 __global__ void __launch_bounds__(256) gemm_splitk_finish_kernel(int64_t M, int N, int ldc, int k_slices, int64_t slice_stride,
                                                                  const float* __restrict__ part, const float* __restrict__ bias,
                                                                  float w_unscale, float* __restrict__ C, __half* __restrict__ C_h1,
@@ -466,7 +472,7 @@ __global__ void __launch_bounds__(256) gemm_splitk_finish_kernel(int64_t M, int 
         for (int u = 0; u < 4; ++u) {
             if (n + u >= N) continue;
             float x = v[u] * w_unscale + (bias ? bias[n + u] : 0.f);
-            if (GELU) x = gelu_erf_u(x);
+            x = epi_act<ACT>(x);
             if (C) C[off + u] = x;
             if (C_h1) { __half a, b; split_half(x, a, b, &ov); C_h1[off + u] = a; C_h2[off + u] = b; }
         }
