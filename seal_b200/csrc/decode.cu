@@ -16,6 +16,7 @@
 #include <memory>
 #include <set>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 using namespace sealb200;
@@ -38,8 +39,13 @@ struct DecLayerW { Lin qkv, o, cq, ckv, co, fc1, fc2; LNp ln_self, ln_cross, ln_
 // graphs captured under an older epoch are discarded.
 uint64_t g_ws_epoch = 0;
 
+// A device buffer that owns its memory: freed when the Buf goes out of scope.
 struct Buf {
     void* p = nullptr; size_t bytes = 0;
+    Buf() = default;
+    Buf(const Buf&) = delete;
+    Buf& operator=(const Buf&) = delete;
+    ~Buf() { release(); }
     void ensure(size_t need) {
         if (need <= bytes) return;
         if (p) { cudaFree(p); p = nullptr; bytes = 0; }
@@ -77,15 +83,15 @@ struct sealbart {
     uint64_t weight_bytes = 0;
     bool finalized = false;
     // workspace
-    Buf enc_tok, enc_mask, ex, eqkv, eattn, etmp, effn, ckv, src_off;
+    Buf enc_tok, enc_mask, ex, eqkv, etmp, ckv, src_off;
     bool enc_packed = false;          // the last encoder_forward ran on the real tokens only (src_off valid)
-    Buf dx, dqkv, dattn, dtmp, dcq, dffn, logits, kc, vc;
+    Buf dx, dqkv, dtmp, dcq, logits, kc, vc;
     Buf ex_hi, ex_lo, eattn_hi, eattn_lo, effn_hi, effn_lo, dx_hi, dx_lo, dattn_hi, dattn_lo, dffn_hi, dffn_lo;   // activation splits (halves or TF32)
     Buf st_scores, st_tokens, st_lo, st_hi, st_pw, st_anc, st_mask;
     Buf st_rowmax, st_rowls, st_rule, st_cval, st_cidx, st_ccnt, st_wide;     // scratch between the kernels of a step
     Buf st_hstat;                     // [R][V / 128] lm_head tile statistics (HeadEpi)
     Buf st_thr;                       // [R][3] top-k warp statistics of each logits row (topk_threshold_kernel)
-    Buf hy_score, hy_len, hy_tok, hy_valid, hy_lo, hy_hi, err, dbg_ids, force_syms, a_hi, a_lo, splitk;
+    Buf hy_score, hy_len, hy_tok, hy_valid, hy_lo, hy_hi, err, dbg_ids, a_hi, a_lo, splitk;
     std::vector<void*> split_allocs;
     int64_t launches = 0;
     uint32_t last_paths = 0;          // OR of the kPath* bits of every kernel branch the last model call took
@@ -301,6 +307,16 @@ SplitOut split_of(const Act& a, int* overflow) {
     return so;
 }
 
+// Buffers hi / lo (and plain, if not null) as an Act from element off on: the TF32 split in gemm_mode 2, the fp16
+// split in the 3xFP16 modes.  plain is null for activations whose producers write the split only.
+Act act_view(int gemm_mode, float* plain, const Buf& hi, const Buf& lo, int64_t off = 0) {
+    Act a;
+    if (plain) a.x = plain + off;
+    if (gemm_mode == 2) { a.hi = hi.as<float>() + off; a.lo = lo.as<float>() + off; }
+    if (gemm_mode >= 3) { a.h1 = hi.as<__half>() + off; a.h2 = lo.as<__half>() + off; }
+    return a;
+}
+
 template <typename T, int ACT, int CL, bool HEAD = false>
 void gemm_launch(cudaStream_t s, int ctas, const CUtensorMap& ahi, const CUtensorMap& alo, const CUtensorMap& whi, const CUtensorMap& wlo,
                  int64_t M, int N, int K, const float* bias, float w_unscale, float* C, T* C1, T* C2, int ldc, int n_fastest, int m_band,
@@ -315,6 +331,13 @@ void gemm_launch(cudaStream_t s, int ctas, const CUtensorMap& ahi, const CUtenso
     cfg.attrs = attr; cfg.numAttrs = 1;
     CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, ahi, alo, whi, wlo, (int)M, N, K, bias, w_unscale, C, C1, C2, ldc, n_fastest, m_band, ovf,
                                   k_slices, slice_stride, he));
+}
+
+// f(std::integral_constant<int, ACT>{}) for the epilogue activation act: kernels are instantiated per activation
+template <typename F> void with_act(int act, F&& f) {
+    if (act == kActGelu) f(std::integral_constant<int, kActGelu>{});
+    else if (act == kActRelu) f(std::integral_constant<int, kActRelu>{});
+    else f(std::integral_constant<int, kActNone>{});
 }
 
 // C = A W^T + b (+ the epilogue activation act: kActNone / kActGelu / kActRelu, wgmma_gemm.cuh) on the tensor cores: gemm_mode 3 / 5 = 3xFP16 (one CTA per tile / clusters of 2 sharing W), 2 = 3xTF32 (fp32
@@ -336,7 +359,6 @@ void gemm(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, const
 
 void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, const Act& C, int ldc, int act) {
     if (M == 0) return;
-    const bool gelu = act == kActGelu;
     if (act == kActRelu) cx.m->last_paths |= kPathT5Relu;
     sealbart* m = cx.m;
     Buf& a_hi = cx.slice ? m->a_hi1 : m->a_hi;
@@ -373,9 +395,9 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
             if (!l.maps2_ready) { make_map(&l.map2_hi, l.w_h1, N, K, K, GN / 2, true); make_map(&l.map2_lo, l.w_h2, N, K, K, GN / 2, true); l.maps2_ready = true; }
             const int groups = (int)((M + 2 * GM - 1) / (2 * GM)) * ((N + GN - 1) / GN);
             const int ctas = 2 * std::min(groups, sm_count() / 2);
-            if (gelu) gemm_launch<__half, kActGelu, 2>(cx.s, ctas, ma1, ma2, l.map2_hi, l.map2_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, 0, ovf, 1, 0);
-            else if (act == kActRelu) gemm_launch<__half, kActRelu, 2>(cx.s, ctas, ma1, ma2, l.map2_hi, l.map2_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, 0, ovf, 1, 0);
-            else gemm_launch<__half, kActNone, 2>(cx.s, ctas, ma1, ma2, l.map2_hi, l.map2_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, 0, ovf, 1, 0);
+            with_act(act, [&](auto A) {
+                gemm_launch<__half, decltype(A)::value, 2>(cx.s, ctas, ma1, ma2, l.map2_hi, l.map2_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, 0, ovf, 1, 0);
+            });
             m->launches++; m->last_paths |= kPathGemmCluster;
             return;
         }
@@ -393,9 +415,9 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
                 return;
             }
             const int fblocks = (int)std::min<int64_t>((M * (ldc / 4) + 255) / 256, (int64_t)sm_count() * 8);
-            if (gelu) launch_k(gemm_splitk_finish_kernel<kActGelu>, fblocks, 256, 0, cx.s, M, N, ldc, k_slices, slice_stride, part, l.b, l.w_unscale, C.x, C.h1, C.h2, ovf);
-            else if (act == kActRelu) launch_k(gemm_splitk_finish_kernel<kActRelu>, fblocks, 256, 0, cx.s, M, N, ldc, k_slices, slice_stride, part, l.b, l.w_unscale, C.x, C.h1, C.h2, ovf);
-            else launch_k(gemm_splitk_finish_kernel<kActNone>, fblocks, 256, 0, cx.s, M, N, ldc, k_slices, slice_stride, part, l.b, l.w_unscale, C.x, C.h1, C.h2, ovf);
+            with_act(act, [&](auto A) {
+                launch_k(gemm_splitk_finish_kernel<decltype(A)::value>, fblocks, 256, 0, cx.s, M, N, ldc, k_slices, slice_stride, part, l.b, l.w_unscale, C.x, C.h1, C.h2, ovf);
+            });
             CUDA_CHECK(cudaGetLastError()); m->launches++; m->last_paths |= kPathSplitKFinish;
             return;
         }
@@ -410,9 +432,10 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
         if (cx.head.stats && act == kActNone) {
             gemm_launch<__half, kActNone, 1, true>(cx.s, ctas, ma1, ma2, l.map_hi, l.map_lo, M, N, K, l.b, l.w_unscale, C.x, nullptr, nullptr, ldc, n_fastest, band, ovf, 1, 0, cx.head);
             cx.head_fused = true;
-        } else if (gelu) gemm_launch<__half, kActGelu, 1>(cx.s, ctas, ma1, ma2, l.map_hi, l.map_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, band, ovf, 1, 0);
-        else if (act == kActRelu) gemm_launch<__half, kActRelu, 1>(cx.s, ctas, ma1, ma2, l.map_hi, l.map_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, band, ovf, 1, 0);
-        else gemm_launch<__half, kActNone, 1>(cx.s, ctas, ma1, ma2, l.map_hi, l.map_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, band, ovf, 1, 0);
+        } else
+            with_act(act, [&](auto A) {
+                gemm_launch<__half, decltype(A)::value, 1>(cx.s, ctas, ma1, ma2, l.map_hi, l.map_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, band, ovf, 1, 0);
+            });
         m->launches++; m->last_paths |= kPathGemmFullTile;
         return;
     }
@@ -427,9 +450,9 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
         make_map(&mah, ahi, M, K, K, GM); make_map(&mal, alo, M, K, K, GM);
         if (!l.maps_ready) { make_map(&l.map_hi, l.w_hi, N, K, K, GN); make_map(&l.map_lo, l.w_lo, N, K, K, GN); l.maps_ready = true; }
         const int ctas = std::min(tiles, sm_count());
-        if (gelu) gemm_launch<float, kActGelu, 1>(cx.s, ctas, mah, mal, l.map_hi, l.map_lo, M, N, K, l.b, 1.0f, C.x, C.hi, C.lo, ldc, n_fastest, 0, m->ovf, 1, 0);
-        else if (act == kActRelu) gemm_launch<float, kActRelu, 1>(cx.s, ctas, mah, mal, l.map_hi, l.map_lo, M, N, K, l.b, 1.0f, C.x, C.hi, C.lo, ldc, n_fastest, 0, m->ovf, 1, 0);
-        else gemm_launch<float, kActNone, 1>(cx.s, ctas, mah, mal, l.map_hi, l.map_lo, M, N, K, l.b, 1.0f, C.x, C.hi, C.lo, ldc, n_fastest, 0, m->ovf, 1, 0);
+        with_act(act, [&](auto A) {
+            gemm_launch<float, decltype(A)::value, 1>(cx.s, ctas, mah, mal, l.map_hi, l.map_lo, M, N, K, l.b, 1.0f, C.x, C.hi, C.lo, ldc, n_fastest, 0, m->ovf, 1, 0);
+        });
         m->launches++; m->last_paths |= kPathGemmTf32;
         return;
     }
@@ -534,11 +557,9 @@ void ensure_workspace(sealbart* m, const Dims& D) {
     const int64_t Tk = D.Q * D.S;
     const int Ld = m->cfg.decoder_layers;
     m->enc_tok.ensure(Tk * 4 * 2); m->enc_mask.ensure(Tk * 4); m->src_off.ensure((D.Q + 1) * 4 + 16 + 16);
-    m->ex.ensure(Tk * D.d * 4); m->eqkv.ensure(Tk * 3 * D.d * 4); m->eattn.ensure(Tk * D.d * 4);
-    m->etmp.ensure(Tk * D.d * 4); m->effn.ensure(Tk * D.f * 4);
+    m->ex.ensure(Tk * D.d * 4); m->eqkv.ensure(Tk * 3 * D.d * 4); m->etmp.ensure(Tk * D.d * 4);
     m->ckv.ensure((size_t)Ld * Tk * 2 * D.d * 4);
-    m->dx.ensure(D.R * D.d * 4); m->dqkv.ensure(D.R * 3 * D.d * 4); m->dattn.ensure(D.R * D.d * 4);
-    m->dtmp.ensure(D.R * D.d * 4); m->dcq.ensure(D.R * D.d * 4); m->dffn.ensure(D.R * D.f * 4);
+    m->dx.ensure(D.R * D.d * 4); m->dqkv.ensure(D.R * 3 * D.d * 4); m->dtmp.ensure(D.R * D.d * 4); m->dcq.ensure(D.R * D.d * 4);
     m->logits.ensure((size_t)D.R * D.ld * 4);
     m->kc.ensure((size_t)Ld * D.T * D.R * D.d * 4); m->vc.ensure((size_t)Ld * D.T * D.R * D.d * 4);
     m->st_scores.ensure(2 * D.R * 4); m->st_tokens.ensure(2 * D.R * D.T * 4);
@@ -590,113 +611,168 @@ void t5_ffn(Ctx& cx, int64_t rows, int d, int f, const Act& x, Lin& fc1, Lin& fc
     cx.defer_rows = 0;
 }
 
-void t5_encoder_layers(Ctx& cx, const Dims& D, int64_t Te, const int32_t* tok, const int32_t* m32, const int32_t* soff) {
+// The activations of one stack's layers as the GEMMs see them.  x: the residual stream (plain) and the next GEMM's
+// operand (split); qkv, tmp, cq: plain GEMM outputs; attn, ffn: the split operands of the o / co and fc2 GEMMs, whose
+// producers write no plain copy; ffn2: the [rows][2 d_ff] output of T5's gated [wi_0; wi_1] GEMM.
+struct Acts { Act x, qkv, attn, tmp, cq, ffn; float* ffn2 = nullptr; };
+
+// One decoder step: rows r0 .. r0 + R of the activation buffers; at the compact first step a row stands for row_mul
+// beams.  Rc: the KV cache's row stride; Tk, ckv_q0, m32, soff_x: the encoder side of the step's queries (packed,
+// src_off holds absolute ckv rows; unpacked, query q's rows are q * S).
+struct DecStep : Acts {
+    int64_t R = 0, Rc = 0, Tk = 0, ckv_q0 = 0; int row_mul = 1, pos = 0; bool compact = false;
+    const int32_t* tokens = nullptr; const int32_t* anc = nullptr; const int32_t* m32 = nullptr; const int32_t* soff_x = nullptr;
+};
+
+// The cross-attention block of decoder layer l: cq = x Wq, attention over the layer's encoder K / V into attn, then
+// co into tmp.  defer_rows: how many rows the norm after the block accepts with co's split-K slices unsummed.
+void cross_attention(Ctx& cx, const Dims& D, const DecStep& S, int l, int64_t defer_rows) {
     sealbart* m = cx.m;
-    const int d = D.d, gm = m->cfg.gemm_mode;
-    const int64_t Tk = D.Q * D.S;
-    auto mk = [&](float* plain, Buf& bh, Buf& bl) {
-        Act a; a.x = plain;
-        if (gm == 2) { a.hi = bh.as<float>(); a.lo = bl.as<float>(); }
-        if (gm >= 3) { a.h1 = bh.as<__half>(); a.h2 = bl.as<__half>(); }
-        return a;
-    };
-    const Act x = mk(m->ex.as<float>(), m->ex_hi, m->ex_lo);
-    const Act qkv{m->eqkv.as<float>()};
-    Act attn = mk(nullptr, m->eattn_hi, m->eattn_lo);
-    Act ffn = mk(nullptr, m->effn_hi, m->effn_lo);
-    const Act tmp{m->etmp.as<float>()};
-    const RelBias rb{m->t5_rel_enc, m->t5_bkt_enc, kT5MaxSource - 1, m->cfg.heads};
-    const int n = (int)m->enc.size();
-    t5_rms(cx, Te, d, tok, 1, x, nullptr, m->enc[0].ln_attn.g, 1.f);
-    for (int i = 0; i < n; ++i) {
-        EncLayerW& L = m->enc[i];
-        gemm(cx, Te, 3 * d, d, x, d, L.qkv, qkv, 3 * d, kActNone);
-        launch_k(t5_enc_self_attn_kernel<kGAttnWarps, kGAttnPasses>, dim3((unsigned)D.Q, m->cfg.heads), kGAttnWarps * 32, 0, cx.s, D.Q, d,
-                 (int)D.S, (const float*)qkv.x, m32, rb, split_of(attn, m->ovf), soff);
-        m->launches++; m->last_paths |= kPathT5EncAttn;
-        cx.defer_rows = INT64_MAX;
-        gemm(cx, Te, d, d, attn, d, L.o, tmp, d, kActNone);
-        cx.defer_rows = 0;
-        t5_rms(cx, Te, d, nullptr, 0, x, tmp.x, L.ln_final.g, 1.f);
-        t5_ffn(cx, Te, d, D.f, x, L.fc1, L.fc2, ffn, m->effn2.as<float>(), tmp);
-        t5_rms(cx, Te, d, nullptr, 0, x, tmp.x, i + 1 < n ? m->enc[i + 1].ln_attn.g : m->enc_ln_emb.g, 1.f);
-    }
-    // the cross-attention K / V of every decoder layer read the encoder's final_layer_norm output
-    for (int l = 0; l < m->cfg.decoder_layers; ++l)
-        gemm(cx, Te, 2 * d, d, x, d, m->dec[l].ckv, Act{m->ckv.as<float>() + (size_t)l * Tk * 2 * d}, 2 * d, kActNone);
+    const int d = D.d, heads = m->cfg.heads;
+    DecLayerW& L = m->dec[l];
+    cx.defer_rows = (D.S <= kXKeys) ? INT64_MAX : 0;      // cross_attn_small_kernel sums a split-K cq itself
+    gemm(cx, S.R, d, d, S.x, d, L.cq, S.cq, d, kActNone);
+    cx.defer_rows = 0;
+    const SplitSrc cq_src = cx.pending;
+    cx.pending = SplitSrc{};
+    const int64_t groups = D.grp_start ? D.G : D.Q;
+    const float* ckv_l = m->ckv.as<float>() + (size_t)l * S.Tk * 2 * d + S.ckv_q0;
+    if (D.S <= kXKeys)
+        launch_k(cross_attn_small_kernel, dim3((unsigned)groups, heads), 128, 0, cx.s, groups, d, heads, S.compact ? 1 : D.B, (int)D.S, (const float*)S.cq.x,
+                 ckv_l, S.m32, D.grp_query, D.grp_start, S.attn.x, split_of(S.attn, m->ovf), S.soff_x, cq_src);
+    else
+        launch_k(cross_attn_kernel, dim3((unsigned)groups, heads), kGAttnWarps * 32, 0, cx.s, groups, d, heads, S.compact ? 1 : D.B, (int)D.S, (const float*)S.cq.x,
+                 ckv_l, S.m32, D.grp_query, D.grp_start, S.attn.x, split_of(S.attn, m->ovf), S.soff_x);
+    m->launches++;
+    m->last_paths |= D.S <= kXKeys ? kPathCrossSmall : kPathCrossGrouped;
+    cx.defer_rows = defer_rows;
+    gemm(cx, S.R, d, d, S.attn, d, L.co, S.tmp, d, kActNone);
+    cx.defer_rows = 0;
 }
 
-// decoder_step for T5 (same contract, same buffers): the self-attention adds the relative position bias, the
-// cross-attention runs the BART kernels on the query projection pre-multiplied by 8 (their 0.125 undoes it exactly).
-void t5_decoder_step(Ctx& cx, const Dims& D, const int32_t* tokens, int cur_len, const int32_t* anc, bool want_logits,
-                     cudaEvent_t ev_layers_done, bool compact, const HeadEpi& head) {
+void t5_encoder_layers(Ctx& cx, const Dims& D, int64_t Te, const Acts& A, const int32_t* tok, const int32_t* m32, const int32_t* soff) {
     sealbart* m = cx.m;
-    const int d = D.d; const int64_t Rc = D.Rb ? D.Rb : D.R; const int64_t Tk = (D.Qb ? D.Qb : D.Q) * D.S;
-    const int64_t R = compact ? D.Q : D.R;
-    const int row_mul = compact ? D.B : 1;
-    const int pos = cur_len - 1;
-    const int gm = m->cfg.gemm_mode;
-    auto mk = [&](float* plain, Buf& bh, Buf& bl, int width) {
-        const int64_t o = D.r0 * width;
-        Act a; a.x = plain ? plain + o : nullptr;
-        if (gm == 2) { a.hi = bh.as<float>() + o; a.lo = bl.as<float>() + o; }
-        if (gm >= 3) { a.h1 = bh.as<__half>() + o; a.h2 = bl.as<__half>() + o; }
-        return a;
-    };
-    int* ovf = m->ovf;
-    const Act x = mk(m->dx.as<float>(), m->dx_hi, m->dx_lo, d);
-    const Act qkv{m->dqkv.as<float>() + D.r0 * 3 * d};
-    const Act attn = mk(nullptr, m->dattn_hi, m->dattn_lo, d);
-    const Act tmp{m->dtmp.as<float>() + D.r0 * d};
-    const Act cq{m->dcq.as<float>() + D.r0 * d};
-    const Act ffn = mk(nullptr, m->dffn_hi, m->dffn_lo, D.f);
-    float* ffn2 = m->dffn2.as<float>() ? m->dffn2.as<float>() + D.r0 * 2 * D.f : nullptr;
-    const int heads = m->cfg.heads;
+    const int d = D.d;
+    const RelBias rb{m->t5_rel_enc, m->t5_bkt_enc, kT5MaxSource - 1, m->cfg.heads};
+    const int n = (int)m->enc.size();
+    t5_rms(cx, Te, d, tok, 1, A.x, nullptr, m->enc[0].ln_attn.g, 1.f);
+    for (int i = 0; i < n; ++i) {
+        EncLayerW& L = m->enc[i];
+        gemm(cx, Te, 3 * d, d, A.x, d, L.qkv, A.qkv, 3 * d, kActNone);
+        launch_k(t5_enc_self_attn_kernel<kGAttnWarps, kGAttnPasses>, dim3((unsigned)D.Q, m->cfg.heads), kGAttnWarps * 32, 0, cx.s, D.Q, d,
+                 (int)D.S, (const float*)A.qkv.x, m32, rb, split_of(A.attn, m->ovf), soff);
+        m->launches++; m->last_paths |= kPathT5EncAttn;
+        cx.defer_rows = INT64_MAX;
+        gemm(cx, Te, d, d, A.attn, d, L.o, A.tmp, d, kActNone);
+        cx.defer_rows = 0;
+        t5_rms(cx, Te, d, nullptr, 0, A.x, A.tmp.x, L.ln_final.g, 1.f);
+        t5_ffn(cx, Te, d, D.f, A.x, L.fc1, L.fc2, A.ffn, A.ffn2, A.tmp);
+        t5_rms(cx, Te, d, nullptr, 0, A.x, A.tmp.x, i + 1 < n ? m->enc[i + 1].ln_attn.g : m->enc_ln_emb.g, 1.f);
+    }
+}
+
+// The T5 decoder layers: the self-attention adds the relative position bias, the cross-attention runs the BART kernels
+// on the query projection pre-multiplied by 8 (their 0.125 undoes it exactly).
+void t5_decoder_layers(Ctx& cx, const Dims& D, const DecStep& S) {
+    sealbart* m = cx.m;
+    const int d = D.d, heads = m->cfg.heads;
     const RelBias rb{m->t5_rel_dec, m->t5_bkt_dec, kMaxLen - 1, heads};
-    const int32_t* m32 = m->enc_mask.as<int32_t>() + D.q0 * D.S;
-    const int32_t* soff_x = m->enc_packed ? m->src_off.as<int32_t>() + D.q0 : nullptr;
-    const int64_t ckv_q0 = m->enc_packed ? 0 : D.q0 * D.S * 2 * d;
     const int n = (int)m->dec.size();
     const float out_scale = m->t5.scale_decoder_outputs ? 1.0f / sqrtf((float)d) : 1.0f;
-    t5_rms(cx, R, d, tokens + pos, (int64_t)(D.T * row_mul), x, nullptr, m->dec[0].ln_self.g, 1.f);
+    t5_rms(cx, S.R, d, S.tokens + S.pos, (int64_t)(D.T * S.row_mul), S.x, nullptr, m->dec[0].ln_self.g, 1.f);
     for (int l = 0; l < n; ++l) {
         DecLayerW& L = m->dec[l];
-        float* kc = m->kc.as<float>() + (size_t)l * D.T * Rc * d + D.r0 * d;
-        float* vc = m->vc.as<float>() + (size_t)l * D.T * Rc * d + D.r0 * d;
-        gemm(cx, R, 3 * d, d, x, d, L.qkv, qkv, 3 * d, kActNone);
-        launch_k(t5_dec_self_attn_kernel, (unsigned)R, 32 * std::min(heads, 16), 0, cx.s, Rc, d, heads, pos, D.T, (const float*)qkv.x, kc, vc,
-                 anc, rb, split_of(attn, ovf), row_mul, row_mul);
+        float* kc = m->kc.as<float>() + (size_t)l * D.T * S.Rc * d + D.r0 * d;
+        float* vc = m->vc.as<float>() + (size_t)l * D.T * S.Rc * d + D.r0 * d;
+        gemm(cx, S.R, 3 * d, d, S.x, d, L.qkv, S.qkv, 3 * d, kActNone);
+        launch_k(t5_dec_self_attn_kernel, (unsigned)S.R, 32 * std::min(heads, 16), 0, cx.s, S.Rc, d, heads, S.pos, D.T, (const float*)S.qkv.x, kc, vc,
+                 S.anc, rb, split_of(S.attn, m->ovf), S.row_mul, S.row_mul);
         m->launches++; m->last_paths |= kPathT5DecAttn;
         cx.defer_rows = INT64_MAX;
-        gemm(cx, R, d, d, attn, d, L.o, tmp, d, kActNone);
+        gemm(cx, S.R, d, d, S.attn, d, L.o, S.tmp, d, kActNone);
         cx.defer_rows = 0;
-        t5_rms(cx, R, d, nullptr, 0, x, tmp.x, L.ln_cross.g, 1.f);
-        cx.defer_rows = (D.S <= kXKeys) ? INT64_MAX : 0;      // cross_attn_small_kernel sums a split-K cq itself
-        gemm(cx, R, d, d, x, d, L.cq, cq, d, kActNone);
-        cx.defer_rows = 0;
-        const SplitSrc cq_src = cx.pending;
-        cx.pending = SplitSrc{};
-        const int64_t groups = D.grp_start ? D.G : D.Q;
-        const float* ckv_l = m->ckv.as<float>() + (size_t)l * Tk * 2 * d + ckv_q0;
-        if (D.S <= kXKeys)
-            launch_k(cross_attn_small_kernel, dim3((unsigned)groups, heads), 128, 0, cx.s, groups, d, heads, compact ? 1 : D.B, (int)D.S, (const float*)cq.x,
-                     ckv_l, m32, D.grp_query, D.grp_start, (float*)nullptr, split_of(attn, ovf), soff_x, cq_src);
-        else
-            launch_k(cross_attn_kernel, dim3((unsigned)groups, heads), kGAttnWarps * 32, 0, cx.s, groups, d, heads, compact ? 1 : D.B, (int)D.S, (const float*)cq.x,
-                     ckv_l, m32, D.grp_query, D.grp_start, (float*)nullptr, split_of(attn, ovf), soff_x);
-        m->launches++;
-        m->last_paths |= D.S <= kXKeys ? kPathCrossSmall : kPathCrossGrouped;
-        cx.defer_rows = INT64_MAX;
-        gemm(cx, R, d, d, attn, d, L.co, tmp, d, kActNone);
-        cx.defer_rows = 0;
-        t5_rms(cx, R, d, nullptr, 0, x, tmp.x, L.ln_final.g, 1.f);
-        t5_ffn(cx, R, d, D.f, x, L.fc1, L.fc2, ffn, ffn2, tmp);
-        t5_rms(cx, R, d, nullptr, 0, x, tmp.x, l + 1 < n ? m->dec[l + 1].ln_self.g : m->dec_ln_emb.g, l + 1 < n ? 1.f : out_scale);
+        t5_rms(cx, S.R, d, nullptr, 0, S.x, S.tmp.x, L.ln_cross.g, 1.f);
+        cross_attention(cx, D, S, l, INT64_MAX);
+        t5_rms(cx, S.R, d, nullptr, 0, S.x, S.tmp.x, L.ln_final.g, 1.f);
+        t5_ffn(cx, S.R, d, D.f, S.x, L.fc1, L.fc2, S.ffn, S.ffn2, S.tmp);
+        t5_rms(cx, S.R, d, nullptr, 0, S.x, S.tmp.x, l + 1 < n ? m->dec[l + 1].ln_self.g : m->dec_ln_emb.g, l + 1 < n ? 1.f : out_scale);
     }
-    if (ev_layers_done) CUDA_CHECK(cudaEventRecord(ev_layers_done, cx.s));
-    cx.head = head;
-    if (want_logits) gemm(cx, R, D.V, d, x, d, m->head, Act{m->logits.as<float>() + D.r0 * D.ld}, D.ld, kActNone);
-    cx.head = HeadEpi{};
+}
+
+void bart_encoder_layers(Ctx& cx, const Dims& D, int64_t Te, const Acts& A, const int32_t* tok, const int32_t* pos, const int32_t* m32,
+                         const int32_t* soff) {
+    sealbart* m = cx.m;
+    const int d = D.d, heads = m->cfg.heads;
+    const float scale = m->cfg.scale_embedding ? sqrtf((float)d) : 1.0f;
+    embed_ln_kernel<<<(unsigned)((Te + 3) / 4), 128, 0, cx.s>>>(Te, d, tok, 1, pos, 0, m->shared, scale, m->enc_pos,
+                                                                m->enc_ln_emb.g, m->enc_ln_emb.b, A.x.x, split_of(A.x, m->ovf));
+    CUDA_CHECK(cudaGetLastError()); m->launches++;
+    for (auto& L : m->enc) {
+        gemm(cx, Te, 3 * d, d, A.x, d, L.qkv, A.qkv, 3 * d, kActNone);
+        enc_self_attn_kernel<<<dim3((unsigned)D.Q, heads), kGAttnWarps * 32, 0, cx.s>>>(D.Q, d, heads, (int)D.S, A.qkv.x, m32, A.attn.x,
+                                                                                       split_of(A.attn, m->ovf), soff);
+        CUDA_CHECK(cudaGetLastError()); m->launches++;
+        cx.defer_rows = kAddLnRowMax;
+        gemm(cx, Te, d, d, A.attn, d, L.o, A.tmp, d, kActNone);
+        cx.defer_rows = 0;
+        add_ln(cx, Te, d, A.x.x, A.tmp.x, L.ln_attn, A.x);
+        gemm(cx, Te, D.f, d, A.x, d, L.fc1, A.ffn, D.f, kActGelu);
+        cx.defer_rows = kAddLnRowMax;
+        gemm(cx, Te, d, D.f, A.ffn, D.f, L.fc2, A.tmp, d, kActNone);
+        cx.defer_rows = 0;
+        add_ln(cx, Te, d, A.x.x, A.tmp.x, L.ln_final, A.x);
+    }
+}
+
+void bart_decoder_layers(Ctx& cx, const Dims& D, const DecStep& S) {
+    sealbart* m = cx.m;
+    const int d = D.d, heads = m->cfg.heads, pos = S.pos;
+    int* ovf = m->ovf;
+    const float scale = m->cfg.scale_embedding ? sqrtf((float)d) : 1.0f;
+    launch_k(embed_ln_kernel, (unsigned)((S.R + 3) / 4), 128, 0, cx.s, S.R, d, S.tokens + pos, (int64_t)(D.T * S.row_mul), (const int32_t*)nullptr, pos,
+             (const float*)m->shared, scale, (const float*)m->dec_pos, (const float*)m->dec_ln_emb.g, (const float*)m->dec_ln_emb.b, S.x.x, split_of(S.x, ovf));
+    m->launches++;
+    for (int l = 0; l < m->cfg.decoder_layers; ++l) {
+        DecLayerW& L = m->dec[l];
+        float* kc = m->kc.as<float>() + (size_t)l * D.T * S.Rc * d + D.r0 * d;
+        float* vc = m->vc.as<float>() + (size_t)l * D.T * S.Rc * d + D.r0 * d;
+        // the beams of a query together, distinct ancestors staged once (not at the compact first step, where a row
+        // stands for all beams, nor for ragged re-scoring groups)
+        static const bool sa_query = [] { const char* e = std::getenv("SEALB200_SELF_ATTN_QUERY"); return !e || std::atoi(e) != 0; }();
+        const size_t saq_smem = self_attn_query_smem(pos + 1, D.B);
+        const bool use_saq = sa_query && !S.compact && !D.grp_start && pos >= 1 && D.B >= 2 && D.B <= 32 && pos + 1 <= 128 && saq_smem <= 112 * 1024;
+        cx.defer_rows = use_saq ? INT64_MAX : 0;               // that kernel sums a split-K qkv itself
+        gemm(cx, S.R, 3 * d, d, S.x, d, L.qkv, S.qkv, 3 * d, kActNone);
+        cx.defer_rows = 0;
+        const SplitSrc qkv_src = cx.pending;
+        cx.pending = SplitSrc{};
+        const unsigned sa_threads = 32 * std::min(heads, 16);
+        const float* qkv = S.qkv.x;
+        if (use_saq) {
+            static size_t saq_set = 0;
+            if (saq_smem > saq_set) { CUDA_CHECK(cudaFuncSetAttribute(dec_self_attn_query_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024)); saq_set = 112 * 1024; }
+            launch_k(dec_self_attn_query_kernel, dim3((unsigned)D.Q, heads), 32 * D.B, saq_smem, cx.s, S.Rc, D.B, d, pos, D.T, qkv, kc, vc, S.anc,
+                     S.attn.x, split_of(S.attn, ovf), qkv_src);
+        } else if (pos + 1 <= 12)
+            launch_k(dec_self_attn_kernel<3>, (unsigned)S.R, sa_threads, 0, cx.s, S.Rc, d, heads, pos, D.T, qkv, kc, vc, S.anc, S.attn.x, split_of(S.attn, ovf), S.row_mul, S.row_mul);
+        else if (pos + 1 <= 32)
+            launch_k(dec_self_attn_kernel<8>, (unsigned)S.R, sa_threads, 0, cx.s, S.Rc, d, heads, pos, D.T, qkv, kc, vc, S.anc, S.attn.x, split_of(S.attn, ovf), S.row_mul, S.row_mul);
+        else
+            launch_k(dec_self_attn_long_kernel, (unsigned)S.R, sa_threads, 0, cx.s, S.Rc, d, heads, pos, D.T, qkv, kc, vc, S.anc, S.attn.x, split_of(S.attn, ovf));
+        m->launches++;
+        m->last_paths |= use_saq ? kPathSelfQuery : pos + 1 <= 12 ? kPathSelfRounds3 : pos + 1 <= 32 ? kPathSelfRounds8 : kPathSelfLong;
+        cx.defer_rows = kAddLnRowMax;
+        gemm(cx, S.R, d, d, S.attn, d, L.o, S.tmp, d, kActNone);
+        cx.defer_rows = 0;
+        add_ln(cx, S.R, d, S.x.x, S.tmp.x, L.ln_self, S.x);
+        cross_attention(cx, D, S, l, kAddLnRowMax);
+        add_ln(cx, S.R, d, S.x.x, S.tmp.x, L.ln_cross, S.x);
+        gemm(cx, S.R, D.f, d, S.x, d, L.fc1, S.ffn, D.f, kActGelu);
+        cx.defer_rows = kAddLnRowMax;
+        gemm(cx, S.R, d, D.f, S.ffn, D.f, L.fc2, S.tmp, d, kActNone);
+        cx.defer_rows = 0;
+        add_ln(cx, S.R, d, S.x.x, S.tmp.x, L.ln_final, S.x);
+    }
 }
 
 // src_tokens_hint: >= 0 the caller's count of real source tokens (right-padded masks): no host synchronisation, the
@@ -733,44 +809,20 @@ void encoder_forward(Ctx& cx, const Dims& D, const int64_t* ids_d, const int64_t
     CUDA_CHECK(cudaGetLastError()); m->launches++;
     m->last_paths |= m->enc_packed ? kPathEncPacked : kPathEncUnpacked;
     const int64_t Te = rows_enc;                    // encoder rows actually computed
-    if (m->arch == 1) { t5_encoder_layers(cx, D, Te, tok, m32, soff); return; }
     const int gm = m->cfg.gemm_mode;
-    auto mk = [&](float* plain, Buf& bh, Buf& bl, bool keep_plain) {
-        Act a;
-        if (keep_plain) a.x = plain;
-        if (gm == 2) { a.hi = bh.as<float>(); a.lo = bl.as<float>(); }
-        if (gm >= 3) { a.h1 = bh.as<__half>(); a.h2 = bl.as<__half>(); }
-        return a;
-    };
-    int* ovf = m->ovf;
-    const Act x = mk(m->ex.as<float>(), m->ex_hi, m->ex_lo, true);
-    const Act qkv{m->eqkv.as<float>()};
-    const Act attn = mk(m->eattn.as<float>(), m->eattn_hi, m->eattn_lo, false);
-    const Act tmp{m->etmp.as<float>()};
-    const Act ffn = mk(m->effn.as<float>(), m->effn_hi, m->effn_lo, false);
-    const float scale = m->cfg.scale_embedding ? sqrtf((float)d) : 1.0f;
-    embed_ln_kernel<<<(unsigned)((Te + 3) / 4), 128, 0, cx.s>>>(Te, d, tok, 1, pos, 0, m->shared, scale, m->enc_pos,
-                                                                m->enc_ln_emb.g, m->enc_ln_emb.b, x.x, split_of(x, ovf));
-    CUDA_CHECK(cudaGetLastError()); m->launches++;
-    const int heads = m->cfg.heads;
-    for (auto& L : m->enc) {
-        gemm(cx, Te, 3 * d, d, x, d, L.qkv, qkv, 3 * d, false);
-        enc_self_attn_kernel<<<dim3((unsigned)D.Q, heads), kGAttnWarps * 32, 0, cx.s>>>(D.Q, d, heads, (int)D.S, qkv.x, m32, attn.x, split_of(attn, ovf), soff);
-        CUDA_CHECK(cudaGetLastError()); m->launches++;
-        cx.defer_rows = kAddLnRowMax;
-        gemm(cx, Te, d, d, attn, d, L.o, tmp, d, false);
-        cx.defer_rows = 0;
-        add_ln(cx, Te, d, x.x, tmp.x, L.ln_attn, x);
-        gemm(cx, Te, D.f, d, x, d, L.fc1, ffn, D.f, true);
-        cx.defer_rows = kAddLnRowMax;
-        gemm(cx, Te, d, D.f, ffn, D.f, L.fc2, tmp, d, false);
-        cx.defer_rows = 0;
-        add_ln(cx, Te, d, x.x, tmp.x, L.ln_final, x);
-    }
-    // per-query cross-attention K/V of every decoder layer, once (the reference recomputes nothing
-    // either: HF caches them after the first step)
+    Acts A;
+    A.x = act_view(gm, m->ex.as<float>(), m->ex_hi, m->ex_lo);
+    A.qkv = Act{m->eqkv.as<float>()};
+    A.attn = act_view(gm, nullptr, m->eattn_hi, m->eattn_lo);
+    A.tmp = Act{m->etmp.as<float>()};
+    A.ffn = act_view(gm, nullptr, m->effn_hi, m->effn_lo);
+    A.ffn2 = m->effn2.as<float>();
+    if (m->arch == 1) t5_encoder_layers(cx, D, Te, A, tok, m32, soff);
+    else bart_encoder_layers(cx, D, Te, A, tok, pos, m32, soff);
+    // per-query cross-attention K/V of every decoder layer, once, from the encoder's output (T5: its final_layer_norm);
+    // the reference recomputes nothing either: HF caches them after the first step
     for (int l = 0; l < m->cfg.decoder_layers; ++l)
-        gemm(cx, Te, 2 * d, d, x, d, m->dec[l].ckv, Act{m->ckv.as<float>() + (size_t)l * Tk * 2 * d}, 2 * d, false);
+        gemm(cx, Te, 2 * d, d, A.x, d, m->dec[l].ckv, Act{m->ckv.as<float>() + (size_t)l * Tk * 2 * d}, 2 * d, kActNone);
 }
 
 // one decoder step for all R rows: token at position pos = cur_len-1 -> logits [R][ld]
@@ -781,98 +833,25 @@ void encoder_forward(Ctx& cx, const Dims& D, const int64_t* ids_d, const int64_t
 void decoder_step(Ctx& cx, const Dims& D, const int32_t* tokens, int cur_len, const int32_t* anc, bool want_logits,
                   cudaEvent_t ev_layers_done, bool compact = false, const HeadEpi& head = HeadEpi{}) {
     sealbart* m = cx.m;
-    const int d = D.d; const int64_t Rc = D.Rb ? D.Rb : D.R; const int64_t Tk = (D.Qb ? D.Qb : D.Q) * D.S;
     if (compact && (cur_len != 1 || D.grp_start || D.Qb)) throw ApiError(SEALFM_EINVAL, "internal: compact step only at position 0 of a generate");
-    if (m->arch == 1) { t5_decoder_step(cx, D, tokens, cur_len, anc, want_logits, ev_layers_done, compact, head); return; }
-    const int64_t R = compact ? D.Q : D.R;          // rows processed
-    const int row_mul = compact ? D.B : 1;
-    const int pos = cur_len - 1;
-    const int gm = m->cfg.gemm_mode;
-    // rows r0 .. r0 + R of the activation buffers ([rows][width])
-    auto mk = [&](float* plain, Buf& bh, Buf& bl, bool keep_plain, int width) {
-        const int64_t o = D.r0 * width;
-        Act a;
-        if (keep_plain) a.x = plain + o;
-        if (gm == 2) { a.hi = bh.as<float>() + o; a.lo = bl.as<float>() + o; }
-        if (gm >= 3) { a.h1 = bh.as<__half>() + o; a.h2 = bl.as<__half>() + o; }
-        return a;
-    };
-    int* ovf = m->ovf;
-    const Act x = mk(m->dx.as<float>(), m->dx_hi, m->dx_lo, true, d);
-    const Act qkv{m->dqkv.as<float>() + D.r0 * 3 * d};
-    const Act attn = mk(m->dattn.as<float>(), m->dattn_hi, m->dattn_lo, false, d);
-    const Act tmp{m->dtmp.as<float>() + D.r0 * d};
-    const Act cq{m->dcq.as<float>() + D.r0 * d};
-    const Act ffn = mk(m->dffn.as<float>(), m->dffn_hi, m->dffn_lo, false, D.f);
-    const float scale = m->cfg.scale_embedding ? sqrtf((float)d) : 1.0f;
-    launch_k(embed_ln_kernel, (unsigned)((R + 3) / 4), 128, 0, cx.s, R, d, tokens + pos, (int64_t)(D.T * row_mul), (const int32_t*)nullptr, pos,
-               (const float*)m->shared, scale, (const float*)m->dec_pos, (const float*)m->dec_ln_emb.g, (const float*)m->dec_ln_emb.b, x.x, split_of(x, ovf));
-    m->launches++;
-    const int heads = m->cfg.heads;
-    // encoder side of queries q0 ..: packed, src_off holds absolute ckv rows; unpacked, query q's rows are q * S
-    const int32_t* m32 = m->enc_mask.as<int32_t>() + D.q0 * D.S;
-    const int32_t* soff_x = m->enc_packed ? m->src_off.as<int32_t>() + D.q0 : nullptr;
-    const int64_t ckv_q0 = m->enc_packed ? 0 : D.q0 * D.S * 2 * d;
-    for (int l = 0; l < m->cfg.decoder_layers; ++l) {
-        DecLayerW& L = m->dec[l];
-        float* kc = m->kc.as<float>() + (size_t)l * D.T * Rc * d + D.r0 * d;
-        float* vc = m->vc.as<float>() + (size_t)l * D.T * Rc * d + D.r0 * d;
-        // the beams of a query together, distinct ancestors staged once (not at the compact first step, where a row
-        // stands for all beams, nor for ragged re-scoring groups)
-        static const bool sa_query = [] { const char* e = std::getenv("SEALB200_SELF_ATTN_QUERY"); return !e || std::atoi(e) != 0; }();
-        const size_t saq_smem = self_attn_query_smem(pos + 1, D.B);
-        const bool use_saq = sa_query && !compact && !D.grp_start && pos >= 1 && D.B >= 2 && D.B <= 32 && pos + 1 <= 128 && saq_smem <= 112 * 1024;
-        cx.defer_rows = use_saq ? INT64_MAX : 0;               // that kernel sums a split-K qkv itself
-        gemm(cx, R, 3 * d, d, x, d, L.qkv, qkv, 3 * d, false);
-        cx.defer_rows = 0;
-        const SplitSrc qkv_src = cx.pending;
-        cx.pending = SplitSrc{};
-        const unsigned sa_threads = 32 * std::min(heads, 16);
-        if (use_saq) {
-            static size_t saq_set = 0;
-            if (saq_smem > saq_set) { CUDA_CHECK(cudaFuncSetAttribute(dec_self_attn_query_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024)); saq_set = 112 * 1024; }
-            launch_k(dec_self_attn_query_kernel, dim3((unsigned)D.Q, heads), 32 * D.B, saq_smem, cx.s, Rc, D.B, d, pos, D.T, (const float*)qkv.x, kc, vc, anc,
-                     attn.x, split_of(attn, ovf), qkv_src);
-        } else if (pos + 1 <= 12)
-            launch_k(dec_self_attn_kernel<3>, (unsigned)R, sa_threads, 0, cx.s, Rc, d, heads, pos, D.T, (const float*)qkv.x, kc, vc, anc, attn.x, split_of(attn, ovf), row_mul, row_mul);
-        else if (pos + 1 <= 32)
-            launch_k(dec_self_attn_kernel<8>, (unsigned)R, sa_threads, 0, cx.s, Rc, d, heads, pos, D.T, (const float*)qkv.x, kc, vc, anc, attn.x, split_of(attn, ovf), row_mul, row_mul);
-        else
-            launch_k(dec_self_attn_long_kernel, (unsigned)R, sa_threads, 0, cx.s, Rc, d, heads, pos, D.T, (const float*)qkv.x, kc, vc, anc, attn.x, split_of(attn, ovf));
-        m->launches++;
-        m->last_paths |= use_saq ? kPathSelfQuery : pos + 1 <= 12 ? kPathSelfRounds3 : pos + 1 <= 32 ? kPathSelfRounds8 : kPathSelfLong;
-        cx.defer_rows = kAddLnRowMax;
-        gemm(cx, R, d, d, attn, d, L.o, tmp, d, false);
-        cx.defer_rows = 0;
-        add_ln(cx, R, d, x.x, tmp.x, L.ln_self, x);
-        cx.defer_rows = (D.S <= kXKeys) ? INT64_MAX : 0;      // cross_attn_small_kernel sums a split-K cq itself
-        gemm(cx, R, d, d, x, d, L.cq, cq, d, false);
-        cx.defer_rows = 0;
-        const SplitSrc cq_src = cx.pending;
-        cx.pending = SplitSrc{};
-        const int64_t groups = D.grp_start ? D.G : D.Q;
-        const float* ckv_l = m->ckv.as<float>() + (size_t)l * Tk * 2 * d + ckv_q0;
-        if (D.S <= kXKeys)
-            launch_k(cross_attn_small_kernel, dim3((unsigned)groups, heads), 128, 0, cx.s, groups, d, heads, compact ? 1 : D.B, (int)D.S, (const float*)cq.x,
-                       ckv_l, m32, D.grp_query, D.grp_start, attn.x, split_of(attn, ovf), soff_x, cq_src);
-        else
-            launch_k(cross_attn_kernel, dim3((unsigned)groups, heads), kGAttnWarps * 32, 0, cx.s, groups, d, heads, compact ? 1 : D.B, (int)D.S, (const float*)cq.x,
-                       ckv_l, m32, D.grp_query, D.grp_start, attn.x, split_of(attn, ovf), soff_x);
-        m->launches++;
-        m->last_paths |= D.S <= kXKeys ? kPathCrossSmall : kPathCrossGrouped;
-        cx.defer_rows = kAddLnRowMax;
-        gemm(cx, R, d, d, attn, d, L.co, tmp, d, false);
-        cx.defer_rows = 0;
-        add_ln(cx, R, d, x.x, tmp.x, L.ln_cross, x);
-        gemm(cx, R, D.f, d, x, d, L.fc1, ffn, D.f, true);
-        cx.defer_rows = kAddLnRowMax;
-        gemm(cx, R, d, D.f, ffn, D.f, L.fc2, tmp, d, false);
-        cx.defer_rows = 0;
-        add_ln(cx, R, d, x.x, tmp.x, L.ln_final, x);
-    }
+    const int d = D.d, gm = m->cfg.gemm_mode;
+    DecStep S;
+    S.x = act_view(gm, m->dx.as<float>(), m->dx_hi, m->dx_lo, D.r0 * d);
+    S.qkv = Act{m->dqkv.as<float>() + D.r0 * 3 * d};
+    S.attn = act_view(gm, nullptr, m->dattn_hi, m->dattn_lo, D.r0 * d);
+    S.tmp = Act{m->dtmp.as<float>() + D.r0 * d};
+    S.cq = Act{m->dcq.as<float>() + D.r0 * d};
+    S.ffn = act_view(gm, nullptr, m->dffn_hi, m->dffn_lo, D.r0 * D.f);
+    S.ffn2 = m->dffn2.as<float>() ? m->dffn2.as<float>() + D.r0 * 2 * D.f : nullptr;
+    S.R = compact ? D.Q : D.R; S.row_mul = compact ? D.B : 1; S.compact = compact;
+    S.Rc = D.Rb ? D.Rb : D.R; S.pos = cur_len - 1; S.tokens = tokens; S.anc = anc;
+    S.Tk = (D.Qb ? D.Qb : D.Q) * D.S; S.ckv_q0 = m->enc_packed ? 0 : D.q0 * D.S * 2 * d;
+    S.m32 = m->enc_mask.as<int32_t>() + D.q0 * D.S; S.soff_x = m->enc_packed ? m->src_off.as<int32_t>() + D.q0 : nullptr;
+    if (m->arch == 1) t5_decoder_layers(cx, D, S);
+    else bart_decoder_layers(cx, D, S);
     if (ev_layers_done) CUDA_CHECK(cudaEventRecord(ev_layers_done, cx.s));
     cx.head = head;                 // only the lm_head may take the statistics epilogue
-    if (want_logits) gemm(cx, R, D.V, d, x, d, m->head, Act{m->logits.as<float>() + D.r0 * D.ld}, D.ld, false);
+    if (want_logits) gemm(cx, S.R, D.V, d, S.x, d, m->head, Act{m->logits.as<float>() + D.r0 * D.ld}, D.ld, kActNone);
     cx.head = HeadEpi{};
 }
 
@@ -916,6 +895,29 @@ void ensure_tf32_splits(sealbart* m) {
     m->tf32_ready = true;
 }
 
+// 3xFP16 operand copies of l (gemm_mode 3 / 5): W * 2^s = w_h1 + w_h2 with max|W| * 2^s in [2^13, 2^14), w_unscale =
+// 2^-s; a weight outside the halves' range raises m->err[1].  h1 / h2 hold n = out * in halves each; null: allocated
+// here and owned by m (split_allocs).  d_max: one device word of scratch.
+void split_lin_half(sealbart* m, Lin& l, unsigned int* d_max, __half* h1 = nullptr, __half* h2 = nullptr) {
+    const uint64_t n = (uint64_t)l.out * l.in;
+    CUDA_CHECK(cudaMemset(d_max, 0, 4));
+    absmax_kernel<<<sm_count() * 4, 256>>>((int64_t)n, l.w, d_max);
+    unsigned int bits = 0; CUDA_CHECK(cudaMemcpy(&bits, d_max, 4, cudaMemcpyDeviceToHost));
+    float mx; std::memcpy(&mx, &bits, 4);
+    int sexp = 0;
+    if (mx > 0.f) { int e; std::frexp(mx, &e); sexp = 14 - e; }
+    l.w_unscale = std::ldexp(1.0f, -sexp);
+    if (!h1) {
+        CUDA_CHECK(cudaMalloc(&h1, n * 2)); m->split_allocs.push_back(h1);
+        CUDA_CHECK(cudaMalloc(&h2, n * 2)); m->split_allocs.push_back(h2);
+        m->weight_bytes += 2 * n * 2;
+    }
+    l.w_h1 = h1; l.w_h2 = h2;
+    split_half_kernel<<<sm_count() * 8, 256>>>((int64_t)n, l.w, std::ldexp(1.0f, sexp), l.w_h1, l.w_h2, m->err.as<int>() + 1);
+    CUDA_CHECK(cudaGetLastError());
+    l.maps_ready = false;
+}
+
 // HF's T5Attention._relative_position_bucket for one relative position (key - query), in its float32 arithmetic:
 // log(rel.float() / max_exact) in fp32, divided by math.log(max_distance / max_exact) (a Python float, rounded to fp32
 // where it meets the fp32 tensor), times (num_buckets - max_exact), truncated.  Computed here once per model: a device
@@ -950,6 +952,18 @@ void t5_bucket_tables(sealbart* m) {
     CUDA_CHECK(cudaMemcpy(m->t5_bkt_dec, dec.data(), dec.size() * 4, cudaMemcpyHostToDevice));
 }
 
+// Returns the number of CUDA devices; none is an error.
+int require_device() {
+    int count = 0;
+    if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) { cudaGetLastError(); throw ApiError(SEALFM_ENODEVICE, "no CUDA device available"); }
+    return count;
+}
+
+void check_gemm_mode(int mode) {
+    if (mode != 2 && mode != 3 && mode != 5)
+        throw ApiError(SEALFM_EINVAL, "gemm_mode must be 3 (3xFP16, one CTA per tile, default), 5 (3xFP16 on 2-CTA clusters) or 2 (3xTF32)");
+}
+
 // sealt5_create's shape checks (before any allocation)
 void check_t5_config(const sealt5_config_t* c) {
     if (c->d_kv != kHeadDim || c->num_heads * kHeadDim != c->d_model)
@@ -962,8 +976,7 @@ void check_t5_config(const sealt5_config_t* c) {
         c->relative_attention_max_distance <= c->relative_attention_num_buckets / 2)
         throw ApiError(SEALFM_EINVAL, "T5: relative_attention_num_buckets must be in [4, 1024] and relative_attention_max_distance > num_buckets / 2");
     if (!(c->layer_norm_epsilon >= 0.f) || !std::isfinite(c->layer_norm_epsilon)) throw ApiError(SEALFM_EINVAL, "T5: bad layer_norm_epsilon");
-    if (c->gemm_mode != 2 && c->gemm_mode != 3 && c->gemm_mode != 5)
-        throw ApiError(SEALFM_EINVAL, "gemm_mode must be 3 (3xFP16, one CTA per tile, default), 5 (3xFP16 on 2-CTA clusters) or 2 (3xTF32)");
+    check_gemm_mode(c->gemm_mode);
 }
 
 }  // namespace
@@ -983,10 +996,7 @@ int sealt5_create(const sealt5_config_t* cfg, int device, sealbart_t** out) {
     return guarded([&] {
         if (!cfg || !out) throw ApiError(SEALFM_EINVAL, "null argument");
         check_t5_config(cfg);
-        int count = 0;
-        cudaError_t e = cudaGetDeviceCount(&count);
-        if (e != cudaSuccess || count == 0) { cudaGetLastError(); throw ApiError(SEALFM_ENODEVICE, "no CUDA device available"); }
-        if (device < 0 || device >= count) throw ApiError(SEALFM_EINVAL, "bad device id");
+        if (device < 0 || device >= require_device()) throw ApiError(SEALFM_EINVAL, "bad device id");
         CUDA_CHECK(cudaSetDevice(device));
         std::unique_ptr<sealbart> m(new sealbart());
         m->arch = 1; m->t5 = *cfg; m->device = device;
@@ -1006,12 +1016,8 @@ int sealbart_create(const sealbart_config_t* cfg, int device, sealbart_t** out) 
         if (cfg->d_model % 128 || cfg->d_model > 1024 || cfg->heads * kHeadDim != cfg->d_model)
             throw ApiError(SEALFM_EINVAL, "d_model must be a multiple of 128, <= 1024, with 64-wide heads");
         if (cfg->ffn_dim % 64 || cfg->vocab_size <= 0) throw ApiError(SEALFM_EINVAL, "bad ffn_dim / vocab_size");
-        if (cfg->gemm_mode != 2 && cfg->gemm_mode != 3 && cfg->gemm_mode != 5)
-            throw ApiError(SEALFM_EINVAL, "gemm_mode must be 3 (3xFP16, one CTA per tile, default), 5 (3xFP16 on 2-CTA clusters) or 2 (3xTF32)");
-        int count = 0;
-        cudaError_t e = cudaGetDeviceCount(&count);
-        if (e != cudaSuccess || count == 0) { cudaGetLastError(); throw ApiError(SEALFM_ENODEVICE, "no CUDA device available"); }
-        if (device < 0 || device >= count) throw ApiError(SEALFM_EINVAL, "bad device id");
+        check_gemm_mode(cfg->gemm_mode);
+        if (device < 0 || device >= require_device()) throw ApiError(SEALFM_EINVAL, "bad device id");
         CUDA_CHECK(cudaSetDevice(device));
         std::unique_ptr<sealbart> m(new sealbart());
         m->cfg = *cfg; m->device = device;
@@ -1026,22 +1032,13 @@ void sealbart_free(sealbart_t* m) {
     for (void* p : m->allocs) cudaFree(p);
     for (void* p : m->split_allocs) cudaFree(p);
     if (m->lm_head_given) cudaFree(m->lm_head);
-    for (Buf* b : {&m->enc_tok, &m->enc_mask, &m->src_off, &m->ex, &m->eqkv, &m->eattn, &m->etmp, &m->effn, &m->ckv, &m->dx, &m->dqkv,
-                   &m->dattn, &m->dtmp, &m->dcq, &m->dffn, &m->logits, &m->kc, &m->vc, &m->st_scores, &m->st_tokens,
-                   &m->st_lo, &m->st_hi, &m->st_pw, &m->st_anc, &m->st_mask, &m->st_rowmax, &m->st_hstat, &m->st_thr, &m->st_rowls, &m->st_rule, &m->st_cval,
-                   &m->st_cidx, &m->st_ccnt, &m->st_wide, &m->hy_score, &m->hy_len, &m->hy_tok,
-                   &m->hy_valid, &m->hy_lo, &m->hy_hi, &m->err, &m->dbg_ids, &m->force_syms, &m->a_hi, &m->a_lo, &m->ex_hi, &m->ex_lo,
-                   &m->eattn_hi, &m->eattn_lo, &m->effn_hi, &m->effn_lo, &m->dx_hi, &m->dx_lo, &m->dattn_hi, &m->dattn_lo,
-                   &m->dffn_hi, &m->dffn_lo, &m->splitk, &m->a_hi1, &m->a_lo1, &m->splitk1, &m->st_wide1, &m->effn2, &m->dffn2})
-        b->release();
     if (m->slice_fork) cudaEventDestroy(m->slice_fork);
     if (m->slice_join) cudaEventDestroy(m->slice_join);
     if (m->slice_stream) cudaStreamDestroy(m->slice_stream);
     for (auto e : m->events) cudaEventDestroy(e);
     for (auto& g : m->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
-    for (Buf* b : {&m->in_ids, &m->in_mask, &m->in_occ}) b->release();
     if (m->stream) cudaStreamDestroy(m->stream);
-    delete m;
+    delete m;                         // frees the workspace (Buf)
 }
 
 int sealbart_set_tensor(sealbart_t* m, const char* key, const float* host, uint64_t numel) {
@@ -1082,41 +1079,19 @@ int sealbart_finalize(sealbart_t* m) {
             if (!m->loaded.count(kv.first)) throw ApiError(SEALFM_EINVAL, "state_dict tensor missing: " + kv.first);
         if (!m->lm_head_given) m->lm_head = m->shared;          // tied (seal/utils.py:48-49; T5: tie_word_embeddings)
         m->head.w = m->lm_head; m->head.b = m->final_bias; m->head.out = m->cfg.vocab_size; m->head.in = m->cfg.d_model;
-        {
-            CUDA_CHECK(cudaSetDevice(m->device));
-            for (void* p : m->split_allocs) cudaFree(p);
-            m->split_allocs.clear();
-            m->tf32_ready = false;
-            for_each_lin(m, [](Lin& l) { l.maps_ready = false; l.maps2_ready = false; });
+        CUDA_CHECK(cudaSetDevice(m->device));
+        for (void* p : m->split_allocs) cudaFree(p);
+        m->split_allocs.clear();
+        m->tf32_ready = false;
+        for_each_lin(m, [](Lin& l) { l.maps_ready = false; l.maps2_ready = false; });
+        if (m->cfg.gemm_mode >= 3) {
             unsigned int* d_max = nullptr;
-            if (m->cfg.gemm_mode >= 3) { CUDA_CHECK(cudaMalloc(&d_max, 4)); m->err.ensure(16); CUDA_CHECK(cudaMemset(m->err.p, 0, 16)); }
-            auto split_lin_half = [&](Lin& l) {
-                const uint64_t n = (uint64_t)l.out * l.in;
-                CUDA_CHECK(cudaMemset(d_max, 0, 4));
-                absmax_kernel<<<sm_count() * 4, 256>>>((int64_t)n, l.w, d_max);
-                unsigned int bits = 0; CUDA_CHECK(cudaMemcpy(&bits, d_max, 4, cudaMemcpyDeviceToHost));
-                float mx; std::memcpy(&mx, &bits, 4);
-                int sexp = 0;
-                if (mx > 0.f) { int e; std::frexp(mx, &e); sexp = 14 - e; }      // max|W| * 2^s in [2^13, 2^14)
-                l.w_unscale = std::ldexp(1.0f, -sexp);
-                CUDA_CHECK(cudaMalloc(&l.w_h1, n * 2)); m->split_allocs.push_back(l.w_h1);
-                CUDA_CHECK(cudaMalloc(&l.w_h2, n * 2)); m->split_allocs.push_back(l.w_h2);
-                split_half_kernel<<<sm_count() * 8, 256>>>((int64_t)n, l.w, std::ldexp(1.0f, sexp), l.w_h1, l.w_h2, m->err.as<int>() + 1);
-                CUDA_CHECK(cudaGetLastError());
-                l.maps_ready = false;
-                m->weight_bytes += 2 * n * 2;
-            };
-            if (m->cfg.gemm_mode >= 3) {
-                for (auto& L : m->enc) { split_lin_half(L.qkv); split_lin_half(L.o); split_lin_half(L.fc1); split_lin_half(L.fc2); }
-                for (auto& L : m->dec) { split_lin_half(L.qkv); split_lin_half(L.o); split_lin_half(L.cq); split_lin_half(L.ckv); split_lin_half(L.co); split_lin_half(L.fc1); split_lin_half(L.fc2); }
-                split_lin_half(m->head);
-                CUDA_CHECK(cudaDeviceSynchronize());
-                cudaFree(d_max);
-                m->finalized = true;
-                return;
-            }
+            CUDA_CHECK(cudaMalloc(&d_max, 4)); m->err.ensure(16); CUDA_CHECK(cudaMemset(m->err.p, 0, 16));
+            for_each_lin(m, [&](Lin& l) { split_lin_half(m, l, d_max); });
+            CUDA_CHECK(cudaDeviceSynchronize());
+            cudaFree(d_max);
+        } else
             ensure_tf32_splits(m);
-        }
         m->finalized = true;
     });
 }
@@ -1186,6 +1161,34 @@ int launch_select_step(cudaStream_t s, const FmView& view, const StepCfg& c, con
     return lists;
 }
 
+// The StepCfg fields every step of a generate shares: the parameters, the groups and the vocabulary size V.  The
+// per-step fields are set by set_step; hyp_base and head_tiles by the caller.
+StepCfg step_cfg(const sealdec_params_t* p, const sealdec_groups_t& grp, int V) {
+    StepCfg c{};
+    c.num_beams = p->num_beams; c.K = 2 * p->num_beams; c.V = V; c.ld = (V + 3) / 4 * 4;
+    c.min_length = p->min_length; c.max_length = p->max_length;
+    c.eos_token_id = p->eos_token_id; c.pad_token_id = p->pad_token_id; c.model_eos_token_id = p->model_eos_token_id;
+    c.forced_eos_token_id = p->forced_eos_token_id; c.forced_bos_token_id = p->forced_bos_token_id;
+    c.stop_at_count = p->stop_at_count; c.always_allow_eos = p->always_allow_eos; c.disable_fm_index = p->disable_fm_index;
+    c.remove_invalid_values = p->remove_invalid_values; c.shift = p->shift; c.T = p->max_length; c.mask_words = (V + 31) / 32;
+    c.hyps_per_query = sealdec_hyps_per_query(p);
+    c.num_groups = grp.num_beam_groups; c.diversity_penalty = grp.diversity_penalty;
+    c.top_k = p->top_k < V ? p->top_k : 0;                 // top_k >= V keeps every logit: the top_k = 0 path
+    return c;
+}
+
+// The fields of step cur_len: whether every row reads the occurring mask (the first step after a forced BOS, or the
+// first), whether the next step's masks are expanded, and how the logits were produced (logits_shared: one row per
+// query, the compact first step; logits_ignored: the forced-EOS step, on which the model did not run).
+void set_step(StepCfg& c, int cur_len, bool logits_shared, bool logits_ignored) {
+    const int eff_len = cur_len - (c.forced_bos_token_id >= 0 ? 1 : 0);
+    c.cur_len = cur_len;
+    c.first_step_shared_mask = (!c.disable_fm_index && eff_len == 1) ? 1 : 0;
+    c.expand_next = (cur_len + 1 < c.T) ? 1 : 0;
+    c.logits_shared = logits_shared ? 1 : 0;
+    c.logits_ignored = logits_ignored ? 1 : 0;
+}
+
 void generate_enqueue(Ctx& cx, const Dims& D, const GenArgs& a, const FmView& view, uint64_t lo0, uint64_t hi0,
                       int64_t src_hint, bool timing) {
     sealbart* m = cx.m;
@@ -1218,16 +1221,7 @@ void generate_enqueue(Ctx& cx, const Dims& D, const GenArgs& a, const FmView& vi
                                                                     lo0, hi0, sc[0], tk[0], lo[0], hi[0], pw[0], an[0]);
     CUDA_CHECK(cudaGetLastError()); m->launches++;
 
-    StepCfg c{};
-    c.num_beams = B; c.K = K; c.V = D.V; c.ld = D.ld;
-    c.min_length = p->min_length; c.max_length = p->max_length;
-    c.eos_token_id = p->eos_token_id; c.pad_token_id = p->pad_token_id; c.model_eos_token_id = p->model_eos_token_id;
-    c.forced_eos_token_id = p->forced_eos_token_id; c.forced_bos_token_id = p->forced_bos_token_id;
-    c.stop_at_count = p->stop_at_count; c.always_allow_eos = p->always_allow_eos; c.disable_fm_index = p->disable_fm_index;
-    c.remove_invalid_values = p->remove_invalid_values; c.shift = p->shift; c.T = T; c.mask_words = D.W;
-    c.hyps_per_query = sealdec_hyps_per_query(p);
-    c.num_groups = G; c.diversity_penalty = a.grp.diversity_penalty;
-    c.top_k = p->top_k < D.V ? p->top_k : 0;                 // top_k >= V keeps every logit: the top_k = 0 path
+    const StepCfg c = step_cfg(p, a.grp, D.V);
     set_select_smem();
     // Query slices.  The rows of a decode step are independent, so after the first step (compact: one row per query,
     // run on the whole batch) queries [0, Q0) and [Q0, Q), Q0 = ceil(Q / 2), run the rest of the decode -- decoder
@@ -1292,22 +1286,24 @@ void generate_enqueue(Ctx& cx, const Dims& D, const GenArgs& a, const FmView& vi
         if (timed) m->fused_head_steps += pc.head_fused ? 1 : 0;
         return pc.head_fused;
     };
+    // A StepState holding only where the hypothesis records of queries q0.. go (each step's and the final beams')
+    auto records = [&](int64_t q0) {
+        StepState st{};
+        st.hyp_score = a.o_score + q0 * H; st.hyp_len = a.o_len + q0 * H; st.hyp_tokens = a.o_tok + q0 * H * T;
+        st.hyp_valid = a.o_valid + q0 * H; st.hyp_lo = a.o_lo ? a.o_lo + q0 * H : nullptr; st.hyp_hi = a.o_hi ? a.o_hi + q0 * H : nullptr;
+        return st;
+    };
     // The selection of step `step` on the rows of PD, from the logits model_part left (head_fused: statistics epilogue).
     auto select_part = [&](Ctx& pc, const Dims& PD, unsigned long long* wide, int step, bool head_fused, bool timed) {
         const int cur = step & 1, cur_len = step + 1;
         const bool compact = compact_first && cur_len == 1;
         const bool dead = is_dead(cur_len);
         const int64_t r0 = PD.r0, q0 = PD.q0;
-        const int eff_len = cur_len - (p->forced_bos_token_id >= 0 ? 1 : 0);
         StepCfg cs = c;
-        cs.cur_len = cur_len;
-        cs.logits_shared = (compact && !dead) ? 1 : 0;
-        cs.logits_ignored = dead ? 1 : 0;
+        set_step(cs, cur_len, compact && !dead, dead);
         cs.head_tiles = head_fused ? head_tiles : 0;
-        cs.first_step_shared_mask = (!p->disable_fm_index && eff_len == 1) ? 1 : 0;
-        cs.expand_next = (cur_len + 1 < T) ? 1 : 0;
         cs.hyp_base = step * K;
-        StepState st{};
+        StepState st = records(q0);
         st.beam_scores_in = sc[cur] + r0; st.beam_scores_out = sc[cur ^ 1] + r0;
         st.tokens_in = tk[cur] + r0 * T; st.tokens_out = tk[cur ^ 1] + r0 * T;
         st.lo_in = lo[cur] + r0; st.lo_out = lo[cur ^ 1] + r0; st.hi_in = hi[cur] + r0; st.hi_out = hi[cur ^ 1] + r0;
@@ -1317,8 +1313,6 @@ void generate_enqueue(Ctx& cx, const Dims& D, const GenArgs& a, const FmView& vi
         // the compact first step wrote one logits row per query (of the whole batch)
         st.occurring_mask = a.occ_d; st.logits = m->logits.as<float>() + (cs.logits_shared ? q0 : r0) * D.ld;
         st.head_stats = m->st_hstat.as<float2>() + r0 * head_tiles;
-        st.hyp_score = a.o_score + q0 * H; st.hyp_len = a.o_len + q0 * H; st.hyp_tokens = a.o_tok + q0 * H * T;
-        st.hyp_valid = a.o_valid + q0 * H; st.hyp_lo = a.o_lo ? a.o_lo + q0 * H : nullptr; st.hyp_hi = a.o_hi ? a.o_hi + q0 * H : nullptr;
         st.error_flag = a.err_d;
         const RowScratch rs{m->st_rowmax.as<float>() + r0, m->st_rowls.as<float>() + r0, m->st_rule.as<uint8_t>() + r0,
                             m->st_cval.as<float>() + r0 * K, m->st_cidx.as<int32_t>() + r0 * K, m->st_ccnt.as<int32_t>() + r0,
@@ -1334,13 +1328,12 @@ void generate_enqueue(Ctx& cx, const Dims& D, const GenArgs& a, const FmView& vi
     };
     auto finalize_part = [&](Ctx& pc, const Dims& PD) {
         const int cur = (T - 1) & 1;
-        const int64_t r0 = PD.r0, q0 = PD.q0;
+        const int64_t r0 = PD.r0;
         StepCfg cs = c;
-        cs.cur_len = T; cs.hyp_base = (T - 1) * K;
-        StepState st{};
-        st.hyp_score = a.o_score + q0 * H; st.hyp_len = a.o_len + q0 * H; st.hyp_tokens = a.o_tok + q0 * H * T;
-        st.hyp_valid = a.o_valid + q0 * H; st.hyp_lo = a.o_lo ? a.o_lo + q0 * H : nullptr; st.hyp_hi = a.o_hi ? a.o_hi + q0 * H : nullptr;
-        finalize_kernel<<<(unsigned)((PD.R + 255) / 256), 256, 0, pc.s>>>(PD.Q, cs, sc[cur] + r0, tk[cur] + r0 * T, lo[cur] + r0, hi[cur] + r0, st);
+        set_step(cs, T, false, false);
+        cs.hyp_base = (T - 1) * K;
+        finalize_kernel<<<(unsigned)((PD.R + 255) / 256), 256, 0, pc.s>>>(PD.Q, cs, sc[cur] + r0, tk[cur] + r0 * T, lo[cur] + r0, hi[cur] + r0,
+                                                                         records(PD.q0));
         CUDA_CHECK(cudaGetLastError()); m->launches++;
     };
     if (!sliced) {
@@ -1429,6 +1422,17 @@ void check_sources(const int64_t* ids, const int64_t* mask, int64_t Q, int64_t S
         if (!any) throw ApiError(SEALFM_EINVAL, "source " + std::to_string(q) + " has an all-zero attention mask");
     }
     check_token_ids(ids, Q * S, V, "source");
+}
+
+// The number of real tokens of host masks [Q][S] whose every row is right-padded ("ones then zeros"), else -1
+int64_t right_padded_tokens(const int64_t* mask, int64_t Q, int64_t S) {
+    int64_t n = 0;
+    for (int64_t q = 0; q < Q; ++q) {
+        int64_t len = 0;
+        for (int64_t s2 = 0; s2 < S; ++s2) { const bool on = mask[q * S + s2] != 0; if (on && s2 != len) return -1; len += on; }
+        n += len;
+    }
+    return n;
 }
 
 // out[r * out_stride] = log_softmax(logits[r] / temperature)[targets[r * tgt_stride]] (0 for a target outside
@@ -1688,13 +1692,8 @@ int sealdec_generate_ex(sealbart_t* m, const sealfm_t* fm, const uint32_t* occ_h
         const int W = (m->cfg.vocab_size + 31) / 32;
         // the caller's buffers are host memory: the real-token count costs nothing to know here, so the encoder
         // never has to ask the device for it (right-padded masks only; anything else takes the padded path)
-        int64_t hint = 0;
-        for (int64_t q = 0; q < Q && hint >= 0; ++q) {
-            int64_t len = 0;
-            for (int64_t s2 = 0; s2 < S; ++s2) { const bool on = mask[q * S + s2] != 0; if (on && s2 != len) { hint = -2; break; } len += on; }
-            if (hint >= 0) hint += len;
-        }
-        if (hint == 0) hint = -2;
+        int64_t hint = right_padded_tokens(mask, Q, S);
+        if (hint <= 0) hint = -2;
         if (!m->stream) CUDA_CHECK(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));
         cudaStream_t s = m->stream;
         m->in_ids.ensure(Q * S * 8); m->in_mask.ensure(Q * S * 8); m->in_occ.ensure((size_t)W * 4);
@@ -1704,30 +1703,27 @@ int sealdec_generate_ex(sealbart_t* m, const sealfm_t* fm, const uint32_t* occ_h
         CUDA_CHECK(cudaMemcpyAsync(m->in_mask.p, mask, Q * S * 8, cudaMemcpyHostToDevice, s));
         if (occ_host) CUDA_CHECK(cudaMemcpyAsync(m->in_occ.p, occ_host, (size_t)W * 4, cudaMemcpyHostToDevice, s));
         int32_t errs[4] = {0, 0, 0, 0};
-        for (int attempt = 0; attempt < 2; ++attempt) {
-            int rc = sealdec_generate_dx_ex(m, fm, occ_host ? m->in_occ.as<uint32_t>() : nullptr, p, m->in_ids.as<int64_t>(),
-                                            m->in_mask.as<int64_t>(), Q, S, s, m->hy_score.as<float>(), m->hy_len.as<int32_t>(),
-                                            m->hy_tok.as<int32_t>(), m->hy_valid.as<uint8_t>(), o_lo ? m->hy_lo.as<uint64_t>() : nullptr,
-                                            o_hi ? m->hy_hi.as<uint64_t>() : nullptr, m->err.as<int32_t>(), hint, groups);
-            if (rc) throw ApiError(rc, last_error());
-            CUDA_CHECK(cudaMemcpyAsync(errs, m->err.p, 16, cudaMemcpyDeviceToHost, s));
-            CUDA_CHECK(cudaStreamSynchronize(s));
-            if (!errs[1] || m->cfg.gemm_mode < 3) break;
+        auto run = [&] {                                       // one pass on the staged inputs
+            return sealdec_generate_dx_ex(m, fm, occ_host ? m->in_occ.as<uint32_t>() : nullptr, p, m->in_ids.as<int64_t>(),
+                                          m->in_mask.as<int64_t>(), Q, S, s, m->hy_score.as<float>(), m->hy_len.as<int32_t>(),
+                                          m->hy_tok.as<int32_t>(), m->hy_valid.as<uint8_t>(), o_lo ? m->hy_lo.as<uint64_t>() : nullptr,
+                                          o_hi ? m->hy_hi.as<uint64_t>() : nullptr, m->err.as<int32_t>(), hint, groups);
+        };
+        if (const int rc = run()) throw ApiError(rc, last_error());
+        CUDA_CHECK(cudaMemcpyAsync(errs, m->err.p, 16, cudaMemcpyDeviceToHost, s));
+        CUDA_CHECK(cudaStreamSynchronize(s));
+        if (errs[1] && m->cfg.gemm_mode >= 3) {
             // An activation left the fp16 range (|x| > 65504; the producers saturate and raise the flag): this pass is
             // redone with the 3xTF32 kernels, which have fp32's range -- the caller gets exact-range results either way.
             const int mode = m->cfg.gemm_mode;
             { const int r0 = sealbart_set_option(m, "gemm_mode", 2); if (r0) throw ApiError(r0, last_error()); }
             m->overflow_fallbacks++;
-            rc = sealdec_generate_dx_ex(m, fm, occ_host ? m->in_occ.as<uint32_t>() : nullptr, p, m->in_ids.as<int64_t>(),
-                                        m->in_mask.as<int64_t>(), Q, S, s, m->hy_score.as<float>(), m->hy_len.as<int32_t>(),
-                                        m->hy_tok.as<int32_t>(), m->hy_valid.as<uint8_t>(), o_lo ? m->hy_lo.as<uint64_t>() : nullptr,
-                                        o_hi ? m->hy_hi.as<uint64_t>() : nullptr, m->err.as<int32_t>(), hint, groups);
+            const int rc = run();
             const int rc2 = sealbart_set_option(m, "gemm_mode", mode);
             if (rc) throw ApiError(rc, last_error());
             if (rc2) throw ApiError(rc2, last_error());
             CUDA_CHECK(cudaMemcpyAsync(errs, m->err.p, 16, cudaMemcpyDeviceToHost, s));
             CUDA_CHECK(cudaStreamSynchronize(s));
-            break;
         }
         CUDA_CHECK(cudaMemcpyAsync(o_score, m->hy_score.p, Q * H * 4, cudaMemcpyDeviceToHost, s));
         CUDA_CHECK(cudaMemcpyAsync(o_len, m->hy_len.p, Q * H * 4, cudaMemcpyDeviceToHost, s));
@@ -1755,16 +1751,9 @@ int sealdec_debug_step_logits_ex(sealbart_t* m, const int64_t* ids, const int64_
             throw ApiError(SEALFM_EINVAL, "bad argument");
         if (S > m->cfg.max_positions) throw ApiError(SEALFM_EINVAL, "source longer than max_positions");
         check_sources(ids, mask, Q, S, m->cfg.vocab_size);
-        if (src_tokens_hint != -1 && src_tokens_hint != -2) {
-            // a count is only valid for right-padded masks; checked here, where the mask is host memory
-            int64_t n = 0; bool prefix = true;
-            for (int64_t q = 0; q < Q; ++q) {
-                int64_t len = 0;
-                for (int64_t s2 = 0; s2 < S; ++s2) { const bool on = mask[q * S + s2] != 0; if (on && s2 != len) prefix = false; len += on; }
-                n += len;
-            }
-            if (!prefix || n != src_tokens_hint) throw ApiError(SEALFM_EINVAL, "src_tokens_hint does not match a right-padded mask");
-        }
+        // a count is only valid for right-padded masks; checked here, where the mask is host memory
+        if (src_tokens_hint != -1 && src_tokens_hint != -2 && right_padded_tokens(mask, Q, S) != src_tokens_hint)
+            throw ApiError(SEALFM_EINVAL, "src_tokens_hint does not match a right-padded mask");
         const int T = (int)t;
         const Dims D = make_dims(m, Q, S, B, T);
         check_token_ids(dec_ids, D.R * T, m->cfg.vocab_size, "decoder");
@@ -1775,7 +1764,6 @@ int sealdec_debug_step_logits_ex(sealbart_t* m, const int64_t* ids, const int64_
         m->ovf = m->err.as<int>() + 1;
         Buf d_ids, d_mask;
         d_ids.ensure(Q * S * 8); d_mask.ensure(Q * S * 8); m->dbg_ids.ensure(D.R * t * 8);
-        struct Rel { Buf *a, *b; ~Rel() { a->release(); b->release(); } } rel{&d_ids, &d_mask};
         cudaStream_t s = nullptr;
         CUDA_CHECK(cudaMemcpyAsync(d_ids.p, ids, Q * S * 8, cudaMemcpyHostToDevice, s));
         CUDA_CHECK(cudaMemcpyAsync(d_mask.p, mask, Q * S * 8, cudaMemcpyHostToDevice, s));
@@ -1818,7 +1806,6 @@ int sealdec_teacher_forced(sealbart_t* m, const int64_t* ids, const int64_t* mas
         cudaStream_t s = nullptr;
         CUDA_CHECK(cudaMemsetAsync(m->ovf, 0, 4, s));          // before the encoder: its producers raise it too
         Buf d_ids, d_mask, d_dec, d_gq, d_gs, d_out, d_full;
-        struct Rel { std::vector<Buf*> v; ~Rel() { for (auto b : v) b->release(); } } rel{{&d_ids, &d_mask, &d_dec, &d_gq, &d_gs, &d_out, &d_full}};
         d_ids.ensure(Q * S * 8); d_mask.ensure(Q * S * 8);
         CUDA_CHECK(cudaMemcpyAsync(d_ids.p, ids, Q * S * 8, cudaMemcpyHostToDevice, s));
         CUDA_CHECK(cudaMemcpyAsync(d_mask.p, mask, Q * S * 8, cudaMemcpyHostToDevice, s));
@@ -1880,13 +1867,11 @@ int debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A, const 
         if (!A || !W || (store && !C) || M <= 0 || N <= 0 || K <= 0 || band < -1) throw ApiError(SEALFM_EINVAL, "bad argument");
         if (head && (mode != 3 || !store || gelu || iters > 0 || !head->mask || !head->stats || !head->fused))
             throw ApiError(SEALFM_EINVAL, "bad argument");
-        int count = 0;
-        if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) { cudaGetLastError(); throw ApiError(SEALFM_ENODEVICE, "no CUDA device available"); }
-        if (mode != 2 && mode != 3 && mode != 5) throw ApiError(SEALFM_EINVAL, "gemm_mode must be 2, 3 or 5");
+        require_device();
+        check_gemm_mode(mode);
         sealbart fake; fake.cfg.gemm_mode = mode;
         CUDA_CHECK(cudaGetDevice(&fake.device));
         Buf dA, dW, dB, dC, whi, wlo;
-        struct Rel { std::vector<Buf*> v; sealbart* f; ~Rel() { for (auto b : v) b->release(); f->a_hi.release(); f->a_lo.release(); f->err.release(); f->splitk.release(); } } rel{{&dA, &dW, &dB, &dC, &whi, &wlo}, &fake};
         const int ldc = (N + 3) / 4 * 4;
         dA.ensure((size_t)M * K * 4); dW.ensure((size_t)N * K * 4); dB.ensure((size_t)N * 4); dC.ensure((size_t)M * ldc * 4);
         CUDA_CHECK(cudaMemcpy(dA.p, A, (size_t)M * K * 4, cudaMemcpyHostToDevice));
@@ -1898,21 +1883,14 @@ int debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A, const 
             whi.ensure((size_t)N * K * 4); wlo.ensure((size_t)N * K * 4);
             l.w_hi = whi.as<float>(); l.w_lo = wlo.as<float>();
             split_into(nullptr, l.w, l.w_hi, l.w_lo, (uint64_t)N * K);
-        } else if (mode >= 3) {
-            whi.ensure((size_t)N * K * 2); wlo.ensure((size_t)N * K * 2);
-            l.w_h1 = whi.as<__half>(); l.w_h2 = wlo.as<__half>();
-            float mx = 0.f;
-            for (int64_t i = 0; i < (int64_t)N * K; ++i) mx = std::max(mx, std::fabs(W[i]));
-            int sexp = 0;
-            if (mx > 0.f) { int e; std::frexp(mx, &e); sexp = 14 - e; }
-            l.w_unscale = std::ldexp(1.0f, -sexp);
-            split_half_kernel<<<sm_count() * 8, 256>>>((int64_t)N * K, l.w, std::ldexp(1.0f, sexp), l.w_h1, l.w_h2, fake.err.as<int>() + 1);
-            CUDA_CHECK(cudaGetLastError());
+        } else {
+            Buf d_max;
+            whi.ensure((size_t)N * K * 2); wlo.ensure((size_t)N * K * 2); d_max.ensure(4);
+            split_lin_half(&fake, l, d_max.as<unsigned int>(), whi.as<__half>(), wlo.as<__half>());
         }
         fake.gemm_band = band;
         Act a{dA.as<float>()};
         Buf ah1, ah2;
-        struct RelA { Buf *x, *y; ~RelA() { x->release(); y->release(); } } rela{&ah1, &ah2};
         if (presplit && mode >= 3) {
             ah1.ensure((size_t)M * K * 2); ah2.ensure((size_t)M * K * 2);
             a.h1 = ah1.as<__half>(); a.h2 = ah2.as<__half>();
@@ -1922,7 +1900,6 @@ int debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A, const 
         const Act c{store ? dC.as<float>() : nullptr};
         Ctx cx{&fake, nullptr};
         Buf dmask, dstats;
-        struct RelH { Buf *x, *y; ~RelH() { x->release(); y->release(); } } relh{&dmask, &dstats};
         const int64_t m_pad = (M + GM - 1) / GM * GM;
         const int n_tiles = (N + GN - 1) / GN, mask_words = (N + 31) / 32;
         if (head) {
@@ -2034,10 +2011,8 @@ int sealdec_debug_select_step(const sealfm_t* fm, const sealdec_params_t* p, con
             if (!fm || sealfm_device(fm) < 0) throw ApiError(SEALFM_ENODEVICE, "FM index not on a device");
             CUDA_CHECK(cudaSetDevice(sealfm_device(fm)));
             view = sealfm_view(fm);
-        } else {
-            int count = 0;
-            if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) { cudaGetLastError(); throw ApiError(SEALFM_ENODEVICE, "no CUDA device available"); }
-        }
+        } else
+            require_device();
         const int64_t R = Q * B;
         for (int64_t r = 0; r < R; ++r) {
             if (lo[r] > hi[r] || (fm_on && hi[r] > view.m + 1)) throw ApiError(SEALFM_EINVAL, "SA range out of the index");
@@ -2047,8 +2022,8 @@ int sealdec_debug_select_step(const sealfm_t* fm, const sealdec_params_t* p, con
         const int ld = (V + 3) / 4 * 4, W = (V + 31) / 32, tiles = (V + GN - 1) / GN;
         const int64_t lrows = logits_shared ? Q : R;
 
-        std::vector<Buf> b(30);
-        struct Rel { std::vector<Buf>& v; ~Rel() { for (auto& x : v) x.release(); } } rel{b};
+        Buf d_lg, d_hs, d_mk, d_occ, d_sc, d_tk, d_an, d_lo, d_hi, d_pw, d_rmax, d_rls, d_rule, d_cval, d_cidx, d_ccnt, d_sco, d_tko,
+            d_ano, d_loo, d_hio, d_pwo, d_hsc, d_hlen, d_htk, d_hval, d_hlo, d_hhi, d_err, d_thr;
         auto up = [&](Buf& d, const void* h, size_t bytes) {
             d.ensure(bytes);
             if (h) CUDA_CHECK(cudaMemcpy(d.p, h, bytes, cudaMemcpyHostToDevice));
@@ -2056,11 +2031,6 @@ int sealdec_debug_select_step(const sealfm_t* fm, const sealdec_params_t* p, con
         };
         // outputs and scratch start as NaN / all-ones bits: a value read before it is written, or never written, shows
         auto poisoned = [&](Buf& d, size_t bytes) { d.ensure(bytes); CUDA_CHECK(cudaMemset(d.p, 0xFF, bytes)); };
-        Buf &d_lg = b[0], &d_hs = b[1], &d_mk = b[2], &d_occ = b[3], &d_sc = b[4], &d_tk = b[5], &d_an = b[6], &d_lo = b[7],
-            &d_hi = b[8], &d_pw = b[9], &d_rmax = b[10], &d_rls = b[11], &d_rule = b[12], &d_cval = b[13], &d_cidx = b[14],
-            &d_ccnt = b[15], &d_sco = b[16], &d_tko = b[17], &d_ano = b[18], &d_loo = b[19], &d_hio = b[20], &d_pwo = b[21],
-            &d_hsc = b[22], &d_hlen = b[23], &d_htk = b[24], &d_hval = b[25], &d_hlo = b[26], &d_hhi = b[27], &d_err = b[28],
-            &d_thr = b[29];
         poisoned(d_lg, (size_t)lrows * ld * 4);                 // the padding columns ld - V stay NaN
         if (!logits_ignored)
             CUDA_CHECK(cudaMemcpy2D(d_lg.p, (size_t)ld * 4, logits, (size_t)V * 4, (size_t)V * 4, lrows, cudaMemcpyHostToDevice));
@@ -2077,19 +2047,10 @@ int sealdec_debug_select_step(const sealfm_t* fm, const sealdec_params_t* p, con
         poisoned(d_hval, (size_t)Q * K); poisoned(d_hlo, (size_t)Q * K * 8); poisoned(d_hhi, (size_t)Q * K * 8);
         d_err.ensure(16); CUDA_CHECK(cudaMemset(d_err.p, 0, 16));
 
-        StepCfg c{};
-        c.num_beams = B; c.K = K; c.V = V; c.ld = ld; c.cur_len = cur_len;
-        c.min_length = p->min_length; c.max_length = p->max_length;
-        c.eos_token_id = p->eos_token_id; c.pad_token_id = p->pad_token_id; c.model_eos_token_id = p->model_eos_token_id;
-        c.forced_eos_token_id = p->forced_eos_token_id; c.forced_bos_token_id = p->forced_bos_token_id;
-        c.stop_at_count = p->stop_at_count; c.always_allow_eos = p->always_allow_eos; c.disable_fm_index = p->disable_fm_index;
-        c.remove_invalid_values = p->remove_invalid_values; c.shift = p->shift; c.T = T; c.mask_words = W;
-        c.first_step_shared_mask = shared_mask ? 1 : 0; c.expand_next = cur_len + 1 < T ? 1 : 0;
-        c.logits_shared = logits_shared ? 1 : 0; c.logits_ignored = logits_ignored ? 1 : 0;
+        StepCfg c = step_cfg(p, grp, V);
+        set_step(c, cur_len, logits_shared, logits_ignored);
         c.hyps_per_query = K; c.hyp_base = 0;                  // the step's 2B records of each query
-        c.num_groups = grp.num_beam_groups; c.diversity_penalty = grp.diversity_penalty;
         c.head_tiles = head_stats ? tiles : 0;
-        c.top_k = p->top_k < V ? p->top_k : 0;
         StepState st{};
         st.beam_scores_in = d_sc.as<float>(); st.beam_scores_out = d_sco.as<float>();
         st.tokens_in = d_tk.as<int32_t>(); st.tokens_out = d_tko.as<int32_t>();
@@ -2121,11 +2082,9 @@ int sealdec_debug_topk_rows(int64_t R, int32_t V, int32_t num_beams, int32_t per
     return guarded([&] {
         if (R <= 0 || V <= 0 || num_beams < 1 || num_beams > kSelMaxBeams || R % num_beams || per_row < 0 || iters <= 0 || !avg_us)
             throw ApiError(SEALFM_EINVAL, "bad argument");
-        int count = 0;
-        if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) { cudaGetLastError(); throw ApiError(SEALFM_ENODEVICE, "no CUDA device available"); }
+        require_device();
         const int ld = (V + 3) / 4 * 4, W = (V + 31) / 32, B = num_beams, K = 2 * B, T = 3;
         Buf lg, mk, sc, tk, pw, rmax, rls, rule, cval, cidx, ccnt;
-        struct Rel { std::vector<Buf*> v; ~Rel() { for (auto b : v) b->release(); } } rel{{&lg, &mk, &sc, &tk, &pw, &rmax, &rls, &rule, &cval, &cidx, &ccnt}};
         lg.ensure((size_t)R * ld * 4); mk.ensure((size_t)R * W * 4); sc.ensure((size_t)R * 4); tk.ensure((size_t)R * T * 4);
         pw.ensure((size_t)R * 8); rmax.ensure((size_t)R * 4); rls.ensure((size_t)R * 4); rule.ensure((size_t)R);
         cval.ensure((size_t)R * K * 4); cidx.ensure((size_t)R * K * 4); ccnt.ensure((size_t)R * 4);
@@ -2164,10 +2123,8 @@ int sealdec_debug_topk_threshold(int64_t R, int32_t V, int64_t ld, const float* 
         if (R <= 0 || V <= 0 || ld < V || !logits || top_k < 1 || !out_thr || !out_max || !out_logsum || (uint64_t)R > INT32_MAX)
             throw ApiError(SEALFM_EINVAL, "bad argument");
         if (V > kTopkMaxVocab) throw ApiError(SEALFM_EINVAL, "V must be <= " + std::to_string(kTopkMaxVocab));
-        int count = 0;
-        if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) { cudaGetLastError(); throw ApiError(SEALFM_ENODEVICE, "no CUDA device available"); }
+        require_device();
         Buf d_lg, d_thr;
-        struct Rel { std::vector<Buf*> v; ~Rel() { for (auto b : v) b->release(); } } rel{{&d_lg, &d_thr}};
         d_lg.ensure((size_t)R * ld * 4); d_thr.ensure((size_t)R * 3 * 4);
         CUDA_CHECK(cudaMemcpy(d_lg.p, logits, (size_t)R * ld * 4, cudaMemcpyHostToDevice));
         CUDA_CHECK(cudaMemset(d_thr.p, 0xFF, (size_t)R * 3 * 4));
@@ -2190,10 +2147,8 @@ int sealdec_debug_target_logprob(int64_t R, int32_t V, int64_t ld, const float* 
         if (out && (!targets || tgt_stride < 1 || out_stride < 1)) throw ApiError(SEALFM_EINVAL, "bad target / output stride");
         if (full && full_ld < V) throw ApiError(SEALFM_EINVAL, "full_ld must be >= V");
         if ((uint64_t)R > INT32_MAX) throw ApiError(SEALFM_EINVAL, "too many rows");
-        int count = 0;
-        if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) { cudaGetLastError(); throw ApiError(SEALFM_ENODEVICE, "no CUDA device available"); }
+        require_device();
         Buf d_lg, d_tg, d_out, d_full;
-        struct Rel { std::vector<Buf*> v; ~Rel() { for (auto b : v) b->release(); } } rel{{&d_lg, &d_tg, &d_out, &d_full}};
         const size_t n_out = out ? (size_t)(R - 1) * out_stride + 1 : 0;
         const size_t n_tg = out ? (size_t)(R - 1) * tgt_stride + 1 : 0;
         const size_t n_full = full ? (size_t)(R - 1) * full_ld + V : 0;
