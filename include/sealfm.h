@@ -48,9 +48,57 @@ int sealfm_build(const uint64_t* symbols, uint64_t n, sealfm_t** out);
 /* Same index as sealfm_build (identical sections, byte for byte), constructed on CUDA device `device`:
  * radix-sort prefix doubling -> BWT -> level-wise wavelet tree -> samples (replaces sdsl::construct_im's
  * qsufsort + wt_int construction, sdsl/construct.hpp:120-166, sdsl/wt_int.hpp:169-256).  n + 1 < 2^32 (32-bit
- * ranks) and ~40 bytes of free device memory per symbol (SEALFM_ENOMEM otherwise); larger texts: sealfm_build.
+ * ranks) and ~40 bytes of free device memory per symbol (SEALFM_ENOMEM otherwise); larger texts: sealfm_build_gpu_ex
+ * or sealfm_build.
  * SEALFM_ENODEVICE without a GPU. */
 int sealfm_build_gpu(const uint64_t* symbols, uint64_t n, int device, sealfm_t** out);
+
+/* Options of sealfm_build_gpu_ex; all-zero (or NULL) selects the defaults. */
+typedef struct {
+    uint64_t device_budget_bytes;   /* 0: free device memory minus 1 GiB                                         */
+    uint64_t chunk_elems;           /* 0: window size derived from the budget; > 0 forces it (at least 16)        */
+    int32_t  force_wide;            /* 1: 64-bit positions and labels even when m < 2^32                          */
+    int32_t  reserved[7];           /* must be 0                                                                  */
+} sealfm_build_opts_t;
+
+/* Same index as sealfm_build (identical sections), constructed on CUDA device `device` for texts of up to 2^40 - 2
+ * symbols.  symbols: n little-endian integers of `width_bytes` (4 or 8) each, all in [1, 2^32).
+ * Suffix sorting is in-place prefix doubling (Larsson-Sadakane labels): the inverse suffix array lives on the device
+ * (4 bytes per symbol while m = n + 1 < 2^32, else 8), the suffix array in pinned host memory (same width), and the
+ * groups still unsorted stream through a device window of chunk_elems entries (~(2w + 34) bytes each, w the position
+ * width, plus CUB scratch).  Groups larger than the window are split by key range in place.  Device memory per phase,
+ * t = 2 bytes per symbol when every symbol is < 2^16, else 4:
+ *   round 0 (sort by first symbol):  w*m + t*m + window
+ *   doubling rounds:                 w*m + window
+ *   BWT and samples:                 t*m + 4*m + window
+ *   wavelet tree:                    12*m + m*L/8   (the BWT, its sorted copy, CUB's alternate keys; L = bits of the largest symbol)
+ * Host: w*m pinned for the suffix array.  The largest phase must fit device_budget_bytes, else SEALFM_ENOMEM before any
+ * large allocation; a pinned allocation that fails is SEALFM_ENOMEM too.  SEALFM_EINVAL: symbol 0, symbols >= 2^32,
+ * m >= 2^40, a width other than 4 or 8, or nonzero reserved fields.  SEALFM_ENODEVICE without a GPU.
+ * *out stays NULL on every failure. */
+int sealfm_build_gpu_ex(const void* symbols, uint64_t n, int width_bytes, int device, const sealfm_build_opts_t* opts,
+                        sealfm_t** out);
+
+/* What the calling thread's last successful sealfm_build_gpu_ex did: window size, which paths ran, time per phase. */
+typedef struct {
+    uint64_t chunk_elems;           /* window size used                                                            */
+    uint64_t windows;               /* windows sorted, all rounds                                                  */
+    uint64_t max_windows_per_round;
+    uint64_t spanning_groups;       /* groups that crossed a window edge: the window was cut at their first row    */
+    uint64_t giant_groups;          /* groups larger than the window, split by key range                           */
+    uint64_t key_partitions;        /* in-place two-way partitions done by those splits                            */
+    uint64_t single_key_buckets;    /* key ranges larger than the window holding one key: relabelled, not sorted  */
+    uint64_t device_peak_bytes;     /* largest sum of the builder's device allocations                             */
+    uint64_t host_pinned_bytes;
+    uint32_t wide;                  /* 1: 64-bit positions                                                         */
+    uint32_t text_bytes;            /* bytes per symbol of the text on the device: 2 or 4                          */
+    uint32_t rounds;                /* sorting rounds, round 0 (first symbol) included                             */
+    uint32_t reserved;
+    double   phase_s[4];            /* round 0 | doubling rounds | BWT and samples | wavelet tree                   */
+    uint64_t round_unsorted[48];    /* rows in the unsorted ranges at the start of round r                          */
+    double   round_s[48];           /* wall time of round r                                                        */
+} sealfm_build_stats_t;
+int sealfm_build_gpu_ex_stats(sealfm_build_stats_t* out);
 /* Adopts index sections computed elsewhere -- exactly what sealfm_section() hands out of a built index: the
  * level-concatenated wavelet-tree bits of csa_wt_int<> (sdsl/wt_int.hpp:202-242; size * max_level bits in n_tree
  * words), the ascending alphabet (sigma symbols incl. the sentinel 0), the cumulative counts C (sigma + 1), SA[32 i]

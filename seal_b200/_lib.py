@@ -32,12 +32,28 @@ def _load():
 
 lib = _load()
 
+
+class BuildOpts(C.Structure):             # sealfm_build_opts_t
+    _fields_ = [("device_budget_bytes", C.c_uint64), ("chunk_elems", C.c_uint64), ("force_wide", C.c_int32),
+                ("reserved", C.c_int32 * 7)]
+
+
+class BuildStats(C.Structure):            # sealfm_build_stats_t
+    _fields_ = [("chunk_elems", C.c_uint64), ("windows", C.c_uint64), ("max_windows_per_round", C.c_uint64),
+                ("spanning_groups", C.c_uint64), ("giant_groups", C.c_uint64), ("key_partitions", C.c_uint64),
+                ("single_key_buckets", C.c_uint64), ("device_peak_bytes", C.c_uint64), ("host_pinned_bytes", C.c_uint64),
+                ("wide", C.c_uint32), ("text_bytes", C.c_uint32), ("rounds", C.c_uint32), ("reserved", C.c_uint32),
+                ("phase_s", C.c_double * 4), ("round_unsorted", C.c_uint64 * 48), ("round_s", C.c_double * 48)]
+
+
 # name -> (restype, argtypes); mirrors include/sealfm.h one to one
 _FM_SIGS = {
     "sealfm_last_error": (cp, []),
     "sealfm_abi_version": (i32, []),
     "sealfm_build": (i32, [vp, u64, C.POINTER(vp)]),
     "sealfm_build_gpu": (i32, [vp, u64, i32, C.POINTER(vp)]),
+    "sealfm_build_gpu_ex": (i32, [vp, u64, i32, i32, C.POINTER(BuildOpts), C.POINTER(vp)]),
+    "sealfm_build_gpu_ex_stats": (i32, [C.POINTER(BuildStats)]),
     "sealfm_save_sdsl": (i32, [vp, cp]),
     "sealfm_from_sections": (i32, [u64, u32, u64, vp, u64, vp, vp, vp, u64, vp, u64, C.POINTER(vp)]),
     "sealfm_build_from_file": (i32, [cp, i32, C.POINTER(vp)]),

@@ -19,6 +19,8 @@ from .._lib import lib, check, vp, u64
 
 __all__ = ["FMIndex", "load_FMIndex"]
 
+_ENOMEM = -3
+
 
 def _u64(a):
     return np.ascontiguousarray(np.asarray(a, dtype=np.uint64))
@@ -37,20 +39,52 @@ def _default_device():
     return 0
 
 
-def _build_on_gpu(n):
-    """Index construction runs on the GPU (sealfm_build_gpu) whenever one is visible, the text fits its 32-bit ranks
-    (n + 1 < 2^32) and ~40 bytes per symbol of device memory are free; SEALB200_BUILD=host selects the host SA-IS
-    builder (the only one without a GPU)."""
-    if os.environ.get("SEALB200_BUILD", "gpu") == "host" or n + 1 >= (1 << 32) - 8:
-        return False
-    try:
-        import torch
-        if not torch.cuda.is_available():
-            return False
-        free_b, _ = torch.cuda.mem_get_info(_default_device())
-        return (n + 1) * 42 + (1 << 30) <= free_b
-    except Exception:
-        return False
+def _large_device_bytes(m, max_symbol=(1 << 32) - 1):
+    """Device memory sealfm_build_gpu_ex needs for m = n + 1 symbols, by its largest phase (include/sealfm.h):
+    round 0 holds the ISA and the text, the BWT phase the text and the BWT, the wavelet-tree phase the BWT, its sorted
+    copy and CUB's alternate keys plus the tree bits; 2 GiB on top for the sorting window."""
+    w = 4 if m < (1 << 32) else 8
+    t = 2 if max_symbol < (1 << 16) else 4
+    L = max(int(max_symbol), 1).bit_length()
+    return max((w + t) * m, (t + 4) * m + m // 4, 12 * m + (m * L + 7) // 8) + (2 << 30)
+
+
+def _large_host_bytes(m):
+    """Pinned host memory of sealfm_build_gpu_ex: the suffix array, 4 bytes per row below 2^32 rows, else 8."""
+    return (4 if m < (1 << 32) else 8) * m
+
+
+def _choose_builder(n, free_dev, host_avail, switch, max_symbol=(1 << 32) - 1):
+    """Which builder constructs an index of n symbols: "gpu" (sealfm_build_gpu, in device memory, while n + 1 < 2^32
+    and ~40 bytes per symbol are free), else "gpu_large" (sealfm_build_gpu_ex, suffix array in pinned host memory) when
+    its device and host budgets fit, else "host" (SA-IS).  free_dev is None without a GPU.  switch is SEALB200_BUILD:
+    "host" and "gpu_large" force that builder.  max_symbol: the text's largest symbol (the worst case when unknown)."""
+    if switch == "host":
+        return "host"
+    if switch == "gpu_large":
+        return "gpu_large"
+    if free_dev is None:
+        return "host"
+    m = n + 1
+    if m < (1 << 32) - 8 and m * 42 + (1 << 30) <= free_dev:
+        return "gpu"
+    if m < (1 << 40) and _large_device_bytes(m, max_symbol) <= free_dev and _large_host_bytes(m) <= host_avail:
+        return "gpu_large"
+    return "host"
+
+
+def _builder(n, max_symbol=(1 << 32) - 1):
+    switch = os.environ.get("SEALB200_BUILD", "gpu")
+    host_avail = os.sysconf("SC_AVPHYS_PAGES") * os.sysconf("SC_PAGE_SIZE")
+    free_dev = None
+    if switch not in ("host", "gpu_large"):
+        try:
+            import torch
+            if torch.cuda.is_available():
+                free_dev, _ = torch.cuda.mem_get_info(_default_device())
+        except Exception:
+            free_dev = None
+    return _choose_builder(n, free_dev, host_avail, switch, max_symbol)
 
 
 class FMIndex:
@@ -103,15 +137,38 @@ class FMIndex:
     def initialize(self, data):                                   # fm_index.cpp:33-41
         a = _u64(data)
         out = vp()
-        if _build_on_gpu(len(a)):
+        how = _builder(len(a), int(a.max()) if len(a) else 1)
+        if how == "gpu":
             check(lib.sealfm_build_gpu(a.ctypes.data, len(a), _default_device(), C.byref(out)))
+        elif how == "gpu_large" and self._build_large(a, 8, out):
+            pass
         else:
             check(lib.sealfm_build(a.ctypes.data, len(a), C.byref(out)))
         self._adopt(out.value)
 
+    @staticmethod
+    def _build_large(a, width, out):
+        """sealfm_build_gpu_ex; False when it ran out of memory and the host builder should take over (only when the
+        streamed builder was picked by its estimate, not forced with SEALB200_BUILD=gpu_large)."""
+        rc = lib.sealfm_build_gpu_ex(a.ctypes.data, len(a), width, _default_device(), None, C.byref(out))
+        if rc == _ENOMEM and os.environ.get("SEALB200_BUILD") != "gpu_large":
+            return False
+        check(rc)
+        return True
+
     def initialize_from_file(self, file, width):                  # fm_index.cpp:43-48
-        if int(width) in (1, 2, 4, 8) and _build_on_gpu(os.path.getsize(file) // int(width)):
-            return FMIndex.initialize(self, np.fromfile(file, dtype=f"<u{int(width)}"))   # not a subclass override
+        w = int(width)
+        how = _builder(os.path.getsize(file) // w) if w in (1, 2, 4, 8) else "host"
+        if how == "gpu_large" and w in (4, 8):          # the file's own integers, not a u64 copy of them
+            a = np.fromfile(file, dtype=f"<u{w}")
+            if _builder(len(a), int(a.max()) if len(a) else 1) == "gpu_large":
+                out = vp()
+                if FMIndex._build_large(a, w, out):
+                    self._adopt(out.value)
+                    return
+            how = "host"
+        if how != "host":
+            return FMIndex.initialize(self, np.fromfile(file, dtype=f"<u{w}"))   # not a subclass override
         out = vp()
         check(lib.sealfm_build_from_file(os.fsencode(file), int(width), C.byref(out)))
         self._adopt(out.value)

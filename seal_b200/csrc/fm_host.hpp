@@ -7,6 +7,8 @@
 #include <string>
 #include <vector>
 
+#include "../../include/sealfm.h"
+
 namespace sealb200 {
 
 struct HostIndex {
@@ -27,6 +29,11 @@ void build_index(const uint64_t* symbols, uint64_t n, HostIndex& out);
 void build_index_from_file(const std::string& path, int width_bytes, HostIndex& out);
 // Same result as build_index, constructed on CUDA device `device` (fm_build.cu); n + 1 < 2^32 and 40 B x n of free device memory.
 void build_index_gpu(const uint64_t* symbols, uint64_t n, int device, HostIndex& out);
+// Same result for n + 1 < 2^40 with the suffix array in pinned host memory (fm_build_large.cu); symbols are
+// `width_bytes` (4 or 8) wide.  Throws ApiError (SEALFM_EINVAL / SEALFM_ENOMEM / SEALFM_ECUDA).
+void build_index_gpu_large(const void* symbols, uint64_t n, int width_bytes, int device, const sealfm_build_opts_t* opts,
+                           HostIndex& out);
+const sealfm_build_stats_t& build_gpu_large_last_stats();        // of the calling thread's last successful build
 void load_index(const std::string& path, HostIndex& out);        // sdsl .fmi or native, auto-detect
 void save_index_native(const HostIndex& idx, const std::string& path);
 // The byte stream sdsl::store_to_file(csa_wt_int<>) writes for this index: loads in the unmodified reference.

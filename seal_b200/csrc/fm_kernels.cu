@@ -461,7 +461,7 @@ FmView sealfm_view(const sealfm_t* h) {
 extern "C" {
 
 const char* sealfm_last_error(void) { return last_error().c_str(); }
-int sealfm_abi_version(void) { return 1; }
+int sealfm_abi_version(void) { return 2; }
 
 int sealfm_build(const uint64_t* symbols, uint64_t n, sealfm_t** out) {
     return guarded([&] {
@@ -482,6 +482,29 @@ int sealfm_build_gpu(const uint64_t* symbols, uint64_t n, int device, sealfm_t**
         std::unique_ptr<sealfm> h(new sealfm());
         build_index_gpu(symbols, n, device, h->host);
         *out = h.release();
+    });
+}
+int sealfm_build_gpu_ex(const void* symbols, uint64_t n, int width_bytes, int device, const sealfm_build_opts_t* opts,
+                        sealfm_t** out) {
+    return guarded([&] {
+        if (!out) throw ApiError(SEALFM_EINVAL, "null argument");
+        *out = nullptr;
+        if (!symbols && n) throw ApiError(SEALFM_EINVAL, "null argument");
+        if (width_bytes != 4 && width_bytes != 8) throw ApiError(SEALFM_EINVAL, "width must be 4 or 8 bytes");
+        int count = 0;
+        if (cudaGetDeviceCount(&count) != cudaSuccess || device < 0 || device >= count) {
+            cudaGetLastError();
+            throw ApiError(SEALFM_ENODEVICE, "no such CUDA device");
+        }
+        std::unique_ptr<sealfm> h(new sealfm());
+        build_index_gpu_large(symbols, n, width_bytes, device, opts, h->host);
+        *out = h.release();
+    });
+}
+int sealfm_build_gpu_ex_stats(sealfm_build_stats_t* out) {
+    return guarded([&] {
+        if (!out) throw ApiError(SEALFM_EINVAL, "null argument");
+        *out = build_gpu_large_last_stats();
     });
 }
 int sealfm_build_from_file(const char* path, int width_bytes, sealfm_t** out) {
