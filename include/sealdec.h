@@ -75,7 +75,8 @@ uint64_t sealbart_device_bytes(const sealbart_t* m);
 
 typedef struct {
     int32_t vocab_size;                      /* 32128 for the released t5 checkpoints                          */
-    int32_t d_model;                         /* multiple of 128, <= 1024 (t5-small 512, t5-base 768, t5-large 1024) */
+    int32_t d_model;                         /* a multiple of 128 up to 1024 (t5-small 512, t5-base 768, t5-large 1024),
+                                                or 2048, 3072 or 4096 (the XL / XXL members of T5 v1.1, Flan-T5, mT5) */
     int32_t num_layers;                      /* encoder blocks                                                 */
     int32_t num_decoder_layers;              /* decoder blocks (may differ from num_layers)                    */
     int32_t num_heads;                       /* num_heads * 64 == d_model                                      */
@@ -91,8 +92,8 @@ typedef struct {
 
 /* Creates a T5 model behind the same opaque handle: sealbart_set_tensor / sealbart_finalize / sealbart_free and every
  * entry point below take it and behave as documented for BART.  A shape the kernels do not cover is rejected with
- * SEALFM_EINVAL before any allocation (d_kv != 64, num_heads * 64 != d_model, d_model not a multiple of 128 or above
- * 1024, d_ff % 64 != 0, an unknown ffn_kind, a bucket count / max distance outside the ranges above).
+ * SEALFM_EINVAL before any allocation (d_kv != 64, num_heads * 64 != d_model, d_model neither a multiple of 128 up to
+ * 1024 nor a multiple of 1024 up to 4096, d_ff % 64 != 0, an unknown ffn_kind, a bucket count / max distance outside the ranges above).
  * sealbart_set_tensor takes HF T5ForConditionalGeneration state_dict keys: "shared.weight" (aliases
  * "encoder.embed_tokens.weight", "decoder.embed_tokens.weight"), "encoder.block.{i}.layer.0.SelfAttention.{q,k,v,o}.weight",
  * "encoder.block.{i}.layer.{0,1}.layer_norm.weight", "encoder.block.{i}.layer.1.DenseReluDense.{wi | wi_0, wi_1, wo}.weight",
@@ -251,8 +252,9 @@ int sealdec_generate_dx_ex(sealbart_t* model, const sealfm_t* fm, const uint32_t
  * and of the T5 forward (a T5 call also sets 6, 7, 10 .. 15 as above; 0 / 1 name its encoder packing):
  *  16 T5 encoder self-attention with the relative position bias
  *  17 T5 decoder self-attention with the relative position bias (one warp per row and head, any position)
- *  18 embedding / add + RMSNorm (one CTA per row; folds a pending split-K GEMM)
- *  19 ReLU feed-forward (ReLU GEMM epilogue)          20 gated-gelu feed-forward (gelu_new(wi_0 x) * wi_1 x kernel) */
+ *  18 embedding / add + RMSNorm (one CTA per row; folds a pending split-K GEMM), d_model <= 1024
+ *  19 ReLU feed-forward (ReLU GEMM epilogue)          20 gated-gelu feed-forward (gelu_new(wi_0 x) * wi_1 x kernel)
+ *  21 embedding / add + RMSNorm as 18, d_model 2048 .. 4096 ("t5_rms_wide"; such a model never sets 18) */
 int     sealbart_set_option(sealbart_t* model, const char* name, int64_t value);
 int64_t sealbart_get_stat(const sealbart_t* model, const char* name);
 

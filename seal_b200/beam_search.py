@@ -223,8 +223,9 @@ def t5_native_config(config, gemm_mode):
     if d_kv != 64 or heads * 64 != d:
         raise ValueError(f"T5 shape not covered: d_kv must be 64 and num_heads * 64 == d_model (d_kv={d_kv}, "
                          f"num_heads={heads}, d_model={d})")
-    if d % 128 or d > 1024:
-        raise ValueError(f"T5 shape not covered: d_model must be a multiple of 128 and <= 1024 (d_model={d})")
+    if not (d > 0 and d % 128 == 0 and d <= 1024) and not (d > 0 and d % 1024 == 0 and d <= 4096):
+        raise ValueError(f"T5 shape not covered: d_model must be a multiple of 128 up to 1 024, or a multiple of 1 024 "
+                         f"up to 4 096 (d_model={d})")
     if d_ff % 64:
         raise ValueError(f"T5 shape not covered: d_ff must be a multiple of 64 (d_ff={d_ff})")
     nb = int(config.relative_attention_num_buckets)

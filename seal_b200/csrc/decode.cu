@@ -284,6 +284,7 @@ enum : uint32_t {
     kPathSplitKDeferred = 1u << 10, kPathSplitKFinish = 1u << 11, kPathGemmFullTile = 1u << 12, kPathGemmCluster = 1u << 13,
     kPathGemmTf32 = 1u << 14, kPathQuerySlices = 1u << 15,
     kPathT5EncAttn = 1u << 16, kPathT5DecAttn = 1u << 17, kPathT5Rms = 1u << 18, kPathT5Relu = 1u << 19, kPathT5Gate = 1u << 20,
+    kPathT5RmsWide = 1u << 21,
 };
 
 void split_into(cudaStream_t s, const float* x, float* hi, float* lo, uint64_t numel) {
@@ -590,10 +591,11 @@ void t5_rms(Ctx& cx, int64_t rows, int d, const int32_t* tok, int64_t tok_stride
             float out_scale) {
     const SplitSrc ps = cx.pending;
     cx.pending = SplitSrc{};
-    launch_k(t5_rms_row_kernel, (unsigned)rows, 128, 0, cx.s, rows, d, tok, tok_stride, (const float*)cx.m->shared, x.x, b, ps, w,
-             cx.m->t5.layer_norm_epsilon, out_scale, split_of(x, cx.m->ovf));
+    const bool wide = d > 4 * 128 * kT5RmsVec;
+    launch_k(wide ? t5_rms_row_kernel<kT5RmsVecWide> : t5_rms_row_kernel<kT5RmsVec>, (unsigned)rows, 128, 0, cx.s, rows, d, tok, tok_stride,
+             (const float*)cx.m->shared, x.x, b, ps, w, cx.m->t5.layer_norm_epsilon, out_scale, split_of(x, cx.m->ovf));
     cx.m->launches++;
-    cx.m->last_paths |= kPathT5Rms;
+    cx.m->last_paths |= wide ? kPathT5RmsWide : kPathT5Rms;
 }
 
 // wi (ReLU epilogue) or [wi_0; wi_1] + gate, then wo into tmp (split-K slices left to the next t5_rms)
@@ -968,7 +970,12 @@ void check_gemm_mode(int mode) {
 void check_t5_config(const sealt5_config_t* c) {
     if (c->d_kv != kHeadDim || c->num_heads * kHeadDim != c->d_model)
         throw ApiError(SEALFM_EINVAL, "T5: d_kv must be 64 and num_heads * 64 == d_model");
-    if (c->d_model % 128 || c->d_model <= 0 || c->d_model > 1024) throw ApiError(SEALFM_EINVAL, "T5: d_model must be a multiple of 128, <= 1024");
+    // the two t5_rms_row_kernel instantiations: 128 threads x 2 float4 up to 1 024; x 8 float4 at the XL / XXL widths
+    // 2 048, 3 072 and 4 096 (the widths in between have no checkpoint with 64-wide heads and are not tested)
+    const bool narrow = c->d_model > 0 && c->d_model % 128 == 0 && c->d_model <= 1024;
+    const bool wide = c->d_model > 0 && c->d_model % 1024 == 0 && c->d_model <= 4096;
+    if (!narrow && !wide)
+        throw ApiError(SEALFM_EINVAL, "T5: d_model must be a multiple of 128 up to 1 024, or a multiple of 1 024 up to 4 096");
     if (c->d_ff <= 0 || c->d_ff % 64) throw ApiError(SEALFM_EINVAL, "T5: d_ff must be a positive multiple of 64");
     if (c->vocab_size <= 0 || c->num_layers < 1 || c->num_decoder_layers < 1) throw ApiError(SEALFM_EINVAL, "T5: bad vocab_size / layer counts");
     if (c->ffn_kind != 0 && c->ffn_kind != 1) throw ApiError(SEALFM_EINVAL, "T5: ffn_kind must be 0 (relu) or 1 (gated-gelu)");

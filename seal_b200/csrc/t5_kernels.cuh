@@ -15,13 +15,16 @@ namespace sealb200 {
 // The longest source the T5 path takes: the encoder bucket table covers distances -(kT5MaxSource-1) .. kT5MaxSource-1.
 constexpr int kT5MaxSource = 1024;
 
-// One CTA of 128 threads per row, d = 4 * n4 <= 1024:
+// One CTA of 128 threads per row, d = 4 * n4 <= 512 * NV (each thread holds NV float4 of the row):
 //   v = embed[tok[r * tok_stride]]            (tok != nullptr: the embedding; T5 does not scale it)
 //   v = x[r] + b[r]                           (otherwise: residual + sub-layer output; b may still be an unsummed
 //                                              split-K GEMM output, bsrc, summed here like add_ln_row_kernel does)
 // then x[r] = v (the fp32 residual stream) and the operand of the next GEMM, written in split form only:
 //   out = (w * (v * rsqrt(mean(v^2) + eps))) * out_scale
 // in HF T5LayerNorm's order; out_scale is the decoder's d_model^-0.5 after its final_layer_norm, else 1.
+// Instantiated for NV = kT5RmsVec (d <= 1024) and kT5RmsVecWide (d <= 4096, the XL / XXL widths).
+constexpr int kT5RmsVec = 2, kT5RmsVecWide = 8;
+template <int NV>
 __global__ void __launch_bounds__(128) t5_rms_row_kernel(int64_t rows, int d, const int32_t* __restrict__ tok, int64_t tok_stride,
                                                          const float* __restrict__ embed, float* __restrict__ x,
                                                          const float* __restrict__ b, SplitSrc bsrc,
@@ -31,20 +34,25 @@ __global__ void __launch_bounds__(128) t5_rms_row_kernel(int64_t rows, int d, co
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int n4 = d / 4;
     const float* src = tok ? embed + (int64_t)tok[r * tok_stride] * d : nullptr;
-    float4 v[2];
+    // The wide form moves the row into the x / b / split-K slice pointers (base): indexed by r * d + 4 * c4 in each of
+    // its 8 slice loops, ptxas keeps the offset's high word in local memory.  The narrow form keeps base = 0.
+    const int64_t base = NV == kT5RmsVec ? 0 : r * d, off = r * d - base;
+    SplitSrc bs = bsrc;
+    if (bs.ks > 1) bs.part += base;
+    float4 v[NV];
     float s = 0.f;
 #pragma unroll
-    for (int i = 0; i < 2; ++i) {
+    for (int i = 0; i < NV; ++i) {
         const int c4 = tid + i * 128;
         v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
         if (c4 < n4) {
             if (src) v[i] = *reinterpret_cast<const float4*>(src + 4 * c4);
             else {
-                const float4 a = *reinterpret_cast<const float4*>(x + r * d + 4 * c4);
-                const float4 y = load_split4(b, bsrc, r * d + 4 * c4, 4 * c4);
+                const float4 a = *reinterpret_cast<const float4*>(x + base + off + 4 * c4);
+                const float4 y = load_split4(b + base, bs, off + 4 * c4, 4 * c4);
                 v[i] = make_float4(a.x + y.x, a.y + y.y, a.z + y.z, a.w + y.w);
             }
-            *reinterpret_cast<float4*>(x + r * d + 4 * c4) = v[i];
+            *reinterpret_cast<float4*>(x + base + off + 4 * c4) = v[i];
             s += (v[i].x * v[i].x + v[i].y * v[i].y) + (v[i].z * v[i].z + v[i].w * v[i].w);
         }
     }
@@ -53,7 +61,7 @@ __global__ void __launch_bounds__(128) t5_rms_row_kernel(int64_t rows, int d, co
     __syncthreads();
     const float rs = rsqrtf(((red[0] + red[1]) + (red[2] + red[3])) / (float)d + eps);
 #pragma unroll
-    for (int i = 0; i < 2; ++i) {
+    for (int i = 0; i < NV; ++i) {
         const int c4 = tid + i * 128;
         if (c4 < n4) {
             const float4 g = *reinterpret_cast<const float4*>(w + 4 * c4);

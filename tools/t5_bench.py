@@ -1,6 +1,8 @@
 """T5 backbones on the benchmark workload: bench.py's corpus (10 M-token index) and queries, beam 15, body n-grams of 10
 (9 decode steps), on random-init T5 models of the t5-base and t5-large shapes (relu feed-forward, tied lm_head with
-the d_model^-0.5 output scale; vocabulary = the corpus's 50 265 ids so that every query and index token is in range).
+the d_model^-0.5 output scale) and of the T5 v1.1 / Flan-T5 XL shape (`--models t5-xl`: d_model 2 048, gated-gelu,
+untied lm_head); vocabulary = the corpus's 50 265 ids so that every query and index token is in range.  The
+fp16-overflow count reflects random weights only.
 
 Per model and batch: queries/s and ms per generate (CUDA events around `--steps` calls on the decode stream, after
 `--warmup` calls; at Q = 20 these replay the call's CUDA graph), the phase split of one more, eager call
@@ -24,14 +26,17 @@ from bench import BEAM, LP, MAX_LEN, MIN_LEN, ClockSampler, build_inputs  # noqa
 from diverse_bench import gpu_info  # noqa: E402
 
 SHAPES = {"t5-base": dict(d_model=768, num_heads=12, d_ff=3072, num_layers=12, num_decoder_layers=12),
-          "t5-large": dict(d_model=1024, num_heads=16, d_ff=4096, num_layers=24, num_decoder_layers=24)}
+          "t5-large": dict(d_model=1024, num_heads=16, d_ff=4096, num_layers=24, num_decoder_layers=24),
+          # the XL member of T5 v1.1 / Flan-T5: ~2.9e9 parameters with this vocabulary, ~23 GB of device weights
+          "t5-xl": dict(d_model=2048, num_heads=32, d_ff=5120, num_layers=24, num_decoder_layers=24,
+                        feed_forward_proj="gated-gelu", tie_word_embeddings=False)}
 
 
 def make_t5(name, vocab):
     import torch
     from transformers import T5Config, T5ForConditionalGeneration
-    cfg = T5Config(vocab_size=vocab, d_kv=64, feed_forward_proj="relu", tie_word_embeddings=True, dropout_rate=0.0,
-                   **SHAPES[name])
+    shape = dict(dict(feed_forward_proj="relu", tie_word_embeddings=True), **SHAPES[name])
+    cfg = T5Config(vocab_size=vocab, d_kv=64, dropout_rate=0.0, **shape)
     torch.manual_seed(0)
     return T5ForConditionalGeneration(cfg).eval().float()
 
