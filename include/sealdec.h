@@ -139,10 +139,11 @@ typedef struct {
  * fill-in pick (a masked candidate, SURVEY.md H4) records -inf when its logit is below tau.  The forcing steps (forced
  * BOS, forced EOS) overwrite every score and are unaffected.  top_k >= V is no warp at all and takes the top_k = 0 path
  * (bit-identical records).  A top_k > 0 step stores the lm_head's logits densely (no statistics epilogue) and runs one
- * more kernel per step whose logits are read.  SEALFM_EINVAL for top_k < 0, for top_k > 0 with num_beam_groups > 1
- * (group_beam_search has no warper) and for top_k > 0 with vocab_size > 53 248 (the row is staged in shared memory;
- * bart-large's 50 265 fits).  The member sits in the struct's former tail padding: a caller that zero-initialises the
- * struct keeps the previous behaviour. */
+ * more kernel per step whose logits are read: one CTA per logits row for vocab_size <= 53 248 (bart-large's 50 265),
+ * one cluster of ceil(vocab_size / 53 248) CTAs per row above (mT5's 250 112: 5).  SEALFM_EINVAL for top_k < 0, for
+ * top_k > 0 with num_beam_groups > 1 (group_beam_search has no warper) and for top_k > 0 with vocab_size > 425 984
+ * (the row is staged in the shared memory of at most 8 CTAs).  The member sits in the struct's former tail padding: a
+ * caller that zero-initialises the struct keeps the previous behaviour. */
 
 /* Number of hypothesis records per query that sealdec_generate writes:
  * (max_length-1) * 2*num_beams + num_beams   (process :662-668 every step + finalize :717-725). */
@@ -238,7 +239,9 @@ int sealdec_generate_dx_ex(sealbart_t* model, const sealfm_t* fm, const uint32_t
  * owns, forked and joined with events on the caller's stream, so a CUDA graph captures both -- with bit-identical
  * records; never while GEMM profiling is on).  Stats: "last_used_graph",
  * "overflow_fallbacks", "gemm_mode", "cached_graphs", "fused_head_steps" (decode steps of the last generate run
- * eagerly that used the statistics epilogue), "last_paths" (-1 for an unknown name).
+ * eagerly that used the statistics epilogue), "topk_cluster_steps" (decode steps of the last generate whose top-k
+ * threshold ran one cluster per logits row, vocab_size > 53 248; a CUDA-graph replay reports the captured call's
+ * count), "last_paths" (-1 for an unknown name).
  * "last_paths" is the OR, over the last generate / teacher-forced / debug-step call (a CUDA-graph replay reports
  * the call it was captured from), of one bit per kernel branch of the BART forward:
  *   0 encoder on the real tokens only (packed)         1 encoder on the padded rows (mask per key)
@@ -358,6 +361,12 @@ int sealdec_debug_target_logprob(int64_t R, int32_t V, int64_t ld, const float* 
  * out_max = the row max, out_logsum = log(sum over x >= tau of exp(x - max)). */
 int sealdec_debug_topk_threshold(int64_t R, int32_t V, int64_t ld, const float* logits, int32_t top_k, float* out_thr,
                                  float* out_max, float* out_logsum);
+/* The same outputs from the threshold kernel the generate runs above V = 53 248: one cluster of ceil(V / 53 248) CTAs
+ * per row, each staging a contiguous slice of the row, with histograms merged over distributed shared memory.  Any
+ * 1 <= V <= 425 984 (so it can be checked at small V too); other arguments as above.  out_logsum is summed in a fixed
+ * order: per CTA as the one-CTA kernel sums a row, then the CTA sums in rank order (decode_kernels.cuh). */
+int sealdec_debug_topk_threshold_cluster(int64_t R, int32_t V, int64_t ld, const float* logits, int32_t top_k,
+                                         float* out_thr, float* out_max, float* out_logsum);
 /* average device time of the decoder's per-row statistics + top-2*beam kernel over R rows of V pseudo-random logits
  * (a later step of constrained beam search, per_row allowed tokens per row) */
 int sealdec_debug_topk_rows(int64_t R, int32_t V, int32_t num_beams, int32_t per_row, int32_t iters, double* avg_us);

@@ -101,6 +101,7 @@ struct sealbart {
     int fused_head = -1;              // -1 $SEALB200_FUSED_HEAD (default on), 0 dense lm_head logits, 1 statistics epilogue
     bool poison_logits = false;
     int fused_head_steps = 0;         // steps of the last enqueued generate whose lm_head used the statistics epilogue       // testing: the logits buffer is filled with NaN before every statistics-epilogue head
+    int topk_cluster_steps = 0;       // steps of the last generate whose top-k threshold ran topk_threshold_cluster_kernel
     int gemm_band = -1;               // sealdec_debug_gemm_ex: -1 tile order chosen by gemm_impl, 0 no bands, > 0 band size
     std::vector<std::pair<cudaEvent_t, cudaEvent_t>> gemm_events;
     double gemm_flops = 0;
@@ -108,7 +109,8 @@ struct sealbart {
     // host-buffer entry point: persistent device staging of the inputs (stable addresses -> CUDA graph reuse)
     Buf in_ids, in_mask, in_occ;
     // CUDA graphs of whole generate calls (small batches are launch-latency-bound: ~1 900 kernels per generate)
-    struct GraphEntry { std::vector<uint8_t> key; uint64_t epoch = 0; cudaGraphExec_t exec = nullptr; int64_t launches = 0; uint32_t paths = 0; uint64_t stamp = 0; };
+    struct GraphEntry { std::vector<uint8_t> key; uint64_t epoch = 0; cudaGraphExec_t exec = nullptr; int64_t launches = 0; uint32_t paths = 0; uint64_t stamp = 0;
+                        int topk_cluster_steps = 0; };
     std::vector<GraphEntry> graphs;
     std::vector<std::vector<uint8_t>> seen_keys;     // shapes run once already (their buffers are sized): capture next time
     uint64_t graph_stamp = 0;
@@ -1137,11 +1139,29 @@ void set_select_smem() {
     CUDA_CHECK(cudaFuncSetAttribute(topk_rows_kernel<512, 8192>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SelSharedT<8192>)));
     CUDA_CHECK(cudaFuncSetAttribute(topk_rows_kernel<256, 4096>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SelSharedT<4096>)));
     CUDA_CHECK(cudaFuncSetAttribute(topk_threshold_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTopkMaxVocab * 4));
+    CUDA_CHECK(cudaFuncSetAttribute(topk_threshold_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTopkMaxVocab * 4));
 }
 
-// (max, log sum exp over x >= tau, tau) of `rows` logits rows of V <= kTopkMaxVocab values at stride ld into row_thr[rows][3]
-// (set_select_smem() first): the generate's top-k steps and sealdec_debug_topk_threshold
+// topk_threshold_cluster_kernel on `rows` rows of 1 <= V <= kTopkClusterMaxVocab values: one cluster of
+// topk_cluster_ctas(V) CTAs per row (set_select_smem() first)
+void launch_topk_threshold_cluster(cudaStream_t s, int64_t rows, int V, int64_t ld, const float* logits, int top_k, float* row_thr) {
+    const int n = topk_cluster_ctas(V);
+    if (rows * n > INT32_MAX) throw ApiError(SEALFM_EINVAL, "too many logits rows for one top-k threshold launch");
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = (unsigned)n; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3((unsigned)(rows * n)); cfg.blockDim = dim3(kTopkThreads);
+    cfg.dynamicSmemBytes = (size_t)topk_cluster_chunk(V) * 4; cfg.stream = s;
+    cfg.attrs = attr; cfg.numAttrs = 1;
+    CUDA_CHECK(cudaLaunchKernelEx(&cfg, topk_threshold_cluster_kernel, V, ld, logits, top_k, row_thr));
+}
+
+// (max, log sum exp over x >= tau, tau) of `rows` logits rows of V values at stride ld into row_thr[rows][3]
+// (set_select_smem() first): one CTA per row up to kTopkMaxVocab, one cluster per row above.  The generate's top-k steps
+// and sealdec_debug_topk_threshold.
 void launch_topk_threshold(cudaStream_t s, int64_t rows, int V, int64_t ld, const float* logits, int top_k, float* row_thr) {
+    if (V > kTopkMaxVocab) { launch_topk_threshold_cluster(s, rows, V, ld, logits, top_k, row_thr); return; }
     launch_k(topk_threshold_kernel, (unsigned)rows, kTopkThreads, (size_t)V * 4, s, V, ld, logits, top_k, row_thr);
 }
 
@@ -1212,6 +1232,7 @@ void generate_enqueue(Ctx& cx, const Dims& D, const GenArgs& a, const FmView& vi
     };
     CUDA_CHECK(cudaMemsetAsync(a.err_d, 0, 16, cx.s));
     m->fused_head_steps = 0;
+    m->topk_cluster_steps = 0;
     mark();
     encoder_forward(cx, D, a.ids_d, a.mask_d, src_hint, a.err_d + 2);
     mark();
@@ -1326,6 +1347,7 @@ void generate_enqueue(Ctx& cx, const Dims& D, const GenArgs& a, const FmView& vi
                             m->st_thr.as<float>() + (cs.logits_shared ? q0 : r0) * 3};
         launch_select_step(pc.s, view, cs, st, rs, PD.Q);
         m->launches += topk_warp_step(cs) ? 3 : 2;
+        if (timed && topk_warp_step(cs) && cs.V > kTopkMaxVocab) m->topk_cluster_steps++;
         if (cs.expand_next && !p->disable_fm_index) {          // successor sets of the new beams -> next step's masks (:107)
             launch_expand_masks(view, pc.s, (uint64_t)PD.R, lo[cur ^ 1] + r0, hi[cur ^ 1] + r0, mk[cur ^ 1] + r0 * D.W, (uint32_t)D.W,
                                 (uint32_t)D.V, (uint32_t)p->shift, wide);
@@ -1397,12 +1419,13 @@ sealdec_groups_t checked_groups(const sealdec_groups_t* g, int num_beams) {
 }
 
 // top_k: 0 = off, > 0 TopKLogitsWarper(top_k) on every step's logits -- only on the single-group path (group_beam_search
-// has no warper, seal/beam_search.py:523-532) and for rows that fit topk_threshold_kernel's shared memory.
+// has no warper, seal/beam_search.py:523-532) and for rows that fit the shared memory of one cluster of
+// topk_threshold_cluster_kernel.
 void check_top_k(int32_t top_k, const sealdec_groups_t& grp, int V) {
     if (top_k < 0) throw ApiError(SEALFM_EINVAL, "top_k must be >= 0 (0 = off)");
     if (top_k > 0 && grp.num_beam_groups > 1) throw ApiError(SEALFM_EINVAL, "top_k > 0 needs num_beam_groups == 1");
-    if (top_k > 0 && V > kTopkMaxVocab)
-        throw ApiError(SEALFM_EINVAL, "top_k > 0 needs vocab_size <= " + std::to_string(kTopkMaxVocab));
+    if (top_k > 0 && V > kTopkClusterMaxVocab)
+        throw ApiError(SEALFM_EINVAL, "top_k > 0 needs vocab_size <= " + std::to_string(kTopkClusterMaxVocab));
 }
 
 void drop_graphs(sealbart* m) {
@@ -1532,6 +1555,7 @@ int sealdec_generate_dx_ex(sealbart_t* m, const sealfm_t* fm, const uint32_t* oc
             if (g.key == key) {
                 CUDA_CHECK(cudaGraphLaunch(g.exec, cx.s));
                 g.stamp = ++m->graph_stamp; m->launches = g.launches; m->last_paths = g.paths; m->last_used_graph = 1;
+                m->topk_cluster_steps = g.topk_cluster_steps;
                 return;
             }
         bool seen = false;
@@ -1575,6 +1599,7 @@ int sealdec_generate_dx_ex(sealbart_t* m, const sealfm_t* fm, const uint32_t* oc
             m->graphs.erase(m->graphs.begin() + victim);
         }
         sealbart::GraphEntry ge; ge.key = std::move(key); ge.epoch = g_ws_epoch; ge.exec = exec; ge.launches = m->launches; ge.paths = m->last_paths; ge.stamp = ++m->graph_stamp;
+        ge.topk_cluster_steps = m->topk_cluster_steps;
         m->graphs.push_back(std::move(ge));
         CUDA_CHECK(cudaGraphLaunch(exec, cx.s));
         m->last_used_graph = 1;
@@ -1631,6 +1656,7 @@ int64_t sealbart_get_stat(const sealbart_t* m, const char* name) {
     if (n == "gemm_mode") return m->cfg.gemm_mode;
     if (n == "cached_graphs") return (int64_t)m->graphs.size();
     if (n == "fused_head_steps") return m->fused_head_steps;
+    if (n == "topk_cluster_steps") return m->topk_cluster_steps;
     if (n == "last_paths") return m->last_paths;
     return -1;
 }
@@ -2124,24 +2150,46 @@ int sealdec_debug_topk_rows(int64_t R, int32_t V, int32_t num_beams, int32_t per
     });
 }
 
-int sealdec_debug_topk_threshold(int64_t R, int32_t V, int64_t ld, const float* logits, int32_t top_k, float* out_thr,
-                                 float* out_max, float* out_logsum) {
+}  // extern "C"
+
+namespace {
+
+// sealdec_debug_topk_threshold (cluster = false: V <= kTopkMaxVocab, the generate's dispatch) and
+// sealdec_debug_topk_threshold_cluster (cluster = true: topk_threshold_cluster_kernel for V <= kTopkClusterMaxVocab)
+int debug_topk_threshold(bool cluster, int64_t R, int32_t V, int64_t ld, const float* logits, int32_t top_k, float* out_thr,
+                         float* out_max, float* out_logsum) {
     return guarded([&] {
         if (R <= 0 || V <= 0 || ld < V || !logits || top_k < 1 || !out_thr || !out_max || !out_logsum || (uint64_t)R > INT32_MAX)
             throw ApiError(SEALFM_EINVAL, "bad argument");
-        if (V > kTopkMaxVocab) throw ApiError(SEALFM_EINVAL, "V must be <= " + std::to_string(kTopkMaxVocab));
+        const int max_v = cluster ? kTopkClusterMaxVocab : kTopkMaxVocab;
+        if (V > max_v) throw ApiError(SEALFM_EINVAL, "V must be <= " + std::to_string(max_v));
         require_device();
         Buf d_lg, d_thr;
         d_lg.ensure((size_t)R * ld * 4); d_thr.ensure((size_t)R * 3 * 4);
         CUDA_CHECK(cudaMemcpy(d_lg.p, logits, (size_t)R * ld * 4, cudaMemcpyHostToDevice));
         CUDA_CHECK(cudaMemset(d_thr.p, 0xFF, (size_t)R * 3 * 4));
         set_select_smem();
-        launch_topk_threshold(nullptr, R, V, ld, d_lg.as<float>(), top_k, d_thr.as<float>());
+        if (cluster) launch_topk_threshold_cluster(nullptr, R, V, ld, d_lg.as<float>(), top_k, d_thr.as<float>());
+        else launch_topk_threshold(nullptr, R, V, ld, d_lg.as<float>(), top_k, d_thr.as<float>());
         CUDA_CHECK(cudaDeviceSynchronize());
         std::vector<float> h((size_t)R * 3);
         CUDA_CHECK(cudaMemcpy(h.data(), d_thr.p, h.size() * 4, cudaMemcpyDeviceToHost));
         for (int64_t r = 0; r < R; ++r) { out_max[r] = h[r * 3]; out_logsum[r] = h[r * 3 + 1]; out_thr[r] = h[r * 3 + 2]; }
     });
+}
+
+}  // namespace
+
+extern "C" {
+
+int sealdec_debug_topk_threshold(int64_t R, int32_t V, int64_t ld, const float* logits, int32_t top_k, float* out_thr,
+                                 float* out_max, float* out_logsum) {
+    return debug_topk_threshold(false, R, V, ld, logits, top_k, out_thr, out_max, out_logsum);
+}
+
+int sealdec_debug_topk_threshold_cluster(int64_t R, int32_t V, int64_t ld, const float* logits, int32_t top_k,
+                                         float* out_thr, float* out_max, float* out_logsum) {
+    return debug_topk_threshold(true, R, V, ld, logits, top_k, out_thr, out_max, out_logsum);
 }
 
 int sealdec_debug_target_logprob(int64_t R, int32_t V, int64_t ld, const float* logits, const int64_t* targets,

@@ -8,6 +8,7 @@
 #include "fm_device.cuh"
 #include "launch.cuh"
 
+#include <cooperative_groups.h>
 #include <cfloat>
 #include <cstdint>
 
@@ -165,7 +166,8 @@ struct RowScratch {
     float* row_max; float* row_logsum; uint8_t* row_rule;     // [R]  log-softmax statistics / index rule of every row
     float* cand_val; int32_t* cand_idx; int32_t* cand_cnt;    // [Q * lists][K] sorted best candidates per candidate list, [Q * lists]
     float* row_thr;                                           // [logits rows][3] (max, log sum exp over x >= tau, tau) of the
-                                                              // top-k warp (topk_threshold_kernel); read on topk_warp_step only
+                                                              // top-k warp (topk_threshold_kernel, or topk_threshold_cluster_kernel
+                                                              // above kTopkMaxVocab); read on topk_warp_step only
 };
 
 // ---- top-k warp (transformers' TopKLogitsWarper before log_softmax, seal/beam_search.py:249-253) ----------------------
@@ -299,6 +301,162 @@ __global__ void __launch_bounds__(kTopkThreads, 1) topk_threshold_kernel(int V, 
         float* o = row_thr + (int64_t)blockIdx.x * 3;
         o[0] = mx; o[1] = logf(se); o[2] = key_float(tau_key);
     }
+}
+
+// Rows of V > kTopkMaxVocab (mT5: 250 112): one cluster of n = ceil(V / kTopkMaxVocab) CTAs per logits row, n <= 8 (the
+// portable cluster size), so V <= kTopkClusterMaxVocab.  It returns what topk_threshold_kernel returns.  CTA `rank`
+// stages the contiguous slice [rank * chunk, min(V, (rank + 1) * chunk)) of the row, chunk = ceil(V / n) rounded up to
+// a multiple of 4 (<= kTopkMaxVocab), as the same keys in its own shared memory; the row is read from HBM once.  Each
+// radix pass sums the CTA's warp histograms into tot[pass & 1], and after a cluster barrier every CTA adds the n totals
+// over DSMEM and takes the same digit decision from the same integer counts, so no broadcast is needed.  tot is double
+// buffered: a CTA overwrites tot[b] two passes after it was read, and every CTA finished that read before the barrier in
+// between.  The max is the largest of the n per-CTA maxima.
+// Summation order of log sum (fixed, independent of scheduling): each CTA sums its slice as topk_threshold_kernel sums
+// a row (per thread strided over ceil(len / 512) keys, the warp's 5-level shuffle tree, the 16 warps in order), then
+// rank 0 adds the n CTA sums in rank order, ((s_0 + s_1) + s_2) + ...: at most ceil(chunk / 512) + 5 + 16 + (n - 1)
+// additions on any term's path.
+constexpr int kTopkClusterMax = 8;
+constexpr int kTopkClusterMaxVocab = kTopkClusterMax * kTopkMaxVocab;   // 425 984
+
+__host__ __device__ __forceinline__ int topk_cluster_ctas(int V) { return (V + kTopkMaxVocab - 1) / kTopkMaxVocab; }
+__host__ __device__ __forceinline__ int topk_cluster_chunk(int V) {
+    const int n = topk_cluster_ctas(V);
+    return ((V + n - 1) / n + 3) / 4 * 4;
+}
+
+__global__ void __launch_bounds__(kTopkThreads, 1) topk_threshold_cluster_kernel(int V, int64_t ld,
+                                                                                 const float* __restrict__ logits,
+                                                                                 int top_k, float* __restrict__ row_thr) {
+    namespace cg = cooperative_groups;
+    extern __shared__ __align__(16) uint32_t keys[];
+    __shared__ uint32_t hist[kTopkWarps][256];
+    __shared__ uint32_t tot[2][256];
+    __shared__ uint32_t s_max[kTopkWarps];
+    __shared__ float red[32];
+    __shared__ uint32_t s_prefix, s_rem, s_cta_max;
+    __shared__ float s_se;
+    cg::cluster_group cluster = cg::this_cluster();
+    const int n = (int)cluster.num_blocks(), rank = (int)cluster.block_rank();
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int chunk = topk_cluster_chunk(V);
+    const int v_begin = rank * chunk < V ? rank * chunk : V;
+    const int len = (v_begin + chunk < V ? v_begin + chunk : V) - v_begin;
+    const float* lp = logits + (int64_t)(blockIdx.x / n) * ld + v_begin;
+    const int k = top_k < 1 ? 1 : (top_k > V ? V : top_k);
+    for (int i = tid; i < kTopkWarps * 256; i += kTopkThreads) (&hist[0][0])[i] = 0u;
+    if (tid == 0) { s_prefix = 0u; s_rem = (uint32_t)k; }
+    __syncthreads();
+    uint32_t mk = 0u;
+    auto stage = [&](int v, float x, bool in) {
+        uint32_t d = 256u;
+        if (in) {
+            const uint32_t key = float_key(x);
+            keys[v] = key;
+            mk = key > mk ? key : mk;
+            d = key >> 24;
+        }
+        warp_hist_add(hist[warp], d);
+    };
+    int v0 = 0;
+    if ((ld & 3) == 0 && (reinterpret_cast<uintptr_t>(logits) & 15) == 0) {        // v_begin is a multiple of 4
+        const int L4 = len >> 2;
+        for (int i0 = 0; i0 < L4; i0 += kTopkThreads) {
+            const int i = i0 + tid;
+            const bool in = i < L4;
+            float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (in) x = reinterpret_cast<const float4*>(lp)[i];
+            const float xs[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll
+            for (int j = 0; j < 4; ++j) stage(4 * i + j, xs[j], in);
+        }
+        v0 = L4 * 4;
+    }
+    for (int b = v0; b < len; b += kTopkThreads) stage(b + tid, b + tid < len ? lp[b + tid] : 0.f, b + tid < len);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { const uint32_t t = __shfl_xor_sync(0xffffffffu, mk, o); mk = t > mk ? t : mk; }
+    if (lane == 0) s_max[warp] = mk;
+    __syncthreads();
+    if (tid == 0) {
+        uint32_t m = s_max[0];
+        for (int w = 1; w < kTopkWarps; ++w) m = s_max[w] > m ? s_max[w] : m;
+        s_cta_max = m;
+    }
+    for (int pass = 0; pass < 4; ++pass) {
+        const int shift = 24 - 8 * pass;
+        if (pass > 0) {
+            const uint32_t prefix = s_prefix;
+            const uint32_t hmask = 0xffffffffu << (shift + 8);
+            for (int b = 0; b < len; b += kTopkThreads) {
+                const int v = b + tid;
+                uint32_t d = 256u;
+                if (v < len) {
+                    const uint32_t key = keys[v];
+                    if ((key & hmask) == prefix) d = (key >> shift) & 0xffu;
+                }
+                warp_hist_add(hist[warp], d);
+            }
+            __syncthreads();
+        }
+        uint32_t* const my_tot = tot[pass & 1];
+        if (tid < 256) {
+            uint32_t c = 0;
+            for (int w = 0; w < kTopkWarps; ++w) c += hist[w][tid];
+            my_tot[tid] = c;
+        }
+        cluster.sync();                                          // every CTA's totals (and, pass 0, its max) are visible
+        if (tid < 256) {                                         // the cluster's count of digit tid, into hist[0]
+            uint32_t c = 0;
+            for (int r = 0; r < n; ++r) c += cluster.map_shared_rank(my_tot, r)[tid];
+            hist[0][tid] = c;
+        }
+        __syncthreads();
+        if (warp == 0) {                                         // the decision of topk_threshold_kernel, same counts
+            uint32_t cnt[8], sum = 0;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) { cnt[j] = hist[0][255 - 8 * lane - j]; sum += cnt[j]; }
+            uint32_t incl = sum;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
+            const uint32_t rem = s_rem, excl = incl - sum;
+            __syncwarp();
+            if (excl < rem && rem <= incl) {
+                uint32_t above = excl;
+                int jd = 7;
+                bool found = false;
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {                    // constant indices: cnt stays in registers
+                    if (found) continue;
+                    if (above + cnt[j] >= rem) { jd = j; found = true; }
+                    else above += cnt[j];
+                }
+                s_prefix |= (uint32_t)(255 - 8 * lane - jd) << shift;
+                s_rem = rem - above;
+            }
+        }
+        __syncthreads();
+        for (int i = tid; i < kTopkWarps * 256; i += kTopkThreads) (&hist[0][0])[i] = 0u;
+        __syncthreads();
+    }
+    uint32_t max_key = 0u;
+    for (int r = 0; r < n; ++r) { const uint32_t m = *cluster.map_shared_rank(&s_cta_max, r); max_key = m > max_key ? m : max_key; }
+    const uint32_t tau_key = s_prefix;
+    const float mx = key_float(max_key);
+    float se = 0.f;
+    if (mx > -INFINITY)
+        for (int v = tid; v < len; v += kTopkThreads) {
+            const uint32_t key = keys[v];
+            if (key >= tau_key) se += expf(key_float(key) - mx);
+        }
+    se = block_reduce_sum(se, red);
+    if (tid == 0) s_se = se;
+    cluster.sync();                                              // every CTA's sum is visible
+    if (rank == 0 && tid == 0) {
+        float total = s_se;
+        for (int r = 1; r < n; ++r) total += *cluster.map_shared_rank(&s_se, r);
+        float* o = row_thr + (int64_t)(blockIdx.x / n) * 3;
+        o[0] = mx; o[1] = logf(total); o[2] = key_float(tau_key);
+    }
+    cluster.sync();                                              // no CTA exits while rank 0 reads its shared memory
 }
 
 // ---- step kernel 1 of 2: row statistics + the best K constrained candidates of a run of beams -----------------------
