@@ -7,7 +7,8 @@
  *   - BeamSearchScorerWithMemory.process/finalize   seal/beam_search.py:614-735
  *   - the BART-large forward the reference gets from transformers 4.13 (call sites
  *     seal/beam_search.py:231-238,481-483; model = BartForConditionalGeneration), or the T5 forward
- *     (T5ForConditionalGeneration, SEALSearcher's 't5' backbone) behind the same handle (sealt5_create)
+ *     (T5ForConditionalGeneration, SEALSearcher's 't5' backbone) behind the same handle (sealt5_create), or the
+ *     pre-LayerNorm BART-family forward of Pegasus and mBART (sealbart_create_ex)
  * Plain pointers and sizes only.  Status codes and sealfm_last_error() as in sealfm.h.
  * Everything runs on the GPU; there is no CPU path.
  */
@@ -70,6 +71,36 @@ int  sealbart_set_tensor(sealbart_t* m, const char* key, const float* host, uint
  * given, derives fused/pre-split copies. */
 int  sealbart_finalize(sealbart_t* m);
 uint64_t sealbart_device_bytes(const sealbart_t* m);
+
+/* ---- pre-LayerNorm BART family (Pegasus, mBART) ---------------------------------------------------- */
+
+#define SEALBART_ACT_GELU 0            /* exact-erf GELU (bart-large, mBART, PegasusConfig() defaults) */
+#define SEALBART_ACT_RELU 1            /* ReLU (released Pegasus checkpoints)                          */
+
+typedef struct {
+    int32_t pre_layer_norm;            /* 1: h += SelfAttn(LN_self(h)); h += CrossAttn(LN_cross(h)); h += fc2(act(fc1(LN_final(h))))
+                                          and the stacks' final "model.{encoder,decoder}.layer_norm" (Pegasus, mBART);
+                                          0: bart-large's post-LayerNorm layer (then only {0, 2, 1, SEALBART_ACT_GELU}) */
+    int32_t position_offset;           /* 0: position p reads table row p (Pegasus's sinusoidal table); 2: row p + 2 (mBART, BART) */
+    int32_t layernorm_embedding;       /* 1: "model.{encoder,decoder}.layernorm_embedding" after the embedding (mBART); 0: none */
+    int32_t activation;                /* SEALBART_ACT_GELU or SEALBART_ACT_RELU, the fc1 epilogue                           */
+} sealbart_variant_t;
+
+/* A BART-family model behind the same handle: every entry point below takes it and behaves as documented for BART.
+ * cfg as for sealbart_create (d_model a multiple of 128 up to 1024, 64-wide heads, ffn_dim % 64 == 0); for a
+ * pre-LayerNorm variant max_positions >= 1 is the number of positions the tables cover: each of
+ * "model.{encoder,decoder}.embed_positions.weight" has max_positions + position_offset rows (Pegasus's
+ * max_position_embeddings rows; mBART's max_position_embeddings + 2).  sealbart_set_tensor takes BART's keys plus
+ * "model.{encoder,decoder}.layer_norm.{weight,bias}"; "model.{encoder,decoder}.layernorm_embedding.*" only with
+ * layernorm_embedding = 1.  Every other key is SEALFM_EINVAL.  An unsupported variant or shape is SEALFM_EINVAL before
+ * any allocation.  sealbart_create is sealbart_create_ex with {0, 2, 1, SEALBART_ACT_GELU}.
+ * Position table: sources longer than max_positions are refused (as for BART), and sealdec_teacher_forced /
+ * sealdec_debug_step_logits refuse decoder inputs longer than max_positions.  A generate may reach decoder positions
+ * past the table (max_length - 2 >= max_positions); those steps read the table's last row, so the records of a beam
+ * that is still alive there are not the model's -- whether such a call may run is the caller's decision
+ * (seal_b200.beam_search raises the reference's IndexError exactly where the reference's forward would read past the
+ * table). */
+int  sealbart_create_ex(const sealbart_config_t* cfg, const sealbart_variant_t* variant, int device, sealbart_t** out);
 
 /* ---- T5 weights ------------------------------------------------------------------------------- */
 
@@ -257,7 +288,11 @@ int sealdec_generate_dx_ex(sealbart_t* model, const sealfm_t* fm, const uint32_t
  *  17 T5 decoder self-attention with the relative position bias (one warp per row and head, any position)
  *  18 embedding / add + RMSNorm (one CTA per row; folds a pending split-K GEMM), d_model <= 1024
  *  19 ReLU feed-forward (ReLU GEMM epilogue)          20 gated-gelu feed-forward (gelu_new(wi_0 x) * wi_1 x kernel)
- *  21 embedding / add + RMSNorm as 18, d_model 2048 .. 4096 ("t5_rms_wide"; such a model never sets 18) */
+ *  21 embedding / add + RMSNorm as 18, d_model 2048 .. 4096 ("t5_rms_wide"; such a model never sets 18)
+ * and of the pre-LayerNorm forward (sealbart_create_ex; it also sets 0 .. 7 and 10 .. 15 as BART does, never 8 / 9;
+ * bit 19 names its ReLU feed-forward, e.g. Pegasus's):
+ *  22 embedding / add + LayerNorm, one CTA per row (preln_row_kernel; folds a pending split-K GEMM)
+ *  23 the embedding form of 22 with layernorm_embedding (mBART: two LayerNorms in one launch) */
 int     sealbart_set_option(sealbart_t* model, const char* name, int64_t value);
 int64_t sealbart_get_stat(const sealbart_t* model, const char* name);
 

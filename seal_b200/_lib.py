@@ -96,6 +96,11 @@ class BartConfig(C.Structure):            # sealbart_config_t
                 ("max_positions", C.c_int32), ("scale_embedding", C.c_int32), ("gemm_mode", C.c_int32)]
 
 
+class BartVariant(C.Structure):           # sealbart_variant_t
+    _fields_ = [("pre_layer_norm", C.c_int32), ("position_offset", C.c_int32), ("layernorm_embedding", C.c_int32),
+                ("activation", C.c_int32)]
+
+
 class T5Config(C.Structure):              # sealt5_config_t
     _fields_ = [("vocab_size", C.c_int32), ("d_model", C.c_int32), ("num_layers", C.c_int32),
                 ("num_decoder_layers", C.c_int32), ("num_heads", C.c_int32), ("d_kv", C.c_int32), ("d_ff", C.c_int32),
@@ -122,6 +127,7 @@ _DEC_SIGS = {
     "sealdec_apply_index_mask_d": (i32, [vp, vp, C.POINTER(ProcessorCfg), vp, C.c_int64, C.c_int64, vp, vp, vp,
                                          C.c_int64, C.c_int64]),
     "sealbart_create": (i32, [C.POINTER(BartConfig), i32, C.POINTER(vp)]),
+    "sealbart_create_ex": (i32, [C.POINTER(BartConfig), C.POINTER(BartVariant), i32, C.POINTER(vp)]),
     "sealbart_free": (None, [vp]),
     "sealt5_create": (i32, [C.POINTER(T5Config), i32, C.POINTER(vp)]),
     "sealt5_relative_buckets": (i32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp]),

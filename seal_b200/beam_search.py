@@ -9,7 +9,8 @@
   groups (``diverse_bs_groups`` / ``diverse_bs_penalty``); ``keep_history=False`` (transformers' stock
   BeamSearchScorer, the signature's default) and ``transformers_output=True`` run the same kernels and replay
   the stock scorer over the per-step records (one beam group only).
-* ``SealBartEngine`` — device copy of an HF ``BartForConditionalGeneration``'s weights.
+* ``SealBartEngine`` — device copy of an HF ``BartForConditionalGeneration``'s weights (``SealPreLnEngine``: Pegasus and
+  mBART, the pre-LayerNorm BART family; ``SealT5Engine``: T5).
 
 No CPU path: CPU tensors are rejected.
 """
@@ -21,7 +22,7 @@ from typing import List, Optional
 
 import numpy as np
 
-from ._lib import lib, check, vp, ProcessorCfg, BartConfig, DecParams, GroupParams, T5Config
+from ._lib import lib, check, vp, ProcessorCfg, BartConfig, BartVariant, DecParams, GroupParams, T5Config
 from .index import FMIndex, SHIFT
 
 stopword_token_ids = [10, 41, 660, 5, 1941, 20, 7, 6]      # beam_search.py:22-31
@@ -126,8 +127,11 @@ class SealBartEngine:
 
     @classmethod
     def from_hf(cls, model, device=None, gemm_mode=None):
-        if getattr(model.config, "model_type", None) == "t5":
+        model_type = getattr(model.config, "model_type", None)
+        if model_type == "t5":
             return SealT5Engine.from_hf(model, device=device, gemm_mode=gemm_mode)
+        if model_type in PRELN_MODEL_TYPES:
+            return SealPreLnEngine.from_hf(model, device=device, gemm_mode=gemm_mode)
         torch = _torch()
         if device is None:
             p = next(model.parameters())
@@ -275,6 +279,113 @@ class SealT5Engine(SealBartEngine):
                    generation_config=getattr(model, "generation_config", None))
 
 
+PRELN_MODEL_TYPES = ("pegasus", "mbart")          # HF model types of the pre-LayerNorm BART family
+PRELN_ACTIVATIONS = {"gelu": 0, "relu": 1}         # sealbart_variant_t.activation (SEALBART_ACT_GELU / _RELU)
+
+
+class PreLnConfigView:
+    """A Pegasus / mBART config as the decode reads it, resolved the way transformers 4.13 (the reference's pin) does for
+    fm_index_generate: decoder_start_token_id from the config, else bos_token_id, else the ValueError of
+    `_get_decoder_start_token_id`; forced_eos_token_id from the config (1 for Pegasus, 2 for mBART), which feeds the
+    ForcedEOS rule; forced_bos_token_id None where the attribute is missing.  Every other attribute is the HF config's."""
+
+    def __init__(self, config):
+        self._hf = config
+        start = getattr(config, "decoder_start_token_id", None)
+        if start is None:
+            start = getattr(config, "bos_token_id", None)
+        if start is None:
+            raise ValueError("`decoder_start_token_id` or `bos_token_id` has to be defined for encoder-decoder generation.")
+        self.decoder_start_token_id = int(start)
+        self.forced_bos_token_id = getattr(config, "forced_bos_token_id", None)
+        self.forced_eos_token_id = getattr(config, "forced_eos_token_id", None)
+
+    def __getattr__(self, name):
+        return getattr(self.__dict__["_hf"], name)
+
+
+def preln_native_config(config, gemm_mode):
+    """(sealbart_config_t, sealbart_variant_t) for an HF Pegasus or mBART config; ValueError for an activation or shape
+    the kernels do not cover (the limits sealbart_create_ex enforces, include/sealdec.h), before anything touches the
+    device."""
+    mt = getattr(config, "model_type", None)
+    if mt not in PRELN_MODEL_TYPES:
+        raise ValueError(f"model_type {mt!r} is not a pre-LayerNorm BART-family model (supported: {list(PRELN_MODEL_TYPES)})")
+    act = getattr(config, "activation_function", "gelu")
+    if act not in PRELN_ACTIVATIONS:
+        raise ValueError(f"{mt} activation_function {act!r} is not implemented (supported: {sorted(PRELN_ACTIVATIONS)})")
+    d = int(config.d_model)
+    heads, ffn = int(config.decoder_attention_heads), int(config.decoder_ffn_dim)
+    if int(config.encoder_attention_heads) != heads or int(config.encoder_ffn_dim) != ffn:
+        raise ValueError(f"{mt} shape not covered: encoder and decoder must have the same heads and ffn_dim "
+                         f"(encoder {config.encoder_attention_heads} / {config.encoder_ffn_dim}, decoder {heads} / {ffn})")
+    if not (0 < d <= 1024 and d % 128 == 0) or heads * 64 != d:
+        raise ValueError(f"{mt} shape not covered: d_model must be a multiple of 128 up to 1 024 with 64-wide heads "
+                         f"(d_model={d}, heads={heads})")
+    if ffn <= 0 or ffn % 64:
+        raise ValueError(f"{mt} shape not covered: ffn_dim must be a positive multiple of 64 (ffn_dim={ffn})")
+    P = int(config.max_position_embeddings)
+    if P < 1:
+        raise ValueError(f"{mt}: max_position_embeddings must be >= 1 (got {P})")
+    cfg = BartConfig(int(config.vocab_size), d, int(config.encoder_layers), int(config.decoder_layers), heads, ffn, P,
+                     int(bool(getattr(config, "scale_embedding", False))), int(gemm_mode))
+    var = BartVariant(1, 2 if mt == "mbart" else 0, 1 if mt == "mbart" else 0, PRELN_ACTIVATIONS[act])
+    return cfg, var
+
+
+class SealPreLnEngine(SealBartEngine):
+    """Device-resident Pegasus / mBART weights + workspace behind the same handle (include/sealdec.h
+    `sealbart_create_ex`): every method of SealBartEngine, and every entry point that takes an engine, works the same
+    way.  `config` is a PreLnConfigView; `max_positions` the rows of the decoder's position table (without mBART's
+    offset of 2)."""
+
+    def __init__(self, state_dict, config, device=0, gemm_mode=None):
+        if gemm_mode is None:
+            gemm_mode = int(os.environ.get("SEALB200_GEMM", "3"))
+        cfg, var = preln_native_config(config, gemm_mode)
+        self.config = PreLnConfigView(config)
+        self.gemm_mode = int(gemm_mode)
+        self.device = int(device)
+        self.max_positions = int(cfg.max_positions)
+        h = vp()
+        check(lib.sealbart_create_ex(C.byref(cfg), C.byref(var), self.device, C.byref(h)))
+        self._h = h.value
+        shared = state_dict.get("model.shared.weight")
+        for k, v in state_dict.items():
+            if shared is not None and k.endswith("embed_tokens.weight"):
+                continue                                    # tied aliases of model.shared.weight
+            if k == "lm_head.weight" and shared is not None and v.data_ptr() == shared.data_ptr():
+                continue
+            a = np.ascontiguousarray(v.detach().to("cpu").float().numpy())
+            check(lib.sealbart_set_tensor(self._h, k.encode(), a.ctypes.data, a.size))
+        check(lib.sealbart_finalize(self._h))
+
+    @classmethod
+    def from_hf(cls, model, device=None, gemm_mode=None):
+        preln_native_config(model.config, 3 if gemm_mode is None else gemm_mode)   # ValueError before any device work
+        PreLnConfigView(model.config)
+        torch = _torch()
+        if device is None:
+            p = next(model.parameters())
+            device = p.device.index if p.is_cuda else torch.cuda.current_device()
+        return cls(model.state_dict(), model.config, device=device, gemm_mode=gemm_mode)
+
+
+def _position_error():
+    # what torch.nn.functional.embedding raises for an index past the position table (the reference's forward)
+    return IndexError("index out of range in self")
+
+
+def _check_decoder_positions(eng, max_length):
+    """A generate that runs every step (keep_history=True, the record entry points) feeds decoder positions
+    0 .. max_length - 2 (cur_len - 1 at cur_len = 1 .. max_length - 1, constrained_beam_search).  A model with a bounded
+    position table (SealPreLnEngine) raises the reference's IndexError before any device work when the last one is
+    past the table."""
+    P = getattr(eng, "max_positions", None)
+    if P is not None and int(max_length) - 2 >= P:
+        raise _position_error()
+
+
 _ENGINES = weakref.WeakKeyDictionary()
 
 
@@ -349,6 +460,7 @@ def generate_records(model, index, input_ids, attention_mask, min_length=3, max_
     num_beam_groups > 1: diverse beam groups (include/sealdec.h sealdec_groups_t), records group by group per step.
     top_k > 0: the top-k logits warp on every step (sealdec_params_t.top_k; one group only)."""
     eng = _engine_for(model)
+    _check_decoder_positions(eng, max_length)
     cfg = eng.config
     if forced_bos_token_id == "config":
         forced_bos_token_id = getattr(cfg, "forced_bos_token_id", None)
@@ -422,16 +534,22 @@ def _side_stream(device):
 def generate_records_device(model, index, input_ids_d, attention_mask_d, min_length=3, max_length=25, length_penalty=1.0,
                             num_beams=3, eos_token_id=None, force_decoding_from=None, always_allow_eos=False,
                             disable_fm_index=False, stop_at_count=0, forced_bos_token_id="config", out=None,
-                            src_tokens=-1, stream=None, num_beam_groups=1, diversity_penalty=0.0, top_k=0):
+                            src_tokens=-1, stream=None, num_beam_groups=1, diversity_penalty=0.0, top_k=0,
+                            check_positions=True):
     """sealdec_generate_dx on DEVICE tensors, asynchronous: input_ids / attention_mask are int64 CUDA tensors
     [Q, S]; the records land in `out` (a DeviceRecords, created if None) on `stream` (default: the current stream if
     it is not the legacy default stream, else a per-device side stream that first waits for the current one).
     `src_tokens`: number of non-zero mask entries if the caller knows it (right-padded masks) — then the call never
     touches the host; -1 = unknown.  Errors are flags inside the buffer (`out.host()["errors"]`, include/sealdec.h).
-    `num_beam_groups` / `diversity_penalty` / `top_k`: diverse beam groups and the top-k warp, as in generate_records."""
+    `num_beam_groups` / `diversity_penalty` / `top_k`: diverse beam groups and the top-k warp, as in generate_records.
+    `check_positions`: raise IndexError for a max_length whose decoder positions pass a bounded position table (Pegasus,
+    mBART), as generate_records does; False leaves it to the caller (fm_index_generate with keep_history=False, whose
+    stock scorer may stop before those steps)."""
     torch = _torch()
     from .sharding import RecordLayout
     eng = _engine_for(model)
+    if check_positions:
+        _check_decoder_positions(eng, max_length)
     cfg = eng.config
     if forced_bos_token_id == "config":
         forced_bos_token_id = getattr(cfg, "forced_bos_token_id", None)
@@ -550,7 +668,7 @@ def records_to_output(rec, length_penalty):
     return out
 
 
-def _replay_beam_search_scorer(rec, num_beams, length_penalty, eos_token_id, pad_token_id, max_length):
+def _replay_beam_search_scorer(rec, num_beams, length_penalty, eos_token_id, pad_token_id, max_length, n_positions=None):
     """keep_history=False (seal/beam_search.py:505-515): the reference hands the loop transformers 4.13's stock
     `BeamSearchScorer` instead of BeamSearchScorerWithMemory.  Both choose the next beams the same way (the first
     num_beams non-EOS candidates of the top 2*num_beams), so the beams evolve identically until a query is `done`,
@@ -559,14 +677,18 @@ def _replay_beam_search_scorer(rec, num_beams, length_penalty, eos_token_id, pad
     "EOS only if ranked inside the top num_beams", finalize's best-num_beams selection with an appended EOS -- is
     replayed here, on the host, over the per-step candidate records (a few thousand scalar operations per query).
     Returns (beams per query [(score, tokens)] in BeamHypotheses order, sequences int64 [Q*num_beams, L],
-    sequence_scores float32 [Q*num_beams]).  transformers 4.13 is not vendored: restated from its published algorithm."""
+    sequence_scores float32 [Q*num_beams]).  transformers 4.13 is not vendored: restated from its published algorithm.
+    n_positions: the decoder's position table rows (None: unbounded).  The reference runs step `st` (decoder position
+    st) while some query is not done, so a query still alive at step st >= n_positions means its forward read past the
+    table: IndexError, unless a query failed the num_beams check at an earlier step, which the reference meets first."""
     scores, lens, toks = rec["scores"], rec["lens"], rec["tokens"]
     Q, H = scores.shape
     B, K = num_beams, 2 * num_beams
     n_steps = (H - B) // K
     all_beams, best, best_scores = [], [], []
+    fail_step, past_table = None, False          # the first step that fails the num_beams check; a step past the table
     for q in range(Q):
-        beams = []; worst = 1e9; done = False
+        beams = []; worst = 1e9; done = False; stopped = False
 
         def add(tokens, sum_logprobs):
             nonlocal worst
@@ -583,6 +705,9 @@ def _replay_beam_search_scorer(rec, num_beams, length_penalty, eos_token_id, pad
         for st in range(n_steps):
             if done:
                 break
+            if n_positions is not None and st >= n_positions:
+                past_table = stopped = True
+                break
             cur_len = st + 1
             base = st * K
             cand_s = scores[q, base:base + K].tolist()
@@ -598,9 +723,13 @@ def _replay_beam_search_scorer(rec, num_beams, length_penalty, eos_token_id, pad
                 if nb == B:
                     break
             if nb < B:
-                raise ValueError(f"At most {B} tokens can be equal to `eos_token_id: {eos_token_id}`.")
+                fail_step = st if fail_step is None else min(fail_step, st)
+                stopped = True
+                break
             if len(beams) >= B:
                 done = worst >= max(cand_s) / cur_len ** length_penalty
+        if stopped:
+            continue
         if not done:
             fb = n_steps * K
             for j in range(B):
@@ -610,6 +739,10 @@ def _replay_beam_search_scorer(rec, num_beams, length_penalty, eos_token_id, pad
         for _ in range(B):
             sc, t = order.pop()
             best.append(t); best_scores.append(sc)
+    if past_table and (fail_step is None or fail_step >= n_positions):
+        raise _position_error()
+    if fail_step is not None:
+        raise ValueError(f"At most {B} tokens can be equal to `eos_token_id: {eos_token_id}`.")
     L = min(max(len(t) for t in best) + 1, max_length) if best else 0
     seq = np.full((len(best), L), pad_token_id, dtype=np.int64)
     for i, t in enumerate(best):
@@ -656,19 +789,23 @@ def fm_index_generate(model, index: FMIndex, input_ids, attention_mask, min_leng
     am_np = np.ascontiguousarray(np.asarray(attention_mask.cpu() if hasattr(attention_mask, "cpu") else attention_mask, dtype=np.int64))
     out = generate_records_device(eng, index, torch.from_numpy(ids_np).to(dev), torch.from_numpy(am_np).to(dev), min_length,
                                   max_length, length_penalty, num_beams, eos_token_id, force_decoding_from, always_allow_eos,
-                                  disable_fm_index, stop_at_count, forced_bos, src_tokens=-2, top_k=top_k)
+                                  disable_fm_index, stop_at_count, forced_bos, src_tokens=-2, top_k=top_k, check_positions=False)
     rec = out.host()
     if rec["errors"][1] and eng.gemm_mode >= 3:        # fp16 range exceeded: redo with the 3xTF32 kernels (sealdec.h)
         check(lib.sealbart_set_option(eng._h, b"gemm_mode", 2))
         try:
             rec = generate_records_device(eng, index, torch.from_numpy(ids_np).to(dev), torch.from_numpy(am_np).to(dev), min_length,
                                           max_length, length_penalty, num_beams, eos_token_id, force_decoding_from, always_allow_eos,
-                                          disable_fm_index, stop_at_count, forced_bos, src_tokens=-2, top_k=top_k).host()
+                                          disable_fm_index, stop_at_count, forced_bos, src_tokens=-2, top_k=top_k,
+                                          check_positions=False).host()
         finally:
             check(lib.sealbart_set_option(eng._h, b"gemm_mode", eng.gemm_mode))
     # the device's "fewer than num_beams non-EOS candidates" flag also fires for queries the stock scorer had already
     # frozen; the replay re-derives the condition per query and step and raises exactly where the reference does
-    beams, seq, _ = _replay_beam_search_scorer(rec, num_beams, length_penalty, eos, cfg.pad_token_id, int(max_length))
+    # with a bounded position table (Pegasus, mBART) the replay raises IndexError where the reference's forward would
+    # first read past it; the steps the kernels ran there (on the table's last row) are never read
+    beams, seq, _ = _replay_beam_search_scorer(rec, num_beams, length_penalty, eos, cfg.pad_token_id, int(max_length),
+                                               n_positions=getattr(eng, "max_positions", None))
     if transformers_output:
         return torch.from_numpy(seq).to(input_ids.device if hasattr(input_ids, "device") else "cpu")     # :388
     return [[(sc * (len(t) ** length_penalty), t) for sc, t in b if sc > float("-inf")] for b in beams]    # :555

@@ -1,10 +1,11 @@
 // Host orchestration + C ABI (include/sealdec.h) of the constrained beam-search decode:
-// BART and T5 weights, workspace, encoder pass, per-step decoder forward, fused select step.
+// BART, pre-LayerNorm BART-family (Pegasus, mBART) and T5 weights, workspace, encoder pass, per-step decoder forward, fused select step.
 #include "../../include/sealdec.h"
 #include "bart_kernels.cuh"
 #include "common.cuh"
 #include "decode_kernels.cuh"
 #include "fm_handle.hpp"
+#include "preln_kernels.cuh"
 #include "t5_kernels.cuh"
 #include "wgmma_gemm.cuh"
 
@@ -64,7 +65,12 @@ struct sealbart {
     // architecture: 0 BART (sealbart_create), 1 T5 (sealt5_create).  For T5 the Lin biases stay zero, LNp::g holds the
     // T5LayerNorm weights (EncLayerW: ln_attn = layer.0, ln_final = layer.1; DecLayerW: ln_self / ln_cross / ln_final =
     // layer.0 / 1 / 2), enc_ln_emb / dec_ln_emb the final_layer_norm of each stack, and fc1 is wi or [wi_0; wi_1].
+    // 2 pre-LayerNorm BART family (sealbart_create_ex): BART's keys and biases; enc_ln_emb / dec_ln_emb hold
+    // layernorm_embedding (allocated only if variant.layernorm_embedding), enc_ln_out / dec_ln_out the stacks' final
+    // layer_norm; the position tables have max_positions + variant.position_offset rows.
     int arch = 0;
+    sealbart_variant_t variant{};
+    LNp enc_ln_out, dec_ln_out;
     sealt5_config_t t5{};
     float* t5_rel_enc = nullptr; float* t5_rel_dec = nullptr;          // layer-0 relative_attention_bias [buckets][heads]
     int32_t* t5_bkt_enc = nullptr; int32_t* t5_bkt_dec = nullptr;      // bucket of distance k - q, see t5_bucket_tables
@@ -198,15 +204,24 @@ void build_slots_t5(sealbart* m) {
     }
 }
 
+// HF BartForConditionalGeneration state_dict keys; a pre-LayerNorm handle (arch 2) registers layernorm_embedding only
+// for a variant that has it, the stacks' final layer_norm, and position tables of max_positions + position_offset rows.
 void build_slots(sealbart* m) {
     const auto& c = m->cfg;
-    const int d = c.d_model, f = c.ffn_dim, V = c.vocab_size, P = c.max_positions + 2;
+    const bool preln = m->arch == 2;
+    const int d = c.d_model, f = c.ffn_dim, V = c.vocab_size, P = c.max_positions + (preln ? m->variant.position_offset : 2);
     m->shared = dalloc(m, (uint64_t)V * d); reg(m, "model.shared.weight", m->shared, (uint64_t)V * d);
     m->enc_pos = dalloc(m, (uint64_t)P * d); reg(m, "model.encoder.embed_positions.weight", m->enc_pos, (uint64_t)P * d);
     m->dec_pos = dalloc(m, (uint64_t)P * d); reg(m, "model.decoder.embed_positions.weight", m->dec_pos, (uint64_t)P * d);
     m->final_bias = dalloc(m, V); reg(m, "final_logits_bias", m->final_bias, V);
-    make_ln(m, m->enc_ln_emb, d); reg_ln(m, "model.encoder.layernorm_embedding", m->enc_ln_emb, d);
-    make_ln(m, m->dec_ln_emb, d); reg_ln(m, "model.decoder.layernorm_embedding", m->dec_ln_emb, d);
+    if (!preln || m->variant.layernorm_embedding) {
+        make_ln(m, m->enc_ln_emb, d); reg_ln(m, "model.encoder.layernorm_embedding", m->enc_ln_emb, d);
+        make_ln(m, m->dec_ln_emb, d); reg_ln(m, "model.decoder.layernorm_embedding", m->dec_ln_emb, d);
+    }
+    if (preln) {
+        make_ln(m, m->enc_ln_out, d); reg_ln(m, "model.encoder.layer_norm", m->enc_ln_out, d);
+        make_ln(m, m->dec_ln_out, d); reg_ln(m, "model.decoder.layer_norm", m->dec_ln_out, d);
+    }
     m->enc.resize(c.encoder_layers);
     for (int i = 0; i < c.encoder_layers; ++i) {
         EncLayerW& L = m->enc[i];
@@ -286,7 +301,7 @@ enum : uint32_t {
     kPathSplitKDeferred = 1u << 10, kPathSplitKFinish = 1u << 11, kPathGemmFullTile = 1u << 12, kPathGemmCluster = 1u << 13,
     kPathGemmTf32 = 1u << 14, kPathQuerySlices = 1u << 15,
     kPathT5EncAttn = 1u << 16, kPathT5DecAttn = 1u << 17, kPathT5Rms = 1u << 18, kPathT5Relu = 1u << 19, kPathT5Gate = 1u << 20,
-    kPathT5RmsWide = 1u << 21,
+    kPathT5RmsWide = 1u << 21, kPathPreLn = 1u << 22, kPathPreLnEmbedLn = 1u << 23,
 };
 
 void split_into(cudaStream_t s, const float* x, float* hi, float* lo, uint64_t numel) {
@@ -728,9 +743,45 @@ void bart_encoder_layers(Ctx& cx, const Dims& D, int64_t Te, const Acts& A, cons
     }
 }
 
-void bart_decoder_layers(Ctx& cx, const Dims& D, const DecStep& S) {
+// The BART decoder self-attention of layer l (BART and the pre-LayerNorm variants): qkv = x Wqkv, then attention over
+// the layer's KV cache (beam ancestry) into attn; the current k / v are persisted to the cache.
+void bart_self_attention(Ctx& cx, const Dims& D, const DecStep& S, int l) {
     sealbart* m = cx.m;
     const int d = D.d, heads = m->cfg.heads, pos = S.pos;
+    int* ovf = m->ovf;
+    DecLayerW& L = m->dec[l];
+    float* kc = m->kc.as<float>() + (size_t)l * D.T * S.Rc * d + D.r0 * d;
+    float* vc = m->vc.as<float>() + (size_t)l * D.T * S.Rc * d + D.r0 * d;
+    // the beams of a query together, distinct ancestors staged once (not at the compact first step, where a row
+    // stands for all beams, nor for ragged re-scoring groups)
+    static const bool sa_query = [] { const char* e = std::getenv("SEALB200_SELF_ATTN_QUERY"); return !e || std::atoi(e) != 0; }();
+    const size_t saq_smem = self_attn_query_smem(pos + 1, D.B);
+    const bool use_saq = sa_query && !S.compact && !D.grp_start && pos >= 1 && D.B >= 2 && D.B <= 32 && pos + 1 <= 128 && saq_smem <= 112 * 1024;
+    cx.defer_rows = use_saq ? INT64_MAX : 0;               // that kernel sums a split-K qkv itself
+    gemm(cx, S.R, 3 * d, d, S.x, d, L.qkv, S.qkv, 3 * d, kActNone);
+    cx.defer_rows = 0;
+    const SplitSrc qkv_src = cx.pending;
+    cx.pending = SplitSrc{};
+    const unsigned sa_threads = 32 * std::min(heads, 16);
+    const float* qkv = S.qkv.x;
+    if (use_saq) {
+        static size_t saq_set = 0;
+        if (saq_smem > saq_set) { CUDA_CHECK(cudaFuncSetAttribute(dec_self_attn_query_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024)); saq_set = 112 * 1024; }
+        launch_k(dec_self_attn_query_kernel, dim3((unsigned)D.Q, heads), 32 * D.B, saq_smem, cx.s, S.Rc, D.B, d, pos, D.T, qkv, kc, vc, S.anc,
+                 S.attn.x, split_of(S.attn, ovf), qkv_src);
+    } else if (pos + 1 <= 12)
+        launch_k(dec_self_attn_kernel<3>, (unsigned)S.R, sa_threads, 0, cx.s, S.Rc, d, heads, pos, D.T, qkv, kc, vc, S.anc, S.attn.x, split_of(S.attn, ovf), S.row_mul, S.row_mul);
+    else if (pos + 1 <= 32)
+        launch_k(dec_self_attn_kernel<8>, (unsigned)S.R, sa_threads, 0, cx.s, S.Rc, d, heads, pos, D.T, qkv, kc, vc, S.anc, S.attn.x, split_of(S.attn, ovf), S.row_mul, S.row_mul);
+    else
+        launch_k(dec_self_attn_long_kernel, (unsigned)S.R, sa_threads, 0, cx.s, S.Rc, d, heads, pos, D.T, qkv, kc, vc, S.anc, S.attn.x, split_of(S.attn, ovf));
+    m->launches++;
+    m->last_paths |= use_saq ? kPathSelfQuery : pos + 1 <= 12 ? kPathSelfRounds3 : pos + 1 <= 32 ? kPathSelfRounds8 : kPathSelfLong;
+}
+
+void bart_decoder_layers(Ctx& cx, const Dims& D, const DecStep& S) {
+    sealbart* m = cx.m;
+    const int d = D.d, pos = S.pos;
     int* ovf = m->ovf;
     const float scale = m->cfg.scale_embedding ? sqrtf((float)d) : 1.0f;
     launch_k(embed_ln_kernel, (unsigned)((S.R + 3) / 4), 128, 0, cx.s, S.R, d, S.tokens + pos, (int64_t)(D.T * S.row_mul), (const int32_t*)nullptr, pos,
@@ -738,33 +789,7 @@ void bart_decoder_layers(Ctx& cx, const Dims& D, const DecStep& S) {
     m->launches++;
     for (int l = 0; l < m->cfg.decoder_layers; ++l) {
         DecLayerW& L = m->dec[l];
-        float* kc = m->kc.as<float>() + (size_t)l * D.T * S.Rc * d + D.r0 * d;
-        float* vc = m->vc.as<float>() + (size_t)l * D.T * S.Rc * d + D.r0 * d;
-        // the beams of a query together, distinct ancestors staged once (not at the compact first step, where a row
-        // stands for all beams, nor for ragged re-scoring groups)
-        static const bool sa_query = [] { const char* e = std::getenv("SEALB200_SELF_ATTN_QUERY"); return !e || std::atoi(e) != 0; }();
-        const size_t saq_smem = self_attn_query_smem(pos + 1, D.B);
-        const bool use_saq = sa_query && !S.compact && !D.grp_start && pos >= 1 && D.B >= 2 && D.B <= 32 && pos + 1 <= 128 && saq_smem <= 112 * 1024;
-        cx.defer_rows = use_saq ? INT64_MAX : 0;               // that kernel sums a split-K qkv itself
-        gemm(cx, S.R, 3 * d, d, S.x, d, L.qkv, S.qkv, 3 * d, kActNone);
-        cx.defer_rows = 0;
-        const SplitSrc qkv_src = cx.pending;
-        cx.pending = SplitSrc{};
-        const unsigned sa_threads = 32 * std::min(heads, 16);
-        const float* qkv = S.qkv.x;
-        if (use_saq) {
-            static size_t saq_set = 0;
-            if (saq_smem > saq_set) { CUDA_CHECK(cudaFuncSetAttribute(dec_self_attn_query_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024)); saq_set = 112 * 1024; }
-            launch_k(dec_self_attn_query_kernel, dim3((unsigned)D.Q, heads), 32 * D.B, saq_smem, cx.s, S.Rc, D.B, d, pos, D.T, qkv, kc, vc, S.anc,
-                     S.attn.x, split_of(S.attn, ovf), qkv_src);
-        } else if (pos + 1 <= 12)
-            launch_k(dec_self_attn_kernel<3>, (unsigned)S.R, sa_threads, 0, cx.s, S.Rc, d, heads, pos, D.T, qkv, kc, vc, S.anc, S.attn.x, split_of(S.attn, ovf), S.row_mul, S.row_mul);
-        else if (pos + 1 <= 32)
-            launch_k(dec_self_attn_kernel<8>, (unsigned)S.R, sa_threads, 0, cx.s, S.Rc, d, heads, pos, D.T, qkv, kc, vc, S.anc, S.attn.x, split_of(S.attn, ovf), S.row_mul, S.row_mul);
-        else
-            launch_k(dec_self_attn_long_kernel, (unsigned)S.R, sa_threads, 0, cx.s, S.Rc, d, heads, pos, D.T, qkv, kc, vc, S.anc, S.attn.x, split_of(S.attn, ovf));
-        m->launches++;
-        m->last_paths |= use_saq ? kPathSelfQuery : pos + 1 <= 12 ? kPathSelfRounds3 : pos + 1 <= 32 ? kPathSelfRounds8 : kPathSelfLong;
+        bart_self_attention(cx, D, S, l);
         cx.defer_rows = kAddLnRowMax;
         gemm(cx, S.R, d, d, S.attn, d, L.o, S.tmp, d, kActNone);
         cx.defer_rows = 0;
@@ -776,6 +801,80 @@ void bart_decoder_layers(Ctx& cx, const Dims& D, const DecStep& S) {
         gemm(cx, S.R, d, D.f, S.ffn, D.f, L.fc2, S.tmp, d, kActNone);
         cx.defer_rows = 0;
         add_ln(cx, S.R, d, S.x.x, S.tmp.x, L.ln_final, S.x);
+    }
+}
+
+// ---- pre-LayerNorm BART family (Pegasus, mBART) ---------------------------------------------------------------
+// The T5 loops' structure with BART's weights and kernels: x (fp32, the residual stream) += sublayer(LN(x)).  The
+// plain half of the Act x holds the residual, its split half the normed operand of the next GEMM: every preln_norm
+// launch adds the previous sublayer's output (or gathers the embedding), stores the residual and writes LN(x) with the
+// next sublayer's norm -- after the last layer the stack's final layer_norm.
+PreLnEmbed preln_embed(const sealbart* m, const int32_t* tok, int64_t tok_stride, const int32_t* pos, int pos_const,
+                       const float* table, const LNp& ln_emb) {
+    PreLnEmbed em;
+    em.tok = tok; em.tok_stride = tok_stride; em.pos = pos; em.pos_const = pos_const;
+    em.pos_offset = m->variant.position_offset; em.pos_rows = m->cfg.max_positions + m->variant.position_offset;
+    em.embed = m->shared; em.scale = m->cfg.scale_embedding ? sqrtf((float)m->cfg.d_model) : 1.0f; em.pos_table = table;
+    em.ln_g = ln_emb.g; em.ln_b = ln_emb.b;
+    return em;
+}
+
+void preln_norm(Ctx& cx, int64_t rows, int d, const PreLnEmbed& em, const Act& x, const float* b, const LNp& ln) {
+    const SplitSrc ps = cx.pending;
+    cx.pending = SplitSrc{};
+    launch_k(preln_row_kernel, (unsigned)rows, 128, 0, cx.s, rows, d, em, x.x, b, ps, (const float*)ln.g, (const float*)ln.b,
+             split_of(x, cx.m->ovf));
+    cx.m->launches++;
+    cx.m->last_paths |= kPathPreLn | (em.tok && em.ln_g ? kPathPreLnEmbedLn : 0u);
+}
+
+// fc1 with the variant's activation epilogue, then fc2 into tmp (split-K slices left to the next preln_norm)
+void preln_ffn(Ctx& cx, int64_t rows, const Dims& D, const Act& x, Lin& fc1, Lin& fc2, const Act& ffn, const Act& tmp) {
+    const int act = cx.m->variant.activation == SEALBART_ACT_RELU ? kActRelu : kActGelu;
+    gemm(cx, rows, D.f, D.d, x, D.d, fc1, ffn, D.f, act);
+    cx.defer_rows = INT64_MAX;
+    gemm(cx, rows, D.d, D.f, ffn, D.f, fc2, tmp, D.d, kActNone);
+    cx.defer_rows = 0;
+}
+
+void preln_encoder_layers(Ctx& cx, const Dims& D, int64_t Te, const Acts& A, const int32_t* tok, const int32_t* pos,
+                          const int32_t* m32, const int32_t* soff) {
+    sealbart* m = cx.m;
+    const int d = D.d, heads = m->cfg.heads;
+    const int n = (int)m->enc.size();
+    preln_norm(cx, Te, d, preln_embed(m, tok, 1, pos, 0, m->enc_pos, m->enc_ln_emb), A.x, nullptr, m->enc[0].ln_attn);
+    for (int i = 0; i < n; ++i) {
+        EncLayerW& L = m->enc[i];
+        gemm(cx, Te, 3 * d, d, A.x, d, L.qkv, A.qkv, 3 * d, kActNone);
+        launch_k(enc_self_attn_kernel, dim3((unsigned)D.Q, heads), kGAttnWarps * 32, 0, cx.s, D.Q, d, heads, (int)D.S, (const float*)A.qkv.x,
+                 m32, A.attn.x, split_of(A.attn, m->ovf), soff);
+        m->launches++;
+        cx.defer_rows = INT64_MAX;
+        gemm(cx, Te, d, d, A.attn, d, L.o, A.tmp, d, kActNone);
+        cx.defer_rows = 0;
+        preln_norm(cx, Te, d, PreLnEmbed{}, A.x, A.tmp.x, L.ln_final);
+        preln_ffn(cx, Te, D, A.x, L.fc1, L.fc2, A.ffn, A.tmp);
+        preln_norm(cx, Te, d, PreLnEmbed{}, A.x, A.tmp.x, i + 1 < n ? m->enc[i + 1].ln_attn : m->enc_ln_out);
+    }
+}
+
+void preln_decoder_layers(Ctx& cx, const Dims& D, const DecStep& S) {
+    sealbart* m = cx.m;
+    const int d = D.d;
+    const int n = (int)m->dec.size();
+    preln_norm(cx, S.R, d, preln_embed(m, S.tokens + S.pos, (int64_t)(D.T * S.row_mul), nullptr, S.pos, m->dec_pos, m->dec_ln_emb),
+               S.x, nullptr, m->dec[0].ln_self);
+    for (int l = 0; l < n; ++l) {
+        DecLayerW& L = m->dec[l];
+        bart_self_attention(cx, D, S, l);
+        cx.defer_rows = INT64_MAX;
+        gemm(cx, S.R, d, d, S.attn, d, L.o, S.tmp, d, kActNone);
+        cx.defer_rows = 0;
+        preln_norm(cx, S.R, d, PreLnEmbed{}, S.x, S.tmp.x, L.ln_cross);
+        cross_attention(cx, D, S, l, INT64_MAX);
+        preln_norm(cx, S.R, d, PreLnEmbed{}, S.x, S.tmp.x, L.ln_final);
+        preln_ffn(cx, S.R, D, S.x, L.fc1, L.fc2, S.ffn, S.tmp);
+        preln_norm(cx, S.R, d, PreLnEmbed{}, S.x, S.tmp.x, l + 1 < n ? m->dec[l + 1].ln_self : m->dec_ln_out);
     }
 }
 
@@ -822,8 +921,10 @@ void encoder_forward(Ctx& cx, const Dims& D, const int64_t* ids_d, const int64_t
     A.ffn = act_view(gm, nullptr, m->effn_hi, m->effn_lo);
     A.ffn2 = m->effn2.as<float>();
     if (m->arch == 1) t5_encoder_layers(cx, D, Te, A, tok, m32, soff);
+    else if (m->arch == 2) preln_encoder_layers(cx, D, Te, A, tok, pos, m32, soff);
     else bart_encoder_layers(cx, D, Te, A, tok, pos, m32, soff);
-    // per-query cross-attention K/V of every decoder layer, once, from the encoder's output (T5: its final_layer_norm);
+    // per-query cross-attention K/V of every decoder layer, once, from the encoder's output (T5 and the pre-LayerNorm
+    // variants: its final layer norm);
     // the reference recomputes nothing either: HF caches them after the first step
     for (int l = 0; l < m->cfg.decoder_layers; ++l)
         gemm(cx, Te, 2 * d, d, A.x, d, m->dec[l].ckv, Act{m->ckv.as<float>() + (size_t)l * Tk * 2 * d}, 2 * d, kActNone);
@@ -852,6 +953,7 @@ void decoder_step(Ctx& cx, const Dims& D, const int32_t* tokens, int cur_len, co
     S.Tk = (D.Qb ? D.Qb : D.Q) * D.S; S.ckv_q0 = m->enc_packed ? 0 : D.q0 * D.S * 2 * d;
     S.m32 = m->enc_mask.as<int32_t>() + D.q0 * D.S; S.soff_x = m->enc_packed ? m->src_off.as<int32_t>() + D.q0 : nullptr;
     if (m->arch == 1) t5_decoder_layers(cx, D, S);
+    else if (m->arch == 2) preln_decoder_layers(cx, D, S);
     else bart_decoder_layers(cx, D, S);
     if (ev_layers_done) CUDA_CHECK(cudaEventRecord(ev_layers_done, cx.s));
     cx.head = head;                 // only the lm_head may take the statistics epilogue
@@ -1019,19 +1121,53 @@ int sealt5_create(const sealt5_config_t* cfg, int device, sealbart_t** out) {
     });
 }
 
+}  // extern "C"
+
+namespace {
+
+// sealbart_create and sealbart_create_ex: var == nullptr is bart-large's post-LayerNorm layer
+void create_bart(const sealbart_config_t* cfg, const sealbart_variant_t* var, int device, sealbart_t** out) {
+    if (!cfg || !out) throw ApiError(SEALFM_EINVAL, "null argument");
+    if (cfg->d_model % 128 || cfg->d_model > 1024 || cfg->heads * kHeadDim != cfg->d_model)
+        throw ApiError(SEALFM_EINVAL, "d_model must be a multiple of 128, <= 1024, with 64-wide heads");
+    if (cfg->ffn_dim % 64 || cfg->vocab_size <= 0) throw ApiError(SEALFM_EINVAL, "bad ffn_dim / vocab_size");
+    if (var && cfg->max_positions < 1) throw ApiError(SEALFM_EINVAL, "max_positions must be >= 1");
+    check_gemm_mode(cfg->gemm_mode);
+    if (device < 0 || device >= require_device()) throw ApiError(SEALFM_EINVAL, "bad device id");
+    CUDA_CHECK(cudaSetDevice(device));
+    std::unique_ptr<sealbart> m(new sealbart());
+    m->cfg = *cfg; m->device = device;
+    if (var) { m->arch = 2; m->variant = *var; }
+    struct Guard { sealbart* m; ~Guard() { if (m) sealbart_free(m); } } guard{m.get()};
+    build_slots(m.get());
+    guard.m = nullptr;
+    *out = m.release();
+}
+
+}  // namespace
+
+extern "C" {
+
 int sealbart_create(const sealbart_config_t* cfg, int device, sealbart_t** out) {
+    return guarded([&] { create_bart(cfg, nullptr, device, out); });
+}
+
+int sealbart_create_ex(const sealbart_config_t* cfg, const sealbart_variant_t* variant, int device, sealbart_t** out) {
     return guarded([&] {
-        if (!cfg || !out) throw ApiError(SEALFM_EINVAL, "null argument");
-        if (cfg->d_model % 128 || cfg->d_model > 1024 || cfg->heads * kHeadDim != cfg->d_model)
-            throw ApiError(SEALFM_EINVAL, "d_model must be a multiple of 128, <= 1024, with 64-wide heads");
-        if (cfg->ffn_dim % 64 || cfg->vocab_size <= 0) throw ApiError(SEALFM_EINVAL, "bad ffn_dim / vocab_size");
-        check_gemm_mode(cfg->gemm_mode);
-        if (device < 0 || device >= require_device()) throw ApiError(SEALFM_EINVAL, "bad device id");
-        CUDA_CHECK(cudaSetDevice(device));
-        std::unique_ptr<sealbart> m(new sealbart());
-        m->cfg = *cfg; m->device = device;
-        build_slots(m.get());
-        *out = m.release();
+        if (!cfg || !variant || !out) throw ApiError(SEALFM_EINVAL, "null argument");
+        const sealbart_variant_t& v = *variant;
+        if (v.activation != SEALBART_ACT_GELU && v.activation != SEALBART_ACT_RELU)
+            throw ApiError(SEALFM_EINVAL, "activation must be SEALBART_ACT_GELU or SEALBART_ACT_RELU");
+        if (!v.pre_layer_norm) {                               // the post-LayerNorm layer exists in bart-large's form only
+            if (v.position_offset != 2 || v.layernorm_embedding != 1 || v.activation != SEALBART_ACT_GELU)
+                throw ApiError(SEALFM_EINVAL, "post-LayerNorm variant: only bart-large's (position_offset 2, layernorm_embedding, gelu)");
+            create_bart(cfg, nullptr, device, out);
+            return;
+        }
+        if (v.pre_layer_norm != 1) throw ApiError(SEALFM_EINVAL, "pre_layer_norm must be 0 or 1");
+        if (v.position_offset != 0 && v.position_offset != 2) throw ApiError(SEALFM_EINVAL, "position_offset must be 0 or 2");
+        if (v.layernorm_embedding != 0 && v.layernorm_embedding != 1) throw ApiError(SEALFM_EINVAL, "layernorm_embedding must be 0 or 1");
+        create_bart(cfg, &v, device, out);
     });
 }
 
@@ -1062,7 +1198,7 @@ int sealbart_set_tensor(sealbart_t* m, const char* key, const float* host, uint6
             CUDA_CHECK(cudaMemcpy(m->lm_head, host, want * 4, cudaMemcpyHostToDevice));
             return;
         }
-        if (m->arch == 0 && (k == "model.encoder.embed_tokens.weight" || k == "model.decoder.embed_tokens.weight")) k = "model.shared.weight";
+        if (m->arch != 1 && (k == "model.encoder.embed_tokens.weight" || k == "model.decoder.embed_tokens.weight")) k = "model.shared.weight";
         if (m->arch == 1 && (k == "encoder.embed_tokens.weight" || k == "decoder.embed_tokens.weight")) k = "shared.weight";
         auto it = m->slots.find(k);
         if (it == m->slots.end()) throw ApiError(SEALFM_EINVAL, "unknown state_dict key: " + k);
@@ -1788,6 +1924,7 @@ int sealdec_debug_step_logits_ex(sealbart_t* m, const int64_t* ids, const int64_
         if (src_tokens_hint != -1 && src_tokens_hint != -2 && right_padded_tokens(mask, Q, S) != src_tokens_hint)
             throw ApiError(SEALFM_EINVAL, "src_tokens_hint does not match a right-padded mask");
         const int T = (int)t;
+        if (m->arch == 2 && T > m->cfg.max_positions) throw ApiError(SEALFM_EINVAL, "decoder inputs longer than the position table");
         const Dims D = make_dims(m, Q, S, B, T);
         check_token_ids(dec_ids, D.R * T, m->cfg.vocab_size, "decoder");
         if (anc)
@@ -1825,6 +1962,7 @@ int sealdec_teacher_forced(sealbart_t* m, const int64_t* ids, const int64_t* mas
             throw ApiError(SEALFM_EINVAL, "bad argument");
         if (S > m->cfg.max_positions) throw ApiError(SEALFM_EINVAL, "source longer than max_positions");
         if (out_full && (out_full_pos < 0 || out_full_pos >= T)) throw ApiError(SEALFM_EINVAL, "out_full_pos must be in [0, T)");
+        if (m->arch == 2 && T > m->cfg.max_positions) throw ApiError(SEALFM_EINVAL, "decoder inputs longer than the position table");
         check_sources(ids, mask, Q, S, m->cfg.vocab_size);
         check_token_ids(dec_ids, N * T, m->cfg.vocab_size, "decoder");
         for (int64_t r = 0; r < N; ++r) {
