@@ -58,14 +58,26 @@ typedef struct {
     int32_t ffn_dim;           /* 4096                                         */
     int32_t max_positions;     /* 1024 (+2 learned offset)                     */
     int32_t scale_embedding;   /* 0 for bart-large                             */
-    int32_t gemm_mode;         /* 3 = 3xFP16, one CTA per 128x128 tile (split-K for small problems; default), 5 = 3xFP16 in clusters of 2 CTAs sharing the W tile (TMA multicast), 2 = 3xTF32 (fp32 range).  All wgmma + TMA. */
+    int32_t gemm_mode;         /* 3 = 3xFP16, one CTA per 128x128 tile (split-K for small problems; default), 5 = 3xFP16 in clusters of 2 CTAs sharing the W tile (TMA multicast), 2 = 3xTF32 (fp32 range),
+                                  6 = 3xBF16 with bf16 weights (see below).  All wgmma + TMA. */
 } sealbart_config_t;
 
 int  sealbart_create(const sealbart_config_t* cfg, int device, sealbart_t** out);
 void sealbart_free(sealbart_t* m);
 /* Copies one tensor of an HF BartForConditionalGeneration state_dict (float32, host pointer,
  * row-major, `numel` elements) by its state_dict key, e.g.
- * "model.decoder.layers.3.encoder_attn.q_proj.weight".  Unknown keys return SEALFM_EINVAL. */
+ * "model.decoder.layers.3.encoder_attn.q_proj.weight".  Unknown keys return SEALFM_EINVAL.
+ * gemm_mode 6 (bf16 weights, for bf16 checkpoints; any handle kind): every GEMM weight matrix, the token-embedding
+ * table and an untied lm_head are stored once, in bf16, rounded to nearest-even here -- exact for values that are
+ * bf16 already.  Biases, LayerNorm / RMSNorm weights, position tables, T5 relative-attention tables and
+ * final_logits_bias stay fp32.  The GEMMs multiply the bf16 W by the activation split into three bf16 pieces
+ * (exact for 2^-100 <= |x| < (2 - 2^-8) 2^127), so each product is exact and only the fp32 accumulation rounds; bf16 has fp32's
+ * exponent range, so error_flag [1] is never raised, sealdec_generate never re-runs ("overflow_fallbacks" stays 0) and
+ * the GEMM sets last_paths bit 24, never 12 or 14.  The mode is fixed at creation: sealbart_set_option "gemm_mode"
+ * refuses to switch into or out of 6 (SEALFM_EINVAL).
+ * sealbart_device_bytes: the bytes of the weights on the device -- in gemm_mode 6, 2 per matrix element plus 4 per
+ * element of every fp32 vector and table; in the other modes 4 per element of everything plus the modes' split
+ * copies (2 x 2 bytes per matrix element for 3 / 5, and 2 x 4 more once 3xTF32 has run). */
 int  sealbart_set_tensor(sealbart_t* m, const char* key, const float* host, uint64_t numel);
 /* After all tensors are set: checks completeness, ties lm_head to model.shared if it was not
  * given, derives fused/pre-split copies. */
@@ -261,7 +273,7 @@ int sealdec_generate_dx_ex(sealbart_t* model, const sealfm_t* fm, const uint32_t
                            int32_t* error_flag_d, int64_t src_tokens_hint, const sealdec_groups_t* groups);
 
 /* Options: "cuda_graph" (-1 auto, 0 off, 1 on), "gemm_mode" (switch between the 3xFP16 modes 3/5 and 2 = 3xTF32;
- * the TF32 operand copies are made on first use), "fused_head" (-1 = $SEALB200_FUSED_HEAD, default on; 0 = the
+ * the TF32 operand copies are made on first use; never into or out of 6), "fused_head" (-1 = $SEALB200_FUSED_HEAD, default on; 0 = the
  * lm_head stores every logit and the select kernel streams them for the log-softmax statistics; 1 = where the select
  * kernels read only the row's allowed tokens, the lm_head emits per-tile statistics and stores only those logits),
  * "poison_logits" (testing: 1 fills the logits buffer with NaN before every such lm_head), "query_slices" (-1 =
@@ -292,7 +304,9 @@ int sealdec_generate_dx_ex(sealbart_t* model, const sealfm_t* fm, const uint32_t
  * and of the pre-LayerNorm forward (sealbart_create_ex; it also sets 0 .. 7 and 10 .. 15 as BART does, never 8 / 9;
  * bit 19 names its ReLU feed-forward, e.g. Pegasus's):
  *  22 embedding / add + LayerNorm, one CTA per row (preln_row_kernel; folds a pending split-K GEMM)
- *  23 the embedding form of 22 with layernorm_embedding (mBART: two LayerNorms in one launch) */
+ *  23 the embedding form of 22 with layernorm_embedding (mBART: two LayerNorms in one launch)
+ * and, for any handle kind:
+ *  24 3xBF16 GEMM (gemm_mode 6; such a call never sets 12, 13 or 14) */
 int     sealbart_set_option(sealbart_t* model, const char* name, int64_t value);
 int64_t sealbart_get_stat(const sealbart_t* model, const char* name);
 
@@ -330,15 +344,16 @@ int sealdec_debug_step_logits_ex(sealbart_t* model, const int64_t* input_ids, co
                                  int64_t Q, int64_t S, int32_t num_beams, const int64_t* decoder_input_ids,
                                  int64_t t, const int32_t* ancestry, int64_t src_tokens_hint, float* out_logits);
 /* Stand-alone GEMM C[M,N] = A[M,K] W[N,K]^T + bias (+GELU) through the model's GEMM kernels
- * (mode 2 = 3xTF32, 3 = 3xFP16, 5 = 3xFP16 on CTA pairs), host pointers; if iters > 0 also reports the average
+ * (mode 2 = 3xTF32, 3 = 3xFP16, 5 = 3xFP16 on CTA pairs, 6 = 3xBF16 with W rounded to bf16 as sealbart_set_tensor
+ * rounds it), host pointers; if iters > 0 also reports the average
  * device time per call (CUDA events, includes the activation split). */
 int sealdec_debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A, const float* W,
                        const float* bias, float* C, int32_t gelu, int32_t iters, double* avg_us);
 /* the same with the tile order (mode 3 without split-K; other paths ignore band) and the store as variables
  * (tools/head_bench.py): band -1 = the order the decoder
  * uses, 0 = no bands (m fastest over all rows when N > M), > 0 = bands of that many 128-row tiles; store 0 = the
- * epilogue writes nothing (C may be NULL, and is not written).  Modes 3 / 5 split A into halves once, outside the
- * timed calls, as the decoder's producers do. */
+ * epilogue writes nothing (C may be NULL, and is not written).  Modes 3 / 5 split A into halves (mode 6 into three
+ * bf16 pieces) once, outside the timed calls, as the decoder's producers do. */
 int sealdec_debug_gemm_ex(int mode, int64_t M, int32_t N, int32_t K, const float* A, const float* W,
                           const float* bias, float* C, int32_t gelu, int32_t iters, double* avg_us, int32_t band,
                           int32_t store);
@@ -352,6 +367,9 @@ int sealdec_debug_gemm_ex(int mode, int64_t M, int32_t N, int32_t K, const float
  * statistics, as the decoder then does. */
 int sealdec_debug_head(int64_t M, int32_t N, int32_t K, const float* A, const float* W, const float* bias,
                        const uint32_t* mask, int32_t eos, int32_t pad, float* C, float* stats, int32_t* fused);
+/* sealdec_debug_head in gemm_mode 3 or 6 (W rounded to bf16); any other mode is SEALFM_EINVAL. */
+int sealdec_debug_head_ex(int mode, int64_t M, int32_t N, int32_t K, const float* A, const float* W, const float* bias,
+                          const uint32_t* mask, int32_t eos, int32_t pad, float* C, float* stats, int32_t* fused);
 /* One decode step's selection (log-softmax statistics or the top-k warp of p->top_k, processors, index mask, top-2*beam, the scorer bookkeeping,
  * the records and the LF step) on caller-supplied inputs, through the same kernel dispatch as the generate entry
  * points.  Host pointers; B = p->num_beams, T = p->max_length, R = Q*B, W = ceil(V/32), G from `groups` (NULL = 1).

@@ -93,14 +93,40 @@ class IndexBasedLogitsProcessor:
         return out
 
 
+# 2-D state_dict tensors that are tables read in fp32, not GEMM operands or the token embedding: they do not take part
+# in choosing the bf16-weight mode
+_FP32_TABLES = ("embed_positions.weight", "relative_attention_bias.weight")
+
+
+def _is_weight_matrix(key, tensor):
+    return key.endswith(".weight") and tensor.dim() == 2 and not key.endswith(_FP32_TABLES)
+
+
+def default_gemm_mode(state_dict):
+    """The gemm_mode an engine gets when none is given: $SEALB200_GEMM if set; else 6 (3xBF16, the weights stored once in
+    bf16) when every weight matrix the GEMMs and the embedding read is torch.bfloat16; else 3 (3xFP16).  fp32, fp16 and
+    mixed-dtype models therefore keep the fp32-master path (their weights are upcast, which is lossless)."""
+    env = os.environ.get("SEALB200_GEMM")
+    if env is not None:
+        return int(env)
+    torch = _torch()
+    mats = [v for k, v in state_dict.items() if _is_weight_matrix(k, v)]
+    return 6 if mats and all(v.dtype == torch.bfloat16 for v in mats) else 3
+
+
+def _weight_dtypes(model):
+    """The set of parameter dtypes of a model: `model.to(torch.bfloat16)` converts in place and changes it."""
+    return frozenset(p.dtype for p in model.parameters())
+
+
 class SealBartEngine:
     """Device-resident BART weights + workspace (include/sealdec.h `sealbart_t`)."""
 
     def __init__(self, state_dict, config, device=0, gemm_mode=None):
-        # gemm_mode: 3 = 3xFP16 with one CTA per tile (default), 5 = 3xFP16 in 2-CTA clusters sharing the W tile, 2 = 3xTF32
-        # (fp32 range, the automatic fallback on fp16 overflow).  $SEALB200_GEMM overrides the default.
+        # gemm_mode: 3 = 3xFP16 with one CTA per tile, 5 = 3xFP16 in 2-CTA clusters sharing the W tile, 2 = 3xTF32 (fp32
+        # range, the automatic fallback on fp16 overflow), 6 = 3xBF16 with bf16 weights; None: default_gemm_mode.
         if gemm_mode is None:
-            gemm_mode = int(os.environ.get("SEALB200_GEMM", "3"))
+            gemm_mode = default_gemm_mode(state_dict)
         self.gemm_mode = int(gemm_mode)
         d = int(config.d_model)
         self.config = config
@@ -250,7 +276,7 @@ class SealT5Engine(SealBartEngine):
 
     def __init__(self, state_dict, config, device=0, gemm_mode=None, generation_config=None):
         if gemm_mode is None:
-            gemm_mode = int(os.environ.get("SEALB200_GEMM", "3"))
+            gemm_mode = default_gemm_mode(state_dict)
         cfg = t5_native_config(config, gemm_mode)
         self.gemm_mode = int(gemm_mode)
         self.config = T5ConfigView(config, generation_config)
@@ -341,7 +367,7 @@ class SealPreLnEngine(SealBartEngine):
 
     def __init__(self, state_dict, config, device=0, gemm_mode=None):
         if gemm_mode is None:
-            gemm_mode = int(os.environ.get("SEALB200_GEMM", "3"))
+            gemm_mode = default_gemm_mode(state_dict)
         cfg, var = preln_native_config(config, gemm_mode)
         self.config = PreLnConfigView(config)
         self.gemm_mode = int(gemm_mode)
@@ -390,13 +416,16 @@ _ENGINES = weakref.WeakKeyDictionary()
 
 
 def _engine_for(model):
+    """The engine of an HF model, built on first use and cached per model object and weight dtypes (a model converted
+    in place, e.g. by `.to(torch.bfloat16)`, gets an engine of the new format)."""
     if isinstance(model, SealBartEngine):
         return model
-    eng = _ENGINES.get(model)
-    if eng is None:
-        eng = SealBartEngine.from_hf(model)
-        _ENGINES[model] = eng
-    return eng
+    key = _weight_dtypes(model)
+    hit = _ENGINES.get(model)
+    if hit is None or hit[0] != key:
+        hit = (key, SealBartEngine.from_hf(model))
+        _ENGINES[model] = hit
+    return hit[1]
 
 
 def _make_params(cfg, num_beams, min_length, max_length, length_penalty, eos_token_id, force_decoding_from,
@@ -791,7 +820,7 @@ def fm_index_generate(model, index: FMIndex, input_ids, attention_mask, min_leng
                                   max_length, length_penalty, num_beams, eos_token_id, force_decoding_from, always_allow_eos,
                                   disable_fm_index, stop_at_count, forced_bos, src_tokens=-2, top_k=top_k, check_positions=False)
     rec = out.host()
-    if rec["errors"][1] and eng.gemm_mode >= 3:        # fp16 range exceeded: redo with the 3xTF32 kernels (sealdec.h)
+    if rec["errors"][1] and eng.gemm_mode in (3, 5):   # fp16 range exceeded: redo with the 3xTF32 kernels (sealdec.h)
         check(lib.sealbart_set_option(eng._h, b"gemm_mode", 2))
         try:
             rec = generate_records_device(eng, index, torch.from_numpy(ids_np).to(dev), torch.from_numpy(am_np).to(dev), min_length,

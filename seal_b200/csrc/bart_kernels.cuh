@@ -3,6 +3,7 @@
 // seal/beam_search.py:231-238,481-483).  Post-LN encoder/decoder layers, learned positions with
 // offset 2, layernorm_embedding, exact-erf GELU, tied lm_head + final_logits_bias.
 #pragma once
+#include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -105,12 +106,58 @@ __device__ __forceinline__ void store_split2(const SplitOut& so, int64_t idx, co
     }
 }
 
+// The operand split of the 3xBF16 GEMM (gemm_mode 6): x = b1 + b2 + b3, each piece the round-to-nearest bf16 of what the
+// previous pieces leave.  Each residual is exact in fp32 and has at most 16, then 8 significant bits, so the three
+// pieces carry x exactly for every 2^-100 <= |x| < (2 - 2^-8) 2^127 (below, b3 may be a bf16 subnormal; from the upper
+// bound on, which only the last 2^-8 of fp32's range reaches, b1 rounds to infinity); bf16 has fp32's exponent range,
+// so nothing saturates.  A producer of a gemm_mode 6 model takes this type in place of SplitOut (its
+// kernels are instantiated per split type); b1 == nullptr: no split wanted.
+struct SplitBf16 { __nv_bfloat16* b1 = nullptr; __nv_bfloat16* b2 = nullptr; __nv_bfloat16* b3 = nullptr; };
+__device__ __forceinline__ void bf16x3_split1(float x, __nv_bfloat16& p1, __nv_bfloat16& p2, __nv_bfloat16& p3) {
+    p1 = __float2bfloat16_rn(x);
+    const float r = x - __bfloat162float(p1);
+    p2 = __float2bfloat16_rn(r);
+    p3 = __float2bfloat16_rn(r - __bfloat162float(p2));
+}
+__device__ __forceinline__ uint32_t bf16_pack(__nv_bfloat16 a, __nv_bfloat16 b) {
+    return (uint32_t)__bfloat16_as_ushort(a) | ((uint32_t)__bfloat16_as_ushort(b) << 16);
+}
+__device__ __forceinline__ void store_split4(const SplitBf16& so, int64_t idx, const float4& o) {
+    if (!so.b1) return;
+    __nv_bfloat16 p[3][4];
+    bf16x3_split1(o.x, p[0][0], p[1][0], p[2][0]); bf16x3_split1(o.y, p[0][1], p[1][1], p[2][1]);
+    bf16x3_split1(o.z, p[0][2], p[1][2], p[2][2]); bf16x3_split1(o.w, p[0][3], p[1][3], p[2][3]);
+    __nv_bfloat16* dst[3] = {so.b1, so.b2, so.b3};
+#pragma unroll
+    for (int j = 0; j < 3; ++j)
+        *reinterpret_cast<uint2*>(dst[j] + idx) = make_uint2(bf16_pack(p[j][0], p[j][1]), bf16_pack(p[j][2], p[j][3]));
+}
+__device__ __forceinline__ void store_split2(const SplitBf16& so, int64_t idx, const float2& o) {
+    if (!so.b1) return;
+    __nv_bfloat16 p[3][2];
+    bf16x3_split1(o.x, p[0][0], p[1][0], p[2][0]); bf16x3_split1(o.y, p[0][1], p[1][1], p[2][1]);
+    *reinterpret_cast<uint32_t*>(so.b1 + idx) = bf16_pack(p[0][0], p[0][1]);
+    *reinterpret_cast<uint32_t*>(so.b2 + idx) = bf16_pack(p[1][0], p[1][1]);
+    *reinterpret_cast<uint32_t*>(so.b3 + idx) = bf16_pack(p[2][0], p[2][1]);
+}
+
+// Element type of the token-embedding table a producer with split type SO gathers from: bf16 in gemm_mode 6
+template <class SO> struct EmbOf { using type = float; };
+template <> struct EmbOf<SplitBf16> { using type = __nv_bfloat16; };
+template <class SO> using EmbT = typename EmbOf<SO>::type;
+__device__ __forceinline__ float4 load_emb4(const float* p) { return *reinterpret_cast<const float4*>(p); }
+__device__ __forceinline__ float4 load_emb4(const __nv_bfloat16* p) {
+    const uint2 u = *reinterpret_cast<const uint2*>(p);
+    return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xFFFF0000u), __uint_as_float(u.y << 16),
+                       __uint_as_float(u.y & 0xFFFF0000u));
+}
+
 // LayerNorm of one row held as `per` float4 per lane (d = 128*per), torch semantics:
 // biased variance, eps inside the sqrt, fp32.
-template <int MAXV>
+template <int MAXV, class SO>
 __device__ __forceinline__ void warp_layernorm(float4 (&v)[MAXV], int nv, int d, const float* __restrict__ gamma,
                                                const float* __restrict__ beta, float eps, float* __restrict__ out,
-                                               const SplitOut& so, int64_t row_off, int lane) {
+                                               const SO& so, int64_t row_off, int lane) {
     float s = 0.f;
 #pragma unroll
     for (int i = 0; i < MAXV; ++i) if (i < nv) s += v[i].x + v[i].y + v[i].z + v[i].w;
@@ -141,25 +188,26 @@ constexpr int kLnMaxVec = 8;     // d_model <= 1024
 
 // out[r] = LN(embed[tok[r]] * scale + pos_table[pos(r) + 2])      (BartEncoder/BartDecoder embedding)
 // tok: int32, row r reads tok[r * tok_stride].  pos(r) = pos_const if pos_per_row == nullptr else pos_per_row[r].
+template <class SO>
 __global__ void __launch_bounds__(128) embed_ln_kernel(int64_t rows, int d, const int32_t* __restrict__ tok,
                                                        int64_t tok_stride,
                                                        const int32_t* __restrict__ pos_per_row, int pos_const,
-                                                       const float* __restrict__ embed, float scale,
+                                                       const EmbT<SO>* __restrict__ embed, float scale,
                                                        const float* __restrict__ pos_table,
                                                        const float* __restrict__ gamma, const float* __restrict__ beta,
-                                                       float* __restrict__ out, SplitOut so) {
+                                                       float* __restrict__ out, SO so) {
     const int lane = threadIdx.x & 31;
     const int64_t r = blockIdx.x * 4LL + (threadIdx.x >> 5);
     if (r >= rows) return;
     const int nv = d / 128;
-    const float* e = embed + (int64_t)tok[r * tok_stride] * d;
+    const EmbT<SO>* e = embed + (int64_t)tok[r * tok_stride] * d;
     const int p = (pos_per_row ? pos_per_row[r] : pos_const) + 2;
     const float* pe = pos_table + (int64_t)p * d;
     float4 v[kLnMaxVec];
 #pragma unroll
     for (int i = 0; i < kLnMaxVec; ++i) if (i < nv) {
         const int col = (i * 32 + lane) * 4;
-        const float4 a = *reinterpret_cast<const float4*>(e + col);
+        const float4 a = load_emb4(e + col);
         const float4 b = *reinterpret_cast<const float4*>(pe + col);
         v[i] = make_float4(a.x * scale + b.x, a.y * scale + b.y, a.z * scale + b.z, a.w * scale + b.w);
     }
@@ -169,10 +217,11 @@ __global__ void __launch_bounds__(128) embed_ln_kernel(int64_t rows, int d, cons
 // out[r] = LN(a[r] + b[r])     (residual + sub-layer output, post-LN)
 // (Folding the split-K finish pass of the preceding GEMM into this kernel was tried: at 300 rows it has 75 CTAs and
 // became slower than the two separate kernels -- reverted.)
+template <class SO>
 __global__ void __launch_bounds__(128) add_ln_kernel(int64_t rows, int d, const float* __restrict__ a,
                                                      const float* __restrict__ b, const float* __restrict__ gamma,
                                                      const float* __restrict__ beta, float* __restrict__ out,
-                                                     SplitOut so) {
+                                                     SO so) {
     const int lane = threadIdx.x & 31;
     const int64_t r = blockIdx.x * 4LL + (threadIdx.x >> 5);
     if (r >= rows) return;
@@ -193,10 +242,11 @@ __global__ void __launch_bounds__(128) add_ln_kernel(int64_t rows, int d, const 
 // (312 launches per generate at batch 20).
 // bsrc: b may still be the raw split-K output of the preceding GEMM (SplitSrc) -- the finish launch of o / co / fc2 is folded in
 // (the same fold into the warp-per-row kernel was slower: 75 CTAs at 300 rows; here a row has its own 128 threads).
+template <class SO>
 __global__ void __launch_bounds__(128) add_ln_row_kernel(int64_t rows, int d, const float* __restrict__ a,
                                                          const float* __restrict__ b, const float* __restrict__ gamma,
                                                          const float* __restrict__ beta, float* __restrict__ out,
-                                                         SplitOut so, SplitSrc bsrc) {
+                                                         SO so, SplitSrc bsrc) {
     __shared__ float red[2][4];
     const int64_t r = blockIdx.x;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -295,7 +345,8 @@ __device__ __forceinline__ float2 warp_attend(const float* __restrict__ q_head, 
     return make_float2(ax / l, ay / l);
 }
 
-__device__ __forceinline__ void store_attn(float2 o, int64_t idx, float* __restrict__ out, const SplitOut& so) {
+template <class SO>
+__device__ __forceinline__ void store_attn(float2 o, int64_t idx, float* __restrict__ out, const SO& so) {
     if (out) *reinterpret_cast<float2*>(out + idx) = o;
     store_split2(so, idx, o);
 }
@@ -375,11 +426,11 @@ __device__ __forceinline__ void self_attend_head(const float* __restrict__ qp, c
     o1 = make_float4(a1.x * inv, a1.y * inv, a1.z * inv, a1.w * inv);
 }
 
-template <int ROUNDS>
+template <int ROUNDS, class SO>
 __global__ void __launch_bounds__(512, ROUNDS <= 3 ? 2 : 1) dec_self_attn_kernel(int64_t R, int d, int heads, int cur_pos, int T,
                                                                const float* __restrict__ qkv, float* kc, float* vc,
                                                                const int32_t* __restrict__ anc,
-                                                               float* __restrict__ out, SplitOut so, int row_mul, int bcast) {
+                                                               float* __restrict__ out, SO so, int row_mul, int bcast) {
     // row_mul / bcast: at the first decode step all beams of a query are the same row (same start token, same
     // source), so the step runs on one row per query: compact row r stands for physical rows r*row_mul ..
     // r*row_mul + bcast - 1, whose cache entries all receive this row's k / v (any of them may become the
@@ -424,10 +475,11 @@ __global__ void __launch_bounds__(512, ROUNDS <= 3 ? 2 : 1) dec_self_attn_kernel
 // grid (Q, heads), block 32 * B threads, dynamic smem self_attn_query_smem(P, B).
 __host__ __device__ inline size_t self_attn_query_smem(int P, int B) { return (size_t)2 * P * B * kHeadDim * 4 + (size_t)2 * P * 32 * 4 + 128 * 4; }
 
+template <class SO>
 __global__ void __launch_bounds__(1024) dec_self_attn_query_kernel(int64_t R, int B, int d, int cur_pos, int T,
                                                                   const float* __restrict__ qkv, float* kc, float* vc,
                                                                   const int32_t* __restrict__ anc,
-                                                                  float* __restrict__ out, SplitOut so, SplitSrc qsrc) {
+                                                                  float* __restrict__ out, SO so, SplitSrc qsrc) {
     extern __shared__ __align__(16) unsigned char sa_smem[];
     const int P = cur_pos + 1;
     float* Ks = reinterpret_cast<float*>(sa_smem);                       // [P][B][64]
@@ -506,10 +558,11 @@ struct AncestryKV {
     __device__ __forceinline__ const float* v(int s) const { return s == cur_pos ? vcur : vc + ((int64_t)s * R + arow[s]) * d + col; }
 };
 
+template <class SO>
 __global__ void __launch_bounds__(512) dec_self_attn_long_kernel(int64_t R, int d, int heads, int cur_pos, int T,
                                                                  const float* __restrict__ qkv, float* kc, float* vc,
                                                                  const int32_t* __restrict__ anc,
-                                                                 float* __restrict__ out, SplitOut so) {
+                                                                 float* __restrict__ out, SO so) {
     __shared__ __align__(16) float q_s[16][kHeadDim];
     const int64_t r = blockIdx.x;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -538,9 +591,9 @@ struct GroupAddr {
     const int32_t* mask;                     // [n_keys], 0 = padded key; nullptr = every key valid (packed sources)
 };
 
-template <int NW, int MAXP>
+template <int NW, int MAXP, class SO>
 __device__ __forceinline__ void grouped_attention(const GroupAddr& g, int rows, int n_keys, int head_off, int64_t out_base,
-                                                  int64_t out_stride, float* __restrict__ out, const SplitOut& so) {
+                                                  int64_t out_stride, float* __restrict__ out, const SO& so) {
     __shared__ float Kt[kHeadDim][33];
     __shared__ __align__(16) float Vs[32][kHeadDim];
     __shared__ __align__(16) float q_s[NW * MAXP][kHeadDim];
@@ -624,12 +677,13 @@ constexpr int kGAttnWarps = 8, kGAttnPasses = 2;               // 16 rows per sw
 // group x head) = the rows that attend to the same source: by default the `beams` rows of query g;
 // with grp_query/grp_start (ragged groups, teacher-forced re-scoring) rows grp_start[g]..grp_start[g+1]
 // of query grp_query[g].
+template <class SO>
 __global__ void __launch_bounds__(kGAttnWarps * 32) cross_attn_kernel(int64_t G, int d, int heads, int beams, int S,
                                                          const float* __restrict__ q, const float* __restrict__ ckv,
                                                          const int32_t* __restrict__ src_mask,
                                                          const int32_t* __restrict__ grp_query,
                                                          const int32_t* __restrict__ grp_start, float* __restrict__ out,
-                                                         SplitOut so, const int32_t* __restrict__ src_off) {
+                                                         SO so, const int32_t* __restrict__ src_off) {
     // src_off (packed sources): query qi's encoder states are rows src_off[qi] .. src_off[qi+1] of ckv, all valid
     const int64_t gi = blockIdx.x;
     const int h = blockIdx.y;
@@ -650,12 +704,13 @@ __global__ void __launch_bounds__(kGAttnWarps * 32) cross_attn_kernel(int64_t G,
 // sweep spends two shared-memory reads per FMA.  Same ragged-group arguments as
 // cross_attn_kernel.
 constexpr int kXKeys = 32, kXRows = 16, kXPad = kHeadDim + 4;
+template <class SO>
 __global__ void __launch_bounds__(128) cross_attn_small_kernel(int64_t G, int d, int heads, int beams, int S_pad,
                                                                const float* __restrict__ q, const float* __restrict__ ckv,
                                                                const int32_t* __restrict__ src_mask,
                                                                const int32_t* __restrict__ grp_query,
                                                                const int32_t* __restrict__ grp_start, float* __restrict__ out,
-                                                               SplitOut so, const int32_t* __restrict__ src_off, SplitSrc qsrc) {
+                                                               SO so, const int32_t* __restrict__ src_off, SplitSrc qsrc) {
     __shared__ __align__(16) float Ks[kXKeys][kXPad];
     __shared__ __align__(16) float Vs[kXKeys][kHeadDim];
     __shared__ __align__(16) float Qs[kXRows][kHeadDim];
@@ -744,10 +799,11 @@ __global__ void __launch_bounds__(128) cross_attn_small_kernel(int64_t G, int d,
 
 // Encoder self attention over the S positions of the same query (bidirectional, key padding mask).
 // qkv [Q*S][3d].  grid (Q, heads).
+template <class SO>
 __global__ void __launch_bounds__(kGAttnWarps * 32) enc_self_attn_kernel(int64_t Q, int d, int heads, int S,
                                                             const float* __restrict__ qkv,
                                                             const int32_t* __restrict__ src_mask,
-                                                            float* __restrict__ out, SplitOut so,
+                                                            float* __restrict__ out, SO so,
                                                             const int32_t* __restrict__ src_off) {
     const int64_t qi = blockIdx.x;
     const int h = blockIdx.y;

@@ -28,6 +28,7 @@ struct Lin {
     float* w = nullptr; float* b = nullptr; int out = 0, in = 0;
     float* w_hi = nullptr; float* w_lo = nullptr;          // TF32 split copies (gemm_mode 2)
     __half* w_h1 = nullptr; __half* w_h2 = nullptr;        // FP16 split copies of W * 2^s (gemm_mode 3)
+    __nv_bfloat16* w_bf = nullptr;                         // gemm_mode 6: the only copy of W (w is null)
     float w_unscale = 1.f;                                 // 2^-s
     CUtensorMap map_hi{}, map_lo{}; bool maps_ready = false;
     CUtensorMap map2_hi{}, map2_lo{}; bool maps2_ready = false;   // 64-row boxes: one CTA's half of a cluster's W tile (gemm_mode 5)
@@ -78,11 +79,13 @@ struct sealbart {
     float* shared = nullptr; float* enc_pos = nullptr; float* dec_pos = nullptr;
     float* lm_head = nullptr; float* final_bias = nullptr;
     bool lm_head_given = false;
+    // gemm_mode 6: the token-embedding / tied lm_head table and an untied lm_head in bf16 (shared / lm_head stay null)
+    __nv_bfloat16* shared_bf = nullptr; __nv_bfloat16* lm_head_bf = nullptr;
     LNp enc_ln_emb, dec_ln_emb;
     Lin head;
     std::vector<EncLayerW> enc;
     std::vector<DecLayerW> dec;
-    struct Slot { float* dst; uint64_t numel; };
+    struct Slot { void* dst; uint64_t numel; bool bf16 = false; };     // bf16: rounded (RNE) into a bf16 matrix (gemm_mode 6)
     std::map<std::string, Slot> slots;
     std::set<std::string> loaded;
     std::vector<void*> allocs;
@@ -145,13 +148,42 @@ float* dalloc(sealbart* m, uint64_t numel) {
     return static_cast<float*>(p);
 }
 
-void make_lin(sealbart* m, Lin& l, int out, int in) { l.out = out; l.in = in; l.w = dalloc(m, (uint64_t)out * in); l.b = dalloc(m, out); }
+__nv_bfloat16* dalloc_bf16(sealbart* m, uint64_t numel) {
+    void* p = nullptr;
+    CUDA_CHECK(cudaMalloc(&p, std::max<uint64_t>(numel, 1) * 2));
+    CUDA_CHECK(cudaMemset(p, 0, std::max<uint64_t>(numel, 1) * 2));
+    m->allocs.push_back(p);
+    m->weight_bytes += numel * 2;
+    return static_cast<__nv_bfloat16*>(p);
+}
+
+// gemm_mode 6 stores every GEMM weight matrix (and the embedding table) once, in bf16; the other modes keep the fp32
+// master and derive their splits from it at finalize
+bool bf16_weights(const sealbart* m) { return m->cfg.gemm_mode == 6; }
+
+void make_lin(sealbart* m, Lin& l, int out, int in) {
+    l.out = out; l.in = in;
+    if (bf16_weights(m)) l.w_bf = dalloc_bf16(m, (uint64_t)out * in);
+    else l.w = dalloc(m, (uint64_t)out * in);
+    l.b = dalloc(m, out);
+}
 void make_ln(sealbart* m, LNp& l, int d) { l.g = dalloc(m, d); l.b = dalloc(m, d); }
 
 void reg(sealbart* m, const std::string& key, float* dst, uint64_t numel) { m->slots[key] = {dst, numel}; }
+void reg_mat(sealbart* m, const std::string& key, Lin& l, int row0, int rows) {
+    const uint64_t off = (uint64_t)row0 * l.in, n = (uint64_t)rows * l.in;
+    if (l.w_bf) m->slots[key] = {l.w_bf + off, n, true};
+    else reg(m, key, l.w + off, n);
+}
 void reg_lin(sealbart* m, const std::string& prefix, Lin& l, int row0, int rows) {
-    reg(m, prefix + ".weight", l.w + (uint64_t)row0 * l.in, (uint64_t)rows * l.in);
+    reg_mat(m, prefix + ".weight", l, row0, rows);
     reg(m, prefix + ".bias", l.b + row0, rows);
+}
+// the [V][d] token-embedding table under `key`
+void make_shared(sealbart* m, const std::string& key) {
+    const uint64_t n = (uint64_t)m->cfg.vocab_size * m->cfg.d_model;
+    if (bf16_weights(m)) { m->shared_bf = dalloc_bf16(m, n); m->slots[key] = {m->shared_bf, n, true}; }
+    else { m->shared = dalloc(m, n); reg(m, key, m->shared, n); }
 }
 void reg_ln(sealbart* m, const std::string& prefix, LNp& l, int d) {
     reg(m, prefix + ".weight", l.g, d);
@@ -163,7 +195,7 @@ void build_slots_t5(sealbart* m) {
     const auto& c = m->cfg;
     const int d = c.d_model, f = c.ffn_dim, V = c.vocab_size, nb = m->t5.relative_attention_num_buckets, H = c.heads;
     const bool gated = m->t5.ffn_kind == 1;
-    m->shared = dalloc(m, (uint64_t)V * d); reg(m, "shared.weight", m->shared, (uint64_t)V * d);
+    make_shared(m, "shared.weight");
     m->final_bias = dalloc(m, V);                                          // zero: T5's lm_head has no bias
     m->enc_ln_emb.g = dalloc(m, d); reg(m, "encoder.final_layer_norm.weight", m->enc_ln_emb.g, d);
     m->dec_ln_emb.g = dalloc(m, d); reg(m, "decoder.final_layer_norm.weight", m->dec_ln_emb.g, d);
@@ -171,7 +203,7 @@ void build_slots_t5(sealbart* m) {
     reg(m, "encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight", m->t5_rel_enc, (uint64_t)nb * H);
     m->t5_rel_dec = dalloc(m, (uint64_t)nb * H);
     reg(m, "decoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight", m->t5_rel_dec, (uint64_t)nb * H);
-    auto reg_w = [&](const std::string& key, Lin& l, int row0, int rows) { reg(m, key + ".weight", l.w + (uint64_t)row0 * l.in, (uint64_t)rows * l.in); };
+    auto reg_w = [&](const std::string& key, Lin& l, int row0, int rows) { reg_mat(m, key + ".weight", l, row0, rows); };
     auto ffn = [&](const std::string& p, Lin& fc1, Lin& fc2) {
         make_lin(m, fc1, gated ? 2 * f : f, d);
         if (gated) { reg_w(p + "DenseReluDense.wi_0", fc1, 0, f); reg_w(p + "DenseReluDense.wi_1", fc1, f, f); }
@@ -210,7 +242,7 @@ void build_slots(sealbart* m) {
     const auto& c = m->cfg;
     const bool preln = m->arch == 2;
     const int d = c.d_model, f = c.ffn_dim, V = c.vocab_size, P = c.max_positions + (preln ? m->variant.position_offset : 2);
-    m->shared = dalloc(m, (uint64_t)V * d); reg(m, "model.shared.weight", m->shared, (uint64_t)V * d);
+    make_shared(m, "model.shared.weight");
     m->enc_pos = dalloc(m, (uint64_t)P * d); reg(m, "model.encoder.embed_positions.weight", m->enc_pos, (uint64_t)P * d);
     m->dec_pos = dalloc(m, (uint64_t)P * d); reg(m, "model.decoder.embed_positions.weight", m->dec_pos, (uint64_t)P * d);
     m->final_bias = dalloc(m, V); reg(m, "final_logits_bias", m->final_bias, V);
@@ -277,13 +309,14 @@ EncodeTiledFn encode_tiled() {
     }
     return fn;
 }
-// row-major [rows][K] fp32 (or fp16), box = 128 bytes of K x box_rows, 128B swizzle, zero fill out of bounds
-void make_map(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t K, uint64_t ld, uint32_t box_rows, bool half = false) {
+// row-major [rows][K] fp32 (or fp16, or bf16), box = 128 bytes of K x box_rows, 128B swizzle, zero fill out of bounds
+void make_map(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t K, uint64_t ld, uint32_t box_rows, bool half = false, bool bf16 = false) {
     cuuint64_t dims[2] = {K, rows};
     cuuint64_t strides[1] = {ld * (half ? 2 : 4)};
     cuuint32_t box[2] = {(cuuint32_t)(128 / (half ? 2 : 4)), box_rows};
     cuuint32_t estr[2] = {1, 1};
-    CUresult r = encode_tiled()(map, half ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(ptr), dims, strides, box, estr,
+    const CUtensorMapDataType dt = bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : half ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+    CUresult r = encode_tiled()(map, dt, 2, const_cast<void*>(ptr), dims, strides, box, estr,
                                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) throw ApiError(SEALFM_ECUDA, "cuTensorMapEncodeTiled failed (" + std::to_string((int)r) + ")");
@@ -301,7 +334,7 @@ enum : uint32_t {
     kPathSplitKDeferred = 1u << 10, kPathSplitKFinish = 1u << 11, kPathGemmFullTile = 1u << 12, kPathGemmCluster = 1u << 13,
     kPathGemmTf32 = 1u << 14, kPathQuerySlices = 1u << 15,
     kPathT5EncAttn = 1u << 16, kPathT5DecAttn = 1u << 17, kPathT5Rms = 1u << 18, kPathT5Relu = 1u << 19, kPathT5Gate = 1u << 20,
-    kPathT5RmsWide = 1u << 21, kPathPreLn = 1u << 22, kPathPreLnEmbedLn = 1u << 23,
+    kPathT5RmsWide = 1u << 21, kPathPreLn = 1u << 22, kPathPreLnEmbedLn = 1u << 23, kPathGemmBf16 = 1u << 24,
 };
 
 void split_into(cudaStream_t s, const float* x, float* hi, float* lo, uint64_t numel) {
@@ -316,6 +349,7 @@ void split_into(cudaStream_t s, const float* x, float* hi, float* lo, uint64_t n
 struct Act {
     float* x = nullptr; float* hi = nullptr; float* lo = nullptr;   // fp32 / TF32 split
     __half* h1 = nullptr; __half* h2 = nullptr;                     // FP16 split
+    __nv_bfloat16* b1 = nullptr; __nv_bfloat16* b2 = nullptr; __nv_bfloat16* b3 = nullptr;   // 3xBF16 split
 };
 
 SplitOut split_of(const Act& a, int* overflow) {
@@ -325,20 +359,34 @@ SplitOut split_of(const Act& a, int* overflow) {
     return so;
 }
 
+// f(so) with the split output a producer of activation a writes: SplitBf16 in gemm_mode 6, SplitOut (split_of)
+// otherwise.  The producer kernels are instantiated per split type, so f launches kernel<decltype(so)>.
+template <typename F> void with_split(const sealbart* m, const Act& a, F&& f) {
+    if (m->cfg.gemm_mode == 6) f(SplitBf16{a.b1, a.b2, a.b3});
+    else f(split_of(a, m->ovf));
+}
+// the embedding table a producer with split type SO gathers from
+template <class SO> const EmbT<SO>* embed_table(const sealbart* m) {
+    if constexpr (std::is_same<SO, SplitBf16>::value) return m->shared_bf;
+    else return m->shared;
+}
+
 // Buffers hi / lo (and plain, if not null) as an Act from element off on: the TF32 split in gemm_mode 2, the fp16
-// split in the 3xFP16 modes.  plain is null for activations whose producers write the split only.
+// split in the 3xFP16 modes, the three bf16 pieces in gemm_mode 6 (b1 and b3 in the two halves of hi -- every split
+// buffer holds 4 bytes per element -- b2 in lo).  plain is null for activations whose producers write the split only.
 Act act_view(int gemm_mode, float* plain, const Buf& hi, const Buf& lo, int64_t off = 0) {
     Act a;
     if (plain) a.x = plain + off;
     if (gemm_mode == 2) { a.hi = hi.as<float>() + off; a.lo = lo.as<float>() + off; }
-    if (gemm_mode >= 3) { a.h1 = hi.as<__half>() + off; a.h2 = lo.as<__half>() + off; }
+    else if (gemm_mode == 6) { a.b1 = hi.as<__nv_bfloat16>() + off; a.b2 = lo.as<__nv_bfloat16>() + off; a.b3 = hi.as<__nv_bfloat16>() + hi.bytes / 4 + off; }
+    else if (gemm_mode >= 3) { a.h1 = hi.as<__half>() + off; a.h2 = lo.as<__half>() + off; }
     return a;
 }
 
 template <typename T, int ACT, int CL, bool HEAD = false>
 void gemm_launch(cudaStream_t s, int ctas, const CUtensorMap& ahi, const CUtensorMap& alo, const CUtensorMap& whi, const CUtensorMap& wlo,
                  int64_t M, int N, int K, const float* bias, float w_unscale, float* C, T* C1, T* C2, int ldc, int n_fastest, int m_band,
-                 int* ovf, int k_slices, int64_t slice_stride, const HeadEpi& he = HeadEpi{}) {
+                 int* ovf, int k_slices, int64_t slice_stride, const HeadEpi& he = HeadEpi{}, T* C3 = nullptr) {
     auto kern = wgmma_gemm_x3_kernel<T, ACT, CL, HEAD>;
     CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, G_SMEM));
     cudaLaunchAttribute attr[1];
@@ -348,7 +396,7 @@ void gemm_launch(cudaStream_t s, int ctas, const CUtensorMap& ahi, const CUtenso
     cfg.gridDim = dim3((unsigned)ctas); cfg.blockDim = dim3(GTHREADS); cfg.dynamicSmemBytes = G_SMEM; cfg.stream = s;
     cfg.attrs = attr; cfg.numAttrs = 1;
     CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, ahi, alo, whi, wlo, (int)M, N, K, bias, w_unscale, C, C1, C2, ldc, n_fastest, m_band, ovf,
-                                  k_slices, slice_stride, he));
+                                  k_slices, slice_stride, he, C3));
 }
 
 // f(std::integral_constant<int, ACT>{}) for the epilogue activation act: kernels are instantiated per activation
@@ -375,6 +423,30 @@ void gemm(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, const
     m->gemm_flops += 2.0 * (double)M * N * K;
 }
 
+// K slices of a 3xFP16 / 3xBF16 GEMM of `tiles` output tiles: skinny problems (a few tiles for the whole GPU) split K
+// so that the serial K loop of a tile is spread over up to 8 CTAs, then sum the partial tiles in a fixed order
+int split_k_slices(int tiles, int kblocks) {
+    int k_slices = 1;
+    static const int force_slices = [] { const char* e = std::getenv("SEALB200_KSLICES"); return e ? std::atoi(e) : 0; }();
+    if (tiles * 2 <= sm_count() && kblocks >= 4) {
+        k_slices = std::min(8, std::min(kblocks / 2, sm_count() / tiles));
+        if (force_slices > 0) k_slices = std::min(force_slices, kblocks);     // experiments only
+        while (k_slices > 1 && kblocks % k_slices) --k_slices;
+    }
+    return k_slices;
+}
+
+// m fastest with more A than a band holds (the lm_head at thousands of rows): bands of m tiles whose A pieces (a_bytes
+// per element: 4 for the two halves, 6 for three bf16 pieces) take <= 8 MB of the 50 MB L2, so A is read from HBM once
+// and W once per band (wgmma_gemm.cuh, tile_coords).  8 MB (16 tiles at K = 1 024 in 3xFP16) measured fastest of
+// 4 / 8 / 16 / 32 MB bands for the lm_head at 15 000 rows (tools/head_bench.py); the band shares the L2 with the
+// streaming W tiles and the logits stores.
+int band_tiles(const sealbart* m, int n_fastest, int64_t M, int K, int a_bytes) {
+    const int64_t a_tile_bytes = (int64_t)GM * K * a_bytes, band_bytes = 8ll << 20;
+    const int band = (!n_fastest && M * K * a_bytes > band_bytes) ? (int)std::max<int64_t>(1, band_bytes / a_tile_bytes) : 0;
+    return m->gemm_band >= 0 ? m->gemm_band : band;
+}
+
 void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, const Act& C, int ldc, int act) {
     if (M == 0) return;
     if (act == kActRelu) cx.m->last_paths |= kPathT5Relu;
@@ -384,7 +456,59 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
     Buf& splitk = cx.slice ? m->splitk1 : m->splitk;
     const int tiles = (int)(((N + GN - 1) / GN) * ((M + GM - 1) / GM));
     const int n_fastest = ((int64_t)M >= (int64_t)N) ? 1 : 0;     // stream the larger operand once
-    if (m->cfg.gemm_mode >= 3 && K % UK16 == 0 && lda == K && l.w_h1) {
+    if (m->cfg.gemm_mode == 6 && K % UK16 == 0 && lda == K && l.w_bf) {
+        // 3xBF16: bf16 W, A in three bf16 pieces (pre-split by the producers); the 3xFP16 path's tile walk, split-K and
+        // bands; no cluster form and no overflow flag
+        const __nv_bfloat16 *p1 = A.b1, *p2 = A.b2, *p3 = A.b3;
+        if (!p1) {
+            a_hi.ensure((size_t)M * K * 4); a_lo.ensure((size_t)M * K * 2);
+            __nv_bfloat16* h = a_hi.as<__nv_bfloat16>();
+            const int blocks = (int)std::min<int64_t>(((int64_t)M * K + 255) / 256, (int64_t)sm_count() * 8);
+            split_bf16x3_kernel<<<blocks, 256, 0, cx.s>>>((int64_t)M * K, A.x, h, a_lo.as<__nv_bfloat16>(), h + (size_t)M * K);
+            CUDA_CHECK(cudaGetLastError()); m->launches++;
+            p1 = h; p2 = a_lo.as<__nv_bfloat16>(); p3 = h + (size_t)M * K;
+        }
+        CUtensorMap ma1, ma2, ma3;
+        make_map(&ma1, p1, M, K, K, GM, true, true); make_map(&ma2, p2, M, K, K, GM, true, true); make_map(&ma3, p3, M, K, K, GM, true, true);
+        if (!l.maps_ready) { make_map(&l.map_hi, l.w_bf, N, K, K, GN, true, true); l.maps_ready = true; }
+        m->last_paths |= kPathGemmBf16;
+        const int k_slices = split_k_slices(tiles, K / UK16);
+        if (k_slices > 1) {
+            const int64_t slice_stride = (int64_t)M * ldc;
+            splitk.ensure((size_t)k_slices * slice_stride * 4);
+            float* part = splitk.as<float>();
+            const int ctas2 = std::min(tiles * k_slices, sm_count());
+            gemm_launch<__nv_bfloat16, kActNone, 1>(cx.s, ctas2, ma1, ma2, l.map_hi, ma3, M, N, K, nullptr, 1.0f, part, nullptr, nullptr, ldc, n_fastest, 0,
+                                                    m->ovf, k_slices, slice_stride);
+            m->launches++;
+            if (M <= cx.defer_rows && act == kActNone && !C.b1 && ldc == N && l.b) {     // summed by the consumer kernel
+                cx.pending = SplitSrc{part, k_slices, slice_stride, l.b, 1.0f};
+                m->last_paths |= kPathSplitKDeferred;
+                return;
+            }
+            const int fblocks = (int)std::min<int64_t>((M * (ldc / 4) + 255) / 256, (int64_t)sm_count() * 8);
+            with_act(act, [&](auto A) {
+                launch_k(gemm_splitk_finish_kernel<decltype(A)::value, __nv_bfloat16>, fblocks, 256, 0, cx.s, M, N, ldc, k_slices, slice_stride, part, l.b, 1.0f,
+                         C.x, C.b1, C.b2, m->ovf, C.b3);
+            });
+            CUDA_CHECK(cudaGetLastError()); m->launches++; m->last_paths |= kPathSplitKFinish;
+            return;
+        }
+        const int band = band_tiles(m, n_fastest, M, K, 6);
+        const int ctas = std::min(tiles, sm_count());
+        if (cx.head.stats && act == kActNone) {
+            gemm_launch<__nv_bfloat16, kActNone, 1, true>(cx.s, ctas, ma1, ma2, l.map_hi, ma3, M, N, K, l.b, 1.0f, C.x, nullptr, nullptr, ldc, n_fastest, band,
+                                                          m->ovf, 1, 0, cx.head);
+            cx.head_fused = true;
+        } else
+            with_act(act, [&](auto A) {
+                gemm_launch<__nv_bfloat16, decltype(A)::value, 1>(cx.s, ctas, ma1, ma2, l.map_hi, ma3, M, N, K, l.b, 1.0f, C.x, C.b1, C.b2, ldc, n_fastest, band,
+                                                                  m->ovf, 1, 0, HeadEpi{}, C.b3);
+            });
+        m->launches++;
+        return;
+    }
+    if ((m->cfg.gemm_mode == 3 || m->cfg.gemm_mode == 5) && K % UK16 == 0 && lda == K && l.w_h1) {
         // 3xFP16; operands pre-split into halves by the producers
         const __half* a1 = A.h1; const __half* a2 = A.h2;
         if (!a1) {
@@ -398,16 +522,7 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
         make_map(&ma1, a1, M, K, K, GM, true); make_map(&ma2, a2, M, K, K, GM, true);
         if (!l.maps_ready) { make_map(&l.map_hi, l.w_h1, N, K, K, GN, true); make_map(&l.map_lo, l.w_h2, N, K, K, GN, true); l.maps_ready = true; }
         int* ovf = m->ovf;
-        // skinny problems (a few tiles for the whole GPU): split K so that the serial K loop of a tile is spread
-        // over up to 8 CTAs, then sum the partial tiles in a fixed order
-        const int kblocks = K / UK16;
-        int k_slices = 1;
-        static const int force_slices = [] { const char* e = std::getenv("SEALB200_KSLICES"); return e ? std::atoi(e) : 0; }();
-        if (tiles * 2 <= sm_count() && kblocks >= 4) {
-            k_slices = std::min(8, std::min(kblocks / 2, sm_count() / tiles));
-            if (force_slices > 0) k_slices = std::min(force_slices, kblocks);     // experiments only
-            while (k_slices > 1 && kblocks % k_slices) --k_slices;
-        }
+        const int k_slices = split_k_slices(tiles, K / UK16);
         if (m->cfg.gemm_mode == 5 && k_slices == 1 && M > GM) {
             // clusters of 2 CTAs on vertically adjacent tiles: the W tile is loaded once (TMA multicast) for both
             if (!l.maps2_ready) { make_map(&l.map2_hi, l.w_h1, N, K, K, GN / 2, true); make_map(&l.map2_lo, l.w_h2, N, K, K, GN / 2, true); l.maps2_ready = true; }
@@ -434,18 +549,13 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
             }
             const int fblocks = (int)std::min<int64_t>((M * (ldc / 4) + 255) / 256, (int64_t)sm_count() * 8);
             with_act(act, [&](auto A) {
-                launch_k(gemm_splitk_finish_kernel<decltype(A)::value>, fblocks, 256, 0, cx.s, M, N, ldc, k_slices, slice_stride, part, l.b, l.w_unscale, C.x, C.h1, C.h2, ovf);
+                launch_k(gemm_splitk_finish_kernel<decltype(A)::value>, fblocks, 256, 0, cx.s, M, N, ldc, k_slices, slice_stride, part, l.b, l.w_unscale, C.x, C.h1, C.h2, ovf,
+                         (__half*)nullptr);
             });
             CUDA_CHECK(cudaGetLastError()); m->launches++; m->last_paths |= kPathSplitKFinish;
             return;
         }
-        // m fastest with more A than a band holds (the lm_head at thousands of rows): bands of m tiles whose A halves
-        // take <= 8 MB of the 50 MB L2, so A is read from HBM once and W once per band (wgmma_gemm.cuh, tile_coords).
-        // 8 MB (16 tiles at K = 1 024) measured fastest of 4 / 8 / 16 / 32 MB bands for the lm_head at 15 000 rows
-        // (tools/head_bench.py); the band shares the L2 with the streaming W tiles and the logits stores.
-        const int64_t a_tile_bytes = (int64_t)GM * K * 4, band_bytes = 8ll << 20;
-        int band = (!n_fastest && M * K * 4 > band_bytes) ? (int)std::max<int64_t>(1, band_bytes / a_tile_bytes) : 0;
-        if (m->gemm_band >= 0) band = m->gemm_band;
+        const int band = band_tiles(m, n_fastest, M, K, 4);
         const int ctas = std::min(tiles, sm_count());
         if (cx.head.stats && act == kActNone) {
             gemm_launch<__half, kActNone, 1, true>(cx.s, ctas, ma1, ma2, l.map_hi, l.map_lo, M, N, K, l.b, l.w_unscale, C.x, nullptr, nullptr, ldc, n_fastest, band, ovf, 1, 0, cx.head);
@@ -474,17 +584,19 @@ void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, 
         m->launches++; m->last_paths |= kPathGemmTf32;
         return;
     }
-    throw ApiError(SEALFM_EINVAL, "GEMM: K must be a multiple of 64 (3xFP16) / 32 (3xTF32) with contiguous operands");
+    throw ApiError(SEALFM_EINVAL, "GEMM: K must be a multiple of 64 (3xFP16, 3xBF16) / 32 (3xTF32) with contiguous operands");
 }
 
 void add_ln(Ctx& cx, int64_t rows, int d, const float* a, const float* b, const LNp& ln, const Act& out) {
     const SplitSrc ps = cx.pending;
     cx.pending = SplitSrc{};
-    if (rows <= kAddLnRowMax)          // small batches: a CTA per row (and the split-K finish of the GEMM before it, if pending)
-        launch_k(add_ln_row_kernel, (unsigned)rows, 128, 0, cx.s, rows, d, a, b, (const float*)ln.g, (const float*)ln.b, out.x,
-                 split_of(out, cx.m->ovf), ps);
-    else
-        launch_k(add_ln_kernel, (unsigned)((rows + 3) / 4), 128, 0, cx.s, rows, d, a, b, (const float*)ln.g, (const float*)ln.b, out.x, split_of(out, cx.m->ovf));
+    with_split(cx.m, out, [&](auto so) {
+        using SO = decltype(so);
+        if (rows <= kAddLnRowMax)          // small batches: a CTA per row (and the split-K finish of the GEMM before it, if pending)
+            launch_k(add_ln_row_kernel<SO>, (unsigned)rows, 128, 0, cx.s, rows, d, a, b, (const float*)ln.g, (const float*)ln.b, out.x, so, ps);
+        else
+            launch_k(add_ln_kernel<SO>, (unsigned)((rows + 3) / 4), 128, 0, cx.s, rows, d, a, b, (const float*)ln.g, (const float*)ln.b, out.x, so);
+    });
     cx.m->launches++;
     cx.m->last_paths |= rows <= kAddLnRowMax ? kPathAddLnRow : kPathAddLnWarp;
 }
@@ -609,8 +721,11 @@ void t5_rms(Ctx& cx, int64_t rows, int d, const int32_t* tok, int64_t tok_stride
     const SplitSrc ps = cx.pending;
     cx.pending = SplitSrc{};
     const bool wide = d > 4 * 128 * kT5RmsVec;
-    launch_k(wide ? t5_rms_row_kernel<kT5RmsVecWide> : t5_rms_row_kernel<kT5RmsVec>, (unsigned)rows, 128, 0, cx.s, rows, d, tok, tok_stride,
-             (const float*)cx.m->shared, x.x, b, ps, w, cx.m->t5.layer_norm_epsilon, out_scale, split_of(x, cx.m->ovf));
+    with_split(cx.m, x, [&](auto so) {
+        using SO = decltype(so);
+        launch_k(wide ? t5_rms_row_kernel<kT5RmsVecWide, SO> : t5_rms_row_kernel<kT5RmsVec, SO>, (unsigned)rows, 128, 0, cx.s, rows, d, tok, tok_stride,
+                 embed_table<SO>(cx.m), x.x, b, ps, w, cx.m->t5.layer_norm_epsilon, out_scale, so);
+    });
     cx.m->launches++;
     cx.m->last_paths |= wide ? kPathT5RmsWide : kPathT5Rms;
 }
@@ -621,7 +736,7 @@ void t5_ffn(Ctx& cx, int64_t rows, int d, int f, const Act& x, Lin& fc1, Lin& fc
     if (m->t5.ffn_kind == 1) {
         gemm(cx, rows, 2 * f, d, x, d, fc1, Act{ffn2}, 2 * f, kActNone);
         const int blocks = (int)std::max<int64_t>(1, std::min<int64_t>((rows * (f / 4) + 255) / 256, (int64_t)sm_count() * 8));
-        launch_k(t5_gate_kernel, (unsigned)blocks, 256, 0, cx.s, rows, f, (const float*)ffn2, split_of(ffn, m->ovf));
+        with_split(m, ffn, [&](auto so) { launch_k(t5_gate_kernel<decltype(so)>, (unsigned)blocks, 256, 0, cx.s, rows, f, (const float*)ffn2, so); });
         m->launches++; m->last_paths |= kPathT5Gate;
     } else
         gemm(cx, rows, f, d, x, d, fc1, ffn, f, kActRelu);
@@ -656,12 +771,15 @@ void cross_attention(Ctx& cx, const Dims& D, const DecStep& S, int l, int64_t de
     cx.pending = SplitSrc{};
     const int64_t groups = D.grp_start ? D.G : D.Q;
     const float* ckv_l = m->ckv.as<float>() + (size_t)l * S.Tk * 2 * d + S.ckv_q0;
-    if (D.S <= kXKeys)
-        launch_k(cross_attn_small_kernel, dim3((unsigned)groups, heads), 128, 0, cx.s, groups, d, heads, S.compact ? 1 : D.B, (int)D.S, (const float*)S.cq.x,
-                 ckv_l, S.m32, D.grp_query, D.grp_start, S.attn.x, split_of(S.attn, m->ovf), S.soff_x, cq_src);
-    else
-        launch_k(cross_attn_kernel, dim3((unsigned)groups, heads), kGAttnWarps * 32, 0, cx.s, groups, d, heads, S.compact ? 1 : D.B, (int)D.S, (const float*)S.cq.x,
-                 ckv_l, S.m32, D.grp_query, D.grp_start, S.attn.x, split_of(S.attn, m->ovf), S.soff_x);
+    with_split(m, S.attn, [&](auto so) {
+        using SO = decltype(so);
+        if (D.S <= kXKeys)
+            launch_k(cross_attn_small_kernel<SO>, dim3((unsigned)groups, heads), 128, 0, cx.s, groups, d, heads, S.compact ? 1 : D.B, (int)D.S, (const float*)S.cq.x,
+                     ckv_l, S.m32, D.grp_query, D.grp_start, S.attn.x, so, S.soff_x, cq_src);
+        else
+            launch_k(cross_attn_kernel<SO>, dim3((unsigned)groups, heads), kGAttnWarps * 32, 0, cx.s, groups, d, heads, S.compact ? 1 : D.B, (int)D.S, (const float*)S.cq.x,
+                     ckv_l, S.m32, D.grp_query, D.grp_start, S.attn.x, so, S.soff_x);
+    });
     m->launches++;
     m->last_paths |= D.S <= kXKeys ? kPathCrossSmall : kPathCrossGrouped;
     cx.defer_rows = defer_rows;
@@ -678,8 +796,10 @@ void t5_encoder_layers(Ctx& cx, const Dims& D, int64_t Te, const Acts& A, const 
     for (int i = 0; i < n; ++i) {
         EncLayerW& L = m->enc[i];
         gemm(cx, Te, 3 * d, d, A.x, d, L.qkv, A.qkv, 3 * d, kActNone);
-        launch_k(t5_enc_self_attn_kernel<kGAttnWarps, kGAttnPasses>, dim3((unsigned)D.Q, m->cfg.heads), kGAttnWarps * 32, 0, cx.s, D.Q, d,
-                 (int)D.S, (const float*)A.qkv.x, m32, rb, split_of(A.attn, m->ovf), soff);
+        with_split(m, A.attn, [&](auto so) {
+            launch_k(t5_enc_self_attn_kernel<kGAttnWarps, kGAttnPasses, decltype(so)>, dim3((unsigned)D.Q, m->cfg.heads), kGAttnWarps * 32, 0, cx.s, D.Q, d,
+                     (int)D.S, (const float*)A.qkv.x, m32, rb, so, soff);
+        });
         m->launches++; m->last_paths |= kPathT5EncAttn;
         cx.defer_rows = INT64_MAX;
         gemm(cx, Te, d, d, A.attn, d, L.o, A.tmp, d, kActNone);
@@ -704,8 +824,10 @@ void t5_decoder_layers(Ctx& cx, const Dims& D, const DecStep& S) {
         float* kc = m->kc.as<float>() + (size_t)l * D.T * S.Rc * d + D.r0 * d;
         float* vc = m->vc.as<float>() + (size_t)l * D.T * S.Rc * d + D.r0 * d;
         gemm(cx, S.R, 3 * d, d, S.x, d, L.qkv, S.qkv, 3 * d, kActNone);
-        launch_k(t5_dec_self_attn_kernel, (unsigned)S.R, 32 * std::min(heads, 16), 0, cx.s, S.Rc, d, heads, S.pos, D.T, (const float*)S.qkv.x, kc, vc,
-                 S.anc, rb, split_of(S.attn, m->ovf), S.row_mul, S.row_mul);
+        with_split(m, S.attn, [&](auto so) {
+            launch_k(t5_dec_self_attn_kernel<decltype(so)>, (unsigned)S.R, 32 * std::min(heads, 16), 0, cx.s, S.Rc, d, heads, S.pos, D.T, (const float*)S.qkv.x, kc, vc,
+                     S.anc, rb, so, S.row_mul, S.row_mul);
+        });
         m->launches++; m->last_paths |= kPathT5DecAttn;
         cx.defer_rows = INT64_MAX;
         gemm(cx, S.R, d, d, S.attn, d, L.o, S.tmp, d, kActNone);
@@ -723,13 +845,18 @@ void bart_encoder_layers(Ctx& cx, const Dims& D, int64_t Te, const Acts& A, cons
     sealbart* m = cx.m;
     const int d = D.d, heads = m->cfg.heads;
     const float scale = m->cfg.scale_embedding ? sqrtf((float)d) : 1.0f;
-    embed_ln_kernel<<<(unsigned)((Te + 3) / 4), 128, 0, cx.s>>>(Te, d, tok, 1, pos, 0, m->shared, scale, m->enc_pos,
-                                                                m->enc_ln_emb.g, m->enc_ln_emb.b, A.x.x, split_of(A.x, m->ovf));
+    with_split(m, A.x, [&](auto so) {
+        using SO = decltype(so);
+        embed_ln_kernel<SO><<<(unsigned)((Te + 3) / 4), 128, 0, cx.s>>>(Te, d, tok, 1, pos, 0, embed_table<SO>(m), scale, m->enc_pos,
+                                                                        m->enc_ln_emb.g, m->enc_ln_emb.b, A.x.x, so);
+    });
     CUDA_CHECK(cudaGetLastError()); m->launches++;
     for (auto& L : m->enc) {
         gemm(cx, Te, 3 * d, d, A.x, d, L.qkv, A.qkv, 3 * d, kActNone);
-        enc_self_attn_kernel<<<dim3((unsigned)D.Q, heads), kGAttnWarps * 32, 0, cx.s>>>(D.Q, d, heads, (int)D.S, A.qkv.x, m32, A.attn.x,
-                                                                                       split_of(A.attn, m->ovf), soff);
+        with_split(m, A.attn, [&](auto so) {
+            enc_self_attn_kernel<decltype(so)><<<dim3((unsigned)D.Q, heads), kGAttnWarps * 32, 0, cx.s>>>(D.Q, d, heads, (int)D.S, A.qkv.x, m32, A.attn.x,
+                                                                                                          so, soff);
+        });
         CUDA_CHECK(cudaGetLastError()); m->launches++;
         cx.defer_rows = kAddLnRowMax;
         gemm(cx, Te, d, d, A.attn, d, L.o, A.tmp, d, kActNone);
@@ -748,7 +875,6 @@ void bart_encoder_layers(Ctx& cx, const Dims& D, int64_t Te, const Acts& A, cons
 void bart_self_attention(Ctx& cx, const Dims& D, const DecStep& S, int l) {
     sealbart* m = cx.m;
     const int d = D.d, heads = m->cfg.heads, pos = S.pos;
-    int* ovf = m->ovf;
     DecLayerW& L = m->dec[l];
     float* kc = m->kc.as<float>() + (size_t)l * D.T * S.Rc * d + D.r0 * d;
     float* vc = m->vc.as<float>() + (size_t)l * D.T * S.Rc * d + D.r0 * d;
@@ -764,17 +890,20 @@ void bart_self_attention(Ctx& cx, const Dims& D, const DecStep& S, int l) {
     cx.pending = SplitSrc{};
     const unsigned sa_threads = 32 * std::min(heads, 16);
     const float* qkv = S.qkv.x;
-    if (use_saq) {
-        static size_t saq_set = 0;
-        if (saq_smem > saq_set) { CUDA_CHECK(cudaFuncSetAttribute(dec_self_attn_query_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024)); saq_set = 112 * 1024; }
-        launch_k(dec_self_attn_query_kernel, dim3((unsigned)D.Q, heads), 32 * D.B, saq_smem, cx.s, S.Rc, D.B, d, pos, D.T, qkv, kc, vc, S.anc,
-                 S.attn.x, split_of(S.attn, ovf), qkv_src);
-    } else if (pos + 1 <= 12)
-        launch_k(dec_self_attn_kernel<3>, (unsigned)S.R, sa_threads, 0, cx.s, S.Rc, d, heads, pos, D.T, qkv, kc, vc, S.anc, S.attn.x, split_of(S.attn, ovf), S.row_mul, S.row_mul);
-    else if (pos + 1 <= 32)
-        launch_k(dec_self_attn_kernel<8>, (unsigned)S.R, sa_threads, 0, cx.s, S.Rc, d, heads, pos, D.T, qkv, kc, vc, S.anc, S.attn.x, split_of(S.attn, ovf), S.row_mul, S.row_mul);
-    else
-        launch_k(dec_self_attn_long_kernel, (unsigned)S.R, sa_threads, 0, cx.s, S.Rc, d, heads, pos, D.T, qkv, kc, vc, S.anc, S.attn.x, split_of(S.attn, ovf));
+    with_split(m, S.attn, [&](auto so) {
+        using SO = decltype(so);
+        if (use_saq) {
+            static size_t saq_set = 0;                     // per instantiation
+            if (saq_smem > saq_set) { CUDA_CHECK(cudaFuncSetAttribute(dec_self_attn_query_kernel<SO>, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024)); saq_set = 112 * 1024; }
+            launch_k(dec_self_attn_query_kernel<SO>, dim3((unsigned)D.Q, heads), 32 * D.B, saq_smem, cx.s, S.Rc, D.B, d, pos, D.T, qkv, kc, vc, S.anc,
+                     S.attn.x, so, qkv_src);
+        } else if (pos + 1 <= 12)
+            launch_k(dec_self_attn_kernel<3, SO>, (unsigned)S.R, sa_threads, 0, cx.s, S.Rc, d, heads, pos, D.T, qkv, kc, vc, S.anc, S.attn.x, so, S.row_mul, S.row_mul);
+        else if (pos + 1 <= 32)
+            launch_k(dec_self_attn_kernel<8, SO>, (unsigned)S.R, sa_threads, 0, cx.s, S.Rc, d, heads, pos, D.T, qkv, kc, vc, S.anc, S.attn.x, so, S.row_mul, S.row_mul);
+        else
+            launch_k(dec_self_attn_long_kernel<SO>, (unsigned)S.R, sa_threads, 0, cx.s, S.Rc, d, heads, pos, D.T, qkv, kc, vc, S.anc, S.attn.x, so);
+    });
     m->launches++;
     m->last_paths |= use_saq ? kPathSelfQuery : pos + 1 <= 12 ? kPathSelfRounds3 : pos + 1 <= 32 ? kPathSelfRounds8 : kPathSelfLong;
 }
@@ -782,10 +911,12 @@ void bart_self_attention(Ctx& cx, const Dims& D, const DecStep& S, int l) {
 void bart_decoder_layers(Ctx& cx, const Dims& D, const DecStep& S) {
     sealbart* m = cx.m;
     const int d = D.d, pos = S.pos;
-    int* ovf = m->ovf;
     const float scale = m->cfg.scale_embedding ? sqrtf((float)d) : 1.0f;
-    launch_k(embed_ln_kernel, (unsigned)((S.R + 3) / 4), 128, 0, cx.s, S.R, d, S.tokens + pos, (int64_t)(D.T * S.row_mul), (const int32_t*)nullptr, pos,
-             (const float*)m->shared, scale, (const float*)m->dec_pos, (const float*)m->dec_ln_emb.g, (const float*)m->dec_ln_emb.b, S.x.x, split_of(S.x, ovf));
+    with_split(m, S.x, [&](auto so) {
+        using SO = decltype(so);
+        launch_k(embed_ln_kernel<SO>, (unsigned)((S.R + 3) / 4), 128, 0, cx.s, S.R, d, S.tokens + pos, (int64_t)(D.T * S.row_mul), (const int32_t*)nullptr, pos,
+                 embed_table<SO>(m), scale, (const float*)m->dec_pos, (const float*)m->dec_ln_emb.g, (const float*)m->dec_ln_emb.b, S.x.x, so);
+    });
     m->launches++;
     for (int l = 0; l < m->cfg.decoder_layers; ++l) {
         DecLayerW& L = m->dec[l];
@@ -822,8 +953,14 @@ PreLnEmbed preln_embed(const sealbart* m, const int32_t* tok, int64_t tok_stride
 void preln_norm(Ctx& cx, int64_t rows, int d, const PreLnEmbed& em, const Act& x, const float* b, const LNp& ln) {
     const SplitSrc ps = cx.pending;
     cx.pending = SplitSrc{};
-    launch_k(preln_row_kernel, (unsigned)rows, 128, 0, cx.s, rows, d, em, x.x, b, ps, (const float*)ln.g, (const float*)ln.b,
-             split_of(x, cx.m->ovf));
+    with_split(cx.m, x, [&](auto so) {
+        using SO = decltype(so);
+        PreLnEmbedT<EmbT<SO>> e;                           // em with the table in the mode's element type
+        e.tok = em.tok; e.tok_stride = em.tok_stride; e.pos = em.pos; e.pos_const = em.pos_const; e.pos_offset = em.pos_offset;
+        e.pos_rows = em.pos_rows; e.embed = em.tok ? embed_table<SO>(cx.m) : nullptr; e.scale = em.scale; e.pos_table = em.pos_table;
+        e.ln_g = em.ln_g; e.ln_b = em.ln_b;
+        launch_k(preln_row_kernel<SO>, (unsigned)rows, 128, 0, cx.s, rows, d, e, x.x, b, ps, (const float*)ln.g, (const float*)ln.b, so);
+    });
     cx.m->launches++;
     cx.m->last_paths |= kPathPreLn | (em.tok && em.ln_g ? kPathPreLnEmbedLn : 0u);
 }
@@ -846,8 +983,10 @@ void preln_encoder_layers(Ctx& cx, const Dims& D, int64_t Te, const Acts& A, con
     for (int i = 0; i < n; ++i) {
         EncLayerW& L = m->enc[i];
         gemm(cx, Te, 3 * d, d, A.x, d, L.qkv, A.qkv, 3 * d, kActNone);
-        launch_k(enc_self_attn_kernel, dim3((unsigned)D.Q, heads), kGAttnWarps * 32, 0, cx.s, D.Q, d, heads, (int)D.S, (const float*)A.qkv.x,
-                 m32, A.attn.x, split_of(A.attn, m->ovf), soff);
+        with_split(m, A.attn, [&](auto so) {
+            launch_k(enc_self_attn_kernel<decltype(so)>, dim3((unsigned)D.Q, heads), kGAttnWarps * 32, 0, cx.s, D.Q, d, heads, (int)D.S, (const float*)A.qkv.x,
+                     m32, A.attn.x, so, soff);
+        });
         m->launches++;
         cx.defer_rows = INT64_MAX;
         gemm(cx, Te, d, d, A.attn, d, L.o, A.tmp, d, kActNone);
@@ -1066,8 +1205,21 @@ int require_device() {
 }
 
 void check_gemm_mode(int mode) {
-    if (mode != 2 && mode != 3 && mode != 5)
-        throw ApiError(SEALFM_EINVAL, "gemm_mode must be 3 (3xFP16, one CTA per tile, default), 5 (3xFP16 on 2-CTA clusters) or 2 (3xTF32)");
+    if (mode != 2 && mode != 3 && mode != 5 && mode != 6)
+        throw ApiError(SEALFM_EINVAL, "gemm_mode must be 3 (3xFP16, one CTA per tile, default), 5 (3xFP16 on 2-CTA clusters), 2 (3xTF32) "
+                                      "or 6 (3xBF16, bf16 weights)");
+}
+
+// fp32 -> bf16 bits, round to nearest even (the weights of a bf16 checkpoint pass through exactly); NaN stays NaN
+uint16_t bf16_rne(float x) {
+    uint32_t u; std::memcpy(&u, &x, 4);
+    if ((u & 0x7FFFFFFFu) > 0x7F800000u) return (uint16_t)((u >> 16) | 0x40u);
+    return (uint16_t)((u + 0x7FFFu + ((u >> 16) & 1u)) >> 16);
+}
+std::vector<uint16_t> to_bf16(const float* x, uint64_t n, float scale = 1.f) {
+    std::vector<uint16_t> out(n);
+    for (uint64_t i = 0; i < n; ++i) out[i] = bf16_rne(x[i] * scale);
+    return out;
 }
 
 // sealt5_create's shape checks (before any allocation)
@@ -1176,7 +1328,7 @@ void sealbart_free(sealbart_t* m) {
     cudaSetDevice(m->device);
     for (void* p : m->allocs) cudaFree(p);
     for (void* p : m->split_allocs) cudaFree(p);
-    if (m->lm_head_given) cudaFree(m->lm_head);
+    if (m->lm_head_given) cudaFree(m->lm_head_bf ? (void*)m->lm_head_bf : (void*)m->lm_head);
     if (m->slice_fork) cudaEventDestroy(m->slice_fork);
     if (m->slice_join) cudaEventDestroy(m->slice_join);
     if (m->slice_stream) cudaStreamDestroy(m->slice_stream);
@@ -1194,6 +1346,12 @@ int sealbart_set_tensor(sealbart_t* m, const char* key, const float* host, uint6
         if (k == "lm_head.weight") {
             const uint64_t want = (uint64_t)m->cfg.vocab_size * m->cfg.d_model;
             if (numel != want) throw ApiError(SEALFM_EINVAL, "lm_head.weight: wrong size");
+            if (bf16_weights(m)) {
+                if (!m->lm_head_given) { CUDA_CHECK(cudaMalloc(&m->lm_head_bf, want * 2)); m->lm_head_given = true; m->weight_bytes += want * 2; }
+                const std::vector<uint16_t> b = to_bf16(host, want);
+                CUDA_CHECK(cudaMemcpy(m->lm_head_bf, b.data(), want * 2, cudaMemcpyHostToDevice));
+                return;
+            }
             if (!m->lm_head_given) { CUDA_CHECK(cudaMalloc(&m->lm_head, want * 4)); m->lm_head_given = true; m->weight_bytes += want * 4; }
             CUDA_CHECK(cudaMemcpy(m->lm_head, host, want * 4, cudaMemcpyHostToDevice));
             return;
@@ -1204,7 +1362,11 @@ int sealbart_set_tensor(sealbart_t* m, const char* key, const float* host, uint6
         if (it == m->slots.end()) throw ApiError(SEALFM_EINVAL, "unknown state_dict key: " + k);
         if (it->second.numel != numel) throw ApiError(SEALFM_EINVAL, "wrong element count for " + k);
         static const std::string kCrossQ = ".layer.1.EncDecAttention.q.weight";
-        if (m->arch == 1 && k.size() > kCrossQ.size() && k.compare(k.size() - kCrossQ.size(), kCrossQ.size(), kCrossQ) == 0) {
+        const bool cross_q = m->arch == 1 && k.size() > kCrossQ.size() && k.compare(k.size() - kCrossQ.size(), kCrossQ.size(), kCrossQ) == 0;
+        if (it->second.bf16) {                                 // gemm_mode 6: rounded into the bf16 matrix (x 8 below is exact)
+            const std::vector<uint16_t> b = to_bf16(host, numel, cross_q ? 8.f : 1.f);
+            CUDA_CHECK(cudaMemcpy(it->second.dst, b.data(), numel * 2, cudaMemcpyHostToDevice));
+        } else if (cross_q) {
             // T5 does not scale attention scores; the cross-attention kernels multiply by 0.125, so q is stored times 8
             // (a power of two: (8q . k) * 0.125 == q . k exactly)
             std::vector<float> q8(host, host + numel);
@@ -1222,14 +1384,17 @@ int sealbart_finalize(sealbart_t* m) {
         if (!m) throw ApiError(SEALFM_EINVAL, "null model");
         for (auto& kv : m->slots)
             if (!m->loaded.count(kv.first)) throw ApiError(SEALFM_EINVAL, "state_dict tensor missing: " + kv.first);
-        if (!m->lm_head_given) m->lm_head = m->shared;          // tied (seal/utils.py:48-49; T5: tie_word_embeddings)
+        if (!m->lm_head_given) { m->lm_head = m->shared; m->lm_head_bf = nullptr; }   // tied (seal/utils.py:48-49; T5: tie_word_embeddings)
         m->head.w = m->lm_head; m->head.b = m->final_bias; m->head.out = m->cfg.vocab_size; m->head.in = m->cfg.d_model;
+        m->head.w_bf = m->lm_head_given ? m->lm_head_bf : m->shared_bf;
         CUDA_CHECK(cudaSetDevice(m->device));
         for (void* p : m->split_allocs) cudaFree(p);
         m->split_allocs.clear();
         m->tf32_ready = false;
         for_each_lin(m, [](Lin& l) { l.maps_ready = false; l.maps2_ready = false; });
-        if (m->cfg.gemm_mode >= 3) {
+        if (bf16_weights(m)) {
+            // the bf16 matrices are the GEMM operands as loaded: nothing to derive
+        } else if (m->cfg.gemm_mode >= 3) {
             unsigned int* d_max = nullptr;
             CUDA_CHECK(cudaMalloc(&d_max, 4)); m->err.ensure(16); CUDA_CHECK(cudaMemset(m->err.p, 0, 16));
             for_each_lin(m, [&](Lin& l) { split_lin_half(m, l, d_max); });
@@ -1439,7 +1604,7 @@ void generate_enqueue(Ctx& cx, const Dims& D, const GenArgs& a, const FmView& vi
         const int eff_len = cur_len - (p->forced_bos_token_id >= 0 ? 1 : 0);
         HeadEpi he{};
         if (fused_head_on(m) && !dead && !compact && !p->disable_fm_index && eff_len > 1 && G == 1 && c.top_k == 0 &&
-            m->cfg.gemm_mode == 3) {
+            (m->cfg.gemm_mode == 3 || m->cfg.gemm_mode == 6)) {
             he = HeadEpi{m->st_hstat.as<float2>() + PD.r0 * head_tiles, mk[cur] + PD.r0 * D.W, (int)D.W, p->eos_token_id, p->pad_token_id};
             if (m->poison_logits) CUDA_CHECK(cudaMemsetAsync(m->logits.as<float>() + PD.r0 * D.ld, 0xFF, (size_t)PD.R * D.ld * 4, pc.s));
         }
@@ -1765,6 +1930,8 @@ int sealbart_set_option(sealbart_t* m, const char* name, int64_t value) {
         else if (n == "gemm_mode") {
             check_model(m);
             if (value == m->cfg.gemm_mode) return;
+            if (value == 6 || m->cfg.gemm_mode == 6)
+                throw ApiError(SEALFM_EINVAL, "gemm_mode 6 (bf16 weights) is chosen at creation: the handle has no fp32 weights to switch to or from");
             if (value == 2 && m->cfg.gemm_mode >= 3) { ensure_tf32_splits(m); m->cfg.gemm_mode = 2; }
             else if ((value == 3 || value == 5) && m->head.w_h1) m->cfg.gemm_mode = (int)value;
             else throw ApiError(SEALFM_EINVAL, "gemm_mode can only switch between the 3xFP16 modes (3, 5) and 2 (3xTF32)");
@@ -1881,7 +2048,7 @@ int sealdec_generate_ex(sealbart_t* m, const sealfm_t* fm, const uint32_t* occ_h
         if (const int rc = run()) throw ApiError(rc, last_error());
         CUDA_CHECK(cudaMemcpyAsync(errs, m->err.p, 16, cudaMemcpyDeviceToHost, s));
         CUDA_CHECK(cudaStreamSynchronize(s));
-        if (errs[1] && m->cfg.gemm_mode >= 3) {
+        if (errs[1] && (m->cfg.gemm_mode == 3 || m->cfg.gemm_mode == 5)) {
             // An activation left the fp16 range (|x| > 65504; the producers saturate and raise the flag): this pass is
             // redone with the 3xTF32 kernels, which have fp32's range -- the caller gets exact-range results either way.
             const int mode = m->cfg.gemm_mode;
@@ -2036,7 +2203,7 @@ int debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A, const 
                const DebugHead* head = nullptr) {
     return guarded([&] {
         if (!A || !W || (store && !C) || M <= 0 || N <= 0 || K <= 0 || band < -1) throw ApiError(SEALFM_EINVAL, "bad argument");
-        if (head && (mode != 3 || !store || gelu || iters > 0 || !head->mask || !head->stats || !head->fused))
+        if (head && ((mode != 3 && mode != 6) || !store || gelu || iters > 0 || !head->mask || !head->stats || !head->fused))
             throw ApiError(SEALFM_EINVAL, "bad argument");
         require_device();
         check_gemm_mode(mode);
@@ -2050,7 +2217,12 @@ int debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A, const 
         if (bias) CUDA_CHECK(cudaMemcpy(dB.p, bias, (size_t)N * 4, cudaMemcpyHostToDevice));
         Lin l; l.w = dW.as<float>(); l.b = bias ? dB.as<float>() : nullptr; l.out = N; l.in = K;
         fake.err.ensure(16); CUDA_CHECK(cudaMemset(fake.err.p, 0, 16)); fake.ovf = fake.err.as<int>() + 1;
-        if (mode == 2) {
+        if (mode == 6) {                                       // W rounded to bf16 (RNE), as sealbart_set_tensor does
+            const std::vector<uint16_t> wb = to_bf16(W, (uint64_t)N * K);
+            whi.ensure((size_t)N * K * 2);
+            CUDA_CHECK(cudaMemcpy(whi.p, wb.data(), (size_t)N * K * 2, cudaMemcpyHostToDevice));
+            l.w_bf = whi.as<__nv_bfloat16>();
+        } else if (mode == 2) {
             whi.ensure((size_t)N * K * 4); wlo.ensure((size_t)N * K * 4);
             l.w_hi = whi.as<float>(); l.w_lo = wlo.as<float>();
             split_into(nullptr, l.w, l.w_hi, l.w_lo, (uint64_t)N * K);
@@ -2062,7 +2234,12 @@ int debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A, const 
         fake.gemm_band = band;
         Act a{dA.as<float>()};
         Buf ah1, ah2;
-        if (presplit && mode >= 3) {
+        if (presplit && mode == 6) {
+            ah1.ensure((size_t)M * K * 4); ah2.ensure((size_t)M * K * 2);
+            a.b1 = ah1.as<__nv_bfloat16>(); a.b2 = ah2.as<__nv_bfloat16>(); a.b3 = a.b1 + (size_t)M * K;
+            split_bf16x3_kernel<<<sm_count() * 8, 256>>>((int64_t)M * K, a.x, a.b1, a.b2, a.b3);
+            CUDA_CHECK(cudaGetLastError());
+        } else if (presplit && mode >= 3) {
             ah1.ensure((size_t)M * K * 2); ah2.ensure((size_t)M * K * 2);
             a.h1 = ah1.as<__half>(); a.h2 = ah2.as<__half>();
             split_half_kernel<<<sm_count() * 8, 256>>>((int64_t)M * K, a.x, 1.0f, a.h1, a.h2, fake.ovf);
@@ -2136,6 +2313,12 @@ int sealdec_debug_head(int64_t M, int32_t N, int32_t K, const float* A, const fl
                        const uint32_t* mask, int32_t eos, int32_t pad, float* C, float* stats, int32_t* fused) {
     const DebugHead h{mask, eos, pad, stats, fused};
     return debug_gemm(3, M, N, K, A, W, bias, C, 0, 0, nullptr, -1, 1, true, &h);
+}
+
+int sealdec_debug_head_ex(int mode, int64_t M, int32_t N, int32_t K, const float* A, const float* W, const float* bias,
+                          const uint32_t* mask, int32_t eos, int32_t pad, float* C, float* stats, int32_t* fused) {
+    const DebugHead h{mask, eos, pad, stats, fused};
+    return debug_gemm(mode, M, N, K, A, W, bias, C, 0, 0, nullptr, -1, 1, true, &h);
 }
 
 int sealdec_debug_select_step(const sealfm_t* fm, const sealdec_params_t* p, const sealdec_groups_t* groups, int64_t Q,

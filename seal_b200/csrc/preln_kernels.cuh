@@ -17,12 +17,15 @@ namespace sealb200 {
 // is rounded before the position row is added.  A position past the table reads its last row: the table is never read
 // out of bounds (the caller decides whether such a position may occur, see sealdec.h).  ln_g / ln_b: mBART's
 // layernorm_embedding, applied to v before it becomes the residual; null for Pegasus.
-struct PreLnEmbed {
+// E: the table's element type (bf16 in gemm_mode 6).
+template <class E>
+struct PreLnEmbedT {
     const int32_t* tok = nullptr; int64_t tok_stride = 0;
     const int32_t* pos = nullptr; int pos_const = 0, pos_offset = 0, pos_rows = 1;
-    const float* embed = nullptr; float scale = 1.f; const float* pos_table = nullptr;
+    const E* embed = nullptr; float scale = 1.f; const float* pos_table = nullptr;
     const float* ln_g = nullptr; const float* ln_b = nullptr;
 };
+using PreLnEmbed = PreLnEmbedT<float>;
 
 // Mean and 1 / sqrt(var + 1e-5) of the row a CTA of 128 threads holds as v[0..1] (float4 c4 = tid + 128 i, n4 of
 // them), in add_ln_row_kernel's order: the mean, then the biased variance of the centred values, then eps.  red:
@@ -60,15 +63,16 @@ __device__ __forceinline__ void preln_stats(const float4 (&v)[2], int n4, int d,
 //   out = LN(v; gamma, beta)
 // gamma / beta: the next sub-layer's norm, or after the last layer the stack's final layer_norm (the encoder's feeds
 // the cross-attention K / V projections, the decoder's the lm_head).
-__global__ void __launch_bounds__(128) preln_row_kernel(int64_t rows, int d, PreLnEmbed em, float* __restrict__ x,
+template <class SO>
+__global__ void __launch_bounds__(128) preln_row_kernel(int64_t rows, int d, PreLnEmbedT<EmbT<SO>> em, float* __restrict__ x,
                                                         const float* __restrict__ b, SplitSrc bsrc,
                                                         const float* __restrict__ gamma, const float* __restrict__ beta,
-                                                        SplitOut so) {
+                                                        SO so) {
     __shared__ float red[2][4];
     const int64_t r = blockIdx.x;
     const int tid = threadIdx.x;
     const int n4 = d / 4;
-    const float* e = nullptr; const float* pe = nullptr;
+    const EmbT<SO>* e = nullptr; const float* pe = nullptr;
     if (em.tok) {
         e = em.embed + (int64_t)em.tok[r * em.tok_stride] * d;
         const int p = min((em.pos ? em.pos[r] : em.pos_const) + em.pos_offset, em.pos_rows - 1);
@@ -81,7 +85,7 @@ __global__ void __launch_bounds__(128) preln_row_kernel(int64_t rows, int d, Pre
         v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
         if (c4 < n4) {
             if (e) {
-                const float4 a = *reinterpret_cast<const float4*>(e + 4 * c4);
+                const float4 a = load_emb4(e + 4 * c4);
                 const float4 q = *reinterpret_cast<const float4*>(pe + 4 * c4);
                 v[i] = make_float4(__fmul_rn(a.x, em.scale) + q.x, __fmul_rn(a.y, em.scale) + q.y,
                                    __fmul_rn(a.z, em.scale) + q.z, __fmul_rn(a.w, em.scale) + q.w);

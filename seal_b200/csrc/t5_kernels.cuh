@@ -24,16 +24,16 @@ constexpr int kT5MaxSource = 1024;
 // in HF T5LayerNorm's order; out_scale is the decoder's d_model^-0.5 after its final_layer_norm, else 1.
 // Instantiated for NV = kT5RmsVec (d <= 1024) and kT5RmsVecWide (d <= 4096, the XL / XXL widths).
 constexpr int kT5RmsVec = 2, kT5RmsVecWide = 8;
-template <int NV>
+template <int NV, class SO>
 __global__ void __launch_bounds__(128) t5_rms_row_kernel(int64_t rows, int d, const int32_t* __restrict__ tok, int64_t tok_stride,
-                                                         const float* __restrict__ embed, float* __restrict__ x,
+                                                         const EmbT<SO>* __restrict__ embed, float* __restrict__ x,
                                                          const float* __restrict__ b, SplitSrc bsrc,
-                                                         const float* __restrict__ w, float eps, float out_scale, SplitOut so) {
+                                                         const float* __restrict__ w, float eps, float out_scale, SO so) {
     __shared__ float red[4];
     const int64_t r = blockIdx.x;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int n4 = d / 4;
-    const float* src = tok ? embed + (int64_t)tok[r * tok_stride] * d : nullptr;
+    const EmbT<SO>* src = tok ? embed + (int64_t)tok[r * tok_stride] * d : nullptr;
     // The wide form moves the row into the x / b / split-K slice pointers (base): indexed by r * d + 4 * c4 in each of
     // its 8 slice loops, ptxas keeps the offset's high word in local memory.  The narrow form keeps base = 0.
     const int64_t base = NV == kT5RmsVec ? 0 : r * d, off = r * d - base;
@@ -46,7 +46,7 @@ __global__ void __launch_bounds__(128) t5_rms_row_kernel(int64_t rows, int d, co
         const int c4 = tid + i * 128;
         v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
         if (c4 < n4) {
-            if (src) v[i] = *reinterpret_cast<const float4*>(src + 4 * c4);
+            if (src) v[i] = load_emb4(src + 4 * c4);
             else {
                 const float4 a = *reinterpret_cast<const float4*>(x + base + off + 4 * c4);
                 const float4 y = load_split4(b + base, bs, off + 4 * c4, 4 * c4);
@@ -78,7 +78,8 @@ __global__ void __launch_bounds__(128) t5_rms_row_kernel(int64_t rows, int d, co
 __device__ __forceinline__ float gelu_new_f(float x) {
     return 0.5f * x * (1.0f + tanhf(0.7978845608028654f * (x + 0.044715f * (x * x * x))));
 }
-__global__ void __launch_bounds__(256) t5_gate_kernel(int64_t rows, int f, const float* __restrict__ h, SplitOut so) {
+template <class SO>
+__global__ void __launch_bounds__(256) t5_gate_kernel(int64_t rows, int f, const float* __restrict__ h, SO so) {
     const int64_t n4 = rows * (f / 4);
     for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < n4; e += (int64_t)gridDim.x * blockDim.x) {
         const int64_t r = e / (f / 4);
@@ -102,10 +103,10 @@ struct RelBias {
 // masked keys excluded).  Scores are q.k + bias(key - query), unscaled.  Structure of grouped_attention
 // (bart_kernels.cuh): 32-key chunks of K (transposed) and V staged in shared memory once per sweep of NW*MAXP rows,
 // online softmax across chunks.
-template <int NW, int MAXP>
+template <int NW, int MAXP, class SO>
 __global__ void __launch_bounds__(NW * 32) t5_enc_self_attn_kernel(int64_t Q, int d, int S, const float* __restrict__ qkv,
                                                                    const int32_t* __restrict__ src_mask, RelBias rb,
-                                                                   SplitOut so, const int32_t* __restrict__ src_off) {
+                                                                   SO so, const int32_t* __restrict__ src_off) {
     __shared__ float Kt[kHeadDim][33];
     __shared__ __align__(16) float Vs[32][kHeadDim];
     __shared__ __align__(16) float q_s[NW * MAXP][kHeadDim];
@@ -195,9 +196,10 @@ __global__ void __launch_bounds__(NW * 32) t5_enc_self_attn_kernel(int64_t Q, in
 // from this step's qkv; the score is q.k + bias(s - cur_pos), unscaled.  One warp per (row, head), lane = key inside a
 // 32-key chunk, chunks merged with an online softmax.  The current k / v are persisted to the cache entries of rows
 // r*row_mul .. r*row_mul + bcast - 1 (the compact first step: one row stands for all beams of a query).
+template <class SO>
 __global__ void __launch_bounds__(512) t5_dec_self_attn_kernel(int64_t R, int d, int heads, int cur_pos, int T,
                                                                const float* __restrict__ qkv, float* kc, float* vc,
-                                                               const int32_t* __restrict__ anc, RelBias rb, SplitOut so,
+                                                               const int32_t* __restrict__ anc, RelBias rb, SO so,
                                                                int row_mul, int bcast) {
     __shared__ __align__(16) float q_s[16][kHeadDim];
     const int64_t r = blockIdx.x, pr = r * row_mul;

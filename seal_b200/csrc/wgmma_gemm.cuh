@@ -15,6 +15,11 @@
 //     BART activation scales that floor is far below the forward's rounding.  Each weight matrix is pre-multiplied by a power of two 2^s so that max|W| ~ 2^14 and the epilogue
 //     multiplies the accumulator by 2^-s (exact).
 //   3xTF32 (gemm_mode 2, fp32 range): hi = x with the 13 low mantissa bits cleared, lo = x - hi (exact).
+//   3xBF16 (gemm_mode 6, bf16 weights): W is stored once in bf16 (exact for a bf16 checkpoint), A = b1 + b2 + b3 in
+//     bf16 pieces (SplitBf16, bart_kernels.cuh; exact for 2^-100 <= |a| < (2 - 2^-8) 2^127) and A*W = b3*W + b2*W + b1*W.  Each
+//     product has 8 x 8 significant bits, exact in the fp32 accumulator, so the only error is the accumulation's --
+//     at any magnitude in fp32's range, with no absolute floor and no overflow flag.  The stage holds A b1, A b2, W and
+//     A b3 in the four 16 KB slots the other modes use for A hi / lo and W hi / lo.
 //
 // Kernel: persistent, 128 x 128 output tile per CTA, three warpgroups.  Warpgroup 0 is the producer (one thread
 // issues the TMA loads of A hi/lo and W hi/lo into 128B-swizzled K-major shared-memory stages); warpgroups 1 and 2
@@ -24,10 +29,13 @@
 // loads half of the W rows and multicasts them to both, which halves the W traffic out of L2.
 #pragma once
 #include <cuda.h>
+#include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <cstdint>
+#include <type_traits>
 
+#include "bart_kernels.cuh"
 #include "launch.cuh"
 
 namespace sealb200 {
@@ -51,6 +59,7 @@ constexpr int UK = 32;                               // 3xTF32 k-block: 32 float
 template <typename T> struct GemmElem;
 template <> struct GemmElem<__half> { static constexpr int KE = 64, KSTEP = 16, CHUNK = 4; };
 template <> struct GemmElem<float> { static constexpr int KE = 32, KSTEP = 8, CHUNK = 2; };
+template <> struct GemmElem<__nv_bfloat16> { static constexpr int KE = 64, KSTEP = 16, CHUNK = 4; };
 
 // ---- PTX wrappers --------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
@@ -134,6 +143,10 @@ __device__ __forceinline__ void wgmma_128(float (&d)[64], uint64_t a, uint64_t b
     asm volatile("wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 " SEAL_WG_D64 ", %64, %65, 1, 1, 1;"
                  : SEAL_WG_OPS(d) : "l"(a), "l"(b));
 }
+__device__ __forceinline__ void wgmma_128(float (&d)[64], uint64_t a, uint64_t b, __nv_bfloat16) {
+    asm volatile("wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " SEAL_WG_D64 ", %64, %65, 1, 1, 1, 0, 0;"
+                 : SEAL_WG_OPS(d) : "l"(a), "l"(b));
+}
 #undef SEAL_WG_D64
 #undef SEAL_WG_OPS
 
@@ -178,6 +191,13 @@ __global__ void __launch_bounds__(256) split_half_kernel(int64_t n, const float*
         if (ov) atomicExch(overflow, 1);
         h1[i] = a; h2[i] = b;
     }
+}
+
+// x -> the three bf16 pieces of the 3xBF16 GEMM (bf16x3_split1); for activations whose producer did not split
+__global__ void __launch_bounds__(256) split_bf16x3_kernel(int64_t n, const float* __restrict__ x, __nv_bfloat16* __restrict__ b1,
+                                                           __nv_bfloat16* __restrict__ b2, __nv_bfloat16* __restrict__ b3) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+        bf16x3_split1(x[i], b1[i], b2[i], b3[i]);
 }
 
 __global__ void __launch_bounds__(256) absmax_kernel(int64_t n, const float* __restrict__ x, unsigned int* __restrict__ out) {
@@ -228,6 +248,24 @@ __device__ __forceinline__ void store_pair(float* C, float* S1, float* S2, int64
     }
 }
 
+// The 3xBF16 form: fp32 and/or the three bf16 pieces of the next GEMM's operand (no saturation, no flag)
+__device__ __forceinline__ void store_pair3(float* C, __nv_bfloat16* S1, __nv_bfloat16* S2, __nv_bfloat16* S3, int64_t off, int n, int N,
+                                            float v0, float v1) {
+    if (n + 1 < N) {
+        if (C) *reinterpret_cast<float2*>(C + off) = make_float2(v0, v1);
+        if (S1) {
+            __nv_bfloat16 p0[3], p1[3];
+            bf16x3_split1(v0, p0[0], p0[1], p0[2]); bf16x3_split1(v1, p1[0], p1[1], p1[2]);
+            *reinterpret_cast<uint32_t*>(S1 + off) = bf16_pack(p0[0], p1[0]);
+            *reinterpret_cast<uint32_t*>(S2 + off) = bf16_pack(p0[1], p1[1]);
+            *reinterpret_cast<uint32_t*>(S3 + off) = bf16_pack(p0[2], p1[2]);
+        }
+    } else if (n < N) {
+        if (C) C[off] = v0;
+        if (S1) bf16x3_split1(v0, S1[off], S2[off], S3[off]);
+    }
+}
+
 // Tile group (mg, n_tile) of work index `tile`.  n_fastest: row-major over (m group, n tile).  Otherwise the m groups
 // are walked in bands of `band` groups (0: one band of all of them), band after band; inside a band the walk is
 // n-major with m fastest, so the concurrent CTAs share W tiles and the band's A rows are re-read from L2, not HBM.
@@ -250,7 +288,8 @@ struct HeadEpi {
     float2* stats = nullptr; const uint32_t* mask = nullptr; int mask_words = 0; int eos = -1, pad = -1;
 };
 
-// T = __half (3xFP16) or float (3xTF32); CL = CTAs per cluster sharing the W tile (1 or 2).
+// T = __half (3xFP16), float (3xTF32) or __nv_bfloat16 (3xBF16: tmA_hi / tmA_lo / tmW_lo are A's pieces b1 / b2 / b3,
+// tmW_hi is W; C_s1 / C_s2 / C_s3 the three output pieces); CL = CTAs per cluster sharing the W tile (1 or 2).
 // Persistent: work unit u = blockIdx.x / CL walks units u, u + gridDim.x / CL, ...  A unit is (tile group, K slice);
 // a tile group is CL vertically adjacent 128 x 128 tiles.  Tile order is chosen by the host (tile_coords): n fastest
 // when the activations dominate (concurrent CTAs then share A tiles and all of W stays in L2), m fastest when the
@@ -272,8 +311,10 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
                      const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo,
                      int M, int N, int K, const float* __restrict__ bias, float w_unscale, float* __restrict__ C,
                      T* __restrict__ C_s1, T* __restrict__ C_s2, int ldc, int n_fastest, int m_band, int* __restrict__ overflow,
-                     int k_slices, int64_t slice_stride, HeadEpi he) {
+                     int k_slices, int64_t slice_stride, HeadEpi he, T* __restrict__ C_s3) {
     using E = GemmElem<T>;
+    constexpr bool kBf16 = std::is_same<T, __nv_bfloat16>::value;
+    static_assert(!kBf16 || CL == 1, "3xBF16 runs one CTA per tile");
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;          // SWIZZLE_128B wants 1024 B alignment
     const uint32_t full0 = base + GSTAGES * G_STAGE, empty0 = full0 + 8 * GSTAGES;
@@ -313,7 +354,10 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
                     mbar_expect_tx(fb, G_STAGE);
                     tma_load_2d(st, &tmA_hi, fb, kx, row_a);
                     tma_load_2d(st + G_AB, &tmA_lo, fb, kx, row_a);
-                    if (CL == 1) {
+                    if (kBf16) {
+                        tma_load_2d(st + 2 * G_AB, &tmW_hi, fb, kx, n_tile * GN);
+                        tma_load_2d(st + 2 * G_AB + G_WB, &tmW_lo, fb, kx, row_a);
+                    } else if (CL == 1) {
                         tma_load_2d(st + 2 * G_AB, &tmW_hi, fb, kx, n_tile * GN);
                         tma_load_2d(st + 2 * G_AB + G_WB, &tmW_lo, fb, kx, n_tile * GN);
                     } else {                                               // this CTA's share of the W rows, to both CTAs
@@ -355,11 +399,21 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
                     const uint64_t w_hi = gmma_desc_sw128(st + 2 * G_AB), w_lo = gmma_desc_sw128(st + 2 * G_AB + G_WB);
                     acc_fence(d);
                     wgmma_fence();
+                    if constexpr (kBf16) {
+                        const uint64_t a_b3 = gmma_desc_sw128(st + 2 * G_AB + G_WB + a_off);   // w_hi = W, a_hi / a_lo = b1 / b2
 #pragma unroll
-                    for (int k = 0; k < E::KE / E::KSTEP; ++k) {           // KSTEP elements = 32 B -> +2 in the address field
-                        wgmma_128(d, a_lo + 2 * k, w_hi + 2 * k, T{});
-                        wgmma_128(d, a_hi + 2 * k, w_lo + 2 * k, T{});
-                        wgmma_128(d, a_hi + 2 * k, w_hi + 2 * k, T{});
+                        for (int k = 0; k < E::KE / E::KSTEP; ++k) {
+                            wgmma_128(d, a_b3 + 2 * k, w_hi + 2 * k, T{});
+                            wgmma_128(d, a_lo + 2 * k, w_hi + 2 * k, T{});
+                            wgmma_128(d, a_hi + 2 * k, w_hi + 2 * k, T{});
+                        }
+                    } else {
+#pragma unroll
+                        for (int k = 0; k < E::KE / E::KSTEP; ++k) {       // KSTEP elements = 32 B -> +2 in the address field
+                            wgmma_128(d, a_lo + 2 * k, w_hi + 2 * k, T{});
+                            wgmma_128(d, a_hi + 2 * k, w_lo + 2 * k, T{});
+                            wgmma_128(d, a_hi + 2 * k, w_hi + 2 * k, T{});
+                        }
                     }
                     wgmma_commit();
                     wgmma_wait<1>();                                       // the previous k-block's MMAs have retired
@@ -436,7 +490,8 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
                         const float x = acc[4 * j + 2 * h + e] * w_unscale + ((bias && n + e < N) ? bias[n + e] : 0.f);
                         v[e] = epi_act<ACT>(x);
                     }
-                    store_pair(Cs, C_s1, C_s2, (int64_t)row * ldc + n, n, N, v[0], v[1], ov);
+                    if constexpr (kBf16) store_pair3(Cs, C_s1, C_s2, C_s3, (int64_t)row * ldc + n, n, N, v[0], v[1]);
+                    else store_pair(Cs, C_s1, C_s2, (int64_t)row * ldc + n, n, N, v[0], v[1], ov);
                 }
             }
             if (ov) atomicExch(overflow, 1);
@@ -450,12 +505,13 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
 }
 
 // Finishes a split-K GEMM: out = act((sum_s part[s]) * w_unscale + bias), slices summed in index order
-// (deterministic), written as fp32 and/or as the half split the next GEMM consumes.
-template <int ACT>
+// (deterministic), written as fp32 and/or as the split the next GEMM consumes: T = __half (two halves) or __nv_bfloat16
+// (three bf16 pieces, C_h3; no saturation, no flag).
+template <int ACT, typename T = __half>
 __global__ void __launch_bounds__(256) gemm_splitk_finish_kernel(int64_t M, int N, int ldc, int k_slices, int64_t slice_stride,
                                                                  const float* __restrict__ part, const float* __restrict__ bias,
-                                                                 float w_unscale, float* __restrict__ C, __half* __restrict__ C_h1,
-                                                                 __half* __restrict__ C_h2, int* __restrict__ overflow) {
+                                                                 float w_unscale, float* __restrict__ C, T* __restrict__ C_h1,
+                                                                 T* __restrict__ C_h2, int* __restrict__ overflow, T* __restrict__ C_h3) {
     const int64_t total = M * (int64_t)(ldc / 4);
     for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
         const int64_t row = e / (ldc / 4);
@@ -474,7 +530,8 @@ __global__ void __launch_bounds__(256) gemm_splitk_finish_kernel(int64_t M, int 
             float x = v[u] * w_unscale + (bias ? bias[n + u] : 0.f);
             x = epi_act<ACT>(x);
             if (C) C[off + u] = x;
-            if (C_h1) { __half a, b; split_half(x, a, b, &ov); C_h1[off + u] = a; C_h2[off + u] = b; }
+            if constexpr (std::is_same<T, __nv_bfloat16>::value) { if (C_h1) bf16x3_split1(x, C_h1[off + u], C_h2[off + u], C_h3[off + u]); }
+            else if (C_h1) { __half a, b; split_half(x, a, b, &ov); C_h1[off + u] = a; C_h2[off + u] = b; }
         }
         if (ov) atomicExch(overflow, 1);
     }
