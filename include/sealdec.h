@@ -423,7 +423,7 @@ int sealdec_debug_topk_threshold_cluster(int64_t R, int32_t V, int64_t ld, const
 /* average device time of the decoder's per-row statistics + top-2*beam kernel over R rows of V pseudo-random logits
  * (a later step of constrained beam search, per_row allowed tokens per row) */
 int sealdec_debug_topk_rows(int64_t R, int32_t V, int32_t num_beams, int32_t per_row, int32_t iters, double* avg_us);
-/* in-kernel timeline of CTA 0 of the mode-3/4 GEMM kernel (development aid): out20 (may be NULL) receives
+/* in-kernel timeline of CTA 0 of the GEMM kernel, in every gemm_mode (development aid): out20 (may be NULL) receives
  * the stamps of the last traced launch -- SM cycles at 0 entry, 1 prologue done, 2 first operands landed,
  * 3 last MMA issued, 4 last chunk complete, 5 tile stored, 6 exit; 7/8 globaltimer ns at entry / exit --
  * 9..16 the epilogue's four store passes (staged / stored) -- then tracing is switched on (enable != 0) or off. */

@@ -13,6 +13,7 @@
 
 #include <cmath>
 #include <cstring>
+#include <iterator>
 #include <map>
 #include <memory>
 #include <set>
@@ -135,6 +136,7 @@ struct sealbart {
     cudaEvent_t slice_fork = nullptr, slice_join = nullptr;
     Buf a_hi1, a_lo1, splitk1, st_wide1;
     Buf effn2, dffn2;                 // T5 gated-gelu: [rows][2 d_ff] output of the [wi_0; wi_1] GEMM
+    ~sealbart() { for (void* p : allocs) cudaFree(p); for (void* p : split_allocs) cudaFree(p); }
 };
 
 namespace {
@@ -157,9 +159,15 @@ __nv_bfloat16* dalloc_bf16(sealbart* m, uint64_t numel) {
     return static_cast<__nv_bfloat16*>(p);
 }
 
+// sealbart_config_t::gemm_mode (include/sealdec.h)
+enum GemmMode : int { kGemmTf32 = 2, kGemmFp16 = 3, kGemmFp16Cluster = 5, kGemmBf16 = 6 };
+// 3xFP16 (one CTA per tile, or 2-CTA clusters): activations in fp16 halves, which an activation can overflow
+bool is_3xfp16(int64_t mode) { return mode == kGemmFp16 || mode == kGemmFp16Cluster; }
+// the modes whose lm_head may take the statistics epilogue (HeadEpi)
+bool head_stats_mode(int mode) { return mode == kGemmFp16 || mode == kGemmBf16; }
 // gemm_mode 6 stores every GEMM weight matrix (and the embedding table) once, in bf16; the other modes keep the fp32
 // master and derive their splits from it at finalize
-bool bf16_weights(const sealbart* m) { return m->cfg.gemm_mode == 6; }
+bool bf16_weights(const sealbart* m) { return m->cfg.gemm_mode == kGemmBf16; }
 
 void make_lin(sealbart* m, Lin& l, int out, int in) {
     l.out = out; l.in = in;
@@ -309,14 +317,16 @@ EncodeTiledFn encode_tiled() {
     }
     return fn;
 }
-// row-major [rows][K] fp32 (or fp16, or bf16), box = 128 bytes of K x box_rows, 128B swizzle, zero fill out of bounds
-void make_map(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t K, uint64_t ld, uint32_t box_rows, bool half = false, bool bf16 = false) {
+// row-major [rows][K] of T (fp32, fp16 or bf16), box = 128 bytes of K x box_rows, 128B swizzle, zero fill out of bounds
+template <typename T> void make_map(CUtensorMap* map, const T* ptr, uint64_t rows, uint64_t K, uint64_t ld, uint32_t box_rows) {
     cuuint64_t dims[2] = {K, rows};
-    cuuint64_t strides[1] = {ld * (half ? 2 : 4)};
-    cuuint32_t box[2] = {(cuuint32_t)(128 / (half ? 2 : 4)), box_rows};
+    cuuint64_t strides[1] = {ld * sizeof(T)};
+    cuuint32_t box[2] = {(cuuint32_t)(128 / sizeof(T)), box_rows};
     cuuint32_t estr[2] = {1, 1};
-    const CUtensorMapDataType dt = bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : half ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
-    CUresult r = encode_tiled()(map, dt, 2, const_cast<void*>(ptr), dims, strides, box, estr,
+    const CUtensorMapDataType dt = std::is_same<T, __nv_bfloat16>::value ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                   : std::is_same<T, __half>::value      ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
+                                                                          : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+    CUresult r = encode_tiled()(map, dt, 2, const_cast<T*>(ptr), dims, strides, box, estr,
                                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) throw ApiError(SEALFM_ECUDA, "cuTensorMapEncodeTiled failed (" + std::to_string((int)r) + ")");
@@ -345,7 +355,7 @@ void split_into(cudaStream_t s, const float* x, float* hi, float* lo, uint64_t n
     CUDA_CHECK(cudaGetLastError());
 }
 
-// An activation tensor as the GEMMs see it: plain fp32 and/or its TF32 split (hi, lo).
+// An activation tensor as the GEMMs see it: plain fp32 and/or its split in the gemm_mode's format (X3Format).
 struct Act {
     float* x = nullptr; float* hi = nullptr; float* lo = nullptr;   // fp32 / TF32 split
     __half* h1 = nullptr; __half* h2 = nullptr;                     // FP16 split
@@ -362,7 +372,7 @@ SplitOut split_of(const Act& a, int* overflow) {
 // f(so) with the split output a producer of activation a writes: SplitBf16 in gemm_mode 6, SplitOut (split_of)
 // otherwise.  The producer kernels are instantiated per split type, so f launches kernel<decltype(so)>.
 template <typename F> void with_split(const sealbart* m, const Act& a, F&& f) {
-    if (m->cfg.gemm_mode == 6) f(SplitBf16{a.b1, a.b2, a.b3});
+    if (bf16_weights(m)) f(SplitBf16{a.b1, a.b2, a.b3});
     else f(split_of(a, m->ovf));
 }
 // the embedding table a producer with split type SO gathers from
@@ -377,9 +387,9 @@ template <class SO> const EmbT<SO>* embed_table(const sealbart* m) {
 Act act_view(int gemm_mode, float* plain, const Buf& hi, const Buf& lo, int64_t off = 0) {
     Act a;
     if (plain) a.x = plain + off;
-    if (gemm_mode == 2) { a.hi = hi.as<float>() + off; a.lo = lo.as<float>() + off; }
-    else if (gemm_mode == 6) { a.b1 = hi.as<__nv_bfloat16>() + off; a.b2 = lo.as<__nv_bfloat16>() + off; a.b3 = hi.as<__nv_bfloat16>() + hi.bytes / 4 + off; }
-    else if (gemm_mode >= 3) { a.h1 = hi.as<__half>() + off; a.h2 = lo.as<__half>() + off; }
+    if (gemm_mode == kGemmTf32) { a.hi = hi.as<float>() + off; a.lo = lo.as<float>() + off; }
+    else if (gemm_mode == kGemmBf16) { a.b1 = hi.as<__nv_bfloat16>() + off; a.b2 = lo.as<__nv_bfloat16>() + off; a.b3 = hi.as<__nv_bfloat16>() + hi.bytes / 4 + off; }
+    else if (is_3xfp16(gemm_mode)) { a.h1 = hi.as<__half>() + off; a.h2 = lo.as<__half>() + off; }
     return a;
 }
 
@@ -406,9 +416,10 @@ template <typename F> void with_act(int act, F&& f) {
     else f(std::integral_constant<int, kActNone>{});
 }
 
-// C = A W^T + b (+ the epilogue activation act: kActNone / kActGelu / kActRelu, wgmma_gemm.cuh) on the tensor cores: gemm_mode 3 / 5 = 3xFP16 (one CTA per tile / clusters of 2 sharing W), 2 = 3xTF32 (fp32
+// C = A W^T + b (+ the epilogue activation act: kActNone / kActGelu / kActRelu, wgmma_gemm.cuh) on the tensor cores:
+// gemm_mode 3 / 5 = 3xFP16 (one CTA per tile / clusters of 2 sharing W), 6 = 3xBF16 (bf16 weights), 2 = 3xTF32 (fp32
 // range: the fallback when an activation leaves the fp16 range).  Operands arrive pre-split from the producing kernel
-// (A.h1/A.h2 or A.hi/A.lo); they are split here only if the producer did not.
+// (A.h1/A.h2, A.b1/A.b2/A.b3 or A.hi/A.lo); they are split here only if the producer did not.
 void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, const Act& C, int ldc, int act);
 
 void gemm(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, const Act& C, int ldc, int act) {
@@ -447,144 +458,146 @@ int band_tiles(const sealbart* m, int n_fastest, int64_t M, int K, int a_bytes) 
     return m->gemm_band >= 0 ? m->gemm_band : band;
 }
 
-void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, const Act& C, int ldc, int act) {
-    if (M == 0) return;
-    if (act == kActRelu) cx.m->last_paths |= kPathT5Relu;
+// The x3 GEMM's operand formats, by element type T: the Act fields of A's pieces (C's split outputs use the same
+// fields), the Lin fields of W's pieces, whether the epilogue unscales W by l.w_unscale, whether split-K, L2 bands and
+// the lm_head statistics epilogue apply (tuned), and the last_paths bits of every call and of the whole-tile launch.
+// 3xBF16's W is one piece; its kernel reads A's third piece in the W lo slot.
+template <typename T> using ActField = T* Act::*;
+template <typename T> using LinField = T* Lin::*;
+template <typename T> struct X3Format;
+template <> struct X3Format<__half> {                 // 3xFP16 (modes 3, 5): A = h1 + h2, W * 2^s = w_h1 + w_h2
+    static constexpr ActField<__half> piece[] = {&Act::h1, &Act::h2};
+    static constexpr LinField<__half> w = &Lin::w_h1, w2 = &Lin::w_h2;
+    static constexpr bool scaled_w = true, tuned = true;
+    static constexpr uint32_t path_call = 0, path_tile = kPathGemmFullTile;
+};
+template <> struct X3Format<__nv_bfloat16> {          // 3xBF16 (mode 6): A = b1 + b2 + b3, W once in bf16
+    static constexpr ActField<__nv_bfloat16> piece[] = {&Act::b1, &Act::b2, &Act::b3};
+    static constexpr LinField<__nv_bfloat16> w = &Lin::w_bf;
+    static constexpr bool scaled_w = false, tuned = true;
+    static constexpr uint32_t path_call = kPathGemmBf16, path_tile = 0;
+};
+template <> struct X3Format<float> {                  // 3xTF32 (mode 2): A = hi + lo, W = w_hi + w_lo; band 0, gemm_band ignored
+    static constexpr ActField<float> piece[] = {&Act::hi, &Act::lo};
+    static constexpr LinField<float> w = &Lin::w_hi, w2 = &Lin::w_lo;
+    static constexpr bool scaled_w = false, tuned = false;    // unscaled: after an overflow fallback l.w_unscale is 3xFP16's
+    static constexpr uint32_t path_call = 0, path_tile = kPathGemmTf32;
+};
+
+// f(T()) with the element type T of gemm_mode's operand format
+template <typename F> void with_format(int mode, F&& f) {
+    if (mode == kGemmBf16) f(__nv_bfloat16());
+    else if (is_3xfp16(mode)) f(__half());
+    else f(0.f);
+}
+
+// x (n fp32 values) split into format T's pieces in hi / lo (grown to fit) on stream s, in act_view's layout but with
+// bf16's third piece n elements into hi.  3xFP16 raises *ovf for a value past the fp16 range.
+template <typename T> Act split_act(cudaStream_t s, float* x, int64_t n, Buf& hi, Buf& lo, int* ovf) {
+    Act a{x};
+    const int blocks = (int)std::min<int64_t>((n + 255) / 256, (int64_t)sm_count() * 8);
+    if constexpr (std::is_same<T, __nv_bfloat16>::value) {
+        hi.ensure((size_t)n * 4); lo.ensure((size_t)n * 2);
+        a.b1 = hi.as<T>(); a.b2 = lo.as<T>(); a.b3 = a.b1 + n;
+        split_bf16x3_kernel<<<blocks, 256, 0, s>>>(n, x, a.b1, a.b2, a.b3);
+    } else if constexpr (std::is_same<T, __half>::value) {
+        hi.ensure((size_t)n * 2); lo.ensure((size_t)n * 2);
+        a.h1 = hi.as<T>(); a.h2 = lo.as<T>();
+        split_half_kernel<<<blocks, 256, 0, s>>>(n, x, 1.0f, a.h1, a.h2, ovf);
+    } else {
+        hi.ensure((size_t)n * 4); lo.ensure((size_t)n * 4);
+        a.hi = hi.as<T>(); a.lo = lo.as<T>();
+        split_into(s, x, a.hi, a.lo, (uint64_t)n);
+    }
+    CUDA_CHECK(cudaGetLastError());
+    return a;
+}
+
+template <typename T> void gemm_x3(Ctx& cx, int64_t M, int N, int K, const Act& A, Lin& l, const Act& C, int ldc, int act) {
+    using F = X3Format<T>;
+    constexpr int pieces = (int)std::size(F::piece);
     sealbart* m = cx.m;
-    Buf& a_hi = cx.slice ? m->a_hi1 : m->a_hi;
-    Buf& a_lo = cx.slice ? m->a_lo1 : m->a_lo;
-    Buf& splitk = cx.slice ? m->splitk1 : m->splitk;
     const int tiles = (int)(((N + GN - 1) / GN) * ((M + GM - 1) / GM));
     const int n_fastest = ((int64_t)M >= (int64_t)N) ? 1 : 0;     // stream the larger operand once
-    if (m->cfg.gemm_mode == 6 && K % UK16 == 0 && lda == K && l.w_bf) {
-        // 3xBF16: bf16 W, A in three bf16 pieces (pre-split by the producers); the 3xFP16 path's tile walk, split-K and
-        // bands; no cluster form and no overflow flag
-        const __nv_bfloat16 *p1 = A.b1, *p2 = A.b2, *p3 = A.b3;
-        if (!p1) {
-            a_hi.ensure((size_t)M * K * 4); a_lo.ensure((size_t)M * K * 2);
-            __nv_bfloat16* h = a_hi.as<__nv_bfloat16>();
-            const int blocks = (int)std::min<int64_t>(((int64_t)M * K + 255) / 256, (int64_t)sm_count() * 8);
-            split_bf16x3_kernel<<<blocks, 256, 0, cx.s>>>((int64_t)M * K, A.x, h, a_lo.as<__nv_bfloat16>(), h + (size_t)M * K);
-            CUDA_CHECK(cudaGetLastError()); m->launches++;
-            p1 = h; p2 = a_lo.as<__nv_bfloat16>(); p3 = h + (size_t)M * K;
-        }
-        CUtensorMap ma1, ma2, ma3;
-        make_map(&ma1, p1, M, K, K, GM, true, true); make_map(&ma2, p2, M, K, K, GM, true, true); make_map(&ma3, p3, M, K, K, GM, true, true);
-        if (!l.maps_ready) { make_map(&l.map_hi, l.w_bf, N, K, K, GN, true, true); l.maps_ready = true; }
-        m->last_paths |= kPathGemmBf16;
-        const int k_slices = split_k_slices(tiles, K / UK16);
-        if (k_slices > 1) {
-            const int64_t slice_stride = (int64_t)M * ldc;
-            splitk.ensure((size_t)k_slices * slice_stride * 4);
-            float* part = splitk.as<float>();
-            const int ctas2 = std::min(tiles * k_slices, sm_count());
-            gemm_launch<__nv_bfloat16, kActNone, 1>(cx.s, ctas2, ma1, ma2, l.map_hi, ma3, M, N, K, nullptr, 1.0f, part, nullptr, nullptr, ldc, n_fastest, 0,
-                                                    m->ovf, k_slices, slice_stride);
-            m->launches++;
-            if (M <= cx.defer_rows && act == kActNone && !C.b1 && ldc == N && l.b) {     // summed by the consumer kernel
-                cx.pending = SplitSrc{part, k_slices, slice_stride, l.b, 1.0f};
-                m->last_paths |= kPathSplitKDeferred;
-                return;
-            }
-            const int fblocks = (int)std::min<int64_t>((M * (ldc / 4) + 255) / 256, (int64_t)sm_count() * 8);
-            with_act(act, [&](auto A) {
-                launch_k(gemm_splitk_finish_kernel<decltype(A)::value, __nv_bfloat16>, fblocks, 256, 0, cx.s, M, N, ldc, k_slices, slice_stride, part, l.b, 1.0f,
-                         C.x, C.b1, C.b2, m->ovf, C.b3);
-            });
-            CUDA_CHECK(cudaGetLastError()); m->launches++; m->last_paths |= kPathSplitKFinish;
-            return;
-        }
-        const int band = band_tiles(m, n_fastest, M, K, 6);
-        const int ctas = std::min(tiles, sm_count());
-        if (cx.head.stats && act == kActNone) {
-            gemm_launch<__nv_bfloat16, kActNone, 1, true>(cx.s, ctas, ma1, ma2, l.map_hi, ma3, M, N, K, l.b, 1.0f, C.x, nullptr, nullptr, ldc, n_fastest, band,
-                                                          m->ovf, 1, 0, cx.head);
-            cx.head_fused = true;
-        } else
-            with_act(act, [&](auto A) {
-                gemm_launch<__nv_bfloat16, decltype(A)::value, 1>(cx.s, ctas, ma1, ma2, l.map_hi, ma3, M, N, K, l.b, 1.0f, C.x, C.b1, C.b2, ldc, n_fastest, band,
-                                                                  m->ovf, 1, 0, HeadEpi{}, C.b3);
-            });
+    Act a = A;
+    if (!(a.*F::piece[0])) {
+        a = split_act<T>(cx.s, A.x, M * K, cx.slice ? m->a_hi1 : m->a_hi, cx.slice ? m->a_lo1 : m->a_lo, m->ovf);
         m->launches++;
-        return;
     }
-    if ((m->cfg.gemm_mode == 3 || m->cfg.gemm_mode == 5) && K % UK16 == 0 && lda == K && l.w_h1) {
-        // 3xFP16; operands pre-split into halves by the producers
-        const __half* a1 = A.h1; const __half* a2 = A.h2;
-        if (!a1) {
-            a_hi.ensure((size_t)M * K * 2); a_lo.ensure((size_t)M * K * 2);
-            const int blocks = (int)std::min<int64_t>(((int64_t)M * K + 255) / 256, (int64_t)sm_count() * 8);
-            split_half_kernel<<<blocks, 256, 0, cx.s>>>((int64_t)M * K, A.x, 1.0f, a_hi.as<__half>(), a_lo.as<__half>(), m->ovf);
-            CUDA_CHECK(cudaGetLastError()); m->launches++;
-            a1 = a_hi.as<__half>(); a2 = a_lo.as<__half>();
-        }
-        CUtensorMap ma1, ma2;
-        make_map(&ma1, a1, M, K, K, GM, true); make_map(&ma2, a2, M, K, K, GM, true);
-        if (!l.maps_ready) { make_map(&l.map_hi, l.w_h1, N, K, K, GN, true); make_map(&l.map_lo, l.w_h2, N, K, K, GN, true); l.maps_ready = true; }
-        int* ovf = m->ovf;
-        const int k_slices = split_k_slices(tiles, K / UK16);
-        if (m->cfg.gemm_mode == 5 && k_slices == 1 && M > GM) {
+    CUtensorMap ma[3];
+    for (int i = 0; i < pieces; ++i) make_map(&ma[i], a.*F::piece[i], M, K, K, GM);
+    if (!l.maps_ready) {
+        make_map(&l.map_hi, l.*F::w, N, K, K, GN);
+        if constexpr (pieces == 2) make_map(&l.map_lo, l.*F::w2, N, K, K, GN);
+        l.maps_ready = true;
+    }
+    const CUtensorMap& w_lo = pieces == 3 ? ma[2] : l.map_lo;
+    T* const c1 = C.*F::piece[0]; T* const c2 = C.*F::piece[1]; T* c3 = nullptr;
+    if constexpr (pieces == 3) c3 = C.*F::piece[2];
+    const float unscale = F::scaled_w ? l.w_unscale : 1.0f;
+    m->last_paths |= F::path_call;
+    const int k_slices = F::tuned ? split_k_slices(tiles, K / UK16) : 1;
+    if constexpr (std::is_same<T, __half>::value) {
+        if (m->cfg.gemm_mode == kGemmFp16Cluster && k_slices == 1 && M > GM) {
             // clusters of 2 CTAs on vertically adjacent tiles: the W tile is loaded once (TMA multicast) for both
-            if (!l.maps2_ready) { make_map(&l.map2_hi, l.w_h1, N, K, K, GN / 2, true); make_map(&l.map2_lo, l.w_h2, N, K, K, GN / 2, true); l.maps2_ready = true; }
+            if (!l.maps2_ready) { make_map(&l.map2_hi, l.w_h1, N, K, K, GN / 2); make_map(&l.map2_lo, l.w_h2, N, K, K, GN / 2); l.maps2_ready = true; }
             const int groups = (int)((M + 2 * GM - 1) / (2 * GM)) * ((N + GN - 1) / GN);
             const int ctas = 2 * std::min(groups, sm_count() / 2);
-            with_act(act, [&](auto A) {
-                gemm_launch<__half, decltype(A)::value, 2>(cx.s, ctas, ma1, ma2, l.map2_hi, l.map2_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, 0, ovf, 1, 0);
+            with_act(act, [&](auto Ac) {
+                gemm_launch<__half, decltype(Ac)::value, 2>(cx.s, ctas, ma[0], ma[1], l.map2_hi, l.map2_lo, M, N, K, l.b, unscale, C.x, c1, c2, ldc, n_fastest, 0, m->ovf, 1, 0);
             });
             m->launches++; m->last_paths |= kPathGemmCluster;
             return;
         }
+    }
+    if constexpr (F::tuned) {
         if (k_slices > 1) {
+            Buf& splitk = cx.slice ? m->splitk1 : m->splitk;
             const int64_t slice_stride = (int64_t)M * ldc;
             splitk.ensure((size_t)k_slices * slice_stride * 4);
             float* part = splitk.as<float>();
             const int ctas2 = std::min(tiles * k_slices, sm_count());
-            gemm_launch<__half, kActNone, 1>(cx.s, ctas2, ma1, ma2, l.map_hi, l.map_lo, M, N, K, nullptr, 1.0f, part, nullptr, nullptr, ldc, n_fastest, 0, ovf,
-                                          k_slices, slice_stride);
+            gemm_launch<T, kActNone, 1>(cx.s, ctas2, ma[0], ma[1], l.map_hi, w_lo, M, N, K, nullptr, 1.0f, part, nullptr, nullptr, ldc, n_fastest, 0,
+                                        m->ovf, k_slices, slice_stride);
             m->launches++;
-            if (M <= cx.defer_rows && act == kActNone && !C.h1 && !C.hi && ldc == N && l.b) {     // summed by the consumer kernel
-                cx.pending = SplitSrc{part, k_slices, slice_stride, l.b, l.w_unscale};
+            if (M <= cx.defer_rows && act == kActNone && !C.hi && !C.h1 && !C.b1 && ldc == N && l.b) {     // C has no split output: summed by the consumer kernel
+                cx.pending = SplitSrc{part, k_slices, slice_stride, l.b, unscale};
                 m->last_paths |= kPathSplitKDeferred;
                 return;
             }
             const int fblocks = (int)std::min<int64_t>((M * (ldc / 4) + 255) / 256, (int64_t)sm_count() * 8);
-            with_act(act, [&](auto A) {
-                launch_k(gemm_splitk_finish_kernel<decltype(A)::value>, fblocks, 256, 0, cx.s, M, N, ldc, k_slices, slice_stride, part, l.b, l.w_unscale, C.x, C.h1, C.h2, ovf,
-                         (__half*)nullptr);
+            with_act(act, [&](auto Ac) {
+                launch_k(gemm_splitk_finish_kernel<decltype(Ac)::value, T>, fblocks, 256, 0, cx.s, M, N, ldc, k_slices, slice_stride, part, l.b, unscale,
+                         C.x, c1, c2, m->ovf, c3);
             });
             CUDA_CHECK(cudaGetLastError()); m->launches++; m->last_paths |= kPathSplitKFinish;
             return;
         }
-        const int band = band_tiles(m, n_fastest, M, K, 4);
-        const int ctas = std::min(tiles, sm_count());
-        if (cx.head.stats && act == kActNone) {
-            gemm_launch<__half, kActNone, 1, true>(cx.s, ctas, ma1, ma2, l.map_hi, l.map_lo, M, N, K, l.b, l.w_unscale, C.x, nullptr, nullptr, ldc, n_fastest, band, ovf, 1, 0, cx.head);
-            cx.head_fused = true;
-        } else
-            with_act(act, [&](auto A) {
-                gemm_launch<__half, decltype(A)::value, 1>(cx.s, ctas, ma1, ma2, l.map_hi, l.map_lo, M, N, K, l.b, l.w_unscale, C.x, C.h1, C.h2, ldc, n_fastest, band, ovf, 1, 0);
-            });
-        m->launches++; m->last_paths |= kPathGemmFullTile;
-        return;
     }
-    if (m->cfg.gemm_mode == 2 && K % UK == 0 && lda == K && l.w_hi) {
-        const float* ahi = A.hi; const float* alo = A.lo;
-        if (!ahi) {
-            a_hi.ensure((size_t)M * K * 4); a_lo.ensure((size_t)M * K * 4);
-            split_into(cx.s, A.x, a_hi.as<float>(), a_lo.as<float>(), (uint64_t)M * K); m->launches++;
-            ahi = a_hi.as<float>(); alo = a_lo.as<float>();
-        }
-        CUtensorMap mah, mal;
-        make_map(&mah, ahi, M, K, K, GM); make_map(&mal, alo, M, K, K, GM);
-        if (!l.maps_ready) { make_map(&l.map_hi, l.w_hi, N, K, K, GN); make_map(&l.map_lo, l.w_lo, N, K, K, GN); l.maps_ready = true; }
-        const int ctas = std::min(tiles, sm_count());
-        with_act(act, [&](auto A) {
-            gemm_launch<float, decltype(A)::value, 1>(cx.s, ctas, mah, mal, l.map_hi, l.map_lo, M, N, K, l.b, 1.0f, C.x, C.hi, C.lo, ldc, n_fastest, 0, m->ovf, 1, 0);
+    const int band = F::tuned ? band_tiles(m, n_fastest, M, K, pieces * (int)sizeof(T)) : 0;
+    const int ctas = std::min(tiles, sm_count());
+    if (F::tuned && cx.head.stats && act == kActNone) {
+        if constexpr (F::tuned)
+            gemm_launch<T, kActNone, 1, true>(cx.s, ctas, ma[0], ma[1], l.map_hi, w_lo, M, N, K, l.b, unscale, C.x, nullptr, nullptr, ldc, n_fastest, band,
+                                              m->ovf, 1, 0, cx.head);
+        cx.head_fused = true;
+    } else
+        with_act(act, [&](auto Ac) {
+            gemm_launch<T, decltype(Ac)::value, 1>(cx.s, ctas, ma[0], ma[1], l.map_hi, w_lo, M, N, K, l.b, unscale, C.x, c1, c2, ldc, n_fastest, band,
+                                                   m->ovf, 1, 0, HeadEpi{}, c3);
         });
-        m->launches++; m->last_paths |= kPathGemmTf32;
-        return;
-    }
-    throw ApiError(SEALFM_EINVAL, "GEMM: K must be a multiple of 64 (3xFP16, 3xBF16) / 32 (3xTF32) with contiguous operands");
+    m->launches++; m->last_paths |= F::path_tile;
+}
+
+void gemm_impl(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, const Act& C, int ldc, int act) {
+    if (M == 0) return;
+    if (act == kActRelu) cx.m->last_paths |= kPathT5Relu;
+    with_format(cx.m->cfg.gemm_mode, [&](auto t) {
+        using T = decltype(t);
+        if (K % GemmElem<T>::KE || lda != K || !(l.*X3Format<T>::w))
+            throw ApiError(SEALFM_EINVAL, "GEMM: K must be a multiple of 64 (3xFP16, 3xBF16) / 32 (3xTF32) with contiguous operands");
+        gemm_x3<T>(cx, M, N, K, A, l, C, ldc, act);
+    });
 }
 
 void add_ln(Ctx& cx, int64_t rows, int d, const float* a, const float* b, const LNp& ln, const Act& out) {
@@ -1125,25 +1138,19 @@ template <typename Fn> void for_each_lin(sealbart* m, Fn&& fn) {
     fn(m->head);
 }
 
-// 3xTF32 operand copies of every weight matrix (gemm_mode 1 / 2; also the range-safe fallback of the 3xFP16 modes)
-void ensure_tf32_splits(sealbart* m) {
-    if (m->tf32_ready) return;
-    CUDA_CHECK(cudaSetDevice(m->device));
-    for_each_lin(m, [&](Lin& l) {
-        const uint64_t n = (uint64_t)l.out * l.in;
-        CUDA_CHECK(cudaMalloc(&l.w_hi, n * 4)); m->split_allocs.push_back(l.w_hi);
-        CUDA_CHECK(cudaMalloc(&l.w_lo, n * 4)); m->split_allocs.push_back(l.w_lo);
-        split_into(nullptr, l.w, l.w_hi, l.w_lo, n);
-        m->weight_bytes += 2 * n * 4;
-    });
-    CUDA_CHECK(cudaDeviceSynchronize());
-    m->tf32_ready = true;
+// 3xTF32 operand copies of l (gemm_mode 2): W = w_hi + w_lo, allocated here and owned by m (split_allocs)
+void split_lin_tf32(sealbart* m, Lin& l) {
+    const uint64_t n = (uint64_t)l.out * l.in;
+    CUDA_CHECK(cudaMalloc(&l.w_hi, n * 4)); m->split_allocs.push_back(l.w_hi);
+    CUDA_CHECK(cudaMalloc(&l.w_lo, n * 4)); m->split_allocs.push_back(l.w_lo);
+    split_into(nullptr, l.w, l.w_hi, l.w_lo, n);
+    m->weight_bytes += 2 * n * 4;
 }
 
 // 3xFP16 operand copies of l (gemm_mode 3 / 5): W * 2^s = w_h1 + w_h2 with max|W| * 2^s in [2^13, 2^14), w_unscale =
-// 2^-s; a weight outside the halves' range raises m->err[1].  h1 / h2 hold n = out * in halves each; null: allocated
-// here and owned by m (split_allocs).  d_max: one device word of scratch.
-void split_lin_half(sealbart* m, Lin& l, unsigned int* d_max, __half* h1 = nullptr, __half* h2 = nullptr) {
+// 2^-s, allocated here and owned by m (split_allocs); a weight outside the halves' range raises m->err[1].  d_max: one
+// device word of scratch.
+void split_lin_half(sealbart* m, Lin& l, unsigned int* d_max) {
     const uint64_t n = (uint64_t)l.out * l.in;
     CUDA_CHECK(cudaMemset(d_max, 0, 4));
     absmax_kernel<<<sm_count() * 4, 256>>>((int64_t)n, l.w, d_max);
@@ -1152,15 +1159,28 @@ void split_lin_half(sealbart* m, Lin& l, unsigned int* d_max, __half* h1 = nullp
     int sexp = 0;
     if (mx > 0.f) { int e; std::frexp(mx, &e); sexp = 14 - e; }
     l.w_unscale = std::ldexp(1.0f, -sexp);
-    if (!h1) {
-        CUDA_CHECK(cudaMalloc(&h1, n * 2)); m->split_allocs.push_back(h1);
-        CUDA_CHECK(cudaMalloc(&h2, n * 2)); m->split_allocs.push_back(h2);
-        m->weight_bytes += 2 * n * 2;
-    }
-    l.w_h1 = h1; l.w_h2 = h2;
+    CUDA_CHECK(cudaMalloc(&l.w_h1, n * 2)); m->split_allocs.push_back(l.w_h1);
+    CUDA_CHECK(cudaMalloc(&l.w_h2, n * 2)); m->split_allocs.push_back(l.w_h2);
+    m->weight_bytes += 2 * n * 2;
     split_half_kernel<<<sm_count() * 8, 256>>>((int64_t)n, l.w, std::ldexp(1.0f, sexp), l.w_h1, l.w_h2, m->err.as<int>() + 1);
     CUDA_CHECK(cudaGetLastError());
     l.maps_ready = false;
+}
+
+// The GEMM operands of l in m's gemm_mode, derived from its loaded weights (gemm_mode 6: the bf16 matrix as loaded).
+// d_max: one device word of scratch for 3xFP16, whose weight split reports into m->err.
+void derive_lin(sealbart* m, Lin& l, unsigned int* d_max) {
+    if (m->cfg.gemm_mode == kGemmTf32) split_lin_tf32(m, l);
+    else if (is_3xfp16(m->cfg.gemm_mode)) split_lin_half(m, l, d_max);
+}
+
+// 3xTF32 operand copies of every weight matrix (gemm_mode 2; also the range-safe fallback of the 3xFP16 modes)
+void ensure_tf32_splits(sealbart* m) {
+    if (m->tf32_ready) return;
+    CUDA_CHECK(cudaSetDevice(m->device));
+    for_each_lin(m, [&](Lin& l) { split_lin_tf32(m, l); });
+    CUDA_CHECK(cudaDeviceSynchronize());
+    m->tf32_ready = true;
 }
 
 // HF's T5Attention._relative_position_bucket for one relative position (key - query), in its float32 arithmetic:
@@ -1205,7 +1225,7 @@ int require_device() {
 }
 
 void check_gemm_mode(int mode) {
-    if (mode != 2 && mode != 3 && mode != 5 && mode != 6)
+    if (mode != kGemmTf32 && !is_3xfp16(mode) && mode != kGemmBf16)
         throw ApiError(SEALFM_EINVAL, "gemm_mode must be 3 (3xFP16, one CTA per tile, default), 5 (3xFP16 on 2-CTA clusters), 2 (3xTF32) "
                                       "or 6 (3xBF16, bf16 weights)");
 }
@@ -1216,10 +1236,19 @@ uint16_t bf16_rne(float x) {
     if ((u & 0x7FFFFFFFu) > 0x7F800000u) return (uint16_t)((u >> 16) | 0x40u);
     return (uint16_t)((u + 0x7FFFu + ((u >> 16) & 1u)) >> 16);
 }
-std::vector<uint16_t> to_bf16(const float* x, uint64_t n, float scale = 1.f) {
-    std::vector<uint16_t> out(n);
-    for (uint64_t i = 0; i < n; ++i) out[i] = bf16_rne(x[i] * scale);
-    return out;
+// n host values times scale (a power of two: exact) into device weights: rounded into bf16 (gemm_mode 6's matrices and
+// embedding table) or copied as fp32
+void upload(void* dst, bool bf16, const float* host, uint64_t n, float scale = 1.f) {
+    if (bf16) {
+        std::vector<uint16_t> b(n);
+        for (uint64_t i = 0; i < n; ++i) b[i] = bf16_rne(host[i] * scale);
+        CUDA_CHECK(cudaMemcpy(dst, b.data(), n * 2, cudaMemcpyHostToDevice));
+    } else if (scale != 1.f) {
+        std::vector<float> x(host, host + n);
+        for (float& v : x) v *= scale;
+        CUDA_CHECK(cudaMemcpy(dst, x.data(), n * 4, cudaMemcpyHostToDevice));
+    } else
+        CUDA_CHECK(cudaMemcpy(dst, host, n * 4, cudaMemcpyHostToDevice));
 }
 
 // sealt5_create's shape checks (before any allocation)
@@ -1326,8 +1355,6 @@ int sealbart_create_ex(const sealbart_config_t* cfg, const sealbart_variant_t* v
 void sealbart_free(sealbart_t* m) {
     if (!m) return;
     cudaSetDevice(m->device);
-    for (void* p : m->allocs) cudaFree(p);
-    for (void* p : m->split_allocs) cudaFree(p);
     if (m->lm_head_given) cudaFree(m->lm_head_bf ? (void*)m->lm_head_bf : (void*)m->lm_head);
     if (m->slice_fork) cudaEventDestroy(m->slice_fork);
     if (m->slice_join) cudaEventDestroy(m->slice_join);
@@ -1335,7 +1362,7 @@ void sealbart_free(sealbart_t* m) {
     for (auto e : m->events) cudaEventDestroy(e);
     for (auto& g : m->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
     if (m->stream) cudaStreamDestroy(m->stream);
-    delete m;                         // frees the workspace (Buf)
+    delete m;                         // frees the weights and the workspace (Buf)
 }
 
 int sealbart_set_tensor(sealbart_t* m, const char* key, const float* host, uint64_t numel) {
@@ -1348,12 +1375,11 @@ int sealbart_set_tensor(sealbart_t* m, const char* key, const float* host, uint6
             if (numel != want) throw ApiError(SEALFM_EINVAL, "lm_head.weight: wrong size");
             if (bf16_weights(m)) {
                 if (!m->lm_head_given) { CUDA_CHECK(cudaMalloc(&m->lm_head_bf, want * 2)); m->lm_head_given = true; m->weight_bytes += want * 2; }
-                const std::vector<uint16_t> b = to_bf16(host, want);
-                CUDA_CHECK(cudaMemcpy(m->lm_head_bf, b.data(), want * 2, cudaMemcpyHostToDevice));
+                upload(m->lm_head_bf, true, host, want);
                 return;
             }
             if (!m->lm_head_given) { CUDA_CHECK(cudaMalloc(&m->lm_head, want * 4)); m->lm_head_given = true; m->weight_bytes += want * 4; }
-            CUDA_CHECK(cudaMemcpy(m->lm_head, host, want * 4, cudaMemcpyHostToDevice));
+            upload(m->lm_head, false, host, want);
             return;
         }
         if (m->arch != 1 && (k == "model.encoder.embed_tokens.weight" || k == "model.decoder.embed_tokens.weight")) k = "model.shared.weight";
@@ -1363,17 +1389,9 @@ int sealbart_set_tensor(sealbart_t* m, const char* key, const float* host, uint6
         if (it->second.numel != numel) throw ApiError(SEALFM_EINVAL, "wrong element count for " + k);
         static const std::string kCrossQ = ".layer.1.EncDecAttention.q.weight";
         const bool cross_q = m->arch == 1 && k.size() > kCrossQ.size() && k.compare(k.size() - kCrossQ.size(), kCrossQ.size(), kCrossQ) == 0;
-        if (it->second.bf16) {                                 // gemm_mode 6: rounded into the bf16 matrix (x 8 below is exact)
-            const std::vector<uint16_t> b = to_bf16(host, numel, cross_q ? 8.f : 1.f);
-            CUDA_CHECK(cudaMemcpy(it->second.dst, b.data(), numel * 2, cudaMemcpyHostToDevice));
-        } else if (cross_q) {
-            // T5 does not scale attention scores; the cross-attention kernels multiply by 0.125, so q is stored times 8
-            // (a power of two: (8q . k) * 0.125 == q . k exactly)
-            std::vector<float> q8(host, host + numel);
-            for (float& v : q8) v *= 8.f;
-            CUDA_CHECK(cudaMemcpy(it->second.dst, q8.data(), numel * 4, cudaMemcpyHostToDevice));
-        } else
-            CUDA_CHECK(cudaMemcpy(it->second.dst, host, numel * 4, cudaMemcpyHostToDevice));
+        // T5 does not scale attention scores; the cross-attention kernels multiply by 0.125, so q is stored times 8
+        // (a power of two: (8q . k) * 0.125 == q . k exactly)
+        upload(it->second.dst, it->second.bf16, host, numel, cross_q ? 8.f : 1.f);
         m->loaded.insert(k);
         m->finalized = false;
     });
@@ -1392,16 +1410,12 @@ int sealbart_finalize(sealbart_t* m) {
         m->split_allocs.clear();
         m->tf32_ready = false;
         for_each_lin(m, [](Lin& l) { l.maps_ready = false; l.maps2_ready = false; });
-        if (bf16_weights(m)) {
-            // the bf16 matrices are the GEMM operands as loaded: nothing to derive
-        } else if (m->cfg.gemm_mode >= 3) {
-            unsigned int* d_max = nullptr;
-            CUDA_CHECK(cudaMalloc(&d_max, 4)); m->err.ensure(16); CUDA_CHECK(cudaMemset(m->err.p, 0, 16));
-            for_each_lin(m, [&](Lin& l) { split_lin_half(m, l, d_max); });
-            CUDA_CHECK(cudaDeviceSynchronize());
-            cudaFree(d_max);
-        } else
-            ensure_tf32_splits(m);
+        unsigned int* d_max = nullptr;
+        if (is_3xfp16(m->cfg.gemm_mode)) { CUDA_CHECK(cudaMalloc(&d_max, 4)); m->err.ensure(16); CUDA_CHECK(cudaMemset(m->err.p, 0, 16)); }
+        for_each_lin(m, [&](Lin& l) { derive_lin(m, l, d_max); });
+        CUDA_CHECK(cudaDeviceSynchronize());
+        cudaFree(d_max);
+        m->tf32_ready = m->cfg.gemm_mode == kGemmTf32;
         m->finalized = true;
     });
 }
@@ -1604,7 +1618,7 @@ void generate_enqueue(Ctx& cx, const Dims& D, const GenArgs& a, const FmView& vi
         const int eff_len = cur_len - (p->forced_bos_token_id >= 0 ? 1 : 0);
         HeadEpi he{};
         if (fused_head_on(m) && !dead && !compact && !p->disable_fm_index && eff_len > 1 && G == 1 && c.top_k == 0 &&
-            (m->cfg.gemm_mode == 3 || m->cfg.gemm_mode == 6)) {
+            head_stats_mode(m->cfg.gemm_mode)) {
             he = HeadEpi{m->st_hstat.as<float2>() + PD.r0 * head_tiles, mk[cur] + PD.r0 * D.W, (int)D.W, p->eos_token_id, p->pad_token_id};
             if (m->poison_logits) CUDA_CHECK(cudaMemsetAsync(m->logits.as<float>() + PD.r0 * D.ld, 0xFF, (size_t)PD.R * D.ld * 4, pc.s));
         }
@@ -1930,10 +1944,10 @@ int sealbart_set_option(sealbart_t* m, const char* name, int64_t value) {
         else if (n == "gemm_mode") {
             check_model(m);
             if (value == m->cfg.gemm_mode) return;
-            if (value == 6 || m->cfg.gemm_mode == 6)
+            if (value == kGemmBf16 || bf16_weights(m))
                 throw ApiError(SEALFM_EINVAL, "gemm_mode 6 (bf16 weights) is chosen at creation: the handle has no fp32 weights to switch to or from");
-            if (value == 2 && m->cfg.gemm_mode >= 3) { ensure_tf32_splits(m); m->cfg.gemm_mode = 2; }
-            else if ((value == 3 || value == 5) && m->head.w_h1) m->cfg.gemm_mode = (int)value;
+            if (value == kGemmTf32 && is_3xfp16(m->cfg.gemm_mode)) { ensure_tf32_splits(m); m->cfg.gemm_mode = kGemmTf32; }
+            else if (is_3xfp16(value) && m->head.w_h1) m->cfg.gemm_mode = (int)value;
             else throw ApiError(SEALFM_EINVAL, "gemm_mode can only switch between the 3xFP16 modes (3, 5) and 2 (3xTF32)");
             for_each_lin(m, [](Lin& l) { l.maps_ready = false; l.maps2_ready = false; });
             drop_graphs(m);
@@ -2048,11 +2062,11 @@ int sealdec_generate_ex(sealbart_t* m, const sealfm_t* fm, const uint32_t* occ_h
         if (const int rc = run()) throw ApiError(rc, last_error());
         CUDA_CHECK(cudaMemcpyAsync(errs, m->err.p, 16, cudaMemcpyDeviceToHost, s));
         CUDA_CHECK(cudaStreamSynchronize(s));
-        if (errs[1] && (m->cfg.gemm_mode == 3 || m->cfg.gemm_mode == 5)) {
+        if (errs[1] && is_3xfp16(m->cfg.gemm_mode)) {
             // An activation left the fp16 range (|x| > 65504; the producers saturate and raise the flag): this pass is
             // redone with the 3xTF32 kernels, which have fp32's range -- the caller gets exact-range results either way.
             const int mode = m->cfg.gemm_mode;
-            { const int r0 = sealbart_set_option(m, "gemm_mode", 2); if (r0) throw ApiError(r0, last_error()); }
+            { const int r0 = sealbart_set_option(m, "gemm_mode", kGemmTf32); if (r0) throw ApiError(r0, last_error()); }
             m->overflow_fallbacks++;
             const int rc = run();
             const int rc2 = sealbart_set_option(m, "gemm_mode", mode);
@@ -2197,54 +2211,34 @@ namespace {
 // the statistics [Mpad][ceil(N/128)] go (host; Mpad = M rounded up to 128 rows) and whether the epilogue ran.
 struct DebugHead { const uint32_t* mask; int eos, pad; float* stats; int32_t* fused; };
 
-// presplit: the activations are split into halves once, outside the timed calls (as the decoder's producers do)
+// presplit: 3xFP16 and 3xBF16 split the activations once, outside the timed calls (as the decoder's producers do)
 int debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A, const float* W, const float* bias, float* C,
                int32_t gelu, int32_t iters, double* avg_us, int32_t band, int32_t store, bool presplit,
                const DebugHead* head = nullptr) {
     return guarded([&] {
         if (!A || !W || (store && !C) || M <= 0 || N <= 0 || K <= 0 || band < -1) throw ApiError(SEALFM_EINVAL, "bad argument");
-        if (head && ((mode != 3 && mode != 6) || !store || gelu || iters > 0 || !head->mask || !head->stats || !head->fused))
+        if (head && (!head_stats_mode(mode) || !store || gelu || iters > 0 || !head->mask || !head->stats || !head->fused))
             throw ApiError(SEALFM_EINVAL, "bad argument");
         require_device();
         check_gemm_mode(mode);
-        sealbart fake; fake.cfg.gemm_mode = mode;
+        sealbart fake; fake.cfg.gemm_mode = mode;              // owns the weights and the scratch, as a model does
         CUDA_CHECK(cudaGetDevice(&fake.device));
-        Buf dA, dW, dB, dC, whi, wlo;
-        const int ldc = (N + 3) / 4 * 4;
-        dA.ensure((size_t)M * K * 4); dW.ensure((size_t)N * K * 4); dB.ensure((size_t)N * 4); dC.ensure((size_t)M * ldc * 4);
-        CUDA_CHECK(cudaMemcpy(dA.p, A, (size_t)M * K * 4, cudaMemcpyHostToDevice));
-        CUDA_CHECK(cudaMemcpy(dW.p, W, (size_t)N * K * 4, cudaMemcpyHostToDevice));
-        if (bias) CUDA_CHECK(cudaMemcpy(dB.p, bias, (size_t)N * 4, cudaMemcpyHostToDevice));
-        Lin l; l.w = dW.as<float>(); l.b = bias ? dB.as<float>() : nullptr; l.out = N; l.in = K;
         fake.err.ensure(16); CUDA_CHECK(cudaMemset(fake.err.p, 0, 16)); fake.ovf = fake.err.as<int>() + 1;
-        if (mode == 6) {                                       // W rounded to bf16 (RNE), as sealbart_set_tensor does
-            const std::vector<uint16_t> wb = to_bf16(W, (uint64_t)N * K);
-            whi.ensure((size_t)N * K * 2);
-            CUDA_CHECK(cudaMemcpy(whi.p, wb.data(), (size_t)N * K * 2, cudaMemcpyHostToDevice));
-            l.w_bf = whi.as<__nv_bfloat16>();
-        } else if (mode == 2) {
-            whi.ensure((size_t)N * K * 4); wlo.ensure((size_t)N * K * 4);
-            l.w_hi = whi.as<float>(); l.w_lo = wlo.as<float>();
-            split_into(nullptr, l.w, l.w_hi, l.w_lo, (uint64_t)N * K);
-        } else {
-            Buf d_max;
-            whi.ensure((size_t)N * K * 2); wlo.ensure((size_t)N * K * 2); d_max.ensure(4);
-            split_lin_half(&fake, l, d_max.as<unsigned int>(), whi.as<__half>(), wlo.as<__half>());
-        }
+        Lin l;                                                 // loaded (sealbart_set_tensor) and derived (sealbart_finalize) as the model's
+        make_lin(&fake, l, N, K);
+        upload(l.w_bf ? (void*)l.w_bf : (void*)l.w, l.w_bf != nullptr, W, (uint64_t)N * K);
+        if (bias) upload(l.b, false, bias, N);
+        else l.b = nullptr;
+        Buf d_max; d_max.ensure(4);
+        derive_lin(&fake, l, d_max.as<unsigned int>());
         fake.gemm_band = band;
+        Buf dA, dC, ah1, ah2;
+        const int ldc = (N + 3) / 4 * 4;
+        dA.ensure((size_t)M * K * 4); dC.ensure((size_t)M * ldc * 4);
+        CUDA_CHECK(cudaMemcpy(dA.p, A, (size_t)M * K * 4, cudaMemcpyHostToDevice));
         Act a{dA.as<float>()};
-        Buf ah1, ah2;
-        if (presplit && mode == 6) {
-            ah1.ensure((size_t)M * K * 4); ah2.ensure((size_t)M * K * 2);
-            a.b1 = ah1.as<__nv_bfloat16>(); a.b2 = ah2.as<__nv_bfloat16>(); a.b3 = a.b1 + (size_t)M * K;
-            split_bf16x3_kernel<<<sm_count() * 8, 256>>>((int64_t)M * K, a.x, a.b1, a.b2, a.b3);
-            CUDA_CHECK(cudaGetLastError());
-        } else if (presplit && mode >= 3) {
-            ah1.ensure((size_t)M * K * 2); ah2.ensure((size_t)M * K * 2);
-            a.h1 = ah1.as<__half>(); a.h2 = ah2.as<__half>();
-            split_half_kernel<<<sm_count() * 8, 256>>>((int64_t)M * K, a.x, 1.0f, a.h1, a.h2, fake.ovf);
-            CUDA_CHECK(cudaGetLastError());
-        }
+        if (presplit && mode != kGemmTf32)
+            with_format(mode, [&](auto t) { a = split_act<decltype(t)>(nullptr, a.x, M * K, ah1, ah2, fake.ovf); });
         const Act c{store ? dC.as<float>() : nullptr};
         Ctx cx{&fake, nullptr};
         Buf dmask, dstats;
