@@ -90,8 +90,16 @@ __device__ __forceinline__ void cluster_sync_all() {
 __device__ __forceinline__ uint32_t map_to_cta(uint32_t addr, uint32_t rank) {
     uint32_t r; asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank)); return r;
 }
+// Consumer release of a stage: one arrive on the empty barrier of each CTA whose producer refills the stage.  The
+// stage was read only by wgmma (async proxy), which wgmma.wait_group has retired, so no generic-proxy writes need to
+// be ordered before the producer's next TMA: the arrive takes the default .release.cta semantics.  A .release.cluster
+// arrive puts a cluster-scope fence in every consumer warp at every k-block: at the benchmark's shapes it cost the
+// one-CTA kernel 18-30 % of its time and the 2-CTA kernel 36 % (H100 SXM, 700 W; DESIGN.md section 4).
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
+    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
@@ -376,6 +384,12 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
         uint32_t empty_peer[CL];
 #pragma unroll
         for (int r = 0; r < CL; ++r) empty_peer[r] = CL > 1 ? map_to_cta(empty0, r) : empty0;
+        auto release = [&](int stage) {
+            if (CL == 1) mbar_arrive(empty0 + 8 * stage);
+            else
+#pragma unroll
+                for (int r = 0; r < CL; ++r) mbar_arrive_cluster(empty_peer[r] + 8 * stage);
+        };
         uint32_t it = 0;
         bool first = true;
         for (int u = unit0; u < total; u += n_units) {
@@ -420,14 +434,14 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
                     acc_fence(d);
                     if (prev_s >= 0) {
                         __syncwarp();
-                        if (lane == 0) for (int r = 0; r < CL; ++r) mbar_arrive_cluster(empty_peer[r] + 8 * prev_s);
+                        if (lane == 0) release(prev_s);
                     }
                     prev_s = s;
                 }
                 wgmma_wait<0>();
                 acc_fence(d);
                 __syncwarp();
-                if (lane == 0) for (int r = 0; r < CL; ++r) mbar_arrive_cluster(empty_peer[r] + 8 * prev_s);
+                if (lane == 0) release(prev_s);
 #pragma unroll
                 for (int j = 0; j < 64; ++j) acc[j] += d[j];              // round-to-nearest promotion
             }
