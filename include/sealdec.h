@@ -408,6 +408,44 @@ int sealdec_debug_select_step(const sealfm_t* fm, const sealdec_params_t* p, con
 int sealdec_debug_target_logprob(int64_t R, int32_t V, int64_t ld, const float* logits, const int64_t* targets,
                                  int64_t tgt_stride, float temperature, float* out, int64_t out_stride, float* full,
                                  int64_t full_ld);
+/* One attention block of the model on caller-supplied activations (sealdec_debug_attention), through the same kernel
+ * choice as the layer loops.  Host pointers throughout; heads = d / 64.
+ *   kind 0 encoder self-attention: Q sources of S positions; qkv [N][3d] with N = Q*S (src_mask int32 [Q][S], 0 = pad)
+ *          or, packed (src_off int32 [Q+1], prefix sums of lengths in [1, S]), N = src_off[Q] rows of real tokens.
+ *   kind 1 decoder self-attention at position pos (keys 0 .. pos) of B beams per query: qkv [R][3d] of this step's rows,
+ *          R = Q*B, or R = Q with compact (the first step, pos 0: row r stands for cache rows r*B .. r*B + B-1); the
+ *          layer's cache kc, vc float32 [T][Q*B][d], key s < pos of row r read from cache row anc[r][s] (int32
+ *          [Q*B][T], entries in [0, Q*B)).  The rows at position pos are filled with NaN on the device first.
+ *   kind 2 cross-attention: q [rows][d] over ckv [N][2d] (k | v of the encoder states, N as for kind 0, src_mask or
+ *          src_off as there); groups of B rows per query (rows = Q*B; compact: 1 row per query), or ragged groups
+ *          (G > 0): group g = rows grp_start[g] .. grp_start[g+1]-1 (grp_start[0] = 0, non-decreasing) of query
+ *          grp_query[g] (in [0, Q)), rows = grp_start[G].
+ *   arch 0 BART (scores q.k / 8), 1 T5 (kinds 0 and 1 add rel_bias [num_buckets][heads] at the bucket of key - query,
+ *          bidirectional for kind 0; scores unscaled; kind 2 runs the BART kernel, as the model does).
+ *   split_ks > 1: qkv (kind 1) or q (kind 2) as split-K GEMM slices split_part [split_ks][rows][cols], element =
+ *          (sum of slices in order) * split_unscale + split_bias[col]; only for the two kernels that sum them (the
+ *          decoder's per-query kernel and the short-source cross kernel); the plain qkv / q is then not read.
+ *   out_split 0 none, 1 TF32 pieces (float32 hi, lo), 2 fp16 halves (h1, h2; overflow raised past 65504), 3 bf16 x3.
+ * Outputs (each filled with NaN on the device first): out float32 [rows][d] (the T5 kernels write only the split; out
+ * then stays NaN, and out_split 0 is refused), split1..3 [rows][d] of the split's element type, *overflow,
+ * kc_out / vc_out [T][Q*B][d] (kind 1), *path = the sealbart_get_stat "last_paths" bit of the kernel that ran (0 for
+ * the BART encoder kernel).  Arguments the model never passes are SEALFM_EINVAL before any device work: a head width
+ * other than 64, d above 1024 (BART) / 4096 (T5), S outside [1, 1024], T outside [pos+1, 128], an ancestry entry out of
+ * range, a query without a valid key, split-K slices for a kernel that does not sum them. */
+typedef struct {
+    int32_t kind, arch, d, heads;
+    int64_t Q, S;
+    int32_t B, pos, T, compact;
+    const float* qkv; const float* q; const float* ckv;
+    const float* kc; const float* vc; const int32_t* anc;
+    const int32_t* src_mask; const int32_t* src_off;
+    int64_t G; const int32_t* grp_query; const int32_t* grp_start;
+    const float* rel_bias; int32_t num_buckets, max_distance;
+    const float* split_part; int32_t split_ks; float split_unscale; const float* split_bias;
+    int32_t out_split;
+} sealdec_attn_case_t;
+int sealdec_debug_attention(const sealdec_attn_case_t* c, float* out, void* split1, void* split2, void* split3,
+                            int32_t* overflow, float* kc_out, float* vc_out, uint32_t* path);
 /* The top-k warp's threshold kernel of the generate (one CTA per row) on caller-supplied rows, through the same launch.
  * Host pointers: logits float32 [R][ld] (ld >= V; columns V .. ld-1 are not read), V <= 53 248, top_k >= 1 (values above
  * V select the smallest value).  Per row: out_thr = tau, the min(top_k, V)-th largest value (-0.0 returned as +0.0),

@@ -123,6 +123,18 @@ class GroupParams(C.Structure):           # sealdec_groups_t
     _fields_ = [("num_beam_groups", C.c_int32), ("diversity_penalty", C.c_float)]
 
 
+class AttnCase(C.Structure):              # sealdec_attn_case_t
+    _fields_ = [("kind", C.c_int32), ("arch", C.c_int32), ("d", C.c_int32), ("heads", C.c_int32),
+                ("Q", C.c_int64), ("S", C.c_int64),
+                ("B", C.c_int32), ("pos", C.c_int32), ("T", C.c_int32), ("compact", C.c_int32),
+                ("qkv", vp), ("q", vp), ("ckv", vp), ("kc", vp), ("vc", vp), ("anc", vp),
+                ("src_mask", vp), ("src_off", vp),
+                ("G", C.c_int64), ("grp_query", vp), ("grp_start", vp),
+                ("rel_bias", vp), ("num_buckets", C.c_int32), ("max_distance", C.c_int32),
+                ("split_part", vp), ("split_ks", C.c_int32), ("split_unscale", C.c_float), ("split_bias", vp),
+                ("out_split", C.c_int32)]
+
+
 _DEC_SIGS = {
     "sealdec_apply_index_mask_d": (i32, [vp, vp, C.POINTER(ProcessorCfg), vp, C.c_int64, C.c_int64, vp, vp, vp,
                                          C.c_int64, C.c_int64]),
@@ -161,6 +173,7 @@ _DEC_SIGS = {
                                         C.c_int32, C.c_int32] + [vp] * 30),
     "sealdec_debug_target_logprob": (i32, [C.c_int64, C.c_int32, C.c_int64, vp, vp, C.c_int64, C.c_float, vp, C.c_int64,
                                            vp, C.c_int64]),
+    "sealdec_debug_attention": (i32, [C.POINTER(AttnCase), vp, vp, vp, vp, vp, vp, vp, vp]),
     "sealdec_debug_topk_threshold": (i32, [C.c_int64, C.c_int32, C.c_int64, vp, C.c_int32, vp, vp, vp]),
     "sealdec_debug_topk_threshold_cluster": (i32, [C.c_int64, C.c_int32, C.c_int64, vp, C.c_int32, vp, vp, vp]),
     "sealdec_debug_topk_rows":(i32, [C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_double)]),

@@ -771,30 +771,108 @@ struct DecStep : Acts {
     const int32_t* tokens = nullptr; const int32_t* anc = nullptr; const int32_t* m32 = nullptr; const int32_t* soff_x = nullptr;
 };
 
+// ---- attention dispatch -----------------------------------------------------------------------------------------
+// Which kernel runs each attention block.  The layer loops and sealdec_debug_attention both go through these, so the
+// debug entry point exercises the model's own choice; each launcher enqueues one kernel and returns its kPath* bit.
+
+// dec_self_attn_query_kernel (the beams of a query together, distinct ancestors staged once): not at the compact first
+// step, where a row stands for all beams, nor for ragged re-scoring groups, and only while the staged K / V of P = pos + 1
+// positions fit in 112 KB of shared memory.  It sums a split-K qkv itself.
+bool use_self_attn_query(int pos, int B, bool compact, bool ragged) {
+    static const bool sa_query = [] { const char* e = std::getenv("SEALB200_SELF_ATTN_QUERY"); return !e || std::atoi(e) != 0; }();
+    const size_t saq_smem = self_attn_query_smem(pos + 1, B);
+    return sa_query && !compact && !ragged && pos >= 1 && B >= 2 && B <= 32 && pos + 1 <= 128 && saq_smem <= 112 * 1024;
+}
+
+// cross_attn_small_kernel for sources of at most kXKeys positions; it sums a split-K cq itself
+bool use_cross_attn_small(int64_t S) { return S <= kXKeys; }
+
+// Decoder self-attention of one step and layer: qkv [R][3d] of the step's rows (at the compact first step row r stands
+// for cache rows r * row_mul .. r * row_mul + row_mul - 1), the layer's cache kc / vc [T][Rc][d] and ancestry anc [Rc][T].
+struct SelfAttnArgs {
+    int64_t Q, R, Rc; int B, d, heads, pos, T, row_mul;
+    const float* qkv; float* kc; float* vc; const int32_t* anc; float* out;
+};
+
+template <class SO>
+uint32_t launch_bart_self_attn(cudaStream_t s, const SelfAttnArgs& a, bool use_saq, const SO& so, const SplitSrc& qkv_src) {
+    const unsigned sa_threads = 32 * std::min(a.heads, 16);
+    if (use_saq) {
+        static size_t saq_set = 0;                     // per instantiation
+        const size_t saq_smem = self_attn_query_smem(a.pos + 1, a.B);
+        if (saq_smem > saq_set) { CUDA_CHECK(cudaFuncSetAttribute(dec_self_attn_query_kernel<SO>, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024)); saq_set = 112 * 1024; }
+        launch_k(dec_self_attn_query_kernel<SO>, dim3((unsigned)a.Q, a.heads), 32 * a.B, saq_smem, s, a.Rc, a.B, a.d, a.pos, a.T, a.qkv, a.kc, a.vc, a.anc,
+                 a.out, so, qkv_src);
+        return kPathSelfQuery;
+    }
+    if (a.pos + 1 <= 12) {
+        launch_k(dec_self_attn_kernel<3, SO>, (unsigned)a.R, sa_threads, 0, s, a.Rc, a.d, a.heads, a.pos, a.T, a.qkv, a.kc, a.vc, a.anc, a.out, so, a.row_mul, a.row_mul);
+        return kPathSelfRounds3;
+    }
+    if (a.pos + 1 <= 32) {
+        launch_k(dec_self_attn_kernel<8, SO>, (unsigned)a.R, sa_threads, 0, s, a.Rc, a.d, a.heads, a.pos, a.T, a.qkv, a.kc, a.vc, a.anc, a.out, so, a.row_mul, a.row_mul);
+        return kPathSelfRounds8;
+    }
+    launch_k(dec_self_attn_long_kernel<SO>, (unsigned)a.R, sa_threads, 0, s, a.Rc, a.d, a.heads, a.pos, a.T, a.qkv, a.kc, a.vc, a.anc, a.out, so);
+    return kPathSelfLong;
+}
+
+template <class SO>
+uint32_t launch_t5_dec_self_attn(cudaStream_t s, const SelfAttnArgs& a, const RelBias& rb, const SO& so) {
+    launch_k(t5_dec_self_attn_kernel<SO>, (unsigned)a.R, 32 * std::min(a.heads, 16), 0, s, a.Rc, a.d, a.heads, a.pos, a.T, a.qkv, a.kc, a.vc,
+             a.anc, rb, so, a.row_mul, a.row_mul);
+    return kPathT5DecAttn;
+}
+
+// Cross-attention of `groups` row groups (beams rows each, or ragged grp_query / grp_start) over ckv [Q*S or packed][2d].
+struct CrossAttnArgs {
+    int64_t groups; int d, heads, beams, S;
+    const float* q; const float* ckv; const int32_t* mask; const int32_t* grp_query; const int32_t* grp_start; float* out;
+    const int32_t* src_off;
+};
+
+template <class SO>
+uint32_t launch_cross_attn(cudaStream_t s, const CrossAttnArgs& a, const SO& so, const SplitSrc& q_src) {
+    if (use_cross_attn_small(a.S)) {
+        launch_k(cross_attn_small_kernel<SO>, dim3((unsigned)a.groups, a.heads), 128, 0, s, a.groups, a.d, a.heads, a.beams, a.S, a.q,
+                 a.ckv, a.mask, a.grp_query, a.grp_start, a.out, so, a.src_off, q_src);
+        return kPathCrossSmall;
+    }
+    launch_k(cross_attn_kernel<SO>, dim3((unsigned)a.groups, a.heads), kGAttnWarps * 32, 0, s, a.groups, a.d, a.heads, a.beams, a.S, a.q,
+             a.ckv, a.mask, a.grp_query, a.grp_start, a.out, so, a.src_off);
+    return kPathCrossGrouped;
+}
+
+// Encoder self-attention of Q sources of S positions: qkv [Q*S or packed][3d]; rb != nullptr: T5 (relative position bias,
+// unscaled scores, no fp32 copy of the output), else the BART kernel.  Returns kPathT5EncAttn or 0 (the BART encoder's
+// attention has no bit of its own: kPathEncPacked / kPathEncUnpacked name its two forms).
+template <class SO>
+uint32_t launch_enc_self_attn(cudaStream_t s, int64_t Q, int d, int heads, int S, const float* qkv, const int32_t* mask,
+                              const RelBias* rb, float* out, const SO& so, const int32_t* src_off) {
+    if (rb) {
+        launch_k(t5_enc_self_attn_kernel<kGAttnWarps, kGAttnPasses, SO>, dim3((unsigned)Q, heads), kGAttnWarps * 32, 0, s, Q, d, S, qkv, mask, *rb,
+                 so, src_off);
+        return kPathT5EncAttn;
+    }
+    launch_k(enc_self_attn_kernel<SO>, dim3((unsigned)Q, heads), kGAttnWarps * 32, 0, s, Q, d, heads, S, qkv, mask, out, so, src_off);
+    return 0;
+}
+
 // The cross-attention block of decoder layer l: cq = x Wq, attention over the layer's encoder K / V into attn, then
 // co into tmp.  defer_rows: how many rows the norm after the block accepts with co's split-K slices unsummed.
 void cross_attention(Ctx& cx, const Dims& D, const DecStep& S, int l, int64_t defer_rows) {
     sealbart* m = cx.m;
     const int d = D.d, heads = m->cfg.heads;
     DecLayerW& L = m->dec[l];
-    cx.defer_rows = (D.S <= kXKeys) ? INT64_MAX : 0;      // cross_attn_small_kernel sums a split-K cq itself
+    cx.defer_rows = use_cross_attn_small(D.S) ? INT64_MAX : 0;
     gemm(cx, S.R, d, d, S.x, d, L.cq, S.cq, d, kActNone);
     cx.defer_rows = 0;
     const SplitSrc cq_src = cx.pending;
     cx.pending = SplitSrc{};
-    const int64_t groups = D.grp_start ? D.G : D.Q;
-    const float* ckv_l = m->ckv.as<float>() + (size_t)l * S.Tk * 2 * d + S.ckv_q0;
-    with_split(m, S.attn, [&](auto so) {
-        using SO = decltype(so);
-        if (D.S <= kXKeys)
-            launch_k(cross_attn_small_kernel<SO>, dim3((unsigned)groups, heads), 128, 0, cx.s, groups, d, heads, S.compact ? 1 : D.B, (int)D.S, (const float*)S.cq.x,
-                     ckv_l, S.m32, D.grp_query, D.grp_start, S.attn.x, so, S.soff_x, cq_src);
-        else
-            launch_k(cross_attn_kernel<SO>, dim3((unsigned)groups, heads), kGAttnWarps * 32, 0, cx.s, groups, d, heads, S.compact ? 1 : D.B, (int)D.S, (const float*)S.cq.x,
-                     ckv_l, S.m32, D.grp_query, D.grp_start, S.attn.x, so, S.soff_x);
-    });
+    const CrossAttnArgs a{D.grp_start ? D.G : D.Q, d, heads, S.compact ? 1 : D.B, (int)D.S, S.cq.x,
+                          m->ckv.as<float>() + (size_t)l * S.Tk * 2 * d + S.ckv_q0, S.m32, D.grp_query, D.grp_start, S.attn.x, S.soff_x};
+    with_split(m, S.attn, [&](auto so) { m->last_paths |= launch_cross_attn(cx.s, a, so, cq_src); });
     m->launches++;
-    m->last_paths |= D.S <= kXKeys ? kPathCrossSmall : kPathCrossGrouped;
     cx.defer_rows = defer_rows;
     gemm(cx, S.R, d, d, S.attn, d, L.co, S.tmp, d, kActNone);
     cx.defer_rows = 0;
@@ -810,10 +888,9 @@ void t5_encoder_layers(Ctx& cx, const Dims& D, int64_t Te, const Acts& A, const 
         EncLayerW& L = m->enc[i];
         gemm(cx, Te, 3 * d, d, A.x, d, L.qkv, A.qkv, 3 * d, kActNone);
         with_split(m, A.attn, [&](auto so) {
-            launch_k(t5_enc_self_attn_kernel<kGAttnWarps, kGAttnPasses, decltype(so)>, dim3((unsigned)D.Q, m->cfg.heads), kGAttnWarps * 32, 0, cx.s, D.Q, d,
-                     (int)D.S, (const float*)A.qkv.x, m32, rb, so, soff);
+            m->last_paths |= launch_enc_self_attn(cx.s, D.Q, d, m->cfg.heads, (int)D.S, A.qkv.x, m32, &rb, A.attn.x, so, soff);
         });
-        m->launches++; m->last_paths |= kPathT5EncAttn;
+        m->launches++;
         cx.defer_rows = INT64_MAX;
         gemm(cx, Te, d, d, A.attn, d, L.o, A.tmp, d, kActNone);
         cx.defer_rows = 0;
@@ -837,11 +914,9 @@ void t5_decoder_layers(Ctx& cx, const Dims& D, const DecStep& S) {
         float* kc = m->kc.as<float>() + (size_t)l * D.T * S.Rc * d + D.r0 * d;
         float* vc = m->vc.as<float>() + (size_t)l * D.T * S.Rc * d + D.r0 * d;
         gemm(cx, S.R, 3 * d, d, S.x, d, L.qkv, S.qkv, 3 * d, kActNone);
-        with_split(m, S.attn, [&](auto so) {
-            launch_k(t5_dec_self_attn_kernel<decltype(so)>, (unsigned)S.R, 32 * std::min(heads, 16), 0, cx.s, S.Rc, d, heads, S.pos, D.T, (const float*)S.qkv.x, kc, vc,
-                     S.anc, rb, so, S.row_mul, S.row_mul);
-        });
-        m->launches++; m->last_paths |= kPathT5DecAttn;
+        const SelfAttnArgs a{D.Q, S.R, S.Rc, D.B, d, heads, S.pos, D.T, S.row_mul, S.qkv.x, kc, vc, S.anc, S.attn.x};
+        with_split(m, S.attn, [&](auto so) { m->last_paths |= launch_t5_dec_self_attn(cx.s, a, rb, so); });
+        m->launches++;
         cx.defer_rows = INT64_MAX;
         gemm(cx, S.R, d, d, S.attn, d, L.o, S.tmp, d, kActNone);
         cx.defer_rows = 0;
@@ -866,11 +941,8 @@ void bart_encoder_layers(Ctx& cx, const Dims& D, int64_t Te, const Acts& A, cons
     CUDA_CHECK(cudaGetLastError()); m->launches++;
     for (auto& L : m->enc) {
         gemm(cx, Te, 3 * d, d, A.x, d, L.qkv, A.qkv, 3 * d, kActNone);
-        with_split(m, A.attn, [&](auto so) {
-            enc_self_attn_kernel<decltype(so)><<<dim3((unsigned)D.Q, heads), kGAttnWarps * 32, 0, cx.s>>>(D.Q, d, heads, (int)D.S, A.qkv.x, m32, A.attn.x,
-                                                                                                          so, soff);
-        });
-        CUDA_CHECK(cudaGetLastError()); m->launches++;
+        with_split(m, A.attn, [&](auto so) { launch_enc_self_attn(cx.s, D.Q, d, heads, (int)D.S, A.qkv.x, m32, nullptr, A.attn.x, so, soff); });
+        m->launches++;
         cx.defer_rows = kAddLnRowMax;
         gemm(cx, Te, d, d, A.attn, d, L.o, A.tmp, d, kActNone);
         cx.defer_rows = 0;
@@ -891,34 +963,15 @@ void bart_self_attention(Ctx& cx, const Dims& D, const DecStep& S, int l) {
     DecLayerW& L = m->dec[l];
     float* kc = m->kc.as<float>() + (size_t)l * D.T * S.Rc * d + D.r0 * d;
     float* vc = m->vc.as<float>() + (size_t)l * D.T * S.Rc * d + D.r0 * d;
-    // the beams of a query together, distinct ancestors staged once (not at the compact first step, where a row
-    // stands for all beams, nor for ragged re-scoring groups)
-    static const bool sa_query = [] { const char* e = std::getenv("SEALB200_SELF_ATTN_QUERY"); return !e || std::atoi(e) != 0; }();
-    const size_t saq_smem = self_attn_query_smem(pos + 1, D.B);
-    const bool use_saq = sa_query && !S.compact && !D.grp_start && pos >= 1 && D.B >= 2 && D.B <= 32 && pos + 1 <= 128 && saq_smem <= 112 * 1024;
-    cx.defer_rows = use_saq ? INT64_MAX : 0;               // that kernel sums a split-K qkv itself
+    const bool use_saq = use_self_attn_query(pos, D.B, S.compact, D.grp_start != nullptr);
+    cx.defer_rows = use_saq ? INT64_MAX : 0;
     gemm(cx, S.R, 3 * d, d, S.x, d, L.qkv, S.qkv, 3 * d, kActNone);
     cx.defer_rows = 0;
     const SplitSrc qkv_src = cx.pending;
     cx.pending = SplitSrc{};
-    const unsigned sa_threads = 32 * std::min(heads, 16);
-    const float* qkv = S.qkv.x;
-    with_split(m, S.attn, [&](auto so) {
-        using SO = decltype(so);
-        if (use_saq) {
-            static size_t saq_set = 0;                     // per instantiation
-            if (saq_smem > saq_set) { CUDA_CHECK(cudaFuncSetAttribute(dec_self_attn_query_kernel<SO>, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024)); saq_set = 112 * 1024; }
-            launch_k(dec_self_attn_query_kernel<SO>, dim3((unsigned)D.Q, heads), 32 * D.B, saq_smem, cx.s, S.Rc, D.B, d, pos, D.T, qkv, kc, vc, S.anc,
-                     S.attn.x, so, qkv_src);
-        } else if (pos + 1 <= 12)
-            launch_k(dec_self_attn_kernel<3, SO>, (unsigned)S.R, sa_threads, 0, cx.s, S.Rc, d, heads, pos, D.T, qkv, kc, vc, S.anc, S.attn.x, so, S.row_mul, S.row_mul);
-        else if (pos + 1 <= 32)
-            launch_k(dec_self_attn_kernel<8, SO>, (unsigned)S.R, sa_threads, 0, cx.s, S.Rc, d, heads, pos, D.T, qkv, kc, vc, S.anc, S.attn.x, so, S.row_mul, S.row_mul);
-        else
-            launch_k(dec_self_attn_long_kernel<SO>, (unsigned)S.R, sa_threads, 0, cx.s, S.Rc, d, heads, pos, D.T, qkv, kc, vc, S.anc, S.attn.x, so);
-    });
+    const SelfAttnArgs a{D.Q, S.R, S.Rc, D.B, d, heads, pos, D.T, S.row_mul, S.qkv.x, kc, vc, S.anc, S.attn.x};
+    with_split(m, S.attn, [&](auto so) { m->last_paths |= launch_bart_self_attn(cx.s, a, use_saq, so, qkv_src); });
     m->launches++;
-    m->last_paths |= use_saq ? kPathSelfQuery : pos + 1 <= 12 ? kPathSelfRounds3 : pos + 1 <= 32 ? kPathSelfRounds8 : kPathSelfLong;
 }
 
 void bart_decoder_layers(Ctx& cx, const Dims& D, const DecStep& S) {
@@ -996,10 +1049,7 @@ void preln_encoder_layers(Ctx& cx, const Dims& D, int64_t Te, const Acts& A, con
     for (int i = 0; i < n; ++i) {
         EncLayerW& L = m->enc[i];
         gemm(cx, Te, 3 * d, d, A.x, d, L.qkv, A.qkv, 3 * d, kActNone);
-        with_split(m, A.attn, [&](auto so) {
-            launch_k(enc_self_attn_kernel<decltype(so)>, dim3((unsigned)D.Q, heads), kGAttnWarps * 32, 0, cx.s, D.Q, d, heads, (int)D.S, (const float*)A.qkv.x,
-                     m32, A.attn.x, so, soff);
-        });
+        with_split(m, A.attn, [&](auto so) { launch_enc_self_attn(cx.s, D.Q, d, heads, (int)D.S, A.qkv.x, m32, nullptr, A.attn.x, so, soff); });
         m->launches++;
         cx.defer_rows = INT64_MAX;
         gemm(cx, Te, d, d, A.attn, d, L.o, A.tmp, d, kActNone);
@@ -2536,6 +2586,150 @@ int sealdec_debug_target_logprob(int64_t R, int32_t V, int64_t ld, const float* 
         CUDA_CHECK(cudaDeviceSynchronize());
         if (out) CUDA_CHECK(cudaMemcpy(out, d_out.p, n_out * 4, cudaMemcpyDeviceToHost));
         if (full) CUDA_CHECK(cudaMemcpy(full, d_full.p, n_full * 4, cudaMemcpyDeviceToHost));
+    });
+}
+
+int sealdec_debug_attention(const sealdec_attn_case_t* c, float* out, void* split1, void* split2, void* split3,
+                            int32_t* overflow, float* kc_out, float* vc_out, uint32_t* path) {
+    return guarded([&] {
+        auto bad = [](const char* what) { return ApiError(SEALFM_EINVAL, what); };
+        if (!c || !out || !path) throw bad("null argument");
+        if (c->kind < 0 || c->kind > 2 || (c->arch != 0 && c->arch != 1)) throw bad("kind must be 0, 1 or 2 and arch 0 or 1");
+        const bool t5 = c->arch == 1, enc = c->kind == 0, self = c->kind == 1, cross = c->kind == 2;
+        const int d = c->d, heads = c->heads;
+        if (heads < 1 || (int64_t)heads * kHeadDim != d) throw bad("heads must be 64 wide (d = 64 * heads)");
+        if (d > (t5 ? 4096 : 1024)) throw bad("d must be <= 1024 (BART) / 4096 (T5)");
+        if (c->Q < 1 || c->Q > (1 << 20)) throw bad("Q must be in [1, 2^20]");
+        if (c->out_split < 0 || c->out_split > 3) throw bad("out_split must be 0..3");
+        if (c->out_split == 0 && t5 && !cross) throw bad("the T5 kernels write only the split: out_split must not be 0");
+        if (c->out_split && (!split1 || !split2 || (c->out_split == 3 && !split3) || (c->out_split == 2 && !overflow)))
+            throw bad("split output missing");
+        if (c->G && !cross) throw bad("ragged groups: cross-attention only");
+        if (c->compact && (enc || c->G)) throw bad("compact: decoder steps without ragged groups only");
+        const int64_t Q = c->Q;
+        const bool t5_bias = t5 && !cross;
+        if (t5_bias && (!c->rel_bias || c->num_buckets < 4 || c->num_buckets > 1024 || c->max_distance <= c->num_buckets / 2))
+            throw bad("T5: rel_bias needed, num_buckets in [4, 1024], max_distance > num_buckets / 2");
+        // the encoder side (kinds 0 and 2): N source rows, packed or masked
+        int64_t N = 0;
+        if (!self) {
+            if (c->S < 1 || c->S > kT5MaxSource) throw bad("S must be in [1, 1024]");
+            if (c->src_off) {
+                if (c->src_off[0] != 0) throw bad("src_off[0] must be 0");
+                for (int64_t qi = 0; qi < Q; ++qi) {
+                    const int64_t len = (int64_t)c->src_off[qi + 1] - c->src_off[qi];
+                    if (len < 1 || len > c->S) throw bad("packed source lengths must be in [1, S]");
+                }
+                N = c->src_off[Q];
+            } else {
+                if (!c->src_mask) throw bad("src_mask or src_off needed");
+                for (int64_t qi = 0; qi < Q; ++qi) {
+                    bool any = false;
+                    for (int64_t s = 0; s < c->S; ++s) any |= c->src_mask[qi * c->S + s] != 0;
+                    if (!any) throw bad("a query without a valid key");
+                }
+                N = Q * c->S;
+            }
+        }
+        int64_t rows = 0, Rc = 0;
+        if (enc) {
+            if (!c->qkv) throw bad("qkv missing");
+            rows = N;
+        } else if (self) {
+            if (c->B < 1 || c->B > 32) throw bad("B must be in [1, 32]");
+            if (c->pos < 0 || c->T < c->pos + 1 || c->T > kMaxLen) throw bad("need 0 <= pos < T <= 128");
+            if (c->compact && c->pos != 0) throw bad("compact: the first step (pos 0) only");
+            if (!c->kc || !c->vc || !c->anc || !kc_out || !vc_out) throw bad("cache, ancestry or cache output missing");
+            Rc = Q * c->B;
+            rows = c->compact ? Q : Rc;
+            for (int64_t i = 0; i < Rc * c->T; ++i)
+                if (c->anc[i] < 0 || c->anc[i] >= Rc) throw bad("ancestor row out of range");
+        } else {
+            if (!c->ckv) throw bad("ckv missing");
+            if (c->G) {
+                if (c->G < 0 || !c->grp_query || !c->grp_start || c->grp_start[0] != 0) throw bad("ragged groups: G, grp_query, grp_start[0] = 0");
+                for (int64_t g = 0; g < c->G; ++g) {
+                    if (c->grp_start[g + 1] < c->grp_start[g]) throw bad("grp_start must be non-decreasing");
+                    if (c->grp_query[g] < 0 || c->grp_query[g] >= Q) throw bad("grp_query out of range");
+                }
+                rows = c->grp_start[c->G];
+            } else {
+                if (c->B < 1) throw bad("B must be >= 1");
+                rows = c->compact ? Q : Q * c->B;
+            }
+        }
+        if (rows < 1) throw bad("no rows");
+        const int cols = cross ? d : 3 * d;                    // the row width of qkv (kinds 0, 1) / q (kind 2)
+        const bool use_saq = self && !t5 && use_self_attn_query(c->pos, c->B, c->compact != 0, false);
+        if (c->split_ks > 1) {
+            if (!(use_saq || (cross && use_cross_attn_small(c->S)))) throw bad("split-K slices: only for the kernels that sum them");
+            if (!c->split_part || !c->split_bias) throw bad("split-K slices or bias missing");
+        } else if (!enc && !(self ? c->qkv : c->q)) throw bad(self ? "qkv missing" : "q missing");
+        require_device();
+
+        Buf d_in, d_ckv, d_kc, d_vc, d_anc, d_mask, d_off, d_gq, d_gs, d_part, d_pb, d_rel, d_bkt, d_out, d_s1, d_s2, d_s3, d_ovf;
+        auto up = [&](Buf& b, const void* h, size_t bytes) { b.ensure(bytes); CUDA_CHECK(cudaMemcpy(b.p, h, bytes, cudaMemcpyHostToDevice)); };
+        auto nan = [&](Buf& b, size_t bytes) { b.ensure(bytes); CUDA_CHECK(cudaMemset(b.p, 0xFF, bytes)); };
+        const size_t in_bytes = (size_t)rows * cols * 4;
+        // qkv (kinds 0, 1) or q; with split-K slices the plain input is not read: NaN
+        if (c->split_ks > 1) {
+            nan(d_in, in_bytes);
+            up(d_part, c->split_part, in_bytes * c->split_ks); up(d_pb, c->split_bias, (size_t)cols * 4);
+        } else up(d_in, enc ? c->qkv : self ? c->qkv : c->q, in_bytes);
+        if (cross) up(d_ckv, c->ckv, (size_t)N * 2 * d * 4);
+        if (!self) {
+            if (c->src_off) up(d_off, c->src_off, (size_t)(Q + 1) * 4);
+            else up(d_mask, c->src_mask, (size_t)Q * c->S * 4);
+        }
+        const size_t cache_bytes = self ? (size_t)c->T * Rc * d * 4 : 0;
+        if (self) {
+            up(d_kc, c->kc, cache_bytes); up(d_vc, c->vc, cache_bytes); up(d_anc, c->anc, (size_t)Rc * c->T * 4);
+            const size_t at_pos = (size_t)c->pos * Rc * d * 4, pos_bytes = (size_t)Rc * d * 4;      // the rows the step writes
+            CUDA_CHECK(cudaMemset(d_kc.as<char>() + at_pos, 0xFF, pos_bytes)); CUDA_CHECK(cudaMemset(d_vc.as<char>() + at_pos, 0xFF, pos_bytes));
+        }
+        if (cross && c->G) { up(d_gq, c->grp_query, (size_t)c->G * 4); up(d_gs, c->grp_start, (size_t)(c->G + 1) * 4); }
+        RelBias rb{};
+        if (t5_bias) {
+            // the model's bucket tables (t5_bucket_tables): distance key - query at entry dist + off
+            const int off = enc ? kT5MaxSource - 1 : kMaxLen - 1;
+            std::vector<int32_t> bkt(enc ? 2 * kT5MaxSource - 1 : kMaxLen);
+            for (int i = 0; i < (int)bkt.size(); ++i) bkt[i] = t5_bucket(i - off, enc, c->num_buckets, c->max_distance);
+            up(d_bkt, bkt.data(), bkt.size() * 4); up(d_rel, c->rel_bias, (size_t)c->num_buckets * heads * 4);
+            rb = RelBias{d_rel.as<float>(), d_bkt.as<int32_t>(), off, heads};
+        }
+        const size_t out_n = (size_t)rows * d, piece = c->out_split == 1 ? 4 : 2;
+        nan(d_out, out_n * 4);
+        if (c->out_split) { nan(d_s1, out_n * piece); nan(d_s2, out_n * piece); }
+        if (c->out_split == 3) nan(d_s3, out_n * piece);
+        d_ovf.ensure(4); CUDA_CHECK(cudaMemset(d_ovf.p, 0, 4));
+        SplitSrc src{};
+        if (c->split_ks > 1) src = SplitSrc{d_part.as<float>(), c->split_ks, (int64_t)rows * cols, d_pb.as<float>(), c->split_unscale};
+
+        const float* in = d_in.as<float>();
+        const int32_t* mask = c->src_off ? nullptr : d_mask.as<int32_t>();
+        const int32_t* soff = c->src_off ? d_off.as<int32_t>() : nullptr;
+        auto run = [&](auto so) -> uint32_t {
+            if (enc) return launch_enc_self_attn(nullptr, Q, d, heads, (int)c->S, in, mask, t5 ? &rb : nullptr, d_out.as<float>(), so, soff);
+            if (self) {
+                const SelfAttnArgs a{Q, rows, Rc, c->B, d, heads, c->pos, c->T, c->compact ? c->B : 1, in, d_kc.as<float>(), d_vc.as<float>(),
+                                     d_anc.as<int32_t>(), d_out.as<float>()};
+                return t5 ? launch_t5_dec_self_attn(nullptr, a, rb, so) : launch_bart_self_attn(nullptr, a, use_saq, so, src);
+            }
+            const CrossAttnArgs a{c->G ? c->G : Q, d, heads, c->compact ? 1 : c->B, (int)c->S, in, d_ckv.as<float>(), mask,
+                                  c->G ? d_gq.as<int32_t>() : nullptr, c->G ? d_gs.as<int32_t>() : nullptr, d_out.as<float>(), soff};
+            return launch_cross_attn(nullptr, a, so, src);
+        };
+        uint32_t bit;
+        if (c->out_split == 3) bit = run(SplitBf16{d_s1.as<__nv_bfloat16>(), d_s2.as<__nv_bfloat16>(), d_s3.as<__nv_bfloat16>()});
+        else bit = run(SplitOut{d_s1.p, d_s2.p, c->out_split, c->out_split == 2 ? d_ovf.as<int>() : nullptr});
+        CUDA_CHECK(cudaDeviceSynchronize());
+        auto down = [&](void* h, const Buf& b, size_t bytes) { CUDA_CHECK(cudaMemcpy(h, b.p, bytes, cudaMemcpyDeviceToHost)); };
+        down(out, d_out, out_n * 4);
+        if (c->out_split) { down(split1, d_s1, out_n * piece); down(split2, d_s2, out_n * piece); }
+        if (c->out_split == 3) down(split3, d_s3, out_n * piece);
+        if (overflow) down(overflow, d_ovf, 4);
+        if (self) { down(kc_out, d_kc, cache_bytes); down(vc_out, d_vc, cache_bytes); }
+        *path = bit;
     });
 }
 

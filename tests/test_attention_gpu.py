@@ -1,0 +1,795 @@
+"""GPU: every attention kernel (bart_kernels.cuh, t5_kernels.cuh) against a float64 attention of the same inputs, through
+sealdec_debug_attention (the layer loops' own kernel choice), on crafted trained-scale scores at the dispatch
+boundaries of decode.cu.
+
+Reference.  numpy float64 on the fp32 inputs the kernel reads (split-K slices summed in fp32 first, in the kernel's
+order): score = q.k / 8 (BART) or q.k + bias[bucket(key - query)][h] (T5, unscaled; buckets from transformers'
+T5Attention._relative_position_bucket), masked keys -inf, softmax, P.V.  Decoder key s < pos comes from cache row
+anc[r][s], key pos from this step's qkv.
+
+Bound, per output element j of row r and head h, with u = 2^-24, derived from the kernels' fp32 arithmetic:
+  E_s = gamma_64 * scale * sum_i |q_i k_si|     the fp32 dot product over 64 dims (any order; scale is exact)
+        + u * |sc_s|                            the scaling or the bias add
+        + u * |sc_s - m|                        the subtraction inside exp (m: the running / final maximum)
+        + 4u                                    expf's 2 ulp
+  is a bound on the relative error of each unnormalised weight p_s = exp(sc_s - m) (chunk corrections included: a
+  correction exp(m_old - m_new) times exp(sc - m_old) carries the same argument error, |sc - m_old| + |m_old - m_new|
+  = |sc - m_new|).  Then
+  |o^_j - o_j| <= sum_s p_s |v_sj - o_j| (E_s + max_t E_t)          perturbed weights, renormalised
+               + c u sum_s p_s |v_sj|                               the P.V accumulation
+               + (2n + 2 n_chunks + 6) u |o_j|                      the sum l of the weights and the division
+               + n 2^-126 max|v|                                    weights that underflow
+  where p_s here is normalised, n is the number of keys and c = 2n + 3 n_chunks + 8: along any path every key adds
+  one fma and at most one correction multiply, every 32-key chunk merge a multiply, an add and a shuffle-tree add.
+The worst err / bound ratio of every case is printed; the near-uniform control sits far below 1.
+
+Score sets include a common offset (maximum near +110, where exp(score) overflows), rows entirely at or below -100
+(where it underflows to 0), and a maximum 110 above a full first chunk (the correction exp(-110) underflows to 0).
+That bound is dominated by the dot-product and accumulation terms, so test_exp_accuracy_probe adds inputs on which
+every kernel's arithmetic is exact except expf and one division: there the bound is 5u (see exp_probe), and an
+exponential whose error grows with |x| fails it.  The last section reruns forward-vs-float64 checks of each model
+family with the query projections scaled by 2^4.
+
+Exact checks: the cache rows at pos equal this step's k / v bit for bit for every beam (all B rows of a query at the
+compact first step) and every other cache row is unchanged (positions past pos hold a sentinel); the TF32 pieces are
+the host split of out (T5: out = hi + lo); the fp16 halves are the host split of out or the overflow flag is raised;
+b1 + b2 + b3 reproduces out exactly."""
+import ctypes as C
+
+import numpy as np
+import pytest
+
+pytestmark = pytest.mark.gpu
+
+U = 2.0 ** -24
+GAMMA64 = 64 * U / (1 - 64 * U)
+PATH = {"self_query": 1 << 2, "self_rounds3": 1 << 3, "self_rounds8": 1 << 4, "self_long": 1 << 5,
+        "cross_small": 1 << 6, "cross_grouped": 1 << 7, "t5_enc": 1 << 16, "t5_dec": 1 << 17, "enc": 0}
+SAQ_SMEM_MAX = 112 * 1024
+SENTINEL = np.float32(7777.0)
+DISTS = ["uniform", "peak_first", "peak_last", "late_max", "rising", "ties", "onehot", "cancel", "voffset", "high", "low",
+         "vbig"]
+
+
+@pytest.fixture(scope="module", autouse=True)
+def need_gpu():
+    import torch
+    assert torch.cuda.is_available(), "-m gpu tests need a CUDA device"
+
+
+def saq_smem(P, B):
+    return 2 * P * B * 64 * 4 + 2 * P * 32 * 4 + 128 * 4
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# crafted scores
+# ---------------------------------------------------------------------------------------------------------------
+
+def key_levels(rng, dist, n):
+    """the intended score of each of n keys (exact small dyadics)"""
+    if dist in ("uniform", "cancel", "voffset", "vbig"):
+        z = rng.integers(-3, 4, n) / 64.0
+        if dist == "cancel":
+            z = rng.integers(-24, 1, n).astype(np.float64)
+    elif dist == "peak_first":
+        z = rng.integers(-80, -8, n).astype(np.float64); z[min(3, n - 1)] = 0
+    elif dist == "peak_last":
+        z = rng.integers(-80, -8, n).astype(np.float64); z[-1] = 0
+    elif dist == "late_max":              # a large first chunk, the maximum 110 above it in a later chunk: corr = 0
+        z = np.full(n, -100.0); z[:min(32, n)] = -rng.integers(0, 3, min(32, n)); z[-1] = 110 if n > 32 else 0
+    elif dist == "high":                  # a common offset: the maximum near 110, where exp(score) overflows
+        z = 110.0 - rng.integers(0, 30, n); z[rng.integers(0, n)] = 110
+    elif dist == "low":                   # every score at or below -100, where exp(score) underflows to 0
+        z = -100.0 - rng.integers(0, 30, n); z[rng.integers(0, n)] = -100
+    elif dist == "rising":
+        z = (np.arange(n) // 32) * 6.0 + rng.integers(0, 4, n)
+    elif dist == "ties":
+        z = rng.integers(-12, -2, n).astype(np.float64); z[rng.choice(n, size=min(n, 3), replace=False)] = 4
+    elif dist == "onehot":
+        z = rng.integers(-60, -40, n).astype(np.float64); z[rng.integers(0, n)] = 0
+    return z
+
+
+def craft_qk(rng, dist, nr, keys, H, bart):
+    """q [nr][H][64], k [keys][H][64] float32 whose scores are z_s (per key) + a small row-dependent term; 'cancel'
+    adds pairs q = (c, c), k = (t, -t) that cancel exactly but make sum |q k| large"""
+    q = np.zeros((nr, H, 64), np.float64); k = np.zeros((keys, H, 64), np.float64)
+    for h in range(H):
+        z = key_levels(rng, dist, keys)
+        q[:, h, 0] = 8.0 if bart else 1.0
+        k[:, h, 0] = z
+        q[:, h, 1] = rng.integers(-8, 9, nr) / 8.0 * (8.0 if bart else 1.0)
+        k[:, h, 1] = rng.integers(-8, 9, keys) / 64.0
+        if dist == "cancel":
+            c = rng.uniform(10, 40, (nr, 31)); t = rng.uniform(10, 40, (keys, 31))
+            q[:, h, 2::2] = c; q[:, h, 3::2] = c
+            k[:, h, 2::2] = t; k[:, h, 3::2] = -t
+        else:
+            q[:, h, 2:] = rng.integers(-4, 5, (nr, 62)) / 16.0
+            k[:, h, 2:] = rng.integers(-4, 5, (keys, 62)) / 64.0
+        if dist == "ties":
+            top = np.flatnonzero(z == z.max())
+            k[top, h, 1:] = k[top[0], h, 1:]
+    return q.astype(np.float32), k.astype(np.float32)
+
+
+def craft_v(rng, dist, keys, H):
+    v = rng.standard_normal((keys, H, 64)).astype(np.float32)
+    if dist == "voffset":
+        v += np.float32(1000.0)
+    if dist == "vbig":                    # past the fp16 range: the halves saturate and raise the overflow flag
+        v += np.float32(1e5)
+    return v
+
+
+def bucket_table(rel, bidirectional, nb, md):
+    import torch
+    from transformers.models.t5.modeling_t5 import T5Attention
+    return T5Attention._relative_position_bucket(torch.as_tensor(rel), bidirectional=bidirectional, num_buckets=nb,
+                                                 max_distance=md).numpy()
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# reference and bound
+# ---------------------------------------------------------------------------------------------------------------
+
+def attend_ref(q, k, v, valid, bias, scale):
+    """q [nr][H][64], k / v [nr or 1][n][H][64] (per-row keys or shared), valid bool [nr or 1][n], bias [nr][H][n] or
+    None.  Returns (o, bound) [nr][H][64] float64."""
+    q64, k64, v64 = q.astype(np.float64), k.astype(np.float64), v.astype(np.float64)
+    nr = q.shape[0]
+    n = k.shape[1]
+    nch = (n + 31) // 32
+    o_all = np.empty(q.shape); b_all = np.empty(q.shape)
+    step = max(1, (1 << 22) // max(1, n * q.shape[1] * 64))
+    for r0 in range(0, nr, step):
+        sl = slice(r0, min(nr, r0 + step))
+        kk = k64[sl] if k64.shape[0] > 1 else k64
+        vv = v64[sl] if v64.shape[0] > 1 else v64
+        ok = valid[sl] if valid.shape[0] > 1 else valid
+        dot = np.einsum("rhi,rshi->rhs", q64[sl], np.broadcast_to(kk, (sl.stop - sl.start,) + kk.shape[1:]))
+        adot = np.einsum("rhi,rshi->rhs", np.abs(q64[sl]), np.abs(np.broadcast_to(kk, (sl.stop - sl.start,) + kk.shape[1:])))
+        sc = dot * scale + (bias[sl] if bias is not None else 0.0)
+        okb = np.broadcast_to(ok[:, None, :], sc.shape)
+        sc = np.where(okb, sc, -np.inf)
+        m = sc.max(-1, keepdims=True)
+        with np.errstate(invalid="ignore"):
+            p = np.where(okb, np.exp(sc - m), 0.0)
+        P = p / p.sum(-1, keepdims=True)
+        vb = np.broadcast_to(vv, (sl.stop - sl.start,) + vv.shape[1:])
+        o = np.einsum("rhs,rshj->rhj", P, vb)
+        with np.errstate(invalid="ignore"):
+            E = np.where(okb, GAMMA64 * scale * adot + U * np.abs(np.where(okb, sc, 0)) + U * np.abs(np.where(okb, sc - m, 0)) + 4 * U, 0.0)
+        Emax = E.max(-1, keepdims=True)
+        dv = np.abs(vb.transpose(0, 2, 1, 3) - o[:, :, None, :])            # [r][h][s][j]
+        t1 = np.einsum("rhs,rhsj->rhj", P * (E + Emax), dv)
+        t2 = (2 * n + 3 * nch + 8) * U * np.einsum("rhs,rshj->rhj", P, np.abs(vb))
+        t3 = (2 * n + 2 * nch + 6) * U * np.abs(o)
+        t4 = n * 2.0 ** -126 * np.abs(vv).max()
+        o_all[sl] = o; b_all[sl] = t1 + t2 + t3 + t4
+    return o_all, b_all
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# the debug call and the split checks
+# ---------------------------------------------------------------------------------------------------------------
+
+def host_half_split(x):
+    h1 = x.astype(np.float16)
+    h2 = (x - h1.astype(np.float32)).astype(np.float16)
+    return h1, h2
+
+
+def run_attention(case, rows, out_split, kc_shape=None):
+    from seal_b200._lib import lib, check, AttnCase
+    c = AttnCase()
+    keep = []
+    for name, val in case.items():
+        if isinstance(val, np.ndarray):
+            keep.append(val)
+            setattr(c, name, val.ctypes.data)
+        else:
+            setattr(c, name, val)
+    c.out_split = out_split
+    d = case["d"]
+    out = np.empty((rows, d), np.float32)
+    dt = {0: np.float32, 1: np.float32, 2: np.float16, 3: np.uint16}[out_split]
+    sp = [np.empty((rows, d), dt) for _ in range(3)]
+    ovf = np.zeros(1, np.int32)
+    kco = np.empty(kc_shape, np.float32) if kc_shape else None
+    vco = np.empty(kc_shape, np.float32) if kc_shape else None
+    path = np.zeros(1, np.uint32)
+    check(lib.sealdec_debug_attention(C.byref(c), out.ctypes.data, *[s.ctypes.data for s in sp], ovf.ctypes.data,
+                                      kco.ctypes.data if kc_shape else None, vco.ctypes.data if kc_shape else None,
+                                      path.ctypes.data))
+    return out, sp, int(ovf[0]), kco, vco, int(path[0])
+
+
+def value_of(out, sp, ovf, out_split, writes_out):
+    """the kernel's fp32 output, checking the split against it exactly"""
+    if out_split == 0:
+        assert writes_out
+        return out
+    if out_split == 1:
+        hi, lo = sp[0], sp[1]
+        if writes_out:
+            hb = (out.view(np.uint32) & np.uint32(0xFFFFE000)).view(np.float32)
+            assert np.array_equal(hi.view(np.uint32), hb.view(np.uint32)) and np.array_equal(lo, out - hb)
+            return out
+        assert np.isnan(out).all()
+        return (hi + lo).astype(np.float32)
+    if out_split == 2:
+        if writes_out:
+            if not ovf:
+                h1, h2 = host_half_split(out)
+                assert np.array_equal(sp[0].view(np.uint16), h1.view(np.uint16))
+                assert np.array_equal(sp[1].view(np.uint16), h2.view(np.uint16))
+            else:
+                assert np.abs(out).max() > 65504
+            return out
+        assert np.isnan(out).all()
+        return None                                       # the halves alone: checked by the caller with their rounding
+    b = [(s.astype(np.uint32) << 16).view(np.float32).astype(np.float64) for s in sp]
+    if writes_out:
+        assert np.array_equal(b[0] + b[1] + b[2], out.astype(np.float64))
+        return out
+    assert np.isnan(out).all()
+    return (b[0] + b[1] + b[2]).astype(np.float32)
+
+
+def compare(label, got, sp, out_split, ref, bound, ovf=0):
+    """got [rows][d] vs ref / bound [rows][H][64]; returns the worst ratio"""
+    rows = ref.shape[0]
+    ref = ref.reshape(rows, -1); bound = bound.reshape(rows, -1)
+    if out_split == 2 and np.abs(ref).max() > 65600:
+        assert ovf == 1, f"{label}: fp16 range exceeded, overflow flag not raised"
+        if got is None:
+            return 0.0
+    elif out_split == 2:
+        assert ovf == 0, f"{label}: overflow flag raised inside the fp16 range"
+    if got is None:                                       # fp16 halves of a T5 kernel: h1 + h2 carries x to 2^-22 |x| + 2^-25
+        x = sp[0].astype(np.float64) + sp[1].astype(np.float64)
+        bound = bound + 2.0 ** -22 * np.abs(ref) + 2.0 ** -25
+    else:
+        x = got.astype(np.float64)
+    assert np.isfinite(x).all(), f"{label}: non-finite output"
+    ratio = (np.abs(x - ref) / bound).max()
+    print(f"{label}: worst err/bound {ratio:.3g}")
+    assert ratio <= 1.0, (label, ratio)
+    return ratio
+
+
+def split_k(rng, x, ks):
+    """split-K slices of x (float32 [rows][cols]): returns (part [ks][rows][cols], bias, unscale, effective fp32 value)"""
+    unscale = np.float32(0.5)
+    bias = rng.integers(-4, 5, x.shape[1]).astype(np.float32) / 8
+    part = (rng.standard_normal((ks,) + x.shape).astype(np.float32) * np.float32(0.01))
+    part[0] = (x - bias) / unscale - part[1:].sum(0, dtype=np.float32)
+    y = part[0].copy()
+    for sl in range(1, ks):
+        y = (y + part[sl]).astype(np.float32)
+    eff = (y * unscale + bias).astype(np.float32)
+    return part, bias, unscale, eff
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# encoder self-attention and cross-attention
+# ---------------------------------------------------------------------------------------------------------------
+
+def source_mask(rng, Q, S, kind):
+    m = np.ones((Q, S), np.int32)
+    for q in range(Q):
+        l = S if q == 0 else int(rng.integers(max(1, S // 2), S + 1))
+        m[q, l:] = 0
+        if kind == "holes" and l >= 3:
+            m[q, rng.choice(np.arange(1, l - 1), size=max(1, (l - 2) // 4), replace=False)] = 0
+        if kind == "left":
+            m[q] = np.roll(m[q], S - l)
+        if kind == "first_chunk" and S > 32:
+            m[q, :32] = 0; m[q, 32:] = 1
+        if kind == "first_two_chunks" and S > 64:
+            m[q, :64] = 0; m[q, 64:] = 1
+        if kind == "last_only":
+            m[q] = 0; m[q, S - 1] = 1
+    return m
+
+
+def make_source(rng, Q, S, H, dist, bart, mask_kind, packed, nr_per_key_rows):
+    """per query: key matrices k, v [S or len][H][64] plus the valid mask; packed: lengths from a right-padded mask"""
+    if packed:
+        lens = [S] + [int(rng.integers(max(1, S // 2), S + 1)) for _ in range(Q - 1)]
+        valid = [np.ones(l, bool) for l in lens]
+    else:
+        m = source_mask(rng, Q, S, mask_kind)
+        valid = [m[q] != 0 for q in range(Q)]
+    return valid
+
+
+def enc_case(arch, Q, S, heads, dist, mask_kind="right", packed=False, seed=0, out_splits=(0, 2, 3)):
+    rng = np.random.default_rng(seed)
+    bart = arch == 0
+    d = heads * 64
+    valid = make_source(rng, Q, S, heads, dist, bart, mask_kind, packed, None)
+    ns = [len(v) for v in valid]
+    N = sum(ns)
+    qkv = np.empty((N, 3 * d), np.float32)
+    nb, md = (32, 128)
+    rel = (rng.uniform(-10, 10, (nb, heads))).astype(np.float32) if not bart else None
+    refs, bounds = [], []
+    r0 = 0
+    for qi, n in enumerate(ns):
+        qm, km = craft_qk(rng, dist, n, n, heads, bart)
+        vm = craft_v(rng, dist, n, heads)
+        qkv[r0:r0 + n, :d] = qm.reshape(n, d); qkv[r0:r0 + n, d:2 * d] = km.reshape(n, d)
+        qkv[r0:r0 + n, 2 * d:] = vm.reshape(n, d)
+        bias = None
+        if not bart:
+            dist_ = np.arange(n)[None, :] - np.arange(n)[:, None]
+            bias = rel[bucket_table(dist_, True, nb, md)].transpose(0, 2, 1).astype(np.float64)
+        o, b = attend_ref(qm, km[None], vm[None], valid[qi][None], bias, 0.125 if bart else 1.0)
+        refs.append(o); bounds.append(b)
+        r0 += n
+    case = dict(kind=0, arch=arch, d=d, heads=heads, Q=Q, S=S, qkv=qkv)
+    if packed:
+        case["src_off"] = np.concatenate([[0], np.cumsum(ns)]).astype(np.int32)
+    else:
+        case["src_mask"] = np.stack(valid).astype(np.int32)
+    if not bart:
+        case.update(rel_bias=rel, num_buckets=nb, max_distance=md)
+    ref, bound = np.concatenate(refs), np.concatenate(bounds)
+    label = f"enc arch={arch} Q={Q} S={S} H={heads} {dist} {mask_kind} packed={packed}"
+    worst = 0.0
+    for osp in out_splits:
+        if not bart and osp == 0:
+            osp = 1
+        out, sp, ovf, _, _, path = run_attention(case, N, osp)
+        assert path == (PATH["enc"] if bart else PATH["t5_enc"])
+        got = value_of(out, sp, ovf, osp, bart)
+        worst = max(worst, compare(f"{label} split={osp}", got, sp, osp, ref, bound, ovf))
+    return worst, path
+
+
+def cross_case(Q, S, B, heads, dist, mask_kind="right", packed=False, ragged=None, ks=1, compact=False, seed=0,
+               out_splits=(0, 2, 3)):
+    rng = np.random.default_rng(seed)
+    d = heads * 64
+    valid = make_source(rng, Q, S, heads, dist, True, mask_kind, packed, None)
+    ns = [len(v) for v in valid]
+    if ragged is not None:
+        grp_query = np.array([g[0] for g in ragged], np.int32)
+        sizes = [g[1] for g in ragged]
+    else:
+        grp_query = np.arange(Q, dtype=np.int32)
+        sizes = [1 if compact else B] * Q
+    rows = sum(sizes)
+    ckv = np.empty((sum(ns) if packed else Q * S, 2 * d), np.float32)
+    q = np.empty((rows, d), np.float32)
+    keys = {}
+    for qi in range(Q):
+        n = ns[qi]
+        keys[qi] = craft_qk(rng, dist, 1, n, heads, True)[1], craft_v(rng, dist, n, heads)
+        k0 = sum(ns[:qi]) if packed else qi * S
+        ckv[k0:k0 + n, :d] = keys[qi][0].reshape(n, d); ckv[k0:k0 + n, d:] = keys[qi][1].reshape(n, d)
+        if not packed and n < S:
+            ckv[k0 + n:k0 + S] = 0
+    refs, bounds = [], []
+    r0 = 0
+    for g, qi in enumerate(grp_query):
+        nr = sizes[g]
+        kq, vq = keys[int(qi)]
+        # rows of the group get scores against this query's keys
+        qm = craft_qk(np.random.default_rng(seed * 1000 + g), dist, nr, len(kq), heads, True)[0]
+        q[r0:r0 + nr] = qm.reshape(nr, d)
+        o, b = attend_ref(qm, kq[None], vq[None], valid[qi][None], None, 0.125)
+        refs.append(o); bounds.append(b)
+        r0 += nr
+    case = dict(kind=2, arch=0, d=d, heads=heads, Q=Q, S=S, B=B, compact=int(compact), ckv=ckv)
+    if packed:
+        case["src_off"] = np.concatenate([[0], np.cumsum(ns)]).astype(np.int32)
+    else:
+        case["src_mask"] = np.stack(valid).astype(np.int32)
+    if ragged is not None:
+        case.update(G=len(ragged), grp_query=grp_query, grp_start=np.concatenate([[0], np.cumsum(sizes)]).astype(np.int32))
+    if ks > 1:
+        part, bias, unscale, eff = split_k(rng, q, ks)
+        case.update(split_part=part, split_ks=ks, split_unscale=float(unscale), split_bias=bias)
+        # the reference on the effective q the kernel forms
+        refs, bounds, r0 = [], [], 0
+        for g, qi in enumerate(grp_query):
+            nr = sizes[g]; kq, vq = keys[int(qi)]
+            o, b = attend_ref(eff[r0:r0 + nr].reshape(nr, heads, 64), kq[None], vq[None], valid[qi][None], None, 0.125)
+            refs.append(o); bounds.append(b); r0 += nr
+    else:
+        case["q"] = q
+    ref, bound = np.concatenate(refs), np.concatenate(bounds)
+    label = f"cross Q={Q} S={S} B={B} H={heads} {dist} {mask_kind} packed={packed} ragged={ragged is not None} ks={ks}"
+    worst = 0.0
+    for osp in out_splits:
+        out, sp, ovf, _, _, path = run_attention(case, rows, osp)
+        assert path == (PATH["cross_small"] if S <= 32 else PATH["cross_grouped"]), (label, path)
+        worst = max(worst, compare(f"{label} split={osp}", value_of(out, sp, ovf, osp, True), sp, osp, ref, bound, ovf))
+    return worst, path
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# decoder self-attention
+# ---------------------------------------------------------------------------------------------------------------
+
+def ancestry(rng, Q, B, T, mode):
+    R = Q * B
+    anc = np.empty((R, T), np.int32)
+    for r in range(R):
+        q0 = (r // B) * B
+        for s in range(T):
+            m = mode if mode != "mixed" else ("one", "distinct", "random")[s % 3]
+            anc[r, s] = q0 if m == "one" else r if m == "distinct" else q0 + rng.integers(0, B)
+    return anc
+
+
+def dec_case(arch, Q, B, P, heads, dist, anc_mode="random", compact=False, ks=1, seed=0, out_splits=(0, 2, 3)):
+    rng = np.random.default_rng(seed)
+    bart = arch == 0
+    d = heads * 64
+    pos = P - 1
+    T = min(128, P + 2)
+    Rc = Q * B
+    R = Q if compact else Rc
+    row_mul = B if compact else 1
+    # per position, per cache row: keys crafted so that position s has level z_s for every row
+    qm, kcur = craft_qk(rng, dist, R, P, heads, bart)        # kcur[s] is the level-s key template
+    kc = np.full((T, Rc, d), SENTINEL, np.float32); vc = np.full((T, Rc, d), SENTINEL, np.float32)
+    amp = 0.0 if dist == "ties" else 1.0                  # ties: every row's key at a position is the same, tied exactly
+    for s in range(pos):
+        noise = (rng.integers(-4, 5, (Rc, heads, 64)) / 256.0 * amp).astype(np.float32)
+        noise[:, :, 0] = 0
+        kc[s] = (kcur[s][None] + noise).reshape(Rc, d)
+        vc[s] = craft_v(rng, dist, Rc, heads).reshape(Rc, d)
+    qkv = np.empty((R, 3 * d), np.float32)
+    qkv[:, :d] = qm.reshape(R, d)
+    qkv[:, d:2 * d] = (kcur[pos][None] + (rng.integers(-4, 5, (R, heads, 64)) / 256.0 * amp)).reshape(R, d).astype(np.float32)
+    qkv[:, 2 * d:] = craft_v(rng, dist, R, heads).reshape(R, d)
+    anc = ancestry(rng, Q, B, T, anc_mode)
+    case = dict(kind=1, arch=arch, d=d, heads=heads, Q=Q, B=B, pos=pos, T=T, compact=int(compact), kc=kc, vc=vc, anc=anc)
+    eff = qkv
+    if ks > 1:
+        part, bias, unscale, eff = split_k(rng, qkv, ks)
+        case.update(split_part=part, split_ks=ks, split_unscale=float(unscale), split_bias=bias)
+    else:
+        case["qkv"] = qkv
+    nb, md = 32, 128
+    bias = None
+    if not bart:
+        rel = rng.uniform(-10, 10, (nb, heads)).astype(np.float32)
+        case.update(rel_bias=rel, num_buckets=nb, max_distance=md)
+        bk = bucket_table(np.arange(P) - pos, False, nb, md)
+        bias = np.broadcast_to(rel[bk].T.astype(np.float64)[None], (R, heads, P))
+    K = np.empty((R, P, heads, 64), np.float32); V = np.empty((R, P, heads, 64), np.float32)
+    for r in range(R):
+        pr = r * row_mul
+        for s in range(pos):
+            K[r, s] = kc[s, anc[pr, s]].reshape(heads, 64); V[r, s] = vc[s, anc[pr, s]].reshape(heads, 64)
+        K[r, pos] = eff[r, d:2 * d].reshape(heads, 64); V[r, pos] = eff[r, 2 * d:].reshape(heads, 64)
+    ref, bound = attend_ref(eff[:, :d].reshape(R, heads, 64), K, V, np.ones((R, P), bool), bias, 0.125 if bart else 1.0)
+    saq = bart and not compact and pos >= 1 and 2 <= B <= 32 and saq_smem(P, B) <= SAQ_SMEM_MAX
+    want = (PATH["t5_dec"] if not bart else PATH["self_query"] if saq else PATH["self_rounds3"] if P <= 12
+            else PATH["self_rounds8"] if P <= 32 else PATH["self_long"])
+    label = f"dec arch={arch} Q={Q} B={B} P={P} H={heads} {dist} anc={anc_mode} compact={compact} ks={ks}"
+    worst = 0.0
+    for osp in out_splits:
+        if not bart and osp == 0:
+            osp = 1
+        out, sp, ovf, kco, vco, path = run_attention(case, R, osp, kc_shape=kc.shape)
+        assert path == want, (label, path, want)
+        worst = max(worst, compare(f"{label} split={osp}", value_of(out, sp, ovf, osp, bart), sp, osp, ref, bound, ovf))
+        # the cache: position pos holds this step's k / v for every beam (all B rows of a query at the compact step)
+        for r in range(R):
+            for b2 in range(row_mul):
+                cr = r * row_mul + b2
+                assert np.array_equal(kco[pos, cr].view(np.uint32), eff[r, d:2 * d].view(np.uint32)), (label, r, b2)
+                assert np.array_equal(vco[pos, cr].view(np.uint32), eff[r, 2 * d:].view(np.uint32)), (label, r, b2)
+        other = np.ones(T, bool); other[pos] = False
+        assert np.array_equal(kco[other].view(np.uint32), kc[other].view(np.uint32)), label
+        assert np.array_equal(vco[other].view(np.uint32), vc[other].view(np.uint32)), label
+    return worst, path
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# the grid
+# ---------------------------------------------------------------------------------------------------------------
+
+def _dist(i):
+    return DISTS[i % len(DISTS)]
+
+
+DEC_BART = (
+    [(1, P, 2) for P in (1, 2, 12, 13, 32, 33, 64, 65, 128)]
+    + [(2, P, 2) for P in (2, 12, 13, 32, 33, 89, 90, 128)]
+    + [(15, P, 2) for P in (2, 14, 15, 33)]
+    + [(16, P, 2) for P in (12, 13)]
+    + [(32, P, 2) for P in (2, 6, 7, 33)]
+    + [(2, 13, 16), (1, 65, 16), (15, 14, 16)]
+)
+DEC_T5 = [(1, 1, 2), (1, 33, 2), (4, 65, 16), (2, 128, 32), (1, 33, 48), (2, 13, 64)]
+ENC = [(S, packed) for S in (1, 31, 32, 33, 256, 1024) for packed in (False, True)]
+CROSS = [(S, B) for S in (1, 31, 32, 33, 64, 65) for B in (1, 15, 16, 17, 32, 33)]
+
+
+@pytest.mark.parametrize("i,B,P,heads", [(i, *c) for i, c in enumerate(DEC_BART)],
+                         ids=[f"B{B}_P{P}_H{h}" for B, P, h in DEC_BART])
+def test_dec_self_attention_bart(i, B, P, heads):
+    anc = ("one", "distinct", "mixed", "random")[i % 4]
+    worst, _ = dec_case(0, 2 if B < 32 else 1, B, P, heads, _dist(i), anc_mode=anc, seed=i)
+    if _dist(i) == "uniform":
+        assert worst < 0.1
+
+
+@pytest.mark.parametrize("i,B,P,heads", [(i, *c) for i, c in enumerate(DEC_T5)], ids=[f"B{B}_P{P}_H{h}" for B, P, h in DEC_T5])
+def test_dec_self_attention_t5(i, B, P, heads):
+    dec_case(1, 2, B, P, heads, _dist(i + 3), anc_mode=("mixed", "random")[i % 2], seed=100 + i, out_splits=(1, 2, 3))
+
+
+@pytest.mark.parametrize("arch", [0, 1])
+@pytest.mark.parametrize("B", [2, 15])
+def test_dec_self_attention_compact_first_step(arch, B):
+    dec_case(arch, 3, B, 1, 2, "uniform", compact=True, seed=7 + B, out_splits=(1, 2, 3) if arch else (0, 2, 3))
+
+
+@pytest.mark.parametrize("dist", DISTS)
+def test_dec_self_attention_distributions(dist):
+    """every score distribution through the per-query kernel and the long kernel (several chunks)"""
+    dec_case(0, 2, 4, 20, 2, dist, anc_mode="mixed", seed=11)
+    dec_case(0, 1, 1, 100, 2, dist, seed=12)
+    dec_case(1, 1, 2, 100, 2, dist, anc_mode="random", seed=13, out_splits=(1, 2, 3))
+
+
+@pytest.mark.parametrize("ks", [2, 8])
+def test_dec_self_attention_query_kernel_split_k(ks):
+    dec_case(0, 2, 8, 20, 2, "peak_last", anc_mode="mixed", ks=ks, seed=20 + ks)
+
+
+@pytest.mark.parametrize("i,S,packed", [(i, *c) for i, c in enumerate(ENC)], ids=[f"S{S}_{'packed' if p else 'masked'}" for S, p in ENC])
+@pytest.mark.parametrize("arch", [0, 1])
+def test_enc_self_attention(arch, i, S, packed):
+    Q = 1 if S >= 256 else 3
+    enc_case(arch, Q, S, 2, _dist(i + arch), packed=packed, seed=30 + i)
+
+
+@pytest.mark.parametrize("mask_kind", ["holes", "left", "first_chunk", "first_two_chunks", "last_only"])
+@pytest.mark.parametrize("arch", [0, 1])
+def test_enc_self_attention_masks(arch, mask_kind):
+    enc_case(arch, 2, 100, 2, "late_max", mask_kind=mask_kind, seed=40)
+
+
+@pytest.mark.parametrize("dist", DISTS)
+def test_enc_self_attention_distributions(dist):
+    enc_case(0, 2, 96, 2, dist, seed=41)
+    enc_case(1, 1, 300, 2, dist, packed=True, seed=42, out_splits=(1, 2, 3))
+
+
+@pytest.mark.parametrize("i,S,B", [(i, *c) for i, c in enumerate(CROSS)], ids=[f"S{S}_B{B}" for S, B in CROSS])
+def test_cross_attention(i, S, B):
+    cross_case(2, S, B, 2, _dist(i), packed=bool(i % 2), seed=50 + i)
+
+
+@pytest.mark.parametrize("mask_kind", ["holes", "left", "first_chunk", "first_two_chunks", "last_only"])
+@pytest.mark.parametrize("S", [20, 100])
+def test_cross_attention_masks(S, mask_kind):
+    cross_case(2, S, 4, 2, "peak_first", mask_kind=mask_kind, seed=60)
+
+
+@pytest.mark.parametrize("dist", DISTS)
+def test_cross_attention_distributions(dist):
+    cross_case(2, 28, 5, 16, dist, seed=61)
+    cross_case(2, 100, 5, 2, dist, packed=True, seed=62)
+
+
+@pytest.mark.parametrize("S", [20, 70])
+def test_cross_attention_ragged_groups(S):
+    cross_case(3, S, 0, 2, "rising", ragged=[(0, 1), (2, 17), (1, 33), (2, 0), (0, 5)], seed=70)
+
+
+@pytest.mark.parametrize("ks", [2, 8])
+def test_cross_attention_split_k(ks):
+    cross_case(2, 30, 17, 2, "peak_last", ks=ks, seed=80 + ks)
+    cross_case(3, 12, 1, 2, "onehot", compact=True, ks=ks, seed=81 + ks)
+
+
+def test_every_attention_path_reached():
+    seen = set()
+    seen.add(dec_case(0, 2, 4, 5, 2, "uniform")[1]); seen.add(dec_case(0, 1, 1, 5, 2, "uniform")[1])
+    seen.add(dec_case(0, 1, 1, 20, 2, "uniform")[1]); seen.add(dec_case(0, 1, 1, 40, 2, "uniform")[1])
+    seen.add(dec_case(1, 1, 1, 5, 2, "uniform", out_splits=(1,))[1])
+    seen.add(cross_case(1, 10, 2, 2, "uniform")[1]); seen.add(cross_case(1, 40, 2, 2, "uniform")[1])
+    seen.add(enc_case(1, 1, 10, 2, "uniform", out_splits=(1,))[1])
+    want = {v for k, v in PATH.items() if v}
+    assert want <= seen, sorted(want - seen)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# the exp probe: a bound tight enough to see expf's accuracy
+# ---------------------------------------------------------------------------------------------------------------
+
+def exp_probe(kind, arch, n, B=1, heads=2, seed=90):
+    """Every kernel on inputs where its fp32 arithmetic is exact except expf and the final division.  q = (8 or 1, 0..),
+    k_s = (z_s, 0..) with integer z: z_0 = 0 and z_s in [-80, -50] after it (T5: integer biases in [-3, 3]), so every
+    score, every max and every sc - m is an exact small integer, key 0 holds the maximum from the first chunk on, and
+    every correction is expf(0) = 1 exactly (CUDA's expf(+-0) returns 1).  V is one-hot per output dimension: column
+    j is 1 at key s_j = 1 + j mod (n - 1), 0 elsewhere, so each fma adds p * 1 to 0 or p * 0 to a sum (exact) and
+    o_j = p_{s_j} / l.  The errors left: expf's 2 ulp on p_{s_j} (4u), the division (u), and the sum l = 1 + (terms
+    <= e^-43), where each add errs by at most its smaller operand, i.e. by at most l - 1: relative error
+    <= adds * (l - 1) with adds <= n + 2 n_chunks.  So |o^_j - o_j| <= (5u + (n + 2 n_chunks) (l - 1)) |o_j|.
+    The arguments x = sc - m lie in [-86, -44], where an exp with an error growing with |x| (__expf: the product
+    x * log2(e) rounded to fp32, ~ u |x| relative) misses the bound by far."""
+    rng = np.random.default_rng(seed)
+    bart = arch == 0
+    d = heads * 64
+    z = np.concatenate([[0.0], rng.integers(-80, -49, n - 1)]).astype(np.float32)
+    kv = np.zeros((n, heads, 64), np.float32); kv[:, :, 0] = z[:, None]
+    vv = np.zeros((n, heads, 64), np.float32)
+    for j in range(64):
+        vv[1 + j % (n - 1), :, j] = 1.0
+    qv = np.zeros((heads, 64), np.float32); qv[:, 0] = 8.0 if bart else 1.0
+    nb, md = 32, 128
+    rel = rng.integers(-3, 4, (nb, heads)).astype(np.float32)
+    case = dict(arch=arch, d=d, heads=heads, Q=1, B=B)
+    if not bart:
+        case.update(rel_bias=rel, num_buckets=nb, max_distance=md)
+    if kind == 0:                                         # row r is query r and key r of one source
+        rows = n
+        qkv = np.concatenate([np.broadcast_to(qv, (n, heads, 64)), kv, vv], axis=1).reshape(n, 3 * d).astype(np.float32)
+        case.update(kind=0, S=n, qkv=qkv, src_mask=np.ones((1, n), np.int32))
+        qpos, kpos = np.arange(n), None
+    elif kind == 1:                                       # positions 0 .. n-1; every cache row at s holds key s
+        rows, pos, T = B, n - 1, n + 1
+        kc = np.full((T, B, d), SENTINEL, np.float32); vc = kc.copy()
+        kc[:pos] = np.broadcast_to(kv[:pos].reshape(pos, 1, d), (pos, B, d)); vc[:pos] = np.broadcast_to(vv[:pos].reshape(pos, 1, d), (pos, B, d))
+        qkv = np.broadcast_to(np.concatenate([qv, kv[pos], vv[pos]]).reshape(1, 3 * d), (B, 3 * d)).copy()
+        anc = np.tile(np.arange(B, dtype=np.int32)[:, None], (1, T))
+        case.update(kind=1, pos=pos, T=T, qkv=qkv, kc=kc, vc=vc, anc=anc)
+        qpos = np.full(B, pos)
+    else:
+        rows = B
+        case.update(kind=2, S=n, q=np.broadcast_to(qv.reshape(1, d), (B, d)).copy(),
+                    ckv=np.concatenate([kv.reshape(n, d), vv.reshape(n, d)], axis=1), src_mask=np.ones((1, n), np.int32))
+        qpos = None
+    bias = None
+    if not bart:
+        bk = bucket_table(np.arange(n)[None, :] - qpos[:, None], kind == 0, nb, md)
+        bias = rel[bk].transpose(0, 2, 1).astype(np.float64)
+    ref, _ = attend_ref(np.broadcast_to(qv, (rows, heads, 64)), kv[None], vv[None], np.ones((1, n), bool), bias,
+                        0.125 if bart else 1.0)
+    sc = (z[None, None, :].astype(np.float64) + (bias if bias is not None else 0.0))
+    l = np.exp(sc - sc.max(-1, keepdims=True)).sum(-1, keepdims=True)              # [rows][H][1]
+    assert (sc.argmax(-1) == 0).all()
+    nch = (n + 31) // 32
+    bound = (5 * U + (n + 2 * nch) * (l - 1)) * np.abs(ref)
+    out_split = 0 if bart else 1
+    out, sp, ovf, _, _, path = run_attention(case, rows, out_split, kc_shape=case["kc"].shape if kind == 1 else None)
+    got = value_of(out, sp, ovf, out_split, bart)
+    ratio = (np.abs(got.astype(np.float64) - ref.reshape(rows, -1)) / bound.reshape(rows, -1)).max()
+    print(f"exp probe kind={kind} arch={arch} n={n} B={B} path={path:#x}: worst err/bound {ratio:.3g}")
+    assert ratio <= 1.0, ratio
+    return path
+
+
+PROBES = [(1, 0, 12, 1, "self_rounds3"), (1, 0, 20, 1, "self_rounds8"), (1, 0, 40, 1, "self_long"), (1, 0, 20, 4, "self_query"),
+          (1, 1, 40, 2, "t5_dec"), (0, 0, 60, 1, "enc"), (0, 1, 60, 1, "t5_enc"), (2, 0, 30, 5, "cross_small"),
+          (2, 0, 60, 5, "cross_grouped")]
+
+
+@pytest.mark.parametrize("kind,arch,n,B,kernel", PROBES, ids=[p[-1] for p in PROBES])
+def test_exp_accuracy_probe(kind, arch, n, B, kernel):
+    assert exp_probe(kind, arch, n, B) == PATH[kernel]
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# model level: the forward-vs-float64 checks with trained-like attention
+# ---------------------------------------------------------------------------------------------------------------
+# Random init leaves every softmax close to uniform.  Multiplying the query projections by 2^4 (weight and bias; T5:
+# q by 2^4 and relative_attention_bias by 2^3) is exact in fp32 and bf16 and scales every score by 16 (T5's biases by
+# 8), so the same models attend the way trained ones do.  The float64 reference is the scaled fp32 model cast to
+# double; the criteria are those of each model family's forward test, run through that test's own runner.
+PEAK_Q, PEAK_BIAS = 16.0, 8.0
+_PEAKED = {}
+
+
+def peak_attention(model):
+    import torch
+    from transformers.models.t5.modeling_t5 import T5Attention
+    with torch.no_grad():
+        for mod in model.modules():
+            if isinstance(mod, T5Attention):
+                mod.q.weight.mul_(PEAK_Q)
+                if mod.has_relative_attention_bias:
+                    mod.relative_attention_bias.weight.mul_(PEAK_BIAS)
+            elif hasattr(mod, "q_proj"):
+                mod.q_proj.weight.mul_(PEAK_Q)
+                mod.q_proj.bias.mul_(PEAK_Q)
+    return model
+
+
+def peaked(family):
+    """register the scaled model of `family` in its forward test's model cache; returns (test module, cache key)"""
+    import copy
+    import torch
+    from seal_b200.beam_search import SealBartEngine
+    key = family + "_peaked"
+    if family == "bart":
+        import test_bart_paths_gpu as mod
+        if key not in _PEAKED:
+            from oracle.decode_oracle import make_bart
+            m32 = peak_attention(make_bart(seed=0, **mod.MODEL_KW["tiny"]))
+            eng = SealBartEngine(m32.state_dict(), m32.config, device=0, gemm_mode=3)
+            _PEAKED[key] = (copy.deepcopy(m32).double().cuda().eval(), m32.cuda().eval(), eng)
+        return mod, _PEAKED[key]
+    if family == "t5":
+        import test_t5_gpu as mod
+        from t5_models import make_t5
+        build = lambda: peak_attention(make_t5("tiny"))
+    elif family == "preln":
+        import test_preln_gpu as mod
+        from preln_models import make_preln
+        build = lambda: peak_attention(make_preln("pegasus_relu"))
+    else:                                                   # gemm_mode 6: bf16 weights
+        import test_bf16_gpu as mod
+        build = lambda: peak_attention(mod.make_model("bart128")).to(torch.bfloat16)
+    if key not in _PEAKED:
+        cpu = build()
+        eng = SealBartEngine.from_hf(cpu, device=0) if family == "bf16" else SealBartEngine.from_hf(cpu, device=0, gemm_mode=3)
+        up = (lambda m: m.float()) if family == "bf16" else (lambda m: m)
+        _PEAKED[key] = (copy.deepcopy(cpu).double().cuda().eval(), up(copy.deepcopy(cpu)).cuda().eval(), cpu, eng)
+    mod._MODELS[key] = _PEAKED[key]
+    return mod, key
+
+
+def bart_peaked_case(name, Q, S, B, t, kind="right", src_tokens=-1, share=False):
+    bp, (m64, m32, eng) = peaked("bart")
+    V = int(eng.config.vocab_size)
+    rng = np.random.default_rng(sum(map(ord, name)))
+    ids, am = bp.src_inputs(rng, Q, S, V, kind)
+    dec, anc = bp.beam_inputs(rng, Q, B, t, V, share and B > 1 and t > 1)
+    got = eng.debug_step_logits(ids, am, B, dec, anc=anc, src_tokens=src_tokens)
+    assert bp.paths(eng) & bp.ATTN_BITS == bp.expected_attn_bits(Q, S, B, t, am, src_tokens)
+    bp.check_bounds("tiny", f"peaked bart {name}", got, bp.hf_logits(m64, ids, am, B, dec), bp.hf_logits(m32, ids, am, B, dec))
+
+
+BART_PEAKED = [("P2", 2, 12, 1, 2, {}), ("P13", 2, 12, 1, 13, {}), ("P40", 2, 12, 1, 40, {}),
+               ("query_B4_P6", 2, 12, 4, 6, dict(share=True)), ("packed_S40", 3, 40, 3, 4, dict(share=True)),
+               ("unpacked_S40", 3, 40, 3, 4, dict(src_tokens=-2, share=True))]
+
+
+@pytest.mark.parametrize("name,Q,S,B,t,kw", BART_PEAKED, ids=[c[0] for c in BART_PEAKED])
+def test_peaked_bart_forward_vs_float64(name, Q, S, B, t, kw):
+    bart_peaked_case(name, Q, S, B, t, **kw)
+
+
+@pytest.mark.parametrize("family,name,Q,S,B,P,kw", [
+    ("t5", "t5_S40", 3, 40, 3, 5, dict(share=True)),
+    ("t5", "t5_P40", 2, 12, 2, 40, dict(share=True)),
+    ("preln", "pegasus_S40", 3, 40, 3, 4, dict(share=True)),
+    ("bf16", "bf16_bart", 3, 40, 3, 4, dict(share=True)),
+], ids=["t5_S40", "t5_P40", "pegasus_S40", "bf16_bart"])
+def test_peaked_forward_vs_float64(family, name, Q, S, B, P, kw):
+    mod, key = peaked(family)
+    if family != "t5":
+        mod.test_forward_vs_float64("peaked_" + name, key, Q, S, B, P, kw)
+        return
+    # T5 with its scores scaled by 16 and its biases by 8 is conditioned so that fp32 HF itself misses test_t5_gpu's
+    # absolute log-prob bound (1e-4; it errs by up to 3e-4 here): the absolute bound would measure the model, not the
+    # kernels.  The criteria kept: the finiteness pattern and the calibration against fp32 HF, on logits and log-probs.
+    m64, m32, cpu, eng = mod.get_model(key)
+    V = int(eng.config.vocab_size)
+    rng = np.random.default_rng(sum(map(ord, "peaked_" + name)))
+    ids, am = mod.t5_sources(rng, Q, S, V, "right")
+    dec, anc = mod.beam_inputs(rng, Q, B, P, V, kw.get("share", False) and B > 1 and P > 1)
+    got = eng.debug_step_logits(ids, am, B, dec, anc=anc, src_tokens=-1)
+    assert mod.paths(eng) & mod.SHAPE_BITS == mod.expected_bits(key, S, am, -1)
+    ref64, ref32 = mod.hf_logits(m64, ids, am, B, dec), mod.hf_logits(m32, ids, am, B, dec)
+    fin = np.isfinite(ref64)
+    assert np.array_equal(np.isfinite(got), fin), "finiteness pattern differs from float64"
+    lg, l64, l32 = mod.log_softmax(got), mod.log_softmax(ref64), mod.log_softmax(ref32)
+    e, h = np.abs(got[fin] - ref64[fin]).max(), np.abs(ref32[fin] - ref64[fin]).max()
+    el, hl = np.abs(lg[fin] - l64[fin]).max(), np.abs(l32[fin] - l64[fin]).max()
+    print(f"peaked t5 {name}: ours |dlogit| {e:.2e} |dlogprob| {el:.2e}   fp32 HF |dlogit| {h:.2e} |dlogprob| {hl:.2e}")
+    assert e <= mod.CAL_C * h + mod.CAL_FLOOR, (name, e, h)
+    assert el <= mod.CAL_C * hl + mod.CAL_FLOOR, (name, el, hl)
