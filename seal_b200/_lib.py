@@ -183,6 +183,18 @@ _DEC_SIGS = {
                                 C.c_double, C.c_double, vp, vp, vp, vp, vp, vp, C.c_int64]),
     "sealev_last_error": (C.c_char_p, []),
     "sealev_set_sum_mode": (None, [i32]),
+    # include/sealev_batch.h
+    "sealev_key_scores": (i32, [C.c_int64, vp, vp, vp, vp, C.c_double, C.c_double, C.c_double, C.c_double, i32, vp]),
+    "sealev_unigram_topk": (i32, [C.c_int64, C.c_int64, vp, C.c_int64, vp, vp, vp, vp]),
+    "sealev_unigram_scores": (i32, [C.c_int64, vp, vp, vp, C.c_double, C.c_double, C.c_double, i32, vp]),
+    "sealev_best_unigrams": (i32, [C.c_int64, vp, vp, vp, vp, vp, vp, vp, vp, C.c_int64]),
+    "sealev_set_device_budget": (None, [u64]),
+    "sealev_batch_first_stage": (i32, [vp, C.c_int64, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, C.c_double, C.c_double,
+                                       C.c_int64, vp, vp, C.c_int64]),
+    "sealev_batch_score_docs": (i32, [vp, C.c_int64, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_int64, i32, i32,
+                                      i32, i32, C.c_double, C.c_double, vp, vp, C.c_int64, vp, vp, vp, vp, vp, vp,
+                                      C.c_int64, vp]),
+    "sealev_batch_phase_us": (None, [vp]),
     "sealdec_last_launch_count": (C.c_int64, [vp]),
     "sealdec_profile_gemm": (i32, [vp, i32, C.POINTER(C.c_double), C.POINTER(C.c_int64), C.POINTER(C.c_double)]),
     "sealdec_last_phase_us": (i32, [vp, C.POINTER(C.c_double)]),

@@ -49,6 +49,12 @@ bool g_compensated_sum = true;      // how the host interpreter's built-in sum()
 
 }  // namespace
 
+namespace sealb200 {
+// the message sealev_last_error() returns, for the batched entry points (include/sealev_batch.h)
+void sealev_set_error(const std::string& msg) { g_err = msg; }
+bool sealev_compensated_sum() { return g_compensated_sum; }
+}  // namespace sealb200
+
 extern "C" {
 
 const char* sealev_last_error(void) { return g_err.c_str(); }

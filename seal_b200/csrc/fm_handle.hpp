@@ -5,8 +5,14 @@
 
 #include <cuda_runtime.h>
 
+#include <vector>
+
 namespace sealb200 {
 FmView sealfm_view(const sealfm_t* h);   // defined in fm_kernels.cu; throws ApiError if not on a device
+// the handle's stream (created on first use); makes the handle's device current.  Throws ApiError if not on a device.
+cudaStream_t sealfm_stream(const sealfm_t* h);
+// document start offsets given to sealfm_set_beginnings (empty before)
+const std::vector<uint64_t>& sealfm_beginnings(const sealfm_t* h);
 // allowed-token bitmask rows of R SA ranges (fm_kernels.cu); `wide` = expand_scratch_bytes(L, R) of device scratch
 size_t expand_scratch_bytes(uint32_t L, uint64_t R);
 void launch_expand_masks(const FmView& v, cudaStream_t s, uint64_t R, const uint64_t* lo_d, const uint64_t* hi_d, uint32_t* mask_d,

@@ -453,6 +453,18 @@ FmView sealfm_view(const sealfm_t* h) {
     if (h->device < 0) throw ApiError(SEALFM_ENODEVICE, "index not bound to a CUDA device (call sealfm_to_device)");
     return h->view;
 }
+
+cudaStream_t sealfm_stream(const sealfm_t* h) {
+    require_device(h);
+    std::lock_guard<std::mutex> lk(h->stage_mu);
+    if (!h->stage_stream) CUDA_CHECK(cudaStreamCreateWithFlags(&h->stage_stream, cudaStreamNonBlocking));
+    return h->stage_stream;
+}
+
+const std::vector<uint64_t>& sealfm_beginnings(const sealfm_t* h) {
+    if (!h) throw ApiError(SEALFM_EINVAL, "null handle");
+    return h->beginnings;
+}
 }  // namespace sealb200
 
 // ------------------------------------------------------------------------------------------------

@@ -353,3 +353,307 @@ def _scan_keys(toks, root):
                     hits.setdefault(end[0], [end[1], []])[1].append((a, i + 1))
         live = keep
     return hits
+
+
+# ------------------------------------------------------------------------------------------------
+# Batched evidence aggregation: aggregate_evidence for a whole batch of queries (include/sealev_batch.h).
+#
+# The scalar scoring of every key and unigram of the batch runs in native host code (sealev_key_scores,
+# sealev_unigram_topk / _scores, sealev_best_unigrams), every distinct SA range of the batch is computed in one
+# backward_search_multi launch, and the two per-query loops -- the first stage and the full scoring of the
+# shortlisted documents -- run as CUDA kernels over all queries at once.  What stays in Python per query is the dict
+# bookkeeping that defines the orders (rare / frequent split, stable sorts by score) and building the result dicts.
+# ------------------------------------------------------------------------------------------------
+import inspect as _inspect
+import time as _time
+
+_AGG_DEFAULTS = {n: q.default for n, q in _inspect.signature(aggregate_evidence).parameters.items()
+                 if n not in ("ngrams_and_scores", "unigram_scores", "index")}
+
+_PY_ERRORS = {"math domain error": ValueError, "math range error": OverflowError,
+              "0.0 cannot be raised to a negative power": ZeroDivisionError}
+
+
+def _evcheck_py(code):
+    """Native scalar scoring: the exception Python's own arithmetic raises, else SealB200Error."""
+    if code != 0:
+        msg = lib.sealev_last_error().decode(errors="replace")
+        if msg in _PY_ERRORS:
+            raise _PY_ERRORS[msg](msg)
+        _evcheck(code)
+
+
+def _i64(x):
+    return np.ascontiguousarray(x, dtype=np.int64) if len(x) else np.zeros(1, dtype=np.int64)
+
+
+def _f64(x):
+    return np.ascontiguousarray(x, dtype=np.float64) if len(x) else np.zeros(1)
+
+
+def batch_aggregate_evidence(list_of_ngrams_and_scores, list_of_unigram_scores=None, index=None, **kw):
+    """aggregate_evidence for a batch of queries: a list of (results, all_ngrams), element q equal (same document
+    order, key order, dict order and floats) to aggregate_evidence(list_of_ngrams_and_scores[q],
+    list_of_unigram_scores[q], index, **kw).  `kw` takes aggregate_evidence's keywords, with its defaults.  Key
+    scores are read with float()."""
+    bad = sorted(set(kw) - set(_AGG_DEFAULTS))
+    if bad:
+        raise TypeError(f"batch_aggregate_evidence() got an unexpected keyword argument {bad[0]!r}")
+    return _batch_evidence(list(list_of_ngrams_and_scores), list_of_unigram_scores, index, {**_AGG_DEFAULTS, **kw})
+
+
+def _batch_evidence(queries, unis, index, p, phases=None):
+    t0 = _time.perf_counter()
+    held = []                              # arrays whose addresses are passed to the native calls below
+
+    def ptr(a):
+        held.append(a)
+        return a.ctypes.data
+
+    Q = len(queries)
+    if Q == 0:
+        return []
+    unis = [None] * Q if unis is None else list(unis)
+    if len(unis) != Q:
+        raise ValueError("list_of_unigram_scores must have one entry per query")
+    from .index import SHIFT
+    fmfreq = bool(p["use_fm_index_frequency"])
+    ntokens = float(index.beginnings[-1])
+    keys = [[((k.tolist() if hasattr(k, "tolist") else list(k)), float(s)) for k, s in q] for q in queries]
+    cutoff = [0.0] * Q
+    if not fmfreq:                                                                          # :198-205
+        cutoff = [min(ks, key=lambda ks: ks[1])[1] - 0.1 if ks else [][0] for ks in keys]
+
+    # -- unigram candidates: the first use_top_k_unigrams of the stable argsort, minus the given tokens ----------
+    top_k = p["use_top_k_unigrams"]
+    kept = [None] * Q                     # int64 arrays of kept tokens
+    V = [-1] * Q
+    uarr = [None] * Q                     # float64 unigram scores
+    out_n = np.zeros(1, dtype=np.int64)
+    for q, us in enumerate(unis):
+        if us is None:
+            continue
+        a = uarr[q] = np.ascontiguousarray(us, dtype=np.float64)
+        v = V[q] = len(a)
+        g = np.fromiter({0, 1, 2} | {k[0] for k, _ in keys[q] if len(k) == 1}, dtype=np.int64)   # :207-211
+        goff = np.array([0, len(g)], dtype=np.int64)
+        kk = v if top_k is None else (min(top_k, v) if top_k >= 0 else max(v + top_k, 0))
+        out = np.zeros(max(kk, 1), dtype=np.int64)
+        _evcheck_py(lib.sealev_unigram_topk(1, v, a.ctypes.data if v else None, v if top_k is None else int(top_k),
+                                            goff.ctypes.data, ptr(_i64(g)), out.ctypes.data, out_n.ctypes.data))
+        kept[q] = out[:out_n[0]]
+
+    # -- every distinct SA range of the batch in one launch: multi-token keys by tuple, single tokens by value ------
+    multi = {}
+    singles = []
+    for ks in keys:
+        for k, _ in ks:
+            if len(k) == 1:
+                singles.append(k[0])
+            else:
+                multi.setdefault(tuple(k), len(multi))
+    uniq = np.unique(np.concatenate([np.asarray(singles, dtype=np.int64)] + [a for a in kept if a is not None]))
+    seqs_multi = list(multi)
+    lens = np.concatenate([np.fromiter((len(s) for s in seqs_multi), dtype=np.int64, count=len(seqs_multi)),
+                           np.ones(len(uniq), dtype=np.int64)])
+    nseq = len(lens)
+    t1 = _time.perf_counter()
+    lo_m = hi_m = lo_u = hi_u = np.zeros(0, dtype=np.int64)
+    if nseq:
+        offs = np.zeros(nseq + 1, dtype=np.uint64); np.cumsum(lens, out=offs[1:])
+        flat = np.concatenate([np.fromiter((t + SHIFT for s in seqs_multi for t in s), dtype=np.int64,
+                                           count=int(lens[:len(seqs_multi)].sum())), uniq + SHIFT]).astype(np.uint64)
+        if len(flat) == 0:
+            flat = np.zeros(1, dtype=np.uint64)
+        lo = np.zeros(nseq, dtype=np.uint64); hi = np.zeros(nseq, dtype=np.uint64)
+        check(lib.sealfm_backward_search_multi(index._dev(), nseq, flat.ctypes.data, offs.ctypes.data,
+                                               lo.ctypes.data, hi.ctypes.data))
+        lo = lo.astype(np.int64); hi = hi.astype(np.int64)
+        lo_m, hi_m, lo_u, hi_u = lo[:len(multi)], hi[:len(multi)], lo[len(multi):], hi[len(multi):]
+    t2 = _time.perf_counter()
+    lo_m, hi_m = lo_m.tolist(), hi_m.tolist()
+
+    def ranges_of(ks):                     # (lo, hi) of each key of a list
+        sing = np.asarray([k[0] for k, _ in ks if len(k) == 1], dtype=np.int64)
+        at = np.searchsorted(uniq, sing)
+        sl, sh = lo_u[at].tolist(), hi_u[at].tolist()
+        out, i = [], 0
+        for k, _ in ks:
+            if len(k) == 1:
+                out.append((sl[i], sh[i])); i += 1
+            else:
+                j = multi[tuple(k)]; out.append((lo_m[j], hi_m[j]))
+        return out
+
+    # -- scalar scoring of every key of the batch ----------------------------------------------------------------
+    rng = [ranges_of(ks) for ks in keys]
+    flat_keys = [(q, k, s, r) for q, ks in enumerate(keys) for (k, s), r in zip(ks, rng[q])]
+    n = len(flat_keys)
+    sr = _f64([s for _, _, s, _ in flat_keys]); cnt = _i64([r[1] - r[0] for _, _, _, r in flat_keys])
+    kl = _i64([len(k) for _, k, _, _ in flat_keys]); co = _f64([cutoff[q] for q, _, _, _ in flat_keys])
+    ksc = np.zeros(max(n, 1))
+    _evcheck_py(lib.sealev_key_scores(n, sr.ctypes.data, cnt.ctypes.data, kl.ctypes.data, co.ctypes.data, ntokens,
+                                      float(p["alpha"]), float(p["length_penalty"]), float(p["smoothing"]), int(fmfreq),
+                                      ksc.ctypes.data))
+    ksc = ksc[:n].tolist()
+    # unigram tables (nonzero entries) and the add_best_unigrams_to_ngrams extras
+    uq = [q for q in range(Q) if kept[q] is not None]
+    tab = [None] * Q
+    extras = [[] for _ in range(Q)]
+    if uq:
+        ut = np.concatenate([kept[q] for q in uq]) if uq else np.zeros(0, dtype=np.int64)
+        at = np.searchsorted(uniq, ut)
+        uc = _i64(hi_u[at] - lo_u[at]) if len(ut) else _i64([])
+        us = _f64(np.concatenate([uarr[q][kept[q]] for q in uq]))
+        uco = _f64(np.concatenate([np.full(len(kept[q]), cutoff[q]) for q in uq]))
+        uv = np.zeros(max(len(ut), 1))
+        _evcheck_py(lib.sealev_unigram_scores(len(ut), us.ctypes.data, uc.ctypes.data, uco.ctypes.data, ntokens,
+                                              float(p["alpha"]), float(p["smoothing"]), int(fmfreq), uv.ctypes.data))
+        uv = uv[:len(ut)]
+        o = 0
+        toff = [0]
+        for q in uq:
+            m = len(kept[q]); t, v = kept[q], uv[o:o + m]; o += m
+            nz = v != 0.0
+            tab[q] = (t[nz], v[nz])
+            toff.append(toff[-1] + int(nz.sum()))
+        if p["add_best_unigrams_to_ngrams"]:                                                # :274-278
+            tt = _i64(np.concatenate([tab[q][0] for q in uq])); tv = _f64(np.concatenate([tab[q][1] for q in uq]))
+            nx = _i64([len(keys[q]) for q in uq]); vv = _i64([V[q] for q in uq])
+            cap = int(sum(min(len(keys[q]), V[q]) for q in uq))
+            xo = np.zeros(len(uq) + 1, dtype=np.int64); xt = np.zeros(max(cap, 1), dtype=np.int64); xv = np.zeros(max(cap, 1))
+            _evcheck_py(lib.sealev_best_unigrams(len(uq), vv.ctypes.data, ptr(_i64(toff)), tt.ctypes.data,
+                                                 tv.ctypes.data, nx.ctypes.data, xo.ctypes.data, xt.ctypes.data,
+                                                 xv.ctypes.data, cap))
+            xt, xv, xo = xt.tolist(), xv.tolist(), xo.tolist()
+            for i, q in enumerate(uq):
+                extras[q] = list(zip(xt[xo[i]:xo[i + 1]], xv[xo[i]:xo[i + 1]]))
+
+    # -- per query: rare / frequent split and all_ngrams, in the reference's dict and sort orders (:280-314) ------
+    mo1, mo2 = p["max_occurrences_1"], p["max_occurrences_2"]
+    by_score = lambda kv: kv[1]
+    uni_at = {}                            # token -> (lo, hi) of the tokens extras can add with a nonzero score
+    fs_tok, fs_off, fs_score, fs_count, fs_lo, fs_rows, fs_q = [], [0], [], [], [], [], [0]
+    sc_tok, sc_off, sc_score, sc_count, sc_q = [], [0], [], [], [0]
+    all_ng, scored_q, empty_count = [], [], []
+    i_key = 0
+    for q in range(Q):
+        ks = keys[q]
+        scores = ksc[i_key:i_key + len(ks)]; i_key += len(ks)
+        rq = rng[q]
+        items = [(tuple(k), sc, r) for (k, _), sc, r in zip(ks, scores, rq)]
+        if extras[q]:
+            ex = [t for t, v in extras[q] if v != 0.0]
+            if ex:
+                at = np.searchsorted(uniq, np.asarray(ex, dtype=np.int64))
+                for t, l, h in zip(ex, lo_u[at].tolist(), hi_u[at].tolist()):
+                    uni_at[t] = (l, h)
+            items += [((t,), v, uni_at.get(t) if v != 0.0 else None) for t, v in extras[q]]
+        counts = {(): len(index)}
+        for k, _, r in items:
+            if r is not None:
+                counts[k] = r[1] - r[0]
+        rare, freq, rr = {}, {}, {}
+        for k, sc, r in items:
+            if sc == 0.0:
+                continue
+            c = r[1] - r[0]
+            if c > mo2:
+                continue
+            (freq if (c > mo1 or sc < 0.0) else rare)[k] = sc
+            rr[k] = r
+        rare = dict(sorted(rare.items(), key=by_score, reverse=True))
+        freq = dict(sorted(freq.items(), key=by_score, reverse=True))
+        all_ngrams = dict(sorted(list(rare.items()) + list(freq.items()), key=by_score, reverse=True))
+        all_ng.append(all_ngrams)
+        empty_count.append(int(counts[()]))
+        for k, sc in rare.items():
+            l, h = rr[k]
+            fs_tok.extend(k); fs_off.append(len(fs_tok)); fs_score.append(sc); fs_count.append(counts[k])
+            fs_lo.append(l); fs_rows.append(max(0, min(h, l + mo1) - l))
+        fs_q.append(len(fs_score))
+        scored = [(k, v) for k, v in all_ngrams.items() if len(k) >= 1 and v > 0.0]        # trie contents, :378-385
+        scored_q.append(scored)
+        for k, v in scored:
+            sc_tok.extend(k); sc_off.append(len(sc_tok)); sc_score.append(v); sc_count.append(counts[k])
+        sc_q.append(len(sc_score))
+    t3 = _time.perf_counter()
+
+    # -- GPU first stage ---------------------------------------------------------------------------------------
+    h = index._dev()
+    sort_mode = 1 if p["sort_by_length"] else (2 if p["sort_by_freq"] else 0)
+    ec = _i64(empty_count)
+    nd_max = int(p["n_docs_complete_score"])
+    rows_q = [sum(fs_rows[fs_q[q]:fs_q[q + 1]]) for q in range(Q)]
+    cap = sum(min(max(nd_max, 0), r) for r in rows_q)
+    so = np.zeros(Q + 1, dtype=np.int64); sd = np.zeros(max(cap, 1), dtype=np.int64)
+    _evcheck(lib.sealev_batch_first_stage(h, Q, ptr(_i64(fs_q)), ptr(_i64(fs_tok)), ptr(_i64(fs_off)),
+                                          ptr(_f64(fs_score)), ptr(_i64(fs_count)),
+                                          ptr(np.ascontiguousarray(_i64(fs_lo), dtype=np.uint64)),
+                                          ptr(_i64(fs_rows)), ec.ctypes.data, sort_mode, int(bool(p["allow_overlaps"])),
+                                          float(p["beta"]), float(p["single_key"]), nd_max, so.ctypes.data, sd.ctypes.data, cap))
+    fs_us = np.zeros(4)
+    lib.sealev_batch_phase_us(fs_us.ctypes.data)
+    t4 = _time.perf_counter()
+
+    # -- GPU scoring of the shortlisted documents -----------------------------------------------------------------
+    so_l = so.tolist()
+    docs = sd[:so_l[-1]]
+    b = np.asarray(index.beginnings, dtype=np.int64)
+    dl = np.maximum(b[docs + 1] - b[docs], 1) if len(docs) else np.zeros(0, dtype=np.int64)
+    tok_cap = int(dl.sum())
+    uo, ut, uv = [0], [], []
+    for q in range(Q):
+        if tab[q] is not None:
+            ut.append(tab[q][0]); uv.append(tab[q][1]); uo.append(uo[-1] + len(tab[q][0]))
+        else:
+            uo.append(uo[-1])
+    ut = _i64(np.concatenate(ut) if ut else []); uv = _f64(np.concatenate(uv) if uv else [])
+    nd = len(docs)
+    dto = np.zeros(nd + 1, dtype=np.int64); dtok = np.zeros(max(tok_cap, 1), dtype=np.int64)
+    out_score = np.zeros(max(nd, 1)); out_best = np.zeros(max(nd, 1), dtype=np.int64); out_bs = np.zeros(max(nd, 1))
+    po = np.zeros(nd + 1, dtype=np.int64)
+    need = C.c_int64(0)
+    pcap = tok_cap * 2 + 16
+    lib.sealev_set_sum_mode(1 if sys.version_info >= (3, 12) else 0)     # how this interpreter's sum() adds floats (:476)
+    args_head = (h, Q, ptr(_i64(sc_q)), ptr(_i64(sc_tok)), ptr(_i64(sc_off)), ptr(_f64(sc_score)),
+                 ptr(_i64(sc_count)), ec.ctypes.data, so.ctypes.data, ptr(_i64(docs)), ptr(_i64(uo)),
+                 ut.ctypes.data, uv.ctypes.data, ptr(_i64(V)), SHIFT, sort_mode, int(bool(p["allow_overlaps"])),
+                 int(bool(p["unigrams_ignore_free_places"])), int(bool(p["single_key_add_unigrams"])), float(p["beta"]),
+                 float(p["single_key"]), dto.ctypes.data, dtok.ctypes.data, tok_cap, out_score.ctypes.data,
+                 out_best.ctypes.data, out_bs.ctypes.data, po.ctypes.data)
+    while True:
+        pk = np.zeros(max(pcap, 1), dtype=np.int64); ps = np.zeros(max(pcap, 1))
+        rc = lib.sealev_batch_score_docs(*args_head, pk.ctypes.data, ps.ctypes.data, pcap, C.byref(need))
+        if rc == -6 and need.value > pcap:               # SEALFM_ECAPACITY: the exact count is known now
+            pcap = need.value
+            continue
+        _evcheck(rc)
+        break
+    sc_us = np.zeros(4)
+    lib.sealev_batch_phase_us(sc_us.ctypes.data)
+    t5 = _time.perf_counter()
+
+    # -- result dicts, as aggregate_evidence builds them ---------------------------------------------------------
+    flat_tok = dtok[:int(dto[-1])].tolist(); dto = dto.tolist()
+    n_pk = int(po[-1])
+    pk, ps, po = pk[:n_pk].tolist(), ps[:n_pk].tolist(), po.tolist()
+    osc, ob, obs = out_score.tolist(), out_best.tolist(), out_bs.tolist()
+    docs = docs.tolist()
+    out = []
+    for q in range(Q):
+        scored = scored_q[q]
+        results = {}
+        for i in range(so_l[q], so_l[q + 1]):
+            picked = [((scored[k][0] if k >= 0 else (-1 - k,)), s) for k, s in zip(pk[po[i]:po[i + 1]], ps[po[i]:po[i + 1]])]
+            bk = ob[i]
+            best = [scored[bk][0], obs[i]] if bk >= 0 else [[], 0.0]
+            results[docs[i]] = [osc[i], picked, None, flat_tok[dto[i]:dto[i + 1]], best]
+        out.append((dict(sorted(results.items(), key=lambda kv: -kv[1][0])), all_ng[q]))   # :496-497
+    t6 = _time.perf_counter()
+    if phases is not None:
+        for name, v in (("host_prep", (t1 - t0) + (t3 - t2)), ("ranges", t2 - t1), ("locate", fs_us[0] * 1e-6),
+                        ("first_stage", fs_us[1] * 1e-6), ("extract", sc_us[2] * 1e-6), ("score", sc_us[3] * 1e-6),
+                        ("python_assembly", (t4 - t3 - (fs_us[0] + fs_us[1]) * 1e-6) + (t5 - t4 - (sc_us[2] + sc_us[3]) * 1e-6) + (t6 - t5))):
+            phases[name] = phases.get(name, 0.0) + v
+    return out
