@@ -466,6 +466,11 @@ int sealdec_debug_topk_rows(int64_t R, int32_t V, int32_t num_beams, int32_t per
  * 3 last MMA issued, 4 last chunk complete, 5 tile stored, 6 exit; 7/8 globaltimer ns at entry / exit --
  * 9..16 the epilogue's four store passes (staged / stored) -- then tracing is switched on (enable != 0) or off. */
 int sealdec_debug_gemm_trace(int enable, int64_t out20[20]);
+/* per-unit timeline of CTA 0 of the last launches traced by sealdec_debug_gemm_trace (development aid): out[4i + e] for
+ * the CTA's i-th work unit (i < 256) = SM cycles at e = 0 its first k-block of MMAs committed, 1 its K loop done,
+ * 2 epilogue start, 3 epilogue end (0 where nothing was stamped).  Copies the first n <= 1 024 entries, then clears
+ * the record.  Only in a library built with GEMM_UNIT_TRACE=1 (seal_b200/csrc/Makefile); otherwise SEALFM_EINVAL. */
+int sealdec_debug_gemm_units(int64_t* out, int32_t n);
 /* kernel launches issued by the last sealdec_generate* call on this model (own kernels only) */
 int64_t sealdec_last_launch_count(const sealbart_t* model);
 /* GEMM profiling: enable != 0 makes every following GEMM launch of this model be bracketed by CUDA

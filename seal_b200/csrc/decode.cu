@@ -2056,6 +2056,21 @@ int sealdec_debug_gemm_trace(int enable, int64_t out20[20]) {
     });
 }
 
+int sealdec_debug_gemm_units(int64_t* out, int32_t n) {
+    return guarded([&] {
+        if (!out || n < 0 || n > 4 * kTraceUnits) throw ApiError(SEALFM_EINVAL, "out is null or n is outside [0, 4 * 256]");
+#ifndef SEAL_GEMM_UNIT_TRACE
+        throw ApiError(SEALFM_EINVAL, "built without the per-unit GEMM timeline (make GEMM_UNIT_TRACE=1)");
+#endif
+        CUDA_CHECK(cudaDeviceSynchronize());
+        std::vector<long long> h(4 * kTraceUnits);
+        CUDA_CHECK(cudaMemcpyFromSymbol(h.data(), g_gemm_units, h.size() * sizeof(long long)));
+        for (int i = 0; i < n; ++i) out[i] = h[i];
+        std::fill(h.begin(), h.end(), 0ll);
+        CUDA_CHECK(cudaMemcpyToSymbol(g_gemm_units, h.data(), h.size() * sizeof(long long)));
+    });
+}
+
 int64_t sealdec_last_launch_count(const sealbart_t* m) { return m ? m->launches : 0; }
 
 int sealdec_profile_gemm(sealbart_t* m, int enable, double* total_us, int64_t* launches, double* flops) {

@@ -229,10 +229,25 @@ __device__ __forceinline__ void gemm_trace(int i) {
         if (i == 0 || i == 6) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); g_gemm_trace[i == 0 ? 7 : 8] = (long long)t; }
     }
 }
+// Per-unit timeline of CTA 0 (consumer warpgroup 1, thread 0) under the same switch (debug ABI
+// sealdec_debug_gemm_units), compiled in only with -DSEAL_GEMM_UNIT_TRACE (make GEMM_UNIT_TRACE=1): the stamps cost the
+// lm_head 5 % even with tracing off (H100 SXM, 700 W), so the default build leaves them out: for its i-th work unit, i < kTraceUnits, SM cycles at 4i + 0 the unit's first k-block of
+// MMAs committed, 1 its K loop done (last chunk promoted), 2 epilogue start, 3 epilogue end.  From these,
+// tools/gemm_epilogue_probe.py reports the epilogue's share of the CTA's time and the tensor-idle gap between a unit's
+// last and the next unit's first MMAs.
+constexpr int kTraceUnits = 256;
+__device__ long long g_gemm_units[4 * kTraceUnits];
+__device__ __forceinline__ void unit_trace(bool on, int unit, int e) {
+#ifdef SEAL_GEMM_UNIT_TRACE
+    if (on && unit < kTraceUnits) g_gemm_units[4 * unit + e] = clock64();
+#endif
+}
 
 // Epilogue store of two adjacent columns (n, n + 1) of one row: fp32 and/or the operand split of the next GEMM.
+// kFull: the caller knows both columns are below N (a tile inside the matrix), so neither is checked.
+template <bool kFull>
 __device__ __forceinline__ void store_pair(float* C, __half* S1, __half* S2, int64_t off, int n, int N, float v0, float v1, int& ov) {
-    if (n + 1 < N) {
+    if (kFull || n + 1 < N) {
         if (C) *reinterpret_cast<float2*>(C + off) = make_float2(v0, v1);
         if (S1) {
             __half a0, b0, a1, b1;
@@ -245,9 +260,10 @@ __device__ __forceinline__ void store_pair(float* C, __half* S1, __half* S2, int
         if (S1) { __half a, b; split_half(v0, a, b, &ov); S1[off] = a; S2[off] = b; }
     }
 }
+template <bool kFull>
 __device__ __forceinline__ void store_pair(float* C, float* S1, float* S2, int64_t off, int n, int N, float v0, float v1, int&) {
     const float h0 = __uint_as_float(__float_as_uint(v0) & 0xFFFFE000u), h1 = __uint_as_float(__float_as_uint(v1) & 0xFFFFE000u);
-    if (n + 1 < N) {
+    if (kFull || n + 1 < N) {
         if (C) *reinterpret_cast<float2*>(C + off) = make_float2(v0, v1);
         if (S1) { *reinterpret_cast<float2*>(S1 + off) = make_float2(h0, h1); *reinterpret_cast<float2*>(S2 + off) = make_float2(v0 - h0, v1 - h1); }
     } else if (n < N) {
@@ -257,9 +273,10 @@ __device__ __forceinline__ void store_pair(float* C, float* S1, float* S2, int64
 }
 
 // The 3xBF16 form: fp32 and/or the three bf16 pieces of the next GEMM's operand (no saturation, no flag)
+template <bool kFull>
 __device__ __forceinline__ void store_pair3(float* C, __nv_bfloat16* S1, __nv_bfloat16* S2, __nv_bfloat16* S3, int64_t off, int n, int N,
                                             float v0, float v1) {
-    if (n + 1 < N) {
+    if (kFull || n + 1 < N) {
         if (C) *reinterpret_cast<float2*>(C + off) = make_float2(v0, v1);
         if (S1) {
             __nv_bfloat16 p0[3], p1[3];
@@ -390,9 +407,10 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
 #pragma unroll
                 for (int r = 0; r < CL; ++r) mbar_arrive_cluster(empty_peer[r] + 8 * stage);
         };
+        const bool tr = blockIdx.x == 0 && t == 0 && wg == 1 && g_gemm_trace_on;
         uint32_t it = 0;
         bool first = true;
-        for (int u = unit0; u < total; u += n_units) {
+        for (int u = unit0, ui = 0; u < total; u += n_units, ++ui) {
             const int tile = u / k_slices;
             float acc[64];
 #pragma unroll
@@ -430,6 +448,7 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
                         }
                     }
                     wgmma_commit();
+                    if (kb == 0) unit_trace(tr, ui, 0);
                     wgmma_wait<1>();                                       // the previous k-block's MMAs have retired
                     acc_fence(d);
                     if (prev_s >= 0) {
@@ -445,6 +464,7 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
 #pragma unroll
                 for (int j = 0; j < 64; ++j) acc[j] += d[j];              // round-to-nearest promotion
             }
+            unit_trace(tr, ui, 1);
             if (first && t == 0 && wg == 1) gemm_trace(4);
             // accumulator layout of m64n128: warp w holds rows 16w + lane/4 (+8); register 4j + {0,1} / {2,3} holds
             // columns 8j + 2 (lane % 4) + {0, 1} of the first / second of those rows
@@ -454,61 +474,73 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
             const int col0 = n_tile * GN + 2 * (lane & 3);
             float* Cs = C ? C + (int64_t)(u % k_slices) * slice_stride : nullptr;
             int ov = 0;
-            if constexpr (HEAD) {
+            unit_trace(tr, ui, 2);
+            // The epilogue is compiled twice: for tiles whose 128 columns all lie below N (every n tile but a ragged
+            // last one), with no per-column bounds checks, and for the edge tile, with them.  On a full tile every
+            // check is true, so both give the same stores; the full form drops the checks and the single-column
+            // fallback stores from the code the tensor cores wait on (DESIGN.md section 10).
+            auto epilogue = [&](auto full) {
+                constexpr bool kFull = decltype(full)::value;
+                if constexpr (HEAD) {
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int row = row0 + 8 * h;
-                    auto xv = [&](int j, int e) {
-                        const int n = col0 + 8 * j + e;
-                        return n < N ? acc[4 * j + 2 * h + e] * w_unscale + (bias ? bias[n] : 0.f) : -INFINITY;
-                    };
-                    // the 4 lanes of a quad hold the row's 128 columns: reduce across them (all lanes take part)
-                    float mx = -INFINITY;
+                    for (int h = 0; h < 2; ++h) {
+                        const int row = row0 + 8 * h;
+                        auto xv = [&](int j, int e) {
+                            const int n = col0 + 8 * j + e;
+                            return kFull || n < N ? acc[4 * j + 2 * h + e] * w_unscale + (bias ? bias[n] : 0.f) : -INFINITY;
+                        };
+                        // the 4 lanes of a quad hold the row's 128 columns: reduce across them (all lanes take part)
+                        float mx = -INFINITY;
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) mx = fmaxf(mx, fmaxf(xv(j, 0), xv(j, 1)));
-                    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-                    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-                    float se = 0.f;
-                    if (mx > -INFINITY) {
+                        for (int j = 0; j < 16; ++j) mx = fmaxf(mx, fmaxf(xv(j, 0), xv(j, 1)));
+                        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+                        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+                        float se = 0.f;
+                        if (mx > -INFINITY) {
 #pragma unroll
-                        for (int j = 0; j < 16; ++j) se += expf(xv(j, 0) - mx) + expf(xv(j, 1) - mx);
+                            for (int j = 0; j < 16; ++j) se += expf(xv(j, 0) - mx) + expf(xv(j, 1) - mx);
+                        }
+                        se += __shfl_xor_sync(0xffffffffu, se, 1);
+                        se += __shfl_xor_sync(0xffffffffu, se, 2);
+                        if (row >= M) continue;
+                        if ((lane & 3) == 0) he.stats[(int64_t)row * n_tiles + n_tile] = make_float2(mx, se);
+                        const uint32_t* mrow = he.mask + (int64_t)row * he.mask_words;
+                        uint32_t w[4];
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) w[i] = kFull || n_tile * 4 + i < he.mask_words ? mrow[n_tile * 4 + i] : 0u;
+#pragma unroll
+                        for (int j = 0; j < 16; ++j) {
+#pragma unroll
+                            for (int e = 0; e < 2; ++e) {
+                                const int n = col0 + 8 * j + e, bit = 8 * (j & 3) + 2 * (lane & 3) + e;
+                                if ((kFull || n < N) && (n_tile == 0 || ((w[j >> 2] >> bit) & 1u) || n == he.eos || n == he.pad)) Cs[(int64_t)row * ldc + n] = xv(j, e);
+                            }
+                        }
                     }
-                    se += __shfl_xor_sync(0xffffffffu, se, 1);
-                    se += __shfl_xor_sync(0xffffffffu, se, 2);
-                    if (row >= M) continue;
-                    if ((lane & 3) == 0) he.stats[(int64_t)row * n_tiles + n_tile] = make_float2(mx, se);
-                    const uint32_t* mrow = he.mask + (int64_t)row * he.mask_words;
-                    uint32_t w[4];
+                } else {
 #pragma unroll
-                    for (int i = 0; i < 4; ++i) w[i] = n_tile * 4 + i < he.mask_words ? mrow[n_tile * 4 + i] : 0u;
+                    for (int h = 0; h < 2; ++h) {
+                        const int row = row0 + 8 * h;
+                        if (row >= M) continue;
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) {
+                        for (int j = 0; j < 16; ++j) {
+                            const int n = col0 + 8 * j;
+                            float v[2];
 #pragma unroll
-                        for (int e = 0; e < 2; ++e) {
-                            const int n = col0 + 8 * j + e, bit = 8 * (j & 3) + 2 * (lane & 3) + e;
-                            if (n < N && (n_tile == 0 || ((w[j >> 2] >> bit) & 1u) || n == he.eos || n == he.pad)) Cs[(int64_t)row * ldc + n] = xv(j, e);
+                            for (int e = 0; e < 2; ++e) {
+                                const float x = acc[4 * j + 2 * h + e] * w_unscale + ((bias && (kFull || n + e < N)) ? bias[n + e] : 0.f);
+                                v[e] = epi_act<ACT>(x);
+                            }
+                            if constexpr (kBf16) store_pair3<kFull>(Cs, C_s1, C_s2, C_s3, (int64_t)row * ldc + n, n, N, v[0], v[1]);
+                            else store_pair<kFull>(Cs, C_s1, C_s2, (int64_t)row * ldc + n, n, N, v[0], v[1], ov);
                         }
                     }
                 }
-            } else
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int row = row0 + 8 * h;
-                if (row >= M) continue;
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const int n = col0 + 8 * j;
-                    float v[2];
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const float x = acc[4 * j + 2 * h + e] * w_unscale + ((bias && n + e < N) ? bias[n + e] : 0.f);
-                        v[e] = epi_act<ACT>(x);
-                    }
-                    if constexpr (kBf16) store_pair3(Cs, C_s1, C_s2, C_s3, (int64_t)row * ldc + n, n, N, v[0], v[1]);
-                    else store_pair(Cs, C_s1, C_s2, (int64_t)row * ldc + n, n, N, v[0], v[1], ov);
-                }
-            }
+            };
+            if ((n_tile + 1) * GN <= N) epilogue(std::true_type{});
+            else epilogue(std::false_type{});
             if (ov) atomicExch(overflow, 1);
+            unit_trace(tr, ui, 3);
             if (first && t == 0 && wg == 1) gemm_trace(5);
             first = false;
         }
