@@ -8,11 +8,10 @@
 #include <cuda_runtime.h>
 #include <cstdint>
 
+#include "decode_types.cuh"
 #include "launch.cuh"
 
 namespace sealb200 {
-
-constexpr int kHeadDim = 64;
 
 // ---- small helpers -----------------------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {
@@ -40,10 +39,7 @@ __device__ __forceinline__ void split4(const float4& v, float4& h, float4& l) {
 // fp32 arrays), 2 = FP16 (two half arrays; saturates at +-65504 and raises *overflow).
 struct SplitOut { void* a = nullptr; void* b = nullptr; int kind = 0; int* overflow = nullptr; };
 
-// A GEMM output that may still be in split-K form: ks > 1 -> value = (sum_s part[s * stride + off]) * unscale + bias[col],
-// the slices summed in index order exactly like gemm_splitk_finish_kernel; ks <= 1 -> plain[off].  Lets the consumer of a
-// small-batch GEMM (add+LN, the attention kernels) do the finish pass itself instead of a separate launch.
-struct SplitSrc { const float* part = nullptr; int ks = 0; int64_t stride = 0; const float* bias = nullptr; float unscale = 1.f; };
+// A GEMM output that may still be in split-K form (SplitSrc, decode_types.cuh), read as the finished value.
 __device__ __forceinline__ float4 load_split4(const float* __restrict__ plain, const SplitSrc& ss, int64_t off, int col) {
     if (ss.ks <= 1) return *reinterpret_cast<const float4*>(plain + off);
     float4 y = *reinterpret_cast<const float4*>(ss.part + off);

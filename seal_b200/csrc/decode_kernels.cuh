@@ -5,6 +5,8 @@
 // Replaces seal/beam_search.py:244-332 + :614-703 and the CPU FM-index work of :62-140 without a single
 // host synchronisation.
 #pragma once
+#include "bart_kernels.cuh"      // warp_sum, warp_max
+#include "decode_types.cuh"
 #include "fm_device.cuh"
 #include "launch.cuh"
 
@@ -16,7 +18,6 @@ namespace sealb200 {
 
 constexpr int kSelMaxK = 64;           // 2*num_beams <= 64
 constexpr int kSelMaxBeams = 32;
-constexpr int kMaxLen = 128;           // max_length <= 128 (SEAL: 10 body, 15 title, README.md:209-216 uses 100)
 
 struct StepCfg {
     int32_t num_beams, K;              // K = 2*num_beams

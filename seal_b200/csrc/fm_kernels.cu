@@ -432,7 +432,7 @@ size_t expand_scratch_bytes(uint32_t L, uint64_t R) { return ((R + 2 + 1) / 2 * 
 
 // Bitmask rows of R SA ranges: narrow ranges by one warp each, wide ones (>= kWideRange rows) by whole CTAs pulling
 // from a device-side work list.  `wide`: expand_scratch_bytes(L, R) of device scratch (work list + the wide CTAs' global
-// frontiers).  Stream-ordered, no host synchronisation; also the tail of every decode step (decode.cu).
+// frontiers).  Stream-ordered, no host synchronisation; also the tail of every decode step (generate.cu).
 void launch_expand_masks(const FmView& v, cudaStream_t s, uint64_t R, const uint64_t* lo_d, const uint64_t* hi_d, uint32_t* mask_d,
                          uint32_t ld_words, uint32_t vocab, uint32_t shift, unsigned long long* wide) {
     if (v.L > kMaxLevels) throw ApiError(SEALFM_EINVAL, "wavelet tree higher than kMaxLevels");

@@ -12,9 +12,6 @@
 
 namespace sealb200 {
 
-// The longest source the T5 path takes: the encoder bucket table covers distances -(kT5MaxSource-1) .. kT5MaxSource-1.
-constexpr int kT5MaxSource = 1024;
-
 // One CTA of 128 threads per row, d = 4 * n4 <= 512 * NV (each thread holds NV float4 of the row):
 //   v = embed[tok[r * tok_stride]]            (tok != nullptr: the embedding; T5 does not scale it)
 //   v = x[r] + b[r]                           (otherwise: residual + sub-layer output; b may still be an unsummed

@@ -36,12 +36,11 @@
 #include <type_traits>
 
 #include "bart_kernels.cuh"
+#include "decode_types.cuh"
 #include "launch.cuh"
 
 namespace sealb200 {
 
-constexpr int GM = 128;                              // tile rows (two consumer warpgroups of 64)
-constexpr int GN = 128;                              // tile columns (wgmma N)
 constexpr int GSTAGES = 3;
 constexpr int GTHREADS = 384;                        // producer warpgroup + 2 consumer warpgroups
 constexpr int G_AB = GM * 128;                       // one A tile (hi or lo): 128 rows x 128 B of K
@@ -160,8 +159,7 @@ __device__ __forceinline__ void wgmma_128(float (&d)[64], uint64_t a, uint64_t b
 
 __device__ __forceinline__ float gelu_erf_u(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
 
-// Epilogue activation (template argument ACT): none, BART's exact-erf GELU, T5's ReLU (torch.relu: NaN stays NaN)
-constexpr int kActNone = 0, kActGelu = 1, kActRelu = 2;
+// Epilogue activation ACT (kActNone, kActGelu, kActRelu: decode_types.cuh)
 template <int ACT> __device__ __forceinline__ float epi_act(float x) {
     return ACT == kActGelu ? gelu_erf_u(x) : ACT == kActRelu ? (x < 0.f ? 0.f : x) : x;
 }
@@ -303,15 +301,6 @@ __device__ __forceinline__ void tile_coords(int tile, int n_fastest, int band, i
     const int r = tile - b0 * n_tiles;
     n_tile = r / rows; mg = b0 + r % rows;
 }
-
-// lm_head epilogue of a constrained-decode step (HEAD = true, 3xFP16, CL = 1, no split-K).  Per (row, n tile) it writes
-// the partial log-softmax statistics (max, sum exp(x - max)) over the tile's columns n < N to stats[row * n_tiles +
-// n_tile], which topk_rows_kernel combines in place of streaming the row, and it stores x only at the columns the select
-// kernels read (the read set): the row's bits of `mask` ([M][mask_words]), eos and pad (topk_rows_kernel, row_bits),
-// and the whole first n tile, columns 0..127 (select_merge_kernel's -inf fill-ins, see generate_enqueue).
-struct HeadEpi {
-    float2* stats = nullptr; const uint32_t* mask = nullptr; int mask_words = 0; int eos = -1, pad = -1;
-};
 
 // T = __half (3xFP16), float (3xTF32) or __nv_bfloat16 (3xBF16: tmA_hi / tmA_lo / tmW_lo are A's pieces b1 / b2 / b3,
 // tmW_hi is W; C_s1 / C_s2 / C_s3 the three output pieces); CL = CTAs per cluster sharing the W tile (1 or 2).

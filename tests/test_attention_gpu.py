@@ -1,6 +1,6 @@
 """GPU: every attention kernel (bart_kernels.cuh, t5_kernels.cuh) against a float64 attention of the same inputs, through
 sealdec_debug_attention (the layer loops' own kernel choice), on crafted trained-scale scores at the dispatch
-boundaries of decode.cu.
+boundaries of forward.cu.
 
 Reference.  numpy float64 on the fp32 inputs the kernel reads (split-K slices summed in fp32 first, in the kernel's
 order): score = q.k / 8 (BART) or q.k + bias[bucket(key - query)][h] (T5, unscaled; buckets from transformers'

@@ -1,5 +1,5 @@
-"""GPU: every kernel branch of the BART forward (seal_b200/csrc/decode.cu: encoder_forward, decoder_step, gemm_impl,
-add_ln) against a float64 forward of the same seeded HF model, at the shapes where decode.cu switches branches.
+"""GPU: every kernel branch of the BART forward (seal_b200/csrc/forward.cu: encoder_forward, decoder_step, add_ln;
+gemm.cu: gemm_impl) against a float64 forward of the same seeded HF model, at the shapes where they switch branches.
 
 The float64 reference is transformers' BartForConditionalGeneration cast to double (the fp32 weights convert exactly),
 re-forwarded over the whole decoder prefix (use_cache=False).  The same model in fp32 runs on the same inputs: its own
@@ -149,7 +149,7 @@ def beam_inputs(rng, Q, B, t, vocab, share):
 
 
 def expected_attn_bits(Q, S, B, t, am, src_tokens):
-    """the shape-determined branches of one debug step call (decode.cu), restated"""
+    """the shape-determined branches of one debug step call (forward.cu, gemm.cu), restated"""
     bits = set()
     right = all(list(row) == sorted(row, reverse=True) for row in am.tolist())
     packed = right and src_tokens != -2
@@ -235,7 +235,7 @@ def run_case(model, Q, S, B, t, kind="right", src_tokens=-1, share=False, gemm_m
     return got_paths
 
 
-# (name, model, Q, S, B, P, kwargs): each case sits next to one threshold of decode.cu and names the branches it needs
+# (name, model, Q, S, B, P, kwargs): each case sits next to one threshold of forward.cu or gemm.cu and names the branches it needs
 CASES = [
     # cross-attention: cross_attn_small_kernel up to kXKeys = 32 keys
     ("S1", "tiny", 3, 1, 2, 2, dict(share=True, must={"cross_small"})),

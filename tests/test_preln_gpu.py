@@ -55,7 +55,7 @@ def paths(eng):
 
 
 def expected_bits(model, Q, S, B, t, am, src_tokens):
-    """the shape-determined branches of one debug step call (decode.cu), restated"""
+    """the shape-determined branches of one debug step call (forward.cu, gemm.cu), restated"""
     cfg = get_model(model)[2].config
     right = all(list(row) == sorted(row, reverse=True) for row in am.tolist())
     bits = {"enc_packed" if right and src_tokens != -2 else "enc_unpacked", "cross_small" if S <= 32 else "cross_grouped",
