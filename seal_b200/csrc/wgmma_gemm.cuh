@@ -22,7 +22,8 @@
 //     A b3 in the four 16 KB slots the other modes use for A hi / lo and W hi / lo.
 //
 // Kernel: persistent, 128 x 128 output tile per CTA, three warpgroups.  Warpgroup 0 is the producer (one thread
-// issues the TMA loads of A hi/lo and W hi/lo into 128B-swizzled K-major shared-memory stages); warpgroups 1 and 2
+// issues the TMA loads of A hi/lo and W hi/lo into 128B-swizzled K-major shared-memory stages, and warp 1 stages each
+// tile's bias slice in shared memory for the epilogue); warpgroups 1 and 2
 // each own 64 rows of the tile and issue wgmma.mma_async (m64n128, both operands from shared memory) into register
 // accumulators.  Stage hand-off uses mbarriers (full: TMA transaction bytes; empty: one arrive per consumer warp).
 // With CL = 2 (gemm_mode 5) two CTAs of a cluster compute vertically adjacent tiles that share the W tile: each CTA
@@ -46,7 +47,10 @@ constexpr int GTHREADS = 384;                        // producer warpgroup + 2 c
 constexpr int G_AB = GM * 128;                       // one A tile (hi or lo): 128 rows x 128 B of K
 constexpr int G_WB = GN * 128;                       // one W tile (hi or lo)
 constexpr int G_STAGE = 2 * G_AB + 2 * G_WB;         // 64 KB
-constexpr int G_SMEM = GSTAGES * G_STAGE + 1024 /*alignment slack*/ + 256 /*barriers*/;
+constexpr int G_BARS = 64;                           // mbarriers: full / empty per stage, bias full / empty
+constexpr int G_BIAS = GN * 4;                       // the unit's 128-column bias slice, fp32
+constexpr int G_SMEM = GSTAGES * G_STAGE + 1024 /*alignment slack*/ + G_BARS + G_BIAS;
+static_assert(8 * (2 * GSTAGES + 2) <= G_BARS, "barrier area");
 constexpr int UK16 = 64;                             // 3xFP16 k-block: 64 halves = one 128-byte swizzle row
 constexpr int UK = 32;                               // 3xTF32 k-block: 32 floats
 
@@ -332,6 +336,8 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;          // SWIZZLE_128B wants 1024 B alignment
     const uint32_t full0 = base + GSTAGES * G_STAGE, empty0 = full0 + 8 * GSTAGES;
+    const uint32_t bias_full = empty0 + 8 * GSTAGES, bias_empty = bias_full + 8;
+    float* const bias_s = reinterpret_cast<float*>(smem_raw + (full0 + G_BARS - smem_u32(smem_raw)));
     const int wg = threadIdx.x >> 7;
     const uint32_t rank = CL > 1 ? cluster_ctarank() : 0;
     if (threadIdx.x == 0) gemm_trace(0);
@@ -345,6 +351,7 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < GSTAGES; ++s) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 8 * CL); }
+        mbar_init(bias_full, 32); mbar_init(bias_empty, 8);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -381,6 +388,23 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
                         tma_load_2d_multicast(st + 2 * G_AB + G_WB + part, &tmW_lo, fb, kx, row_w, (uint16_t)((1u << CL) - 1));
                     }
                 }
+            }
+        } else if (threadIdx.x >> 5 == 1) {
+            // Warp 1 stages each unit's bias slice (0 past N, or everywhere without a bias) in shared memory during the
+            // unit's K loop, so that the epilogue reads no global memory: a global load issued there waits behind the
+            // next unit's operand stages, which the producer has already put in flight (DESIGN.md section 10).  One
+            // buffer: it is refilled after both consumer warpgroups have finished the previous unit's epilogue, a whole
+            // K loop before it is read.
+            const int lane = threadIdx.x & 31;
+            for (int u = unit0, ui = 0; u < total; u += n_units, ++ui) {
+                int mg, n_tile;
+                tile_coords(u / k_slices, n_fastest, m_band, m_groups, n_tiles, mg, n_tile);
+                mbar_wait(bias_empty, (ui & 1) ^ 1);
+                for (int i = lane; i < GN; i += 32) {
+                    const int n = n_tile * GN + i;
+                    bias_s[i] = bias && n < N ? bias[n] : 0.f;
+                }
+                mbar_arrive(bias_full);
             }
         }
     } else {
@@ -462,7 +486,9 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
             const int row0 = (mg * CL + (int)rank) * GM + (wg - 1) * 64 + warp * 16 + (lane >> 2);
             const int col0 = n_tile * GN + 2 * (lane & 3);
             float* Cs = C ? C + (int64_t)(u % k_slices) * slice_stride : nullptr;
+            const float* const bq = bias_s + 2 * (lane & 3);               // the bias of column col0 + 8 j + e is bq[8 j + e]
             int ov = 0;
+            mbar_wait(bias_full, ui & 1);
             unit_trace(tr, ui, 2);
             // The epilogue is compiled twice: for tiles whose 128 columns all lie below N (every n tile but a ragged
             // last one), with no per-column bounds checks, and for the edge tile, with them.  On a full tile every
@@ -474,10 +500,21 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
 #pragma unroll
                     for (int h = 0; h < 2; ++h) {
                         const int row = row0 + 8 * h;
-                        auto xv = [&](int j, int e) {
-                            const int n = col0 + 8 * j + e;
-                            return kFull || n < N ? acc[4 * j + 2 * h + e] * w_unscale + (bias ? bias[n] : 0.f) : -INFINITY;
-                        };
+                        // the row's logits, computed once in place (acc is not read again) and read by the three passes
+#pragma unroll
+                        for (int j = 0; j < 16; ++j) {
+#pragma unroll
+                            for (int e = 0; e < 2; ++e) {
+                                float& x = acc[4 * j + 2 * h + e];
+                                x = kFull || col0 + 8 * j + e < N ? x * w_unscale + bq[8 * j + e] : -INFINITY;
+                            }
+                        }
+                        auto xv = [&](int j, int e) { return acc[4 * j + 2 * h + e]; };
+                        // the mask words are loaded before the reductions, whose arithmetic hides their latency
+                        const uint32_t* mrow = he.mask + (int64_t)row * he.mask_words;
+                        uint32_t w[4];
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) w[i] = row < M && (kFull || n_tile * 4 + i < he.mask_words) ? mrow[n_tile * 4 + i] : 0u;
                         // the 4 lanes of a quad hold the row's 128 columns: reduce across them (all lanes take part)
                         float mx = -INFINITY;
 #pragma unroll
@@ -493,10 +530,6 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
                         se += __shfl_xor_sync(0xffffffffu, se, 2);
                         if (row >= M) continue;
                         if ((lane & 3) == 0) he.stats[(int64_t)row * n_tiles + n_tile] = make_float2(mx, se);
-                        const uint32_t* mrow = he.mask + (int64_t)row * he.mask_words;
-                        uint32_t w[4];
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) w[i] = kFull || n_tile * 4 + i < he.mask_words ? mrow[n_tile * 4 + i] : 0u;
 #pragma unroll
                         for (int j = 0; j < 16; ++j) {
 #pragma unroll
@@ -516,10 +549,7 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
                             const int n = col0 + 8 * j;
                             float v[2];
 #pragma unroll
-                            for (int e = 0; e < 2; ++e) {
-                                const float x = acc[4 * j + 2 * h + e] * w_unscale + ((bias && (kFull || n + e < N)) ? bias[n + e] : 0.f);
-                                v[e] = epi_act<ACT>(x);
-                            }
+                            for (int e = 0; e < 2; ++e) v[e] = epi_act<ACT>(acc[4 * j + 2 * h + e] * w_unscale + bq[8 * j + e]);
                             if constexpr (kBf16) store_pair3<kFull>(Cs, C_s1, C_s2, C_s3, (int64_t)row * ldc + n, n, N, v[0], v[1]);
                             else store_pair<kFull>(Cs, C_s1, C_s2, (int64_t)row * ldc + n, n, N, v[0], v[1], ov);
                         }
@@ -528,6 +558,8 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
             };
             if ((n_tile + 1) * GN <= N) epilogue(std::true_type{});
             else epilogue(std::false_type{});
+            __syncwarp();
+            if (lane == 0) mbar_arrive(bias_empty);                        // this warp has read the bias slice
             if (ov) atomicExch(overflow, 1);
             unit_trace(tr, ui, 3);
             if (first && t == 0 && wg == 1) gemm_trace(5);

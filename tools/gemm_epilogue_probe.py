@@ -10,10 +10,12 @@ first k-block of MMAs committed (F), its K loop done (L), epilogue start (E0) an
 The lm_head runs twice: through sealdec_debug_gemm_ex without storing (the plain GEMM's tile loop) and through
 sealdec_debug_head with the statistics epilogue the decoder uses (HEAD).  Card name, power limit and SM clocks are
 sampled in the same run.  Needs a GPU.
+--variant no-bias passes no bias to every shape; --variant no-store stores no output at any shape but the HEAD one
+(whose sparse logits are its output).  Set against the default, they show what the bias loads and the stores cost.
 
 Needs the library built with the timeline compiled in: make -C seal_b200/csrc GEMM_UNIT_TRACE=1 (after make clean).
 
-Usage: gemm_epilogue_probe.py [--iters 5] [--out FILE.json]"""
+Usage: gemm_epilogue_probe.py [--iters 5] [--variant as-is|no-bias|no-store] [--out FILE.json]"""
 import argparse
 import ctypes as C
 import json
@@ -63,6 +65,7 @@ def summarize(t20, u):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=5)
+    ap.add_argument("--variant", default="as-is", choices=["as-is", "no-bias", "no-store"])
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     rng = np.random.default_rng(0)
@@ -72,6 +75,7 @@ def main():
             A = rng.standard_normal((M, K), dtype=np.float32)
             W = (rng.standard_normal((N, K), dtype=np.float32) * 0.05).astype(np.float32)
             b = rng.standard_normal(N, dtype=np.float32)
+            bp = None if args.variant == "no-bias" else b.ctypes.data
             dev_us = C.c_double(0)
             if name == "lm_head HEAD":
                 words = (N + 31) // 32
@@ -81,15 +85,15 @@ def main():
                 out = np.empty((mpad, N), dtype=np.float32)
                 stats = np.empty((mpad, -(-N // 128), 2), dtype=np.float32)
                 fused = C.c_int32(0)
-                call = lambda: check(lib.sealdec_debug_head(M, N, K, A.ctypes.data, W.ctypes.data, b.ctypes.data,  # noqa: E731
+                call = lambda: check(lib.sealdec_debug_head(M, N, K, A.ctypes.data, W.ctypes.data, bp,  # noqa: E731
                                                             mask.ctypes.data, 2, 1, out.ctypes.data, stats.ctypes.data,
                                                             C.byref(fused)))
                 call()
                 assert fused.value == 1, "the lm_head took the split-K path"
             else:
-                store = 0 if name == "lm_head" else 1
+                store = 0 if name == "lm_head" or args.variant == "no-store" else 1
                 out = np.empty((M, N), dtype=np.float32) if store else None
-                call = lambda: check(lib.sealdec_debug_gemm_ex(3, M, N, K, A.ctypes.data, W.ctypes.data, b.ctypes.data,  # noqa: E731
+                call = lambda: check(lib.sealdec_debug_gemm_ex(3, M, N, K, A.ctypes.data, W.ctypes.data, bp,  # noqa: E731
                                                                out.ctypes.data if store else None, gelu, args.iters,
                                                                C.byref(dev_us), -1, store))
                 call()                                                                   # warm-up
@@ -98,7 +102,7 @@ def main():
             rows.append(r)
             del A, W, out
     card = smp.summary()
-    print(f"{card['gpu']}, power limit {card['power_limit_w']} W, median SM clock {card['sm_mhz_median']} MHz")
+    print(f"variant {args.variant}: {card['gpu']}, power limit {card['power_limit_w']} W, median SM clock {card['sm_mhz_median']} MHz")
     print(f"{'shape':13s} {'M':>6s} {'N':>6s} {'K':>5s} {'units':>5s} {'call ms':>8s} {'K loop us':>9s} {'epi us':>7s} "
           f"{'epi %':>6s} {'gap us':>7s} {'gap %':>6s}")
     for r in rows:
@@ -107,7 +111,7 @@ def main():
               f"{r['epilogue_us']:7.2f} {r['epilogue_share'] * 100:5.1f}% {r['gap_us']:7.2f} {r['gap_share'] * 100:5.1f}%")
     if args.out:
         with open(args.out, "w") as f:
-            json.dump({"card": card, "iters": args.iters, "rows": rows}, f, indent=1)
+            json.dump({"card": card, "variant": args.variant, "iters": args.iters, "rows": rows}, f, indent=1)
     return 0
 
 
