@@ -343,10 +343,10 @@ int sealdec_debug_step_logits(sealbart_t* model, const int64_t* input_ids, const
 int sealdec_debug_step_logits_ex(sealbart_t* model, const int64_t* input_ids, const int64_t* attention_mask,
                                  int64_t Q, int64_t S, int32_t num_beams, const int64_t* decoder_input_ids,
                                  int64_t t, const int32_t* ancestry, int64_t src_tokens_hint, float* out_logits);
-/* Stand-alone GEMM C[M,N] = A[M,K] W[N,K]^T + bias (+GELU) through the model's GEMM kernels
+/* Stand-alone GEMM C[M,N] = A[M,K] W[N,K]^T + bias (+ the epilogue activation) through the model's GEMM kernels
  * (mode 2 = 3xTF32, 3 = 3xFP16, 5 = 3xFP16 on CTA pairs, 6 = 3xBF16 with W rounded to bf16 as sealbart_set_tensor
- * rounds it), host pointers; if iters > 0 also reports the average
- * device time per call (CUDA events, includes the activation split). */
+ * rounds it), host pointers; gelu: 0 = no activation, 1 = exact-erf GELU, 2 = ReLU.  If iters > 0 also reports the
+ * average device time per call (CUDA events, includes the activation split). */
 int sealdec_debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A, const float* W,
                        const float* bias, float* C, int32_t gelu, int32_t iters, double* avg_us);
 /* the same with the tile order (mode 3 without split-K; other paths ignore band) and the store as variables
@@ -357,6 +357,25 @@ int sealdec_debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A
 int sealdec_debug_gemm_ex(int mode, int64_t M, int32_t N, int32_t K, const float* A, const float* W,
                           const float* bias, float* C, int32_t gelu, int32_t iters, double* avg_us, int32_t band,
                           int32_t store);
+/* The GEMM's other outputs, as the forward uses them (tests/test_gemm_split_out_gpu.py): one sealdec_debug_gemm_ex call
+ * (A split once beforehand; bias may be NULL) with
+ *   act       0 = no activation, 1 = exact-erf GELU, 2 = ReLU;
+ *   outputs   bit 0: the fp32 C [M][N]; bit 1: the operand split of the next GEMM, row stride N, in the mode's format:
+ *             mode 2 float s1 / s2 (TF32 hi / lo), modes 3 / 5 fp16 s1 / s2 (h1 / h2, saturated at +-65504), mode 6
+ *             bf16 s1 / s2 / s3 (the three pieces).  1, 2 or 3; s3 is only read in mode 6.  Whatever the GEMM does
+ *             not write comes back as NaN;
+ *   *overflow the GEMM's own fp16 range flag (1 if its epilogue or finish pass saturated a value; the flag the input
+ *             split may raise is cleared before the GEMM runs);
+ *   defer_rows as the forward passes it: a split-K result of at most this many rows, without activation or split
+ *             output, with a bias and N a multiple of 4, is left unsummed for its consumer.  If the call deferred,
+ *             *k_slices > 1, slices [k_slices][M][N] receives the raw slices (room for 8 is needed) and *unscale the
+ *             factor the consumer applies before the bias (finished = (sum of the slices in index order) * unscale +
+ *             bias); otherwise *k_slices = 0.  slices and unscale may be NULL when defer_rows is 0;
+ *   *paths    the "last_paths" bits of the call (10 .. 14, 24; 19 for ReLU). */
+int sealdec_debug_gemm_split(int mode, int64_t M, int32_t N, int32_t K, const float* A, const float* W,
+                             const float* bias, int32_t act, int32_t outputs, float* C, void* s1, void* s2, void* s3,
+                             int32_t* overflow, int64_t defer_rows, float* slices, int32_t* k_slices, float* unscale,
+                             uint32_t* paths);
 /* The lm_head GEMM of a decode step with the statistics epilogue requested (gemm_mode 3, through the same GEMM
  * dispatch as the decoder; tests/test_select_step_gpu.py): C[M,N] = A W^T + bias with the row masks
  * mask uint32 [M][ceil(N/32)] and eos / pad defining each row's read set.  Host pointers.  With Mpad = M rounded up

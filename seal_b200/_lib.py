@@ -167,6 +167,8 @@ _DEC_SIGS = {
                                  C.POINTER(C.c_double)]),
     "sealdec_debug_gemm_ex": (i32, [i32, C.c_int64, C.c_int32, C.c_int32, vp, vp, vp, vp, C.c_int32, C.c_int32,
                                     C.POINTER(C.c_double), C.c_int32, C.c_int32]),
+    "sealdec_debug_gemm_split": (i32, [i32, C.c_int64, C.c_int32, C.c_int32, vp, vp, vp, C.c_int32, C.c_int32, vp, vp, vp,
+                                       vp, vp, C.c_int64, vp, vp, vp, vp]),
     "sealdec_debug_head": (i32, [C.c_int64, C.c_int32, C.c_int32, vp, vp, vp, vp, C.c_int32, C.c_int32, vp, vp, vp]),
     "sealdec_debug_head_ex": (i32, [i32, C.c_int64, C.c_int32, C.c_int32, vp, vp, vp, vp, C.c_int32, C.c_int32, vp, vp, vp]),
     "sealdec_debug_select_step": (i32, [vp, C.POINTER(DecParams), C.POINTER(GroupParams), C.c_int64, C.c_int32, C.c_int32,

@@ -368,13 +368,24 @@ namespace {
 // the statistics [Mpad][ceil(N/128)] go (host; Mpad = M rounded up to 128 rows) and whether the epilogue ran.
 struct DebugHead { const uint32_t* mask; int eos, pad; float* stats; int32_t* fused; };
 
+// The other outputs of sealdec_debug_gemm_split (host pointers): the operand split of the next GEMM into s[0..2] when
+// `split` is set, the epilogue's overflow flag, defer_rows with the deferred slices, and the call's last_paths bits.
+struct DebugSplit {
+    bool split; void* s[3]; int32_t* overflow; int64_t defer_rows; float* slices; int32_t* k_slices; float* unscale; uint32_t* paths;
+};
+
 // presplit: 3xFP16 and 3xBF16 split the activations once, outside the timed calls (as the decoder's producers do)
+// act: kActNone, kActGelu or kActRelu
 int debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A, const float* W, const float* bias, float* C,
-               int32_t gelu, int32_t iters, double* avg_us, int32_t band, int32_t store, bool presplit,
-               const DebugHead* head = nullptr) {
+               int32_t act, int32_t iters, double* avg_us, int32_t band, int32_t store, bool presplit,
+               const DebugHead* head = nullptr, const DebugSplit* so = nullptr) {
     return guarded([&] {
-        if (!A || !W || (store && !C) || M <= 0 || N <= 0 || K <= 0 || band < -1) throw ApiError(SEALFM_EINVAL, "bad argument");
-        if (head && (!head_stats_mode(mode) || !store || gelu || iters > 0 || !head->mask || !head->stats || !head->fused))
+        if (!A || !W || (store && !C) || M <= 0 || N <= 0 || K <= 0 || band < -1 || act < kActNone || act > kActRelu)
+            throw ApiError(SEALFM_EINVAL, "bad argument");
+        if (head && (!head_stats_mode(mode) || !store || act || iters > 0 || !head->mask || !head->stats || !head->fused))
+            throw ApiError(SEALFM_EINVAL, "bad argument");
+        if (so && (head || iters > 0 || (!store && !so->split) || (so->split && (!so->s[0] || !so->s[1] || (mode == kGemmBf16 && !so->s[2]))) ||
+                   !so->overflow || !so->paths || !so->k_slices || so->defer_rows < 0 || (so->defer_rows > 0 && (!so->slices || !so->unscale))))
             throw ApiError(SEALFM_EINVAL, "bad argument");
         require_device();
         check_gemm_mode(mode);
@@ -396,7 +407,26 @@ int debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A, const 
         Act a{dA.as<float>()};
         if (presplit && mode != kGemmTf32)
             with_format(mode, [&](auto t) { a = split_act<decltype(t)>(nullptr, a.x, M * K, ah1, ah2, fake.ovf); });
-        const Act c{store ? dC.as<float>() : nullptr};
+        Act c{store ? dC.as<float>() : nullptr};
+        Buf ds[3];
+        size_t elem = 4;
+        if (so) {
+            // only the epilogue's flag is reported: clear what the input split raised.  Every output starts poisoned
+            // (all-ones bits: NaN in fp32, fp16 and bf16), so an element the GEMM does not write comes back as NaN.
+            CUDA_CHECK(cudaDeviceSynchronize());
+            CUDA_CHECK(cudaMemset(fake.ovf, 0, sizeof(int)));
+            CUDA_CHECK(cudaMemset(dC.p, 0xFF, (size_t)M * ldc * 4));
+            if (so->split)
+                with_format(mode, [&](auto t) {
+                    using T = decltype(t);
+                    elem = sizeof(T);
+                    for (int i = 0; i < (int)std::size(X3Format<T>::piece); ++i) {
+                        ds[i].ensure((size_t)M * ldc * elem);
+                        CUDA_CHECK(cudaMemset(ds[i].p, 0xFF, (size_t)M * ldc * elem));
+                        c.*X3Format<T>::piece[i] = ds[i].as<T>();
+                    }
+                });
+        }
         Ctx cx{&fake, nullptr};
         Buf dmask, dstats;
         const int64_t m_pad = (M + GM - 1) / GM * GM;
@@ -411,8 +441,20 @@ int debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A, const 
             CUDA_CHECK(cudaMemcpy(dmask.p, head->mask, (size_t)M * mask_words * 4, cudaMemcpyHostToDevice));
             cx.head = HeadEpi{dstats.as<float2>(), dmask.as<uint32_t>(), mask_words, head->eos, head->pad};
         }
-        gemm(cx, M, N, K, a, K, l, head ? Act{dC.as<float>()} : c, ldc, gelu ? kActGelu : kActNone);
+        gemm(cx, M, N, K, a, K, l, head ? Act{dC.as<float>()} : c, ldc, act, so ? so->defer_rows : 0);
         CUDA_CHECK(cudaDeviceSynchronize());
+        if (so) {
+            CUDA_CHECK(cudaMemcpy(so->overflow, fake.ovf, sizeof(int32_t), cudaMemcpyDeviceToHost));
+            *so->paths = fake.last_paths;
+            const SplitSrc& p = cx.pending;
+            *so->k_slices = p.ks;
+            if (p.ks > 0) {                                    // deferred: [k_slices][M][ldc] raw slices (ldc == N)
+                CUDA_CHECK(cudaMemcpy(so->slices, p.part, (size_t)p.ks * p.stride * 4, cudaMemcpyDeviceToHost));
+                *so->unscale = p.unscale;
+            }
+            for (int i = 0; i < 3; ++i)
+                if (ds[i].p) CUDA_CHECK(cudaMemcpy2D(so->s[i], (size_t)N * elem, ds[i].p, (size_t)ldc * elem, (size_t)N * elem, M, cudaMemcpyDeviceToHost));
+        }
         if (head) {
             *head->fused = cx.head_fused ? 1 : 0;
             CUDA_CHECK(cudaMemcpy2D(C, (size_t)N * 4, dC.p, (size_t)ldc * 4, (size_t)N * 4, m_pad, cudaMemcpyDeviceToHost));
@@ -422,7 +464,7 @@ int debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A, const 
         if (iters > 0 && avg_us) {
             cudaEvent_t e0, e1; CUDA_CHECK(cudaEventCreate(&e0)); CUDA_CHECK(cudaEventCreate(&e1));
             CUDA_CHECK(cudaEventRecord(e0, nullptr));
-            for (int i = 0; i < iters; ++i) gemm(cx, M, N, K, a, K, l, c, ldc, gelu ? kActGelu : kActNone);
+            for (int i = 0; i < iters; ++i) gemm(cx, M, N, K, a, K, l, c, ldc, act);
             CUDA_CHECK(cudaEventRecord(e1, nullptr));
             CUDA_CHECK(cudaEventSynchronize(e1));
             float ms = 0; CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
@@ -445,6 +487,14 @@ int sealdec_debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A
 int sealdec_debug_gemm_ex(int mode, int64_t M, int32_t N, int32_t K, const float* A, const float* W, const float* bias, float* C,
                           int32_t gelu, int32_t iters, double* avg_us, int32_t band, int32_t store) {
     return debug_gemm(mode, M, N, K, A, W, bias, C, gelu, iters, avg_us, band, store, true);
+}
+
+int sealdec_debug_gemm_split(int mode, int64_t M, int32_t N, int32_t K, const float* A, const float* W, const float* bias,
+                             int32_t act, int32_t outputs, float* C, void* s1, void* s2, void* s3, int32_t* overflow,
+                             int64_t defer_rows, float* slices, int32_t* k_slices, float* unscale, uint32_t* paths) {
+    if (outputs < 1 || outputs > 3) return guarded([] { throw ApiError(SEALFM_EINVAL, "outputs must be 1, 2 or 3"); });
+    const DebugSplit so{(outputs & 2) != 0, {s1, s2, s3}, overflow, defer_rows, slices, k_slices, unscale, paths};
+    return debug_gemm(mode, M, N, K, A, W, bias, C, act, 0, nullptr, -1, outputs & 1, true, nullptr, &so);
 }
 
 int sealdec_debug_head(int64_t M, int32_t N, int32_t K, const float* A, const float* W, const float* bias,

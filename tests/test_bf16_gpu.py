@@ -2,7 +2,7 @@
 (wgmma_gemm.cuh, include/sealdec.h).  The oracle is the same bf16 model upcast to float64, which is exact.
 
   1. the GEMM alone (sealdec_debug_gemm_ex / sealdec_debug_gemm, mode 6) against float64 on activations from 2^-30 to
-     2^40, on whole tiles, bands, split-K with its finish pass, the GELU epilogue and unsplit operands, held to the
+     2^40, on whole tiles, bands, split-K with its finish pass, the GELU and ReLU epilogues and unsplit operands, held to the
      accumulation bound (48 + K / 256 + 8) 2^-23 sum|a w| with no absolute floor; A W with W = I returns A bit for bit
      (the device split is exact);
   2. the lm_head statistics epilogue in mode 6 (sealdec_debug_head_ex) with test_select_step_gpu.py's checks;
@@ -54,17 +54,18 @@ def bf16_round(x):
 
 # ---- 1. the GEMM alone ------------------------------------------------------------------------------------------------
 
-def run_gemm(A, W, b, gelu, band=-1, presplit=True):
+def run_gemm(A, W, b, act, band=-1, presplit=True):
+    """act: 0 none, 1 GELU, 2 ReLU"""
     from seal_b200._lib import check, lib
     M, K = A.shape; N = W.shape[0]
     out = np.empty((M, N), dtype=np.float32)
     us = C.c_double(0)
     bp = b.ctypes.data if b is not None else None
     if presplit:
-        check(lib.sealdec_debug_gemm_ex(6, M, N, K, A.ctypes.data, W.ctypes.data, bp, out.ctypes.data, int(gelu), 0,
+        check(lib.sealdec_debug_gemm_ex(6, M, N, K, A.ctypes.data, W.ctypes.data, bp, out.ctypes.data, act, 0,
                                         C.byref(us), band, 1))
     else:
-        check(lib.sealdec_debug_gemm(6, M, N, K, A.ctypes.data, W.ctypes.data, bp, out.ctypes.data, int(gelu), 0, C.byref(us)))
+        check(lib.sealdec_debug_gemm(6, M, N, K, A.ctypes.data, W.ctypes.data, bp, out.ctypes.data, act, 0, C.byref(us)))
     return out
 
 
@@ -75,31 +76,34 @@ def gelu64(x):
 
 ROW_EXPS = [-30, -20, -10, 0, 10, 20, 30, 40]
 
-# (label, M, N, K, gelu, band, presplit): whole tiles (80 tiles > 132 / 2), ragged edges and an odd N, bands (m fastest,
-# 2 tiles per band), split-K (8 tiles) with the plain and the GELU finish, an operand the GEMM splits itself
+# (label, M, N, K, act, band, presplit): whole tiles (80 tiles > 132 / 2), ragged edges and an odd N, bands (m fastest,
+# 2 tiles per band), split-K (8 tiles) with the plain, the GELU and the ReLU finish, an operand the GEMM splits itself;
+# act 0 none, 1 GELU, 2 ReLU
 GEMM_CASES = [("tiles", 1280, 1024, 1024, 0, -1, True), ("tiles_gelu", 1280, 1024, 1024, 1, -1, True),
               ("ragged", 1300, 1157, 192, 0, -1, True), ("bands", 1024, 4096, 512, 0, 2, True),
               ("splitk", 64, 1024, 1024, 0, -1, True), ("splitk_gelu", 64, 1024, 4096, 1, -1, True),
-              ("unsplit", 300, 512, 256, 1, -1, False)]
+              ("splitk_relu", 64, 1024, 2048, 2, -1, True), ("unsplit", 300, 512, 256, 1, -1, False)]
 
 
-@pytest.mark.parametrize("label,M,N,K,gelu,band,presplit", GEMM_CASES, ids=[c[0] for c in GEMM_CASES])
-def test_gemm_vs_float64(label, M, N, K, gelu, band, presplit):
+@pytest.mark.parametrize("label,M,N,K,act,band,presplit", GEMM_CASES, ids=[c[0] for c in GEMM_CASES])
+def test_gemm_vs_float64(label, M, N, K, act, band, presplit):
     rng = np.random.default_rng(M + N + K)
     scale = np.array([2.0 ** ROW_EXPS[i % len(ROW_EXPS)] for i in range(M)])
     A = (rng.standard_normal((M, K)) * scale[:, None]).astype(np.float32)
     W = rng.standard_normal((N, K)).astype(np.float32) / np.float32(math.sqrt(K))
     b = rng.standard_normal(N).astype(np.float32)
     b[::2] *= 0                                               # bias-free columns: the products alone at every scale
-    got = run_gemm(A, W, b, gelu, band, presplit)
+    got = run_gemm(A, W, b, act, band, presplit)
     A64, W64 = A.astype(np.float64), bf16_round(W).astype(np.float64)     # the library rounds W to bf16
     pre = A64 @ W64.T + b.astype(np.float64)
     mag = np.abs(A64) @ np.abs(W64).T
     tol = (48 + K // 256 + 8) * 2.0 ** -23 * mag + 2.0 ** -23 * np.abs(pre)
     exp = pre
-    if gelu:                                                  # |gelu'| <= 1.13; erff's error relative to |x|
+    if act == 1:                                              # |gelu'| <= 1.13; erff's error relative to |x|
         exp = gelu64(pre)
         tol = 1.2 * tol + 2.0 ** -22 * (np.abs(pre) + np.abs(exp))
+    elif act == 2:                                            # ReLU is 1-Lipschitz: the same bound
+        exp = np.maximum(pre, 0.0)
     assert np.isfinite(got).all(), label
     err = np.abs(got - exp)
     ratio = err / np.maximum(tol, 1e-300)

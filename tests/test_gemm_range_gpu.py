@@ -31,13 +31,14 @@ def need_gpu():
     assert torch.cuda.is_available(), "-m gpu tests need a CUDA device"
 
 
-def run_gemm(mode, A, W, b, gelu):
+def run_gemm(mode, A, W, b, act):
+    """act: 0 none, 1 GELU, 2 ReLU"""
     from seal_b200._lib import lib, check
     M, K = A.shape; N = W.shape[0]
     out = np.empty((M, N), dtype=np.float32)
     us = C.c_double(0)
     check(lib.sealdec_debug_gemm(mode, M, N, K, A.ctypes.data, W.ctypes.data, b.ctypes.data if b is not None else None,
-                                 out.ctypes.data, int(gelu), 0, C.byref(us)))
+                                 out.ctypes.data, act, 0, C.byref(us)))
     return out
 
 
@@ -54,8 +55,8 @@ def make_a(kind, M, K, rng):
     return gelu64(rng.standard_normal((M, K)) * 3.0).astype(np.float32)
 
 
-def check_elementwise(mode, A, W, b, gelu, label, floor_ok=True):
-    got = run_gemm(mode, A, W, b, gelu)
+def check_elementwise(mode, A, W, b, act, label, floor_ok=True):
+    got = run_gemm(mode, A, W, b, act)
     A64, W64 = A.astype(np.float64), W.astype(np.float64)
     pre = A64 @ W64.T + (b.astype(np.float64) if b is not None else 0.0)
     mag = np.abs(A64) @ np.abs(W64).T
@@ -64,9 +65,11 @@ def check_elementwise(mode, A, W, b, gelu, label, floor_ok=True):
     if mode != 2 and floor_ok:
         tol = tol + floor
     exp = pre
-    if gelu:              # |gelu'| <= 1.13; erff's own error is relative to |x| where 1 + erf cancels
+    if act == 1:          # |gelu'| <= 1.13; erff's own error is relative to |x| where 1 + erf cancels
         exp = gelu64(pre)
         tol = 1.2 * tol + ULP * (np.abs(pre) + np.abs(exp))
+    elif act == 2:        # |relu(x) - relu(y)| <= |x - y|: the same bound
+        exp = np.maximum(pre, 0.0)
     assert np.isfinite(got).all(), label
     err = np.abs(got - exp)
     worst = np.unravel_index(np.argmax(err / tol), err.shape)
@@ -77,30 +80,31 @@ def check_elementwise(mode, A, W, b, gelu, label, floor_ok=True):
     assert (err <= tol).all(), (label, worst, err[worst], tol[worst])
 
 
+@pytest.mark.parametrize("act", [0, 2], ids=["none", "relu"])
 @pytest.mark.parametrize("mode", [2, 3, 5])
 @pytest.mark.parametrize("kind", ["scaled", "gelu_rows"])
 @pytest.mark.parametrize("M", [1, 129])
 @pytest.mark.parametrize("N", [1, 3, 129])
 @pytest.mark.parametrize("K", [64, 320])        # one k-block; five, the last promotion chunk partly filled
-def test_gemm_per_element_vs_float64(mode, kind, M, N, K):
+def test_gemm_per_element_vs_float64(mode, kind, M, N, K, act):
     rng = np.random.default_rng(M * 1000 + N * 10 + K)
     A = make_a(kind, M, K, rng)
     W = (rng.standard_normal((N, K)) * 0.05).astype(np.float32)
     b = rng.standard_normal(N).astype(np.float32) if N != 3 else None
-    check_elementwise(mode, A, W, b, False, f"mode {mode} {kind} {M}x{N}x{K}")
+    check_elementwise(mode, A, W, b, act, f"mode {mode} {kind} {M}x{N}x{K} act={act}")
 
 
 @pytest.mark.parametrize("mode", [3, 5])
-@pytest.mark.parametrize("gelu", [False, True])
+@pytest.mark.parametrize("act", [0, 1, 2], ids=["none", "gelu", "relu"])
 @pytest.mark.parametrize("K", [512, 2048])
-def test_gemm_split_k_per_element_vs_float64(mode, gelu, K):
+def test_gemm_split_k_per_element_vs_float64(mode, act, K):
     """129 x 129: four tiles, so K is split over 4 (K = 512) or 8 (K = 2048) CTAs and summed by the finish pass"""
-    rng = np.random.default_rng(K + gelu)
+    rng = np.random.default_rng(K + act)
     for kind in ("scaled", "gelu_rows"):
         A = make_a(kind, 129, K, rng)
         W = (rng.standard_normal((129, K)) * 0.05).astype(np.float32)
         b = rng.standard_normal(129).astype(np.float32) if kind == "scaled" else None
-        check_elementwise(mode, A, W, b, gelu, f"mode {mode} split-K {kind} 129x129x{K} gelu={gelu}")
+        check_elementwise(mode, A, W, b, act, f"mode {mode} split-K {kind} 129x129x{K} act={act}")
 
 
 @pytest.mark.parametrize("mode", [2, 3, 5])
@@ -111,7 +115,7 @@ def test_gemm_fp32_level_above_fp16_floor(mode, M, N, K):
     A = (np.exp2(rng.uniform(-3.0, 2.0, size=(M, K))) * rng.choice([-1.0, 1.0], size=(M, K))).astype(np.float32)
     W = (rng.standard_normal((N, K)) * 0.05).astype(np.float32)
     b = rng.standard_normal(N).astype(np.float32)
-    check_elementwise(mode, A, W, b, False, f"mode {mode} |a| in [2^-3, 4) {M}x{N}x{K}", floor_ok=False)
+    check_elementwise(mode, A, W, b, 0, f"mode {mode} |a| in [2^-3, 4) {M}x{N}x{K}", floor_ok=False)
 
 
 @pytest.mark.parametrize("mode", [3, 5])
@@ -119,6 +123,6 @@ def test_fp16_modes_reject_k_not_multiple_of_64(mode):
     from seal_b200._lib import SealB200Error
     A = np.ones((4, 96), dtype=np.float32); W = np.ones((8, 96), dtype=np.float32)
     with pytest.raises(SealB200Error) as ei:
-        run_gemm(mode, A, W, None, False)
+        run_gemm(mode, A, W, None, 0)
     assert ei.value.code == -1
-    run_gemm(2, A, W, None, False)                # 3xTF32 takes K in steps of 32
+    run_gemm(2, A, W, None, 0)                # 3xTF32 takes K in steps of 32
