@@ -10,6 +10,7 @@
 
 #include "decode_types.cuh"
 #include "launch.cuh"
+#include "operand_split.cuh"
 
 namespace sealb200 {
 
@@ -23,16 +24,6 @@ __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
     return v;
-}
-
-// TF32 split used by the 3xTF32 GEMM (wgmma_gemm.cuh): hi keeps sign/exponent/10 mantissa bits,
-// lo = x - hi exactly.  Producers write the split directly so no separate pass is needed.
-__device__ __forceinline__ void split1(float x, float& h, float& l) {
-    h = __uint_as_float(__float_as_uint(x) & 0xFFFFE000u);
-    l = x - h;
-}
-__device__ __forceinline__ void split4(const float4& v, float4& h, float4& l) {
-    split1(v.x, h.x, l.x); split1(v.y, h.y, l.y); split1(v.z, h.z, l.z); split1(v.w, h.w, l.w);
 }
 
 // Where a producer writes the operand split its consumer GEMM wants: kind 0 = none, 1 = TF32 (two
@@ -61,80 +52,36 @@ __device__ __forceinline__ float2 load_split2(const float* __restrict__ plain, c
     return make_float2(y.x * ss.unscale + bb.x, y.y * ss.unscale + bb.y);
 }
 
-__device__ __forceinline__ void half_split1(float x, __half& h1, __half& h2, int& ov) {
-    if (fabsf(x) > 65504.f) { ov = 1; x = copysignf(65504.f, x); }
-    h1 = __float2half_rn(x);
-    h2 = __float2half_rn(x - __half2float(h1));
-}
-__device__ __forceinline__ void store_split4(const SplitOut& so, int64_t idx, const float4& o) {
+// The producers' split stores (operand_split.cuh): SplitOut kind 1 / 2 stores the 3xTF32 / 3xFP16 pieces, and raises
+// *overflow once per store whose values the fp16 split saturated.
+template <int V> __device__ __forceinline__ void store_split(const SplitOut& so, int64_t idx, const float (&v)[V]) {
+    int ov = 0;
     if (so.kind == 1) {
-        float4 h, l;
-        split4(o, h, l);
-        *reinterpret_cast<float4*>(static_cast<float*>(so.a) + idx) = h;
-        *reinterpret_cast<float4*>(static_cast<float*>(so.b) + idx) = l;
+        float* const s[2] = {static_cast<float*>(so.a), static_cast<float*>(so.b)};
+        store_split<float, V>(s, idx, v, ov);
     } else if (so.kind == 2) {
-        __half h1[4], h2[4];
-        int ov = 0;
-        half_split1(o.x, h1[0], h2[0], ov); half_split1(o.y, h1[1], h2[1], ov);
-        half_split1(o.z, h1[2], h2[2], ov); half_split1(o.w, h1[3], h2[3], ov);
+        __half* const s[2] = {static_cast<__half*>(so.a), static_cast<__half*>(so.b)};
+        __half q[V][2];
+        split_values(v, q, ov);
         if (ov) atomicExch(so.overflow, 1);
-        *reinterpret_cast<uint2*>(static_cast<__half*>(so.a) + idx) = make_uint2(
-            (uint32_t)__half_as_ushort(h1[0]) | ((uint32_t)__half_as_ushort(h1[1]) << 16),
-            (uint32_t)__half_as_ushort(h1[2]) | ((uint32_t)__half_as_ushort(h1[3]) << 16));
-        *reinterpret_cast<uint2*>(static_cast<__half*>(so.b) + idx) = make_uint2(
-            (uint32_t)__half_as_ushort(h2[0]) | ((uint32_t)__half_as_ushort(h2[1]) << 16),
-            (uint32_t)__half_as_ushort(h2[2]) | ((uint32_t)__half_as_ushort(h2[3]) << 16));
-    }
-}
-__device__ __forceinline__ void store_split2(const SplitOut& so, int64_t idx, const float2& o) {
-    if (so.kind == 1) {
-        float2 h, l;
-        split1(o.x, h.x, l.x); split1(o.y, h.y, l.y);
-        *reinterpret_cast<float2*>(static_cast<float*>(so.a) + idx) = h;
-        *reinterpret_cast<float2*>(static_cast<float*>(so.b) + idx) = l;
-    } else if (so.kind == 2) {
-        __half a0, a1, b0, b1;
-        int ov = 0;
-        half_split1(o.x, a0, b0, ov); half_split1(o.y, a1, b1, ov);
-        if (ov) atomicExch(so.overflow, 1);
-        *reinterpret_cast<uint32_t*>(static_cast<__half*>(so.a) + idx) = (uint32_t)__half_as_ushort(a0) | ((uint32_t)__half_as_ushort(a1) << 16);
-        *reinterpret_cast<uint32_t*>(static_cast<__half*>(so.b) + idx) = (uint32_t)__half_as_ushort(b0) | ((uint32_t)__half_as_ushort(b1) << 16);
+        store_pieces(s, idx, q);
     }
 }
 
-// The operand split of the 3xBF16 GEMM (gemm_mode 6): x = b1 + b2 + b3, each piece the round-to-nearest bf16 of what the
-// previous pieces leave.  Each residual is exact in fp32 and has at most 16, then 8 significant bits, so the three
-// pieces carry x exactly for every 2^-100 <= |x| < (2 - 2^-8) 2^127 (below, b3 may be a bf16 subnormal; from the upper
-// bound on, which only the last 2^-8 of fp32's range reaches, b1 rounds to infinity); bf16 has fp32's exponent range,
-// so nothing saturates.  A producer of a gemm_mode 6 model takes this type in place of SplitOut (its
-// kernels are instantiated per split type); b1 == nullptr: no split wanted.
+// The producer split of a gemm_mode 6 model, the three bf16 pieces (operand_split.cuh).  A producer takes this type in
+// place of SplitOut (its kernels are instantiated per split type); b1 == nullptr: no split wanted.
 struct SplitBf16 { __nv_bfloat16* b1 = nullptr; __nv_bfloat16* b2 = nullptr; __nv_bfloat16* b3 = nullptr; };
-__device__ __forceinline__ void bf16x3_split1(float x, __nv_bfloat16& p1, __nv_bfloat16& p2, __nv_bfloat16& p3) {
-    p1 = __float2bfloat16_rn(x);
-    const float r = x - __bfloat162float(p1);
-    p2 = __float2bfloat16_rn(r);
-    p3 = __float2bfloat16_rn(r - __bfloat162float(p2));
-}
-__device__ __forceinline__ uint32_t bf16_pack(__nv_bfloat16 a, __nv_bfloat16 b) {
-    return (uint32_t)__bfloat16_as_ushort(a) | ((uint32_t)__bfloat16_as_ushort(b) << 16);
-}
-__device__ __forceinline__ void store_split4(const SplitBf16& so, int64_t idx, const float4& o) {
+template <int V> __device__ __forceinline__ void store_split(const SplitBf16& so, int64_t idx, const float (&v)[V]) {
     if (!so.b1) return;
-    __nv_bfloat16 p[3][4];
-    bf16x3_split1(o.x, p[0][0], p[1][0], p[2][0]); bf16x3_split1(o.y, p[0][1], p[1][1], p[2][1]);
-    bf16x3_split1(o.z, p[0][2], p[1][2], p[2][2]); bf16x3_split1(o.w, p[0][3], p[1][3], p[2][3]);
-    __nv_bfloat16* dst[3] = {so.b1, so.b2, so.b3};
-#pragma unroll
-    for (int j = 0; j < 3; ++j)
-        *reinterpret_cast<uint2*>(dst[j] + idx) = make_uint2(bf16_pack(p[j][0], p[j][1]), bf16_pack(p[j][2], p[j][3]));
+    __nv_bfloat16* const s[3] = {so.b1, so.b2, so.b3};
+    int ov = 0;
+    store_split<__nv_bfloat16, V>(s, idx, v, ov);
 }
-__device__ __forceinline__ void store_split2(const SplitBf16& so, int64_t idx, const float2& o) {
-    if (!so.b1) return;
-    __nv_bfloat16 p[3][2];
-    bf16x3_split1(o.x, p[0][0], p[1][0], p[2][0]); bf16x3_split1(o.y, p[0][1], p[1][1], p[2][1]);
-    *reinterpret_cast<uint32_t*>(so.b1 + idx) = bf16_pack(p[0][0], p[0][1]);
-    *reinterpret_cast<uint32_t*>(so.b2 + idx) = bf16_pack(p[1][0], p[1][1]);
-    *reinterpret_cast<uint32_t*>(so.b3 + idx) = bf16_pack(p[2][0], p[2][1]);
+template <class SO> __device__ __forceinline__ void store_split4(const SO& so, int64_t idx, const float4& o) {
+    store_split<4>(so, idx, {o.x, o.y, o.z, o.w});
+}
+template <class SO> __device__ __forceinline__ void store_split2(const SO& so, int64_t idx, const float2& o) {
+    store_split<2>(so, idx, {o.x, o.y});
 }
 
 // Element type of the token-embedding table a producer with split type SO gathers from: bf16 in gemm_mode 6

@@ -10,6 +10,7 @@
 #include "../../include/sealdec.h"
 #include "common.cuh"
 #include "decode_types.cuh"
+#include "operand_split.cuh"
 
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -101,12 +102,12 @@ struct sealbart {
     Buf enc_tok, enc_mask, ex, eqkv, etmp, ckv, src_off;
     bool enc_packed = false;          // the last encoder_forward ran on the real tokens only (src_off valid)
     Buf dx, dqkv, dtmp, dcq, logits, kc, vc;
-    Buf ex_hi, ex_lo, eattn_hi, eattn_lo, effn_hi, effn_lo, dx_hi, dx_lo, dattn_hi, dattn_lo, dffn_hi, dffn_lo;   // activation splits (halves or TF32)
+    Buf ex_split, eattn_split, effn_split, dx_split, dattn_split, dffn_split;   // activation splits (split_view)
     Buf st_scores, st_tokens, st_lo, st_hi, st_pw, st_anc, st_mask;
     Buf st_rowmax, st_rowls, st_rule, st_cval, st_cidx, st_ccnt, st_wide;     // scratch between the kernels of a step
     Buf st_hstat;                     // [R][V / 128] lm_head tile statistics (HeadEpi)
     Buf st_thr;                       // [R][3] top-k warp statistics of each logits row (topk_threshold_kernel)
-    Buf hy_score, hy_len, hy_tok, hy_valid, hy_lo, hy_hi, err, dbg_ids, a_hi, a_lo, splitk;
+    Buf hy_score, hy_len, hy_tok, hy_valid, hy_lo, hy_hi, err, dbg_ids, a_split, splitk;
     std::vector<void*> split_allocs;
     int64_t launches = 0;
     uint32_t last_paths = 0;          // OR of the kPath* bits of every kernel branch the last model call took
@@ -139,7 +140,7 @@ struct sealbart {
     int query_slices = -1;            // -1 $SEALB200_QUERY_SLICES (default on), 0 off, 1 on
     cudaStream_t slice_stream = nullptr;
     cudaEvent_t slice_fork = nullptr, slice_join = nullptr;
-    Buf a_hi1, a_lo1, splitk1, st_wide1;
+    Buf a_split1, splitk1, st_wide1;
     Buf effn2, dffn2;                 // T5 gated-gelu: [rows][2 d_ff] output of the [wi_0; wi_1] GEMM
     ~sealbart() { for (void* p : allocs) cudaFree(p); for (void* p : split_allocs) cudaFree(p); }
 };
@@ -158,18 +159,34 @@ inline bool bf16_weights(const sealbart* m) { return m->cfg.gemm_mode == kGemmBf
 
 constexpr int64_t kAddLnRowMax = 2048;      // up to this many rows add+LN runs one CTA per row
 
-// An activation tensor as the GEMMs see it: plain fp32 and/or its split in the gemm_mode's format (X3Format).
+// f(T()) with the element type T of gemm_mode's operand format (operand_split.cuh)
+template <typename F> void with_format(int mode, F&& f) {
+    if (mode == kGemmBf16) f(__nv_bfloat16());
+    else if (is_3xfp16(mode)) f(__half());
+    else f(0.f);
+}
+
+// An activation tensor as the GEMMs see it: plain fp32 x and/or its split in the gemm_mode's format T (with_format):
+// p[i] is piece i, an array of T, for i < kPieces<T>; p[0] == nullptr: no split.
 struct Act {
-    float* x = nullptr; float* hi = nullptr; float* lo = nullptr;   // fp32 / TF32 split
-    __half* h1 = nullptr; __half* h2 = nullptr;                     // FP16 split
-    __nv_bfloat16* b1 = nullptr; __nv_bfloat16* b2 = nullptr; __nv_bfloat16* b3 = nullptr;   // 3xBF16 split
+    float* x = nullptr; void* p[3] = {};
+    template <typename T> T* piece(int i) const { return static_cast<T*>(p[i]); }
 };
+
+// Every split buffer holds 8 bytes per element, whatever the format: with cap = b.bytes / 8 elements, piece i of format
+// T starts at element i * cap of T.  The view of b from element off on, with plain (if not null) as the fp32 copy.
+template <typename T> Act split_view(float* plain, const Buf& b, int64_t off = 0) {
+    Act a{plain ? plain + off : nullptr};
+    const int64_t cap = (int64_t)(b.bytes / 8);
+    for (int i = 0; i < kPieces<T>; ++i) a.p[i] = b.as<T>() + i * cap + off;
+    return a;
+}
 
 // The stream and the per-call state the launches of one forward share.
 // pending: a split-K GEMM whose slices are still unsummed (gemm's defer_rows) -- its consumer (add+LN on small batches,
 // the attention kernels) folds the finish pass in
 // head: the lm_head GEMM may use the statistics epilogue (HeadEpi); head_fused reports that it did
-// slice: 1 = the second query slice of a generate, which has its own GEMM scratch (a_hi1, a_lo1, splitk1)
+// slice: 1 = the second query slice of a generate, which has its own GEMM scratch (a_split1, splitk1)
 struct Ctx { sealbart* m; cudaStream_t s; SplitSrc pending{}; HeadEpi head{}; bool head_fused = false; int slice = 0; };
 
 struct Dims {
@@ -203,7 +220,7 @@ int32_t t5_bucket(int32_t rel, bool bidirectional, int num_buckets, int max_dist
 // C = A W^T + b (+ the epilogue activation act: kActNone / kActGelu / kActRelu, decode_types.cuh) on the tensor cores:
 // gemm_mode 3 / 5 = 3xFP16 (one CTA per tile / clusters of 2 sharing W), 6 = 3xBF16 (bf16 weights), 2 = 3xTF32 (fp32
 // range: the fallback when an activation leaves the fp16 range).  Operands arrive pre-split from the producing kernel
-// (A.h1/A.h2, A.b1/A.b2/A.b3 or A.hi/A.lo); they are split here only if the producer did not.
+// (A.p); they are split here only if the producer did not.
 // defer_rows: a split-K result of at most this many rows may be left unsummed in cx.pending for the kernel that consumes
 // C (plain fp32 C of a biased GEMM without activation only); 0: the GEMM finishes it itself.
 void gemm(Ctx& cx, int64_t M, int N, int K, const Act& A, int lda, Lin& l, const Act& C, int ldc, int act, int64_t defer_rows = 0);

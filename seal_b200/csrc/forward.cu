@@ -22,18 +22,19 @@ SplitSrc take_pending(Ctx& cx) {
     return ps;
 }
 
-SplitOut split_of(const Act& a, int* overflow) {
-    SplitOut so;
-    if (a.hi) { so.a = a.hi; so.b = a.lo; so.kind = 1; }
-    else if (a.h1) { so.a = a.h1; so.b = a.h2; so.kind = 2; so.overflow = overflow; }
-    return so;
+// The split a producer of activation a writes in format T (bart_kernels.cuh): SplitOut kind 1 / 2 for 3xTF32 / 3xFP16
+// (kind 0 if a has no split), SplitBf16 for 3xBF16
+template <typename T> auto producer_split(const Act& a, int* overflow) {
+    if constexpr (std::is_same<T, __nv_bfloat16>::value) return SplitBf16{a.piece<T>(0), a.piece<T>(1), a.piece<T>(2)};
+    else if (!a.p[0]) return SplitOut{};
+    else if constexpr (std::is_same<T, float>::value) return SplitOut{a.p[0], a.p[1], 1};
+    else return SplitOut{a.p[0], a.p[1], 2, overflow};
 }
 
-// f(so) with the split output a producer of activation a writes: SplitBf16 in gemm_mode 6, SplitOut (split_of)
-// otherwise.  The producer kernels are instantiated per split type, so f launches kernel<decltype(so)>.
+// f(so) with the split a producer of activation a writes in m's gemm_mode.  The producer kernels are instantiated per
+// split type, so f launches kernel<decltype(so)>.
 template <typename F> void with_split(const sealbart* m, const Act& a, F&& f) {
-    if (bf16_weights(m)) f(SplitBf16{a.b1, a.b2, a.b3});
-    else f(split_of(a, m->ovf));
+    with_format(m->cfg.gemm_mode, [&](auto t) { f(producer_split<decltype(t)>(a, m->ovf)); });
 }
 // the embedding table a producer with split type SO gathers from
 template <class SO> const EmbT<SO>* embed_table(const sealbart* m) {
@@ -41,15 +42,11 @@ template <class SO> const EmbT<SO>* embed_table(const sealbart* m) {
     else return m->shared;
 }
 
-// Buffers hi / lo (and plain, if not null) as an Act from element off on: the TF32 split in gemm_mode 2, the fp16
-// split in the 3xFP16 modes, the three bf16 pieces in gemm_mode 6 (b1 and b3 in the two halves of hi -- every split
-// buffer holds 4 bytes per element -- b2 in lo).  plain is null for activations whose producers write the split only.
-Act act_view(int gemm_mode, float* plain, const Buf& hi, const Buf& lo, int64_t off = 0) {
+// Split buffer b (and plain, if not null) as an Act in gemm_mode's format from element off on (split_view).  plain is
+// null for activations whose producers write the split only.
+Act act_view(int gemm_mode, float* plain, const Buf& b, int64_t off = 0) {
     Act a;
-    if (plain) a.x = plain + off;
-    if (gemm_mode == kGemmTf32) { a.hi = hi.as<float>() + off; a.lo = lo.as<float>() + off; }
-    else if (gemm_mode == kGemmBf16) { a.b1 = hi.as<__nv_bfloat16>() + off; a.b2 = lo.as<__nv_bfloat16>() + off; a.b3 = hi.as<__nv_bfloat16>() + hi.bytes / 4 + off; }
-    else if (is_3xfp16(gemm_mode)) { a.h1 = hi.as<__half>() + off; a.h2 = lo.as<__half>() + off; }
+    with_format(gemm_mode, [&](auto t) { a = split_view<decltype(t)>(plain, b, off); });
     return a;
 }
 
@@ -486,11 +483,11 @@ void encoder_forward(Ctx& cx, const Dims& D, const int64_t* ids_d, const int64_t
     const int64_t Te = rows_enc;                    // encoder rows actually computed
     const int gm = m->cfg.gemm_mode;
     Acts A;
-    A.x = act_view(gm, m->ex.as<float>(), m->ex_hi, m->ex_lo);
+    A.x = act_view(gm, m->ex.as<float>(), m->ex_split);
     A.qkv = Act{m->eqkv.as<float>()};
-    A.attn = act_view(gm, nullptr, m->eattn_hi, m->eattn_lo);
+    A.attn = act_view(gm, nullptr, m->eattn_split);
     A.tmp = Act{m->etmp.as<float>()};
-    A.ffn = act_view(gm, nullptr, m->effn_hi, m->effn_lo);
+    A.ffn = act_view(gm, nullptr, m->effn_split);
     A.ffn2 = m->effn2.as<float>();
     if (m->arch == 1) t5_encoder_layers(cx, D, Te, A, tok, m32, soff);
     else if (m->arch == 2) preln_encoder_layers(cx, D, Te, A, tok, pos, m32, soff);
@@ -513,12 +510,12 @@ void decoder_step(Ctx& cx, const Dims& D, const int32_t* tokens, int cur_len, co
     if (compact && (cur_len != 1 || D.grp_start || D.Qb)) throw ApiError(SEALFM_EINVAL, "internal: compact step only at position 0 of a generate");
     const int d = D.d, gm = m->cfg.gemm_mode;
     DecStep S;
-    S.x = act_view(gm, m->dx.as<float>(), m->dx_hi, m->dx_lo, D.r0 * d);
+    S.x = act_view(gm, m->dx.as<float>(), m->dx_split, D.r0 * d);
     S.qkv = Act{m->dqkv.as<float>() + D.r0 * 3 * d};
-    S.attn = act_view(gm, nullptr, m->dattn_hi, m->dattn_lo, D.r0 * d);
+    S.attn = act_view(gm, nullptr, m->dattn_split, D.r0 * d);
     S.tmp = Act{m->dtmp.as<float>() + D.r0 * d};
     S.cq = Act{m->dcq.as<float>() + D.r0 * d};
-    S.ffn = act_view(gm, nullptr, m->dffn_hi, m->dffn_lo, D.r0 * D.f);
+    S.ffn = act_view(gm, nullptr, m->dffn_split, D.r0 * D.f);
     S.ffn2 = m->dffn2.as<float>() ? m->dffn2.as<float>() + D.r0 * 2 * D.f : nullptr;
     S.R = compact ? D.Q : D.R; S.row_mul = compact ? D.B : 1; S.compact = compact;
     S.Rc = D.Rb ? D.Rb : D.R; S.pos = cur_len - 1; S.tokens = tokens; S.anc = anc;
@@ -617,7 +614,7 @@ int sealdec_debug_attention(const sealdec_attn_case_t* c, float* out, void* spli
         } else if (!enc && !(self ? c->qkv : c->q)) throw bad(self ? "qkv missing" : "q missing");
         require_device();
 
-        Buf d_in, d_ckv, d_kc, d_vc, d_anc, d_mask, d_off, d_gq, d_gs, d_part, d_pb, d_rel, d_bkt, d_out, d_s1, d_s2, d_s3, d_ovf;
+        Buf d_in, d_ckv, d_kc, d_vc, d_anc, d_mask, d_off, d_gq, d_gs, d_part, d_pb, d_rel, d_bkt, d_out, d_split, d_ovf;
         auto up = [&](Buf& b, const void* h, size_t bytes) { b.ensure(bytes); CUDA_CHECK(cudaMemcpy(b.p, h, bytes, cudaMemcpyHostToDevice)); };
         auto nan = [&](Buf& b, size_t bytes) { b.ensure(bytes); CUDA_CHECK(cudaMemset(b.p, 0xFF, bytes)); };
         const size_t in_bytes = (size_t)rows * cols * 4;
@@ -647,10 +644,9 @@ int sealdec_debug_attention(const sealdec_attn_case_t* c, float* out, void* spli
             up(d_bkt, bkt.data(), bkt.size() * 4); up(d_rel, c->rel_bias, (size_t)c->num_buckets * heads * 4);
             rb = RelBias{d_rel.as<float>(), d_bkt.as<int32_t>(), off, heads};
         }
-        const size_t out_n = (size_t)rows * d, piece = c->out_split == 1 ? 4 : 2;
+        const size_t out_n = (size_t)rows * d;
         nan(d_out, out_n * 4);
-        if (c->out_split) { nan(d_s1, out_n * piece); nan(d_s2, out_n * piece); }
-        if (c->out_split == 3) nan(d_s3, out_n * piece);
+        if (c->out_split) nan(d_split, out_n * 8);
         d_ovf.ensure(4); CUDA_CHECK(cudaMemset(d_ovf.p, 0, 4));
         SplitSrc src{};
         if (c->split_ks > 1) src = SplitSrc{d_part.as<float>(), c->split_ks, (int64_t)rows * cols, d_pb.as<float>(), c->split_unscale};
@@ -669,16 +665,25 @@ int sealdec_debug_attention(const sealdec_attn_case_t* c, float* out, void* spli
                                   c->G ? d_gq.as<int32_t>() : nullptr, c->G ? d_gs.as<int32_t>() : nullptr, d_out.as<float>(), soff};
             return launch_cross_attn(nullptr, a, so, src);
         };
-        uint32_t bit;
-        if (c->out_split == 3) bit = run(SplitBf16{d_s1.as<__nv_bfloat16>(), d_s2.as<__nv_bfloat16>(), d_s3.as<__nv_bfloat16>()});
-        else bit = run(SplitOut{d_s1.p, d_s2.p, c->out_split, c->out_split == 2 ? d_ovf.as<int>() : nullptr});
+        // out_split 1 / 2 / 3: the split of gemm_mode 2 / 3 / 6, laid out as the model's split buffers (split_view)
+        uint32_t bit = 0;
+        Act split;
+        size_t elem = 0;
+        if (c->out_split)
+            with_format(c->out_split == 1 ? kGemmTf32 : c->out_split == 2 ? kGemmFp16 : kGemmBf16, [&](auto t) {
+                using T = decltype(t);
+                split = split_view<T>(nullptr, d_split); elem = sizeof(T);
+                bit = run(producer_split<T>(split, d_ovf.as<int>()));
+            });
+        else bit = run(SplitOut{});
         CUDA_CHECK(cudaDeviceSynchronize());
-        auto down = [&](void* h, const Buf& b, size_t bytes) { CUDA_CHECK(cudaMemcpy(h, b.p, bytes, cudaMemcpyDeviceToHost)); };
-        down(out, d_out, out_n * 4);
-        if (c->out_split) { down(split1, d_s1, out_n * piece); down(split2, d_s2, out_n * piece); }
-        if (c->out_split == 3) down(split3, d_s3, out_n * piece);
-        if (overflow) down(overflow, d_ovf, 4);
-        if (self) { down(kc_out, d_kc, cache_bytes); down(vc_out, d_vc, cache_bytes); }
+        auto down = [&](void* h, const void* d, size_t bytes) { CUDA_CHECK(cudaMemcpy(h, d, bytes, cudaMemcpyDeviceToHost)); };
+        down(out, d_out.p, out_n * 4);
+        void* const split_out[3] = {split1, split2, split3};
+        for (int i = 0; i < 3; ++i)
+            if (split.p[i]) down(split_out[i], split.p[i], out_n * elem);
+        if (overflow) down(overflow, d_ovf.p, 4);
+        if (self) { down(kc_out, d_kc.p, cache_bytes); down(vc_out, d_vc.p, cache_bytes); }
         *path = bit;
     });
 }

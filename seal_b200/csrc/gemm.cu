@@ -9,7 +9,6 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
-#include <iterator>
 #include <type_traits>
 #include <vector>
 
@@ -45,11 +44,11 @@ template <typename T> void make_map(CUtensorMap* map, const T* ptr, uint64_t row
     if (r != CUDA_SUCCESS) throw ApiError(SEALFM_ECUDA, "cuTensorMapEncodeTiled failed (" + std::to_string((int)r) + ")");
 }
 
-void split_into(cudaStream_t s, const float* x, float* hi, float* lo, uint64_t numel) {
-    const int64_t n4 = (int64_t)(numel / 4);
-    const int blocks = (int)std::min<int64_t>((n4 + 255) / 256, (int64_t)sm_count() * 8);
-    split_tf32_kernel<<<std::max(blocks, 1), 256, 0, s>>>(n4, reinterpret_cast<const float4*>(x), reinterpret_cast<float4*>(hi),
-                                                          reinterpret_cast<float4*>(lo));
+// the n values of x times scale split into format T's pieces p0, p1 (, p2) on stream s; 3xFP16 raises *ovf for a value
+// past the fp16 range
+template <typename T> void split_into(cudaStream_t s, const float* x, float scale, int64_t n, T* p0, T* p1, T* p2, int* ovf) {
+    const int blocks = (int)std::min<int64_t>((n + 255) / 256, (int64_t)sm_count() * 8);
+    split_kernel<T><<<std::max(blocks, 1), 256, 0, s>>>(n, x, scale, p0, p1, p2, ovf);
     CUDA_CHECK(cudaGetLastError());
 }
 
@@ -100,83 +99,57 @@ int band_tiles(const sealbart* m, int n_fastest, int64_t M, int K, int a_bytes) 
     return m->gemm_band >= 0 ? m->gemm_band : band;
 }
 
-// The x3 GEMM's operand formats, by element type T: the Act fields of A's pieces (C's split outputs use the same
-// fields), the Lin fields of W's pieces, whether the epilogue unscales W by l.w_unscale, whether split-K, L2 bands and
-// the lm_head statistics epilogue apply (tuned), and the last_paths bits of every call and of the whole-tile launch.
-// 3xBF16's W is one piece; its kernel reads A's third piece in the W lo slot.
-template <typename T> using ActField = T* Act::*;
+// The x3 GEMM's operand formats, by element type T: the Lin fields of W's pieces, whether the epilogue unscales W by
+// l.w_unscale, whether split-K, L2 bands and the lm_head statistics epilogue apply (tuned), and the last_paths bits of
+// every call and of the whole-tile launch.  3xBF16's W is one piece; its kernel reads A's third piece in the W lo slot.
 template <typename T> using LinField = T* Lin::*;
 template <typename T> struct X3Format;
 template <> struct X3Format<__half> {                 // 3xFP16 (modes 3, 5): A = h1 + h2, W * 2^s = w_h1 + w_h2
-    static constexpr ActField<__half> piece[] = {&Act::h1, &Act::h2};
     static constexpr LinField<__half> w = &Lin::w_h1, w2 = &Lin::w_h2;
     static constexpr bool scaled_w = true, tuned = true;
     static constexpr uint32_t path_call = 0, path_tile = kPathGemmFullTile;
 };
 template <> struct X3Format<__nv_bfloat16> {          // 3xBF16 (mode 6): A = b1 + b2 + b3, W once in bf16
-    static constexpr ActField<__nv_bfloat16> piece[] = {&Act::b1, &Act::b2, &Act::b3};
     static constexpr LinField<__nv_bfloat16> w = &Lin::w_bf;
     static constexpr bool scaled_w = false, tuned = true;
     static constexpr uint32_t path_call = kPathGemmBf16, path_tile = 0;
 };
 template <> struct X3Format<float> {                  // 3xTF32 (mode 2): A = hi + lo, W = w_hi + w_lo; band 0, gemm_band ignored
-    static constexpr ActField<float> piece[] = {&Act::hi, &Act::lo};
     static constexpr LinField<float> w = &Lin::w_hi, w2 = &Lin::w_lo;
     static constexpr bool scaled_w = false, tuned = false;    // unscaled: after an overflow fallback l.w_unscale is 3xFP16's
     static constexpr uint32_t path_call = 0, path_tile = kPathGemmTf32;
 };
 
-// f(T()) with the element type T of gemm_mode's operand format
-template <typename F> void with_format(int mode, F&& f) {
-    if (mode == kGemmBf16) f(__nv_bfloat16());
-    else if (is_3xfp16(mode)) f(__half());
-    else f(0.f);
-}
-
-// x (n fp32 values) split into format T's pieces in hi / lo (grown to fit) on stream s, in act_view's layout but with
-// bf16's third piece n elements into hi.  3xFP16 raises *ovf for a value past the fp16 range.
-template <typename T> Act split_act(cudaStream_t s, float* x, int64_t n, Buf& hi, Buf& lo, int* ovf) {
-    Act a{x};
-    const int blocks = (int)std::min<int64_t>((n + 255) / 256, (int64_t)sm_count() * 8);
-    if constexpr (std::is_same<T, __nv_bfloat16>::value) {
-        hi.ensure((size_t)n * 4); lo.ensure((size_t)n * 2);
-        a.b1 = hi.as<T>(); a.b2 = lo.as<T>(); a.b3 = a.b1 + n;
-        split_bf16x3_kernel<<<blocks, 256, 0, s>>>(n, x, a.b1, a.b2, a.b3);
-    } else if constexpr (std::is_same<T, __half>::value) {
-        hi.ensure((size_t)n * 2); lo.ensure((size_t)n * 2);
-        a.h1 = hi.as<T>(); a.h2 = lo.as<T>();
-        split_half_kernel<<<blocks, 256, 0, s>>>(n, x, 1.0f, a.h1, a.h2, ovf);
-    } else {
-        hi.ensure((size_t)n * 4); lo.ensure((size_t)n * 4);
-        a.hi = hi.as<T>(); a.lo = lo.as<T>();
-        split_into(s, x, a.hi, a.lo, (uint64_t)n);
-    }
-    CUDA_CHECK(cudaGetLastError());
+// x (n fp32 values) split into format T's pieces in buf, grown to 8 bytes per element and viewed as split_view.
+// 3xFP16 raises *ovf for a value past the fp16 range.
+template <typename T> Act split_act(cudaStream_t s, float* x, int64_t n, Buf& buf, int* ovf) {
+    buf.ensure((size_t)n * 8);
+    const Act a = split_view<T>(x, buf);
+    split_into(s, x, 1.0f, n, a.piece<T>(0), a.piece<T>(1), a.piece<T>(2), ovf);
     return a;
 }
 
 template <typename T>
 void gemm_x3(Ctx& cx, int64_t M, int N, int K, const Act& A, Lin& l, const Act& C, int ldc, int act, int64_t defer_rows) {
     using F = X3Format<T>;
-    constexpr int pieces = (int)std::size(F::piece);
+    constexpr int pieces = kPieces<T>;
     sealbart* m = cx.m;
     const int tiles = (int)(((N + GN - 1) / GN) * ((M + GM - 1) / GM));
     const int n_fastest = ((int64_t)M >= (int64_t)N) ? 1 : 0;     // stream the larger operand once
     Act a = A;
-    if (!(a.*F::piece[0])) {
-        a = split_act<T>(cx.s, A.x, M * K, cx.slice ? m->a_hi1 : m->a_hi, cx.slice ? m->a_lo1 : m->a_lo, m->ovf);
+    if (!a.p[0]) {
+        a = split_act<T>(cx.s, A.x, M * K, cx.slice ? m->a_split1 : m->a_split, m->ovf);
         m->launches++;
     }
     CUtensorMap ma[3];
-    for (int i = 0; i < pieces; ++i) make_map(&ma[i], a.*F::piece[i], M, K, K, GM);
+    for (int i = 0; i < pieces; ++i) make_map(&ma[i], a.piece<T>(i), M, K, K, GM);
     if (!l.maps_ready) {
         make_map(&l.map_hi, l.*F::w, N, K, K, GN);
         if constexpr (pieces == 2) make_map(&l.map_lo, l.*F::w2, N, K, K, GN);
         l.maps_ready = true;
     }
     const CUtensorMap& w_lo = pieces == 3 ? ma[2] : l.map_lo;
-    T* const c1 = C.*F::piece[0]; T* const c2 = C.*F::piece[1]; T* c3 = nullptr;
-    if constexpr (pieces == 3) c3 = C.*F::piece[2];
+    T* const c1 = C.piece<T>(0); T* const c2 = C.piece<T>(1); T* const c3 = C.piece<T>(2);
     const float unscale = F::scaled_w ? l.w_unscale : 1.0f;
     m->last_paths |= F::path_call;
     const int k_slices = F::tuned ? split_k_slices(tiles, K / UK16) : 1;
@@ -203,7 +176,7 @@ void gemm_x3(Ctx& cx, int64_t M, int N, int K, const Act& A, Lin& l, const Act& 
             gemm_launch<T, kActNone, 1>(cx.s, ctas2, ma[0], ma[1], l.map_hi, w_lo, M, N, K, nullptr, 1.0f, part, nullptr, nullptr, ldc, n_fastest, 0,
                                         m->ovf, k_slices, slice_stride);
             m->launches++;
-            if (M <= defer_rows && act == kActNone && !C.hi && !C.h1 && !C.b1 && ldc == N && l.b) {     // C has no split output: summed by the consumer kernel
+            if (M <= defer_rows && act == kActNone && !C.p[0] && ldc == N && l.b) {     // C has no split output: summed by the consumer kernel
                 cx.pending = SplitSrc{part, k_slices, slice_stride, l.b, unscale};
                 m->last_paths |= kPathSplitKDeferred;
                 return;
@@ -248,7 +221,7 @@ void split_lin_tf32(sealbart* m, Lin& l) {
     const uint64_t n = (uint64_t)l.out * l.in;
     CUDA_CHECK(cudaMalloc(&l.w_hi, n * 4)); m->split_allocs.push_back(l.w_hi);
     CUDA_CHECK(cudaMalloc(&l.w_lo, n * 4)); m->split_allocs.push_back(l.w_lo);
-    split_into(nullptr, l.w, l.w_hi, l.w_lo, n);
+    split_into<float>(nullptr, l.w, 1.0f, (int64_t)n, l.w_hi, l.w_lo, nullptr, nullptr);
     m->weight_bytes += 2 * n * 4;
 }
 
@@ -267,8 +240,7 @@ void split_lin_half(sealbart* m, Lin& l, unsigned int* d_max) {
     CUDA_CHECK(cudaMalloc(&l.w_h1, n * 2)); m->split_allocs.push_back(l.w_h1);
     CUDA_CHECK(cudaMalloc(&l.w_h2, n * 2)); m->split_allocs.push_back(l.w_h2);
     m->weight_bytes += 2 * n * 2;
-    split_half_kernel<<<sm_count() * 8, 256>>>((int64_t)n, l.w, std::ldexp(1.0f, sexp), l.w_h1, l.w_h2, m->err.as<int>() + 1);
-    CUDA_CHECK(cudaGetLastError());
+    split_into<__half>(nullptr, l.w, std::ldexp(1.0f, sexp), (int64_t)n, l.w_h1, l.w_h2, nullptr, m->err.as<int>() + 1);
     l.maps_ready = false;
 }
 
@@ -400,15 +372,14 @@ int debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A, const 
         Buf d_max; d_max.ensure(4);
         derive_lin(&fake, l, d_max.as<unsigned int>());
         fake.gemm_band = band;
-        Buf dA, dC, ah1, ah2;
+        Buf dA, dC, dA_split, dC_split;
         const int ldc = (N + 3) / 4 * 4;
         dA.ensure((size_t)M * K * 4); dC.ensure((size_t)M * ldc * 4);
         CUDA_CHECK(cudaMemcpy(dA.p, A, (size_t)M * K * 4, cudaMemcpyHostToDevice));
         Act a{dA.as<float>()};
         if (presplit && mode != kGemmTf32)
-            with_format(mode, [&](auto t) { a = split_act<decltype(t)>(nullptr, a.x, M * K, ah1, ah2, fake.ovf); });
+            with_format(mode, [&](auto t) { a = split_act<decltype(t)>(nullptr, a.x, M * K, dA_split, fake.ovf); });
         Act c{store ? dC.as<float>() : nullptr};
-        Buf ds[3];
         size_t elem = 4;
         if (so) {
             // only the epilogue's flag is reported: clear what the input split raised.  Every output starts poisoned
@@ -416,16 +387,11 @@ int debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A, const 
             CUDA_CHECK(cudaDeviceSynchronize());
             CUDA_CHECK(cudaMemset(fake.ovf, 0, sizeof(int)));
             CUDA_CHECK(cudaMemset(dC.p, 0xFF, (size_t)M * ldc * 4));
-            if (so->split)
-                with_format(mode, [&](auto t) {
-                    using T = decltype(t);
-                    elem = sizeof(T);
-                    for (int i = 0; i < (int)std::size(X3Format<T>::piece); ++i) {
-                        ds[i].ensure((size_t)M * ldc * elem);
-                        CUDA_CHECK(cudaMemset(ds[i].p, 0xFF, (size_t)M * ldc * elem));
-                        c.*X3Format<T>::piece[i] = ds[i].as<T>();
-                    }
-                });
+            if (so->split) {
+                dC_split.ensure((size_t)M * ldc * 8);
+                CUDA_CHECK(cudaMemset(dC_split.p, 0xFF, (size_t)M * ldc * 8));
+                with_format(mode, [&](auto t) { c = split_view<decltype(t)>(c.x, dC_split); elem = sizeof(t); });
+            }
         }
         Ctx cx{&fake, nullptr};
         Buf dmask, dstats;
@@ -453,7 +419,7 @@ int debug_gemm(int mode, int64_t M, int32_t N, int32_t K, const float* A, const 
                 *so->unscale = p.unscale;
             }
             for (int i = 0; i < 3; ++i)
-                if (ds[i].p) CUDA_CHECK(cudaMemcpy2D(so->s[i], (size_t)N * elem, ds[i].p, (size_t)ldc * elem, (size_t)N * elem, M, cudaMemcpyDeviceToHost));
+                if (c.p[i]) CUDA_CHECK(cudaMemcpy2D(so->s[i], (size_t)N * elem, c.p[i], (size_t)ldc * elem, (size_t)N * elem, M, cudaMemcpyDeviceToHost));
         }
         if (head) {
             *head->fused = cx.head_fused ? 1 : 0;

@@ -289,14 +289,8 @@ void ensure_workspace(sealbart* m, const Dims& D) {
     m->st_thr.ensure((size_t)D.R * 3 * 4);
     m->st_cval.ensure((size_t)D.R * 2 * D.B * 4); m->st_cidx.ensure((size_t)D.R * 2 * D.B * 4); m->st_ccnt.ensure(D.R * 4);
     if (m->arch == 1 && m->t5.ffn_kind == 1) { m->effn2.ensure(Tk * 2 * D.f * 4); m->dffn2.ensure(D.R * 2 * D.f * 4); }
-    {
-        m->ex_hi.ensure(Tk * D.d * 4); m->ex_lo.ensure(Tk * D.d * 4);
-        m->eattn_hi.ensure(Tk * D.d * 4); m->eattn_lo.ensure(Tk * D.d * 4);
-        m->effn_hi.ensure(Tk * D.f * 4); m->effn_lo.ensure(Tk * D.f * 4);
-        m->dx_hi.ensure(D.R * D.d * 4); m->dx_lo.ensure(D.R * D.d * 4);
-        m->dattn_hi.ensure(D.R * D.d * 4); m->dattn_lo.ensure(D.R * D.d * 4);
-        m->dffn_hi.ensure(D.R * D.f * 4); m->dffn_lo.ensure(D.R * D.f * 4);
-    }
+    m->ex_split.ensure(Tk * D.d * 8); m->eattn_split.ensure(Tk * D.d * 8); m->effn_split.ensure(Tk * D.f * 8);
+    m->dx_split.ensure(D.R * D.d * 8); m->dattn_split.ensure(D.R * D.d * 8); m->dffn_split.ensure(D.R * D.f * 8);
     m->err.ensure(16);
 }
 

@@ -3,7 +3,7 @@
 // computed on the tensor cores as an error-compensated 3-pass product
 //   A*W ~= A_lo*W_hi + A_hi*W_lo + A_hi*W_hi,
 // which keeps the fp32-level accuracy the 1e-4 beam-score parity needs (a single TF32/FP16 pass does not).
-// Two operand splits:
+// Three operand splits (operand_split.cuh):
 //   3xFP16 (gemm_mode 3 / 5): x = h1 + h2, h1 = rn_half(x), h2 = rn_half(x - h1).  fp16 products are exact in the
 //     fp32 accumulator, so the accuracy class is that of 3xTF32 at half the operand bytes and twice the tensor rate --
 //     for activations of magnitude at least 2^-3.  Activations are used unscaled (|x| must stay below 65504; the
@@ -16,7 +16,7 @@
 //     multiplies the accumulator by 2^-s (exact).
 //   3xTF32 (gemm_mode 2, fp32 range): hi = x with the 13 low mantissa bits cleared, lo = x - hi (exact).
 //   3xBF16 (gemm_mode 6, bf16 weights): W is stored once in bf16 (exact for a bf16 checkpoint), A = b1 + b2 + b3 in
-//     bf16 pieces (SplitBf16, bart_kernels.cuh; exact for 2^-100 <= |a| < (2 - 2^-8) 2^127) and A*W = b3*W + b2*W + b1*W.  Each
+//     bf16 pieces (exact for 2^-100 <= |a| < (2 - 2^-8) 2^127) and A*W = b3*W + b2*W + b1*W.  Each
 //     product has 8 x 8 significant bits, exact in the fp32 accumulator, so the only error is the accumulation's --
 //     at any magnitude in fp32's range, with no absolute floor and no overflow flag.  The stage holds A b1, A b2, W and
 //     A b3 in the four 16 KB slots the other modes use for A hi / lo and W hi / lo.
@@ -36,9 +36,9 @@
 #include <cstdint>
 #include <type_traits>
 
-#include "bart_kernels.cuh"
 #include "decode_types.cuh"
 #include "launch.cuh"
+#include "operand_split.cuh"
 
 namespace sealb200 {
 
@@ -168,46 +168,17 @@ template <int ACT> __device__ __forceinline__ float epi_act(float x) {
     return ACT == kActGelu ? gelu_erf_u(x) : ACT == kActRelu ? (x < 0.f ? 0.f : x) : x;
 }
 
-// x -> (hi, lo): hi keeps the TF32 bits (sign, exponent, 10 mantissa bits), lo = x - hi exactly.
-__global__ void __launch_bounds__(256) split_tf32_kernel(int64_t n4, const float4* __restrict__ x, float4* __restrict__ hi,
-                                                         float4* __restrict__ lo) {
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
-        const float4 v = x[i];
-        float4 h, l;
-        h.x = __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u); l.x = v.x - h.x;
-        h.y = __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u); l.y = v.y - h.y;
-        h.z = __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u); l.z = v.z - h.z;
-        h.w = __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u); l.w = v.w - h.w;
-        hi[i] = h; lo[i] = l;
-    }
-}
-
-constexpr float kHalfMax = 65504.f;
-
-__device__ __forceinline__ void split_half(float x, __half& h1, __half& h2, int* overflow) {
-    if (fabsf(x) > kHalfMax) { if (overflow) *overflow = 1; x = copysignf(kHalfMax, x); }
-    h1 = __float2half_rn(x);
-    h2 = __float2half_rn(x - __half2float(h1));
-}
-
-// x * scale -> (h1, h2) halves; used for weights (once) and for activations whose producer did not split
-__global__ void __launch_bounds__(256) split_half_kernel(int64_t n, const float* __restrict__ x, float scale,
-                                                         __half* __restrict__ h1, __half* __restrict__ h2,
-                                                         int* __restrict__ overflow) {
+// x * scale -> format T's pieces p0, p1 (, p2), for weights (once) and for activations whose producer did not split;
+// a value the fp16 split saturated raises *overflow
+template <typename T>
+__global__ void __launch_bounds__(256) split_kernel(int64_t n, const float* __restrict__ x, float scale, T* __restrict__ p0,
+                                                    T* __restrict__ p1, T* __restrict__ p2, int* __restrict__ overflow) {
+    T* const s[3] = {p0, p1, p2};
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-        __half a, b;
         int ov = 0;
-        split_half(x[i] * scale, a, b, &ov);
+        store_split<T, 1>(s, i, {x[i] * scale}, ov);
         if (ov) atomicExch(overflow, 1);
-        h1[i] = a; h2[i] = b;
     }
-}
-
-// x -> the three bf16 pieces of the 3xBF16 GEMM (bf16x3_split1); for activations whose producer did not split
-__global__ void __launch_bounds__(256) split_bf16x3_kernel(int64_t n, const float* __restrict__ x, __nv_bfloat16* __restrict__ b1,
-                                                           __nv_bfloat16* __restrict__ b2, __nv_bfloat16* __restrict__ b3) {
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
-        bf16x3_split1(x[i], b1[i], b2[i], b3[i]);
 }
 
 __global__ void __launch_bounds__(256) absmax_kernel(int64_t n, const float* __restrict__ x, unsigned int* __restrict__ out) {
@@ -245,51 +216,17 @@ __device__ __forceinline__ void unit_trace(bool on, int unit, int e) {
 #endif
 }
 
-// Epilogue store of two adjacent columns (n, n + 1) of one row: fp32 and/or the operand split of the next GEMM.
-// kFull: the caller knows both columns are below N (a tile inside the matrix), so neither is checked.
-template <bool kFull>
-__device__ __forceinline__ void store_pair(float* C, __half* S1, __half* S2, int64_t off, int n, int N, float v0, float v1, int& ov) {
+// Epilogue store of two adjacent columns (n, n + 1) of one row: fp32 to C and/or format T's split of the next GEMM's
+// operand to S (S[0] == nullptr: none).  kFull: the caller knows both columns are below N (a tile inside the matrix),
+// so neither is checked.
+template <bool kFull, typename T>
+__device__ __forceinline__ void store_pair(float* C, T* const* S, int64_t off, int n, int N, float v0, float v1, int& ov) {
     if (kFull || n + 1 < N) {
         if (C) *reinterpret_cast<float2*>(C + off) = make_float2(v0, v1);
-        if (S1) {
-            __half a0, b0, a1, b1;
-            split_half(v0, a0, b0, &ov); split_half(v1, a1, b1, &ov);
-            *reinterpret_cast<__half2*>(S1 + off) = __halves2half2(a0, a1);
-            *reinterpret_cast<__half2*>(S2 + off) = __halves2half2(b0, b1);
-        }
+        if (S[0]) store_split<T, 2>(S, off, {v0, v1}, ov);
     } else if (n < N) {
         if (C) C[off] = v0;
-        if (S1) { __half a, b; split_half(v0, a, b, &ov); S1[off] = a; S2[off] = b; }
-    }
-}
-template <bool kFull>
-__device__ __forceinline__ void store_pair(float* C, float* S1, float* S2, int64_t off, int n, int N, float v0, float v1, int&) {
-    const float h0 = __uint_as_float(__float_as_uint(v0) & 0xFFFFE000u), h1 = __uint_as_float(__float_as_uint(v1) & 0xFFFFE000u);
-    if (kFull || n + 1 < N) {
-        if (C) *reinterpret_cast<float2*>(C + off) = make_float2(v0, v1);
-        if (S1) { *reinterpret_cast<float2*>(S1 + off) = make_float2(h0, h1); *reinterpret_cast<float2*>(S2 + off) = make_float2(v0 - h0, v1 - h1); }
-    } else if (n < N) {
-        if (C) C[off] = v0;
-        if (S1) { S1[off] = h0; S2[off] = v0 - h0; }
-    }
-}
-
-// The 3xBF16 form: fp32 and/or the three bf16 pieces of the next GEMM's operand (no saturation, no flag)
-template <bool kFull>
-__device__ __forceinline__ void store_pair3(float* C, __nv_bfloat16* S1, __nv_bfloat16* S2, __nv_bfloat16* S3, int64_t off, int n, int N,
-                                            float v0, float v1) {
-    if (kFull || n + 1 < N) {
-        if (C) *reinterpret_cast<float2*>(C + off) = make_float2(v0, v1);
-        if (S1) {
-            __nv_bfloat16 p0[3], p1[3];
-            bf16x3_split1(v0, p0[0], p0[1], p0[2]); bf16x3_split1(v1, p1[0], p1[1], p1[2]);
-            *reinterpret_cast<uint32_t*>(S1 + off) = bf16_pack(p0[0], p1[0]);
-            *reinterpret_cast<uint32_t*>(S2 + off) = bf16_pack(p0[1], p1[1]);
-            *reinterpret_cast<uint32_t*>(S3 + off) = bf16_pack(p0[2], p1[2]);
-        }
-    } else if (n < N) {
-        if (C) C[off] = v0;
-        if (S1) bf16x3_split1(v0, S1[off], S2[off], S3[off]);
+        if (S[0]) store_split<T, 1>(S, off, {v0}, ov);
     }
 }
 
@@ -486,6 +423,7 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
             const int row0 = (mg * CL + (int)rank) * GM + (wg - 1) * 64 + warp * 16 + (lane >> 2);
             const int col0 = n_tile * GN + 2 * (lane & 3);
             float* Cs = C ? C + (int64_t)(u % k_slices) * slice_stride : nullptr;
+            T* const S[3] = {C_s1, C_s2, C_s3};                             // the split outputs (C_s3: 3xBF16 only)
             const float* const bq = bias_s + 2 * (lane & 3);               // the bias of column col0 + 8 j + e is bq[8 j + e]
             int ov = 0;
             mbar_wait(bias_full, ui & 1);
@@ -550,8 +488,7 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
                             float v[2];
 #pragma unroll
                             for (int e = 0; e < 2; ++e) v[e] = epi_act<ACT>(acc[4 * j + 2 * h + e] * w_unscale + bq[8 * j + e]);
-                            if constexpr (kBf16) store_pair3<kFull>(Cs, C_s1, C_s2, C_s3, (int64_t)row * ldc + n, n, N, v[0], v[1]);
-                            else store_pair<kFull>(Cs, C_s1, C_s2, (int64_t)row * ldc + n, n, N, v[0], v[1], ov);
+                            store_pair<kFull>(Cs, S, (int64_t)row * ldc + n, n, N, v[0], v[1], ov);
                         }
                     }
                 }
@@ -572,8 +509,8 @@ wgmma_gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_co
 }
 
 // Finishes a split-K GEMM: out = act((sum_s part[s]) * w_unscale + bias), slices summed in index order
-// (deterministic), written as fp32 and/or as the split the next GEMM consumes: T = __half (two halves) or __nv_bfloat16
-// (three bf16 pieces, C_h3; no saturation, no flag).
+// (deterministic), written as fp32 and/or as format T's split the next GEMM consumes: T = __half (C_h1, C_h2) or
+// __nv_bfloat16 (C_h1, C_h2, C_h3).
 template <int ACT, typename T = __half>
 __global__ void __launch_bounds__(256) gemm_splitk_finish_kernel(int64_t M, int N, int ldc, int k_slices, int64_t slice_stride,
                                                                  const float* __restrict__ part, const float* __restrict__ bias,
@@ -591,14 +528,14 @@ __global__ void __launch_bounds__(256) gemm_splitk_finish_kernel(int64_t M, int 
             acc.x += p.x; acc.y += p.y; acc.z += p.z; acc.w += p.w;
         }
         float v[4] = {acc.x, acc.y, acc.z, acc.w};
+        T* const S[3] = {C_h1, C_h2, C_h3};
         int ov = 0;
         for (int u = 0; u < 4; ++u) {
             if (n + u >= N) continue;
             float x = v[u] * w_unscale + (bias ? bias[n + u] : 0.f);
             x = epi_act<ACT>(x);
             if (C) C[off + u] = x;
-            if constexpr (std::is_same<T, __nv_bfloat16>::value) { if (C_h1) bf16x3_split1(x, C_h1[off + u], C_h2[off + u], C_h3[off + u]); }
-            else if (C_h1) { __half a, b; split_half(x, a, b, &ov); C_h1[off + u] = a; C_h2[off + u] = b; }
+            if (C_h1) store_split<T, 1>(S, off + u, {x}, ov);
         }
         if (ov) atomicExch(overflow, 1);
     }

@@ -16,7 +16,7 @@ K_T5_MAX_SOURCE, K_MAX_LEN = 1024, 128          # t5_kernels.cuh / decode_kernel
 
 
 def split3(a):
-    """b1, b2, b3 (as float32 tensors) of bf16x3_split1 (bart_kernels.cuh) computed with torch's RNE conversion"""
+    """b1, b2, b3 (as float32 tensors) of the bf16 split_value (operand_split.cuh) computed with torch's RNE conversion"""
     import torch
     b1 = a.to(torch.bfloat16).float()
     r = a - b1

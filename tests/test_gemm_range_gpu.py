@@ -5,7 +5,7 @@ Here every element j of row i is held to the standard dot-product bound
     |C - C64| <= REL * sum_k |a_ik w_jk| + ULP * |C64|                      (3xTF32, gemm_mode 2)
 plus, for the 3xFP16 modes 3 / 5, an absolute floor
     + FLOOR * sum_k |w_jk|
-because activations enter the fp16 split unscaled (wgmma_gemm.cuh, split_half): the low half h2 = rn_half(x - h1)
+because activations enter the fp16 split unscaled (operand_split.cuh, split_value): the low half h2 = rn_half(x - h1)
 has |x - h1| <= 2^-11 |x|, so below |x| ~ 2^-3 it is an fp16 subnormal with an absolute spacing of 2^-24 (below 2^-14
 h1 is too), each such activation carries an error of up to 2^-25 whatever its size, and values below 2^-25 flush to
 zero.  Standard-normal rows have entries on both sides of 2^-3; rows scaled by 2^-6 and less sit entirely below it.

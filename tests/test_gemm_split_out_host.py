@@ -1,11 +1,11 @@
-"""CPU: the exact references of the GEMM's split outputs (wgmma_gemm.cuh) that test_gemm_split_out_gpu.py compares the
+"""CPU: the exact references of the GEMM's split outputs (operand_split.cuh) that test_gemm_split_out_gpu.py compares the
 device with bit for bit, and the C signature of the hook it calls.
 
-  - split_half (3xFP16, gemm_mode 3 / 5): saturate to +-65 504, h1 = rn_half(x), h2 = rn_half(x - h1), numpy's
+  - split_half (3xFP16, gemm_mode 3 / 5, split_value for __half): saturate to +-65 504, h1 = rn_half(x), h2 = rn_half(x - h1), numpy's
     round-to-nearest-even conversion.  h1 + h2 == x wherever the pair can hold x: |x| in [2^-14, 65 504] with at most
     22 significant bits on fp16's 2^-24 grid; elsewhere within the documented error max(2^-23 |x|, 2^-25).  Past the
     range the pair is (+-65 504, 0).
-  - split_tf32 (3xTF32, gemm_mode 2): hi = x with the 13 low mantissa bits cleared, lo = x - hi; hi + lo == x for every
+  - split_tf32 (3xTF32, gemm_mode 2, split_value for float): hi = x with the 13 low mantissa bits cleared, lo = x - hi; hi + lo == x for every
     finite x.
   - 3xBF16 (gemm_mode 6) uses test_bf16_host.split3, whose exactness that module tests.
   - the ctypes signature of sealdec_debug_gemm_split (seal_b200/_lib.py) matches include/sealdec.h argument by
@@ -20,14 +20,14 @@ HALF_MAX = 65504.0
 
 
 def split_half(x):
-    """(h1, h2) float16 arrays of split_half (wgmma_gemm.cuh) for float32 x"""
+    """(h1, h2) float16 arrays of the fp16 split_value (operand_split.cuh) for float32 x"""
     x = np.clip(np.asarray(x, dtype=np.float32), -HALF_MAX, HALF_MAX)
     h1 = x.astype(np.float16)
     return h1, (x - h1.astype(np.float32)).astype(np.float16)
 
 
 def split_tf32(x):
-    """(hi, lo) float32 arrays of store_pair's 3xTF32 split (wgmma_gemm.cuh) for float32 x"""
+    """(hi, lo) float32 arrays of the TF32 split_value (operand_split.cuh) for float32 x"""
     x = np.asarray(x, dtype=np.float32)
     hi = (x.view(np.uint32) & np.uint32(0xFFFFE000)).view(np.float32)
     return hi, x - hi
