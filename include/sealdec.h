@@ -106,12 +106,12 @@ typedef struct {
  * "model.{encoder,decoder}.layer_norm.{weight,bias}"; "model.{encoder,decoder}.layernorm_embedding.*" only with
  * layernorm_embedding = 1.  Every other key is SEALFM_EINVAL.  An unsupported variant or shape is SEALFM_EINVAL before
  * any allocation.  sealbart_create is sealbart_create_ex with {0, 2, 1, SEALBART_ACT_GELU}.
- * Position table: sources longer than max_positions are refused (as for BART), and sealdec_teacher_forced /
- * sealdec_debug_step_logits refuse decoder inputs longer than max_positions.  A generate may reach decoder positions
- * past the table (max_length - 2 >= max_positions); those steps read the table's last row, so the records of a beam
- * that is still alive there are not the model's -- whether such a call may run is the caller's decision
- * (seal_b200.beam_search raises the reference's IndexError exactly where the reference's forward would read past the
- * table). */
+ * Position table (BART's learned table of max_positions + 2 rows too): sources longer than max_positions are refused,
+ * and sealdec_teacher_forced / sealdec_debug_step_logits refuse decoder inputs longer than max_positions.  A generate
+ * may reach decoder positions past the table (max_length - 2 >= max_positions); those steps read the table's last
+ * row, so the records of a beam that is still alive there are not the model's -- whether such a call may run is the
+ * caller's decision (seal_b200.beam_search raises the reference's IndexError exactly where the reference's forward
+ * would read past the table). */
 int  sealbart_create_ex(const sealbart_config_t* cfg, const sealbart_variant_t* variant, int device, sealbart_t** out);
 
 /* ---- T5 weights ------------------------------------------------------------------------------- */
@@ -465,6 +465,48 @@ typedef struct {
 } sealdec_attn_case_t;
 int sealdec_debug_attention(const sealdec_attn_case_t* c, float* out, void* split1, void* split2, void* split3,
                             int32_t* overflow, float* kc_out, float* vc_out, uint32_t* path);
+/* One row-norm or gate producer of the model on caller-supplied rows (sealdec_debug_rownorm), through the same
+ * launchers as the layer loops: the kernels that write every GEMM operand that is not an attention output.  Host
+ * pointers throughout; `rows` rows of width d.
+ *   kind 0 BART embedding + layernorm_embedding: out[r] = LN(embed[tok[r * tok_stride]] * scale
+ *          + pos_table[min(p + 2, pos_rows - 1)]; gamma, beta), p = pos[r] or pos_const (pos NULL).
+ *   kind 1 BART add + LayerNorm: out[r] = LN(a[r] + b[r]; gamma, beta), run in place as the layers run it (out == a);
+ *          a CTA per row up to 2 048 rows, a warp per row above.
+ *   kind 2 T5 RMSNorm: the residual x_out[r] = embed[tok[r * tok_stride]] (tok given) or a[r] + b[r] (a given), and
+ *          the split of (gamma * (x_out * rsqrt(mean(x_out^2) + eps))) * out_scale.
+ *   kind 3 pre-LayerNorm row: the residual x_out[r] = embed[tok] * scale + pos_table[min(p + pos_offset, pos_rows - 1)],
+ *          then LN(.; ln_emb_g, ln_emb_b) if ln_emb_g is given (tok given), or a[r] + b[r] (a given); and the split of
+ *          LN(x_out; gamma, beta).
+ *   kind 4 T5 gated-gelu: h [rows][2d] (d = d_ff) -> the split of gelu_new(h[:, :d]) * h[:, d:].
+ * embed float32 [V][d] (rounded to bf16 as sealbart_set_tensor rounds it for out_split 3), pos_table float32
+ * [pos_rows][d], gamma / beta / ln_emb_g / ln_emb_b float32 [d].  b may be given as split-K slices instead (split_ks in
+ * 2 .. 8): split_part [split_ks][rows][d], element = (sum of slices in index order) * split_unscale + split_bias[col];
+ * only where the kernel sums them (kind 1 up to 2 048 rows, the add forms of kinds 2 and 3).
+ * out_split 0 none (kinds 0, 1 only), 1 TF32 pieces (float32 hi, lo), 2 fp16 halves (h1, h2; overflow raised past
+ * 65504), 3 bf16 x3 (the splits of gemm_mode 2 / 3 / 6).
+ * Outputs, each filled with NaN on the device first: out float32 [rows][d] (the LayerNorm of kinds 0 and 1, the
+ * residual x_out of kinds 2 and 3; not written for kind 4, may be NULL there), split1..3 [rows][d] of the split's
+ * element type, *overflow, *path = the sealbart_get_stat "last_paths" bit(s) of the kernel that ran (0 for kind 0).
+ * The position table is followed on the device by NaN rows up to row 1 026, so a read past its last row shows as NaN.
+ * Arguments the model never passes are SEALFM_EINVAL before any device work: d outside the family's widths (kinds 0,
+ * 1, 3: multiples of 128 up to 1 024; kind 2: also 2 048, 3 072, 4 096; kind 4: multiples of 64 up to 65 536), rows
+ * outside [1, 2^20], split_ks outside 2 .. 8 (0 and 1: no slices), slices where the kernel does not sum them, a token id
+ * outside [0, V), a position outside [0, 1 024], pos_rows outside [pos_offset + 1, 1 026], pos_offset other than 0 or 2
+ * (kind 0 always uses 2), out_split 0 for kinds 2 .. 4, both tok and a (kinds 2, 3), or a missing input or output. */
+typedef struct {
+    int32_t kind, d;
+    int64_t rows;
+    const int32_t* tok; int64_t tok_stride; int32_t V; const float* embed; float scale;
+    const int32_t* pos; int32_t pos_const, pos_offset, pos_rows; const float* pos_table;
+    const float* ln_emb_g; const float* ln_emb_b;
+    const float* a; const float* b;
+    const float* split_part; int32_t split_ks; float split_unscale; const float* split_bias;
+    const float* gamma; const float* beta; float eps, out_scale;
+    const float* h;
+    int32_t out_split;
+} sealdec_norm_case_t;
+int sealdec_debug_rownorm(const sealdec_norm_case_t* c, float* out, void* split1, void* split2, void* split3,
+                          int32_t* overflow, uint32_t* path);
 /* The top-k warp's threshold kernel of the generate (one CTA per row) on caller-supplied rows, through the same launch.
  * Host pointers: logits float32 [R][ld] (ld >= V; columns V .. ld-1 are not read), V <= 53 248, top_k >= 1 (values above
  * V select the smallest value).  Per row: out_thr = tau, the min(top_k, V)-th largest value (-0.0 returned as +0.0),

@@ -135,6 +135,18 @@ class AttnCase(C.Structure):              # sealdec_attn_case_t
                 ("out_split", C.c_int32)]
 
 
+class NormCase(C.Structure):              # sealdec_norm_case_t
+    _fields_ = [("kind", C.c_int32), ("d", C.c_int32), ("rows", C.c_int64),
+                ("tok", vp), ("tok_stride", C.c_int64), ("V", C.c_int32), ("embed", vp), ("scale", C.c_float),
+                ("pos", vp), ("pos_const", C.c_int32), ("pos_offset", C.c_int32), ("pos_rows", C.c_int32), ("pos_table", vp),
+                ("ln_emb_g", vp), ("ln_emb_b", vp),
+                ("a", vp), ("b", vp),
+                ("split_part", vp), ("split_ks", C.c_int32), ("split_unscale", C.c_float), ("split_bias", vp),
+                ("gamma", vp), ("beta", vp), ("eps", C.c_float), ("out_scale", C.c_float),
+                ("h", vp),
+                ("out_split", C.c_int32)]
+
+
 _DEC_SIGS = {
     "sealdec_apply_index_mask_d": (i32, [vp, vp, C.POINTER(ProcessorCfg), vp, C.c_int64, C.c_int64, vp, vp, vp,
                                          C.c_int64, C.c_int64]),
@@ -176,6 +188,7 @@ _DEC_SIGS = {
     "sealdec_debug_target_logprob": (i32, [C.c_int64, C.c_int32, C.c_int64, vp, vp, C.c_int64, C.c_float, vp, C.c_int64,
                                            vp, C.c_int64]),
     "sealdec_debug_attention": (i32, [C.POINTER(AttnCase), vp, vp, vp, vp, vp, vp, vp, vp]),
+    "sealdec_debug_rownorm": (i32, [C.POINTER(NormCase), vp, vp, vp, vp, vp, vp]),
     "sealdec_debug_topk_threshold": (i32, [C.c_int64, C.c_int32, C.c_int64, vp, C.c_int32, vp, vp, vp]),
     "sealdec_debug_topk_threshold_cluster": (i32, [C.c_int64, C.c_int32, C.c_int64, vp, C.c_int32, vp, vp, vp]),
     "sealdec_debug_topk_rows":(i32, [C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_double)]),

@@ -164,6 +164,12 @@ class SealBartEngine:
             device = p.device.index if p.is_cuda else torch.cuda.current_device()
         return cls(model.state_dict(), model.config, device=device, gemm_mode=gemm_mode)
 
+    @property
+    def max_positions(self):
+        """the positions the decoder's position table covers (without BART's and mBART's offset of 2); None for T5,
+        which has no table"""
+        return int(self.config.max_position_embeddings)
+
     def __del__(self):
         h = self.__dict__.get("_h")
         if h:
@@ -274,6 +280,8 @@ class SealT5Engine(SealBartEngine):
     """Device-resident T5 weights + workspace behind the same handle (include/sealdec.h `sealt5_create`): every method
     of SealBartEngine, and every entry point that takes an engine, works the same way.  `config` is a T5ConfigView."""
 
+    max_positions = None
+
     def __init__(self, state_dict, config, device=0, gemm_mode=None, generation_config=None):
         if gemm_mode is None:
             gemm_mode = default_gemm_mode(state_dict)
@@ -362,8 +370,7 @@ def preln_native_config(config, gemm_mode):
 class SealPreLnEngine(SealBartEngine):
     """Device-resident Pegasus / mBART weights + workspace behind the same handle (include/sealdec.h
     `sealbart_create_ex`): every method of SealBartEngine, and every entry point that takes an engine, works the same
-    way.  `config` is a PreLnConfigView; `max_positions` the rows of the decoder's position table (without mBART's
-    offset of 2)."""
+    way.  `config` is a PreLnConfigView."""
 
     def __init__(self, state_dict, config, device=0, gemm_mode=None):
         if gemm_mode is None:
@@ -372,7 +379,6 @@ class SealPreLnEngine(SealBartEngine):
         self.config = PreLnConfigView(config)
         self.gemm_mode = int(gemm_mode)
         self.device = int(device)
-        self.max_positions = int(cfg.max_positions)
         h = vp()
         check(lib.sealbart_create_ex(C.byref(cfg), C.byref(var), self.device, C.byref(h)))
         self._h = h.value
@@ -404,8 +410,8 @@ def _position_error():
 
 def _check_decoder_positions(eng, max_length):
     """A generate that runs every step (keep_history=True, the record entry points) feeds decoder positions
-    0 .. max_length - 2 (cur_len - 1 at cur_len = 1 .. max_length - 1, constrained_beam_search).  A model with a bounded
-    position table (SealPreLnEngine) raises the reference's IndexError before any device work when the last one is
+    0 .. max_length - 2 (cur_len - 1 at cur_len = 1 .. max_length - 1, constrained_beam_search).  A model with a
+    position table (BART, Pegasus, mBART) raises the reference's IndexError before any device work when the last one is
     past the table."""
     P = getattr(eng, "max_positions", None)
     if P is not None and int(max_length) - 2 >= P:

@@ -129,14 +129,15 @@ __device__ __forceinline__ void warp_layernorm(float4 (&v)[MAXV], int nv, int d,
 
 constexpr int kLnMaxVec = 8;     // d_model <= 1024
 
-// out[r] = LN(embed[tok[r]] * scale + pos_table[pos(r) + 2])      (BartEncoder/BartDecoder embedding)
+// out[r] = LN(embed[tok[r]] * scale + pos_table[min(pos(r) + 2, pos_rows - 1)])      (BartEncoder/BartDecoder embedding)
 // tok: int32, row r reads tok[r * tok_stride].  pos(r) = pos_const if pos_per_row == nullptr else pos_per_row[r].
+// A position past the table of pos_rows rows reads its last row, as preln_row_kernel does (see sealdec.h).
 template <class SO>
 __global__ void __launch_bounds__(128) embed_ln_kernel(int64_t rows, int d, const int32_t* __restrict__ tok,
                                                        int64_t tok_stride,
                                                        const int32_t* __restrict__ pos_per_row, int pos_const,
                                                        const EmbT<SO>* __restrict__ embed, float scale,
-                                                       const float* __restrict__ pos_table,
+                                                       const float* __restrict__ pos_table, int pos_rows,
                                                        const float* __restrict__ gamma, const float* __restrict__ beta,
                                                        float* __restrict__ out, SO so) {
     const int lane = threadIdx.x & 31;
@@ -144,7 +145,7 @@ __global__ void __launch_bounds__(128) embed_ln_kernel(int64_t rows, int d, cons
     if (r >= rows) return;
     const int nv = d / 128;
     const EmbT<SO>* e = embed + (int64_t)tok[r * tok_stride] * d;
-    const int p = (pos_per_row ? pos_per_row[r] : pos_const) + 2;
+    const int p = min((pos_per_row ? pos_per_row[r] : pos_const) + 2, pos_rows - 1);
     const float* pe = pos_table + (int64_t)p * d;
     float4 v[kLnMaxVec];
 #pragma unroll

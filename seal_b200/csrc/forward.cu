@@ -50,17 +50,76 @@ Act act_view(int gemm_mode, float* plain, const Buf& b, int64_t off = 0) {
     return a;
 }
 
+// ---- producer dispatch -------------------------------------------------------------------------------------------
+// The kernels that normalise or gate a row and write the next GEMM's split operand.  The layer loops and
+// sealdec_debug_rownorm both go through these launchers; each enqueues one kernel and returns its kPath* bit (0 for
+// the BART embedding, which has none).  b_src: the split-K GEMM output b still is, if it was left unsummed.
+
+// BART's embedding + layernorm_embedding: row r = LN(embed[tok[r * tok_stride]] * scale + pos_table[pos(r) + 2]), pos(r) =
+// pos[r] or pos_const, the row clamped to the table's pos_rows - 1
+template <class SO>
+uint32_t launch_embed_ln(cudaStream_t s, int64_t rows, int d, const int32_t* tok, int64_t tok_stride, const int32_t* pos, int pos_const,
+                         const EmbT<SO>* embed, float scale, const float* pos_table, int pos_rows, const float* g, const float* beta,
+                         float* out, const SO& so) {
+    launch_k(embed_ln_kernel<SO>, (unsigned)((rows + 3) / 4), 128, 0, s, rows, d, tok, tok_stride, pos, pos_const, embed, scale, pos_table,
+             pos_rows, g, beta, out, so);
+    return 0;
+}
+
+// BART's post-LN add: out = LN(a + b), a CTA per row up to kAddLnRowMax rows (which also sums a split-K b), else a
+// warp per row (the GEMM never defers there)
+template <class SO>
+uint32_t launch_add_ln(cudaStream_t s, int64_t rows, int d, const float* a, const float* b, const SplitSrc& b_src, const float* g,
+                       const float* beta, float* out, const SO& so) {
+    if (rows <= kAddLnRowMax) {
+        launch_k(add_ln_row_kernel<SO>, (unsigned)rows, 128, 0, s, rows, d, a, b, g, beta, out, so, b_src);
+        return kPathAddLnRow;
+    }
+    launch_k(add_ln_kernel<SO>, (unsigned)((rows + 3) / 4), 128, 0, s, rows, d, a, b, g, beta, out, so);
+    return kPathAddLnWarp;
+}
+
+// T5's embedding (tok != nullptr) or add, then RMSNorm (t5_kernels.cuh); the wide kernel above d = 1024
+template <class SO>
+uint32_t launch_t5_rms(cudaStream_t s, int64_t rows, int d, const int32_t* tok, int64_t tok_stride, const EmbT<SO>* embed, float* x,
+                       const float* b, const SplitSrc& b_src, const float* w, float eps, float out_scale, const SO& so) {
+    const bool wide = d > 4 * 128 * kT5RmsVec;
+    launch_k(wide ? t5_rms_row_kernel<kT5RmsVecWide, SO> : t5_rms_row_kernel<kT5RmsVec, SO>, (unsigned)rows, 128, 0, s, rows, d, tok,
+             tok_stride, embed, x, b, b_src, w, eps, out_scale, so);
+    return wide ? kPathT5RmsWide : kPathT5Rms;
+}
+
+// the pre-LayerNorm family's embedding (em.tok != nullptr) or add, then LayerNorm (preln_kernels.cuh)
+template <class SO>
+uint32_t launch_preln_norm(cudaStream_t s, int64_t rows, int d, const PreLnEmbedT<EmbT<SO>>& em, float* x, const float* b,
+                           const SplitSrc& b_src, const float* g, const float* beta, const SO& so) {
+    launch_k(preln_row_kernel<SO>, (unsigned)rows, 128, 0, s, rows, d, em, x, b, b_src, g, beta, so);
+    return kPathPreLn | (em.tok && em.ln_g ? kPathPreLnEmbedLn : 0u);
+}
+
+// T5's gated-gelu: h [rows][2f] -> gelu_new(h[:, :f]) * h[:, f:], a grid-stride loop of at most 8 CTAs per SM
+template <class SO> uint32_t launch_t5_gate(cudaStream_t s, int64_t rows, int f, const float* h, const SO& so) {
+    const int blocks = (int)std::max<int64_t>(1, std::min<int64_t>((rows * (f / 4) + 255) / 256, (int64_t)sm_count() * 8));
+    launch_k(t5_gate_kernel<SO>, (unsigned)blocks, 256, 0, s, rows, f, h, so);
+    return kPathT5Gate;
+}
+
 void add_ln(Ctx& cx, int64_t rows, int d, const float* a, const float* b, const LNp& ln, const Act& out) {
     const SplitSrc ps = take_pending(cx);
-    with_split(cx.m, out, [&](auto so) {
-        using SO = decltype(so);
-        if (rows <= kAddLnRowMax)          // small batches: a CTA per row (and the split-K finish of the GEMM before it, if pending)
-            launch_k(add_ln_row_kernel<SO>, (unsigned)rows, 128, 0, cx.s, rows, d, a, b, (const float*)ln.g, (const float*)ln.b, out.x, so, ps);
-        else
-            launch_k(add_ln_kernel<SO>, (unsigned)((rows + 3) / 4), 128, 0, cx.s, rows, d, a, b, (const float*)ln.g, (const float*)ln.b, out.x, so);
-    });
+    with_split(cx.m, out, [&](auto so) { cx.m->last_paths |= launch_add_ln(cx.s, rows, d, a, b, ps, ln.g, ln.b, out.x, so); });
     cx.m->launches++;
-    cx.m->last_paths |= rows <= kAddLnRowMax ? kPathAddLnRow : kPathAddLnWarp;
+}
+
+// the BART embedding of rows tok[r * tok_stride] at positions pos[r] or pos_const, through the table pos_table
+void embed_ln(Ctx& cx, int64_t rows, int d, const int32_t* tok, int64_t tok_stride, const int32_t* pos, int pos_const,
+              const float* pos_table, const LNp& ln, const Act& x) {
+    sealbart* m = cx.m;
+    const float scale = m->cfg.scale_embedding ? sqrtf((float)d) : 1.0f;
+    with_split(m, x, [&](auto so) {
+        launch_embed_ln(cx.s, rows, d, tok, tok_stride, pos, pos_const, embed_table<decltype(so)>(m), scale, pos_table,
+                        m->cfg.max_positions + 2, ln.g, ln.b, x.x, so);
+    });
+    m->launches++;
 }
 
 __global__ void prep_enc_kernel(int64_t n, int S, const int64_t* __restrict__ ids, const int64_t* __restrict__ mask,
@@ -125,14 +184,11 @@ __global__ void prep_enc_packed_kernel(int64_t n, int S, const int64_t* __restri
 void t5_rms(Ctx& cx, int64_t rows, int d, const int32_t* tok, int64_t tok_stride, const Act& x, const float* b, const float* w,
             float out_scale) {
     const SplitSrc ps = take_pending(cx);
-    const bool wide = d > 4 * 128 * kT5RmsVec;
     with_split(cx.m, x, [&](auto so) {
-        using SO = decltype(so);
-        launch_k(wide ? t5_rms_row_kernel<kT5RmsVecWide, SO> : t5_rms_row_kernel<kT5RmsVec, SO>, (unsigned)rows, 128, 0, cx.s, rows, d, tok, tok_stride,
-                 embed_table<SO>(cx.m), x.x, b, ps, w, cx.m->t5.layer_norm_epsilon, out_scale, so);
+        cx.m->last_paths |= launch_t5_rms(cx.s, rows, d, tok, tok_stride, embed_table<decltype(so)>(cx.m), x.x, b, ps, w,
+                                          cx.m->t5.layer_norm_epsilon, out_scale, so);
     });
     cx.m->launches++;
-    cx.m->last_paths |= wide ? kPathT5RmsWide : kPathT5Rms;
 }
 
 // wi (ReLU epilogue) or [wi_0; wi_1] + gate, then wo into tmp (split-K slices left to the next t5_rms)
@@ -140,9 +196,8 @@ void t5_ffn(Ctx& cx, int64_t rows, int d, int f, const Act& x, Lin& fc1, Lin& fc
     sealbart* m = cx.m;
     if (m->t5.ffn_kind == 1) {
         gemm(cx, rows, 2 * f, d, x, d, fc1, Act{ffn2}, 2 * f, kActNone);
-        const int blocks = (int)std::max<int64_t>(1, std::min<int64_t>((rows * (f / 4) + 255) / 256, (int64_t)sm_count() * 8));
-        with_split(m, ffn, [&](auto so) { launch_k(t5_gate_kernel<decltype(so)>, (unsigned)blocks, 256, 0, cx.s, rows, f, (const float*)ffn2, so); });
-        m->launches++; m->last_paths |= kPathT5Gate;
+        with_split(m, ffn, [&](auto so) { m->last_paths |= launch_t5_gate(cx.s, rows, f, ffn2, so); });
+        m->launches++;
     } else
         gemm(cx, rows, f, d, x, d, fc1, ffn, f, kActRelu);
     gemm(cx, rows, d, f, ffn, f, fc2, tmp, d, kActNone, INT64_MAX);
@@ -313,13 +368,7 @@ void bart_encoder_layers(Ctx& cx, const Dims& D, int64_t Te, const Acts& A, cons
                          const int32_t* soff) {
     sealbart* m = cx.m;
     const int d = D.d, heads = m->cfg.heads;
-    const float scale = m->cfg.scale_embedding ? sqrtf((float)d) : 1.0f;
-    with_split(m, A.x, [&](auto so) {
-        using SO = decltype(so);
-        embed_ln_kernel<SO><<<(unsigned)((Te + 3) / 4), 128, 0, cx.s>>>(Te, d, tok, 1, pos, 0, embed_table<SO>(m), scale, m->enc_pos,
-                                                                        m->enc_ln_emb.g, m->enc_ln_emb.b, A.x.x, so);
-    });
-    CUDA_CHECK(cudaGetLastError()); m->launches++;
+    embed_ln(cx, Te, d, tok, 1, pos, 0, m->enc_pos, m->enc_ln_emb, A.x);
     for (auto& L : m->enc) {
         gemm(cx, Te, 3 * d, d, A.x, d, L.qkv, A.qkv, 3 * d, kActNone);
         with_split(m, A.attn, [&](auto so) { launch_enc_self_attn(cx.s, D.Q, d, heads, (int)D.S, A.qkv.x, m32, nullptr, A.attn.x, so, soff); });
@@ -351,13 +400,7 @@ void bart_self_attention(Ctx& cx, const Dims& D, const DecStep& S, int l) {
 void bart_decoder_layers(Ctx& cx, const Dims& D, const DecStep& S) {
     sealbart* m = cx.m;
     const int d = D.d, pos = S.pos;
-    const float scale = m->cfg.scale_embedding ? sqrtf((float)d) : 1.0f;
-    with_split(m, S.x, [&](auto so) {
-        using SO = decltype(so);
-        launch_k(embed_ln_kernel<SO>, (unsigned)((S.R + 3) / 4), 128, 0, cx.s, S.R, d, S.tokens + pos, (int64_t)(D.T * S.row_mul), (const int32_t*)nullptr, pos,
-                 embed_table<SO>(m), scale, (const float*)m->dec_pos, (const float*)m->dec_ln_emb.g, (const float*)m->dec_ln_emb.b, S.x.x, so);
-    });
-    m->launches++;
+    embed_ln(cx, S.R, d, S.tokens + pos, (int64_t)(D.T * S.row_mul), nullptr, pos, m->dec_pos, m->dec_ln_emb, S.x);
     for (int l = 0; l < m->cfg.decoder_layers; ++l) {
         DecLayerW& L = m->dec[l];
         bart_self_attention(cx, D, S, l);
@@ -394,10 +437,9 @@ void preln_norm(Ctx& cx, int64_t rows, int d, const PreLnEmbed& em, const Act& x
         e.tok = em.tok; e.tok_stride = em.tok_stride; e.pos = em.pos; e.pos_const = em.pos_const; e.pos_offset = em.pos_offset;
         e.pos_rows = em.pos_rows; e.embed = em.tok ? embed_table<SO>(cx.m) : nullptr; e.scale = em.scale; e.pos_table = em.pos_table;
         e.ln_g = em.ln_g; e.ln_b = em.ln_b;
-        launch_k(preln_row_kernel<SO>, (unsigned)rows, 128, 0, cx.s, rows, d, e, x.x, b, ps, (const float*)ln.g, (const float*)ln.b, so);
+        cx.m->last_paths |= launch_preln_norm(cx.s, rows, d, e, x.x, b, ps, ln.g, ln.b, so);
     });
     cx.m->launches++;
-    cx.m->last_paths |= kPathPreLn | (em.tok && em.ln_g ? kPathPreLnEmbedLn : 0u);
 }
 
 // fc1 with the variant's activation epilogue, then fc2 into tmp (split-K slices left to the next preln_norm)
@@ -684,6 +726,149 @@ int sealdec_debug_attention(const sealdec_attn_case_t* c, float* out, void* spli
             if (split.p[i]) down(split_out[i], split.p[i], out_n * elem);
         if (overflow) down(overflow, d_ovf.p, 4);
         if (self) { down(kc_out, d_kc.p, cache_bytes); down(vc_out, d_vc.p, cache_bytes); }
+        *path = bit;
+    });
+}
+
+}  // extern "C"
+
+extern "C" {
+
+int sealdec_debug_rownorm(const sealdec_norm_case_t* c, float* out, void* split1, void* split2, void* split3, int32_t* overflow,
+                          uint32_t* path) {
+    return guarded([&] {
+        auto bad = [](const char* what) { return ApiError(SEALFM_EINVAL, what); };
+        constexpr int kMaxPos = 1024;                                     // the largest position accepted
+        if (!c || !path) throw bad("null argument");
+        if (c->kind < 0 || c->kind > 4) throw bad("kind must be 0..4");
+        const int kind = c->kind, d = c->d;
+        const int64_t rows = c->rows;
+        const bool t5 = kind == 2 || kind == 4;
+        if (kind == 4 ? (d < 64 || d > 65536 || d % 64) : t5 ? !((d > 0 && d <= 1024 && d % 128 == 0) || (d > 0 && d <= 4096 && d % 1024 == 0))
+                                                          : (d < 128 || d > 1024 || d % 128))
+            throw bad("d outside the family's widths (BART / pre-LN: multiples of 128 up to 1024; T5: also 2048, 3072, 4096; "
+                      "gate: multiples of 64 up to 65536)");
+        if (rows < 1 || rows > (1 << 20)) throw bad("rows must be in [1, 2^20]");
+        if (c->out_split < 0 || c->out_split > 3) throw bad("out_split must be 0..3");
+        if (c->out_split == 0 && kind >= 2) throw bad("kinds 2..4 write the split only: out_split must not be 0");
+        if (c->out_split && (!split1 || !split2 || (c->out_split == 3 && !split3) || (c->out_split == 2 && !overflow)))
+            throw bad("split output missing");
+        if (kind != 4 && !out) throw bad("out missing");
+        // the input form: the embedding (kind 0; kinds 2, 3 with tok), the add (kind 1; kinds 2, 3 with a), the gate's h
+        const bool emb = kind == 0 || ((kind == 2 || kind == 3) && c->tok);
+        const bool add = kind == 1 || ((kind == 2 || kind == 3) && !c->tok);
+        if ((kind == 2 || kind == 3) && c->tok && c->a) throw bad("tok and a: one input form only");
+        const bool sums = add && (kind != 1 || rows <= kAddLnRowMax);      // the kernels that sum split-K slices
+        if (c->split_ks != 0 && c->split_ks != 1) {
+            if (c->split_ks < 2 || c->split_ks > 8) throw bad("split_ks must be 2..8");
+            if (!sums) throw bad("split-K slices: only for the kernels that sum them");
+            if (!c->split_part || !c->split_bias) throw bad("split-K slices or bias missing");
+        }
+        const bool sliced = c->split_ks > 1;
+        if (add && (!c->a || (!sliced && !c->b))) throw bad("a or b missing");
+        if (kind == 4 && !c->h) throw bad("h missing");
+        if (kind != 4 && !c->gamma) throw bad("gamma missing");
+        if ((kind == 0 || kind == 1 || kind == 3) && !c->beta) throw bad("beta missing");
+        if (kind == 2 && !(std::isfinite(c->eps) && c->eps >= 0.f && std::isfinite(c->out_scale))) throw bad("eps and out_scale must be finite");
+        const bool has_pos = kind == 0 || (kind == 3 && emb);
+        const int pos_offset = kind == 0 ? 2 : c->pos_offset;
+        if (emb) {
+            if (!c->embed || c->V < 1 || c->tok_stride < 1) throw bad("embedding: embed, V >= 1 and tok_stride >= 1 needed");
+            for (int64_t r = 0; r < rows; ++r)
+                if (c->tok[r * c->tok_stride] < 0 || c->tok[r * c->tok_stride] >= c->V) throw bad("token id outside [0, V)");
+        }
+        if (has_pos) {
+            if (kind == 3 && pos_offset != 0 && pos_offset != 2) throw bad("pos_offset must be 0 or 2");
+            if (!c->pos_table || c->pos_rows < pos_offset + 1 || c->pos_rows > kMaxPos + 2) throw bad("pos_table of pos_offset + 1 .. 1026 rows needed");
+            for (int64_t r = 0; r < (c->pos ? rows : 1); ++r) {
+                const int p = c->pos ? c->pos[r] : c->pos_const;
+                if (p < 0 || p > kMaxPos) throw bad("position outside [0, 1024]");
+            }
+            if (kind == 3 && !c->ln_emb_g != !c->ln_emb_b) throw bad("ln_emb_g and ln_emb_b together");
+        }
+        require_device();
+
+        Buf d_tok, d_pos, d_emb, d_ptab, d_lg, d_lb, d_a, d_b, d_part, d_pb, d_g, d_beta, d_h, d_out, d_split, d_ovf;
+        auto up = [&](Buf& b, const void* h, size_t bytes) { b.ensure(bytes); CUDA_CHECK(cudaMemcpy(b.p, h, bytes, cudaMemcpyHostToDevice)); };
+        auto nan = [&](Buf& b, size_t bytes) { b.ensure(bytes); CUDA_CHECK(cudaMemset(b.p, 0xFF, bytes)); };
+        const size_t n = (size_t)rows * d;
+        if (emb) {
+            std::vector<int32_t> tok((size_t)rows);                        // row r's token at r (tok_stride 1 on the device)
+            for (int64_t r = 0; r < rows; ++r) tok[r] = c->tok[r * c->tok_stride];
+            up(d_tok, tok.data(), tok.size() * 4);
+            const size_t ne = (size_t)c->V * d;
+            d_emb.ensure(ne * (c->out_split == 3 ? 2 : 4));
+            upload(d_emb.p, c->out_split == 3, c->embed, ne);               // bf16 as sealbart_set_tensor rounds it (gemm_mode 6)
+        }
+        if (has_pos) {
+            if (c->pos) up(d_pos, c->pos, (size_t)rows * 4);
+            // the table, then NaN guard rows up to row 1026 = the last one an accepted position can name
+            const size_t tab = (size_t)c->pos_rows * d * 4, all = (size_t)std::max(c->pos_rows, kMaxPos + 3) * d * 4;
+            nan(d_ptab, all);
+            CUDA_CHECK(cudaMemcpy(d_ptab.p, c->pos_table, tab, cudaMemcpyHostToDevice));
+        }
+        if (kind == 3 && emb && c->ln_emb_g) { up(d_lg, c->ln_emb_g, (size_t)d * 4); up(d_lb, c->ln_emb_b, (size_t)d * 4); }
+        if (kind != 4) up(d_g, c->gamma, (size_t)d * 4);
+        if (kind != 4 && kind != 2) up(d_beta, c->beta, (size_t)d * 4);
+        if (kind == 4) up(d_h, c->h, n * 2 * 4);
+        // the residual: out for kind 1 (add_ln runs in place, out == a), x_out for kinds 2 and 3; NaN where not an input
+        nan(d_out, n * 4);
+        if (add) CUDA_CHECK(cudaMemcpy(d_out.p, c->a, n * 4, cudaMemcpyHostToDevice));
+        SplitSrc src{};
+        if (add) {
+            if (sliced) {
+                nan(d_b, n * 4);                                          // not read
+                up(d_part, c->split_part, n * 4 * c->split_ks); up(d_pb, c->split_bias, (size_t)d * 4);
+                src = SplitSrc{d_part.as<float>(), c->split_ks, (int64_t)n, d_pb.as<float>(), c->split_unscale};
+            } else up(d_b, c->b, n * 4);
+        }
+        if (c->out_split) nan(d_split, n * 8);
+        d_ovf.ensure(4); CUDA_CHECK(cudaMemset(d_ovf.p, 0, 4));
+
+        float* x = d_out.as<float>();
+        const int32_t* tok = d_tok.as<int32_t>();
+        const int32_t* pos = c->pos ? d_pos.as<int32_t>() : nullptr;
+        auto run = [&](auto so) -> uint32_t {
+            using SO = decltype(so);
+            const EmbT<SO>* table = d_emb.as<EmbT<SO>>();
+            switch (kind) {
+            case 0:
+                return launch_embed_ln(nullptr, rows, d, tok, 1, pos, c->pos_const, table, c->scale, d_ptab.as<float>(), c->pos_rows,
+                                       d_g.as<float>(), d_beta.as<float>(), x, so);
+            case 1: return launch_add_ln(nullptr, rows, d, x, d_b.as<float>(), src, d_g.as<float>(), d_beta.as<float>(), x, so);
+            case 2:
+                return launch_t5_rms(nullptr, rows, d, emb ? tok : nullptr, 1, table, x, d_b.as<float>(), src, d_g.as<float>(), c->eps,
+                                     c->out_scale, so);
+            case 3: {
+                PreLnEmbedT<EmbT<SO>> e;
+                if (emb) {
+                    e.tok = tok; e.tok_stride = 1; e.pos = pos; e.pos_const = c->pos_const; e.pos_offset = pos_offset;
+                    e.pos_rows = c->pos_rows; e.embed = table; e.scale = c->scale; e.pos_table = d_ptab.as<float>();
+                    e.ln_g = d_lg.as<float>(); e.ln_b = d_lb.as<float>();
+                }
+                return launch_preln_norm(nullptr, rows, d, e, x, d_b.as<float>(), src, d_g.as<float>(), d_beta.as<float>(), so);
+            }
+            default: return launch_t5_gate(nullptr, rows, d, d_h.as<float>(), so);
+            }
+        };
+        // out_split 1 / 2 / 3: the split of gemm_mode 2 / 3 / 6, laid out as the model's split buffers (split_view)
+        uint32_t bit = 0;
+        Act split;
+        size_t elem = 0;
+        if (c->out_split)
+            with_format(c->out_split == 1 ? kGemmTf32 : c->out_split == 2 ? kGemmFp16 : kGemmBf16, [&](auto t) {
+                using T = decltype(t);
+                split = split_view<T>(nullptr, d_split); elem = sizeof(T);
+                bit = run(producer_split<T>(split, d_ovf.as<int>()));
+            });
+        else bit = run(SplitOut{});
+        CUDA_CHECK(cudaDeviceSynchronize());
+        auto down = [&](void* h, const void* dp, size_t bytes) { CUDA_CHECK(cudaMemcpy(h, dp, bytes, cudaMemcpyDeviceToHost)); };
+        if (kind != 4) down(out, d_out.p, n * 4);
+        void* const split_out[3] = {split1, split2, split3};
+        for (int i = 0; i < 3; ++i)
+            if (split.p[i]) down(split_out[i], split.p[i], n * elem);
+        if (overflow) down(overflow, d_ovf.p, 4);
         *path = bit;
     });
 }

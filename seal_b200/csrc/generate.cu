@@ -648,7 +648,7 @@ int sealdec_teacher_forced(sealbart_t* m, const int64_t* ids, const int64_t* mas
             throw ApiError(SEALFM_EINVAL, "bad argument");
         if (S > m->cfg.max_positions) throw ApiError(SEALFM_EINVAL, "source longer than max_positions");
         if (out_full && (out_full_pos < 0 || out_full_pos >= T)) throw ApiError(SEALFM_EINVAL, "out_full_pos must be in [0, T)");
-        if (m->arch == 2 && T > m->cfg.max_positions) throw ApiError(SEALFM_EINVAL, "decoder inputs longer than the position table");
+        if (m->arch != 1 && T > m->cfg.max_positions) throw ApiError(SEALFM_EINVAL, "decoder inputs longer than the position table");
         check_sources(ids, mask, Q, S, m->cfg.vocab_size);
         check_token_ids(dec_ids, N * T, m->cfg.vocab_size, "decoder");
         for (int64_t r = 0; r < N; ++r) {
@@ -828,7 +828,7 @@ int sealdec_debug_step_logits_ex(sealbart_t* m, const int64_t* ids, const int64_
         if (src_tokens_hint != -1 && src_tokens_hint != -2 && right_padded_tokens(mask, Q, S) != src_tokens_hint)
             throw ApiError(SEALFM_EINVAL, "src_tokens_hint does not match a right-padded mask");
         const int T = (int)t;
-        if (m->arch == 2 && T > m->cfg.max_positions) throw ApiError(SEALFM_EINVAL, "decoder inputs longer than the position table");
+        if (m->arch != 1 && T > m->cfg.max_positions) throw ApiError(SEALFM_EINVAL, "decoder inputs longer than the position table");
         const Dims D = make_dims(m, Q, S, B, T);
         check_token_ids(dec_ids, D.R * T, m->cfg.vocab_size, "decoder");
         if (anc)

@@ -107,7 +107,7 @@ def test_keep_history_position_limit():
     _check_decoder_positions(eng, 61)
     with pytest.raises(IndexError, match="index out of range in self"):
         _check_decoder_positions(eng, 62)
-    _check_decoder_positions(type("B", (), {})(), 128)          # BART / T5 engines: no bound here
+    _check_decoder_positions(type("B", (), {})(), 128)          # no position table (T5): no bound
     # the HF forward at the boundary: position 59 runs, position 60 raises the same IndexError
     model = make_preln("pegasus_relu")
     ids, am = preln_sources(np.random.default_rng(0), 1, 6, 2000)
