@@ -8,9 +8,10 @@
  *   - the BART-large forward the reference gets from transformers 4.13 (call sites
  *     seal/beam_search.py:231-238,481-483; model = BartForConditionalGeneration), or the T5 forward
  *     (T5ForConditionalGeneration, SEALSearcher's 't5' backbone) behind the same handle (sealt5_create), or the
- *     pre-LayerNorm BART-family forward of Pegasus and mBART (sealbart_create_ex)
+ *     pre-LayerNorm BART-family forward of Pegasus and mBART (sealbart_create with a variant)
  * Plain pointers and sizes only.  Status codes and sealfm_last_error() as in sealfm.h.
  * Everything runs on the GPU; there is no CPU path.
+ * This header is ABI version 3 (sealfm_abi_version()); the prototypes that changed in it say so.
  */
 #ifndef SEALDEC_H
 #define SEALDEC_H
@@ -45,7 +46,7 @@ int sealdec_apply_index_mask_d(const sealfm_t* fm, sealfm_stream_t stream,
                                const uint32_t* occurring_mask_d,
                                const float* scores_in_d, float* scores_out_d, int64_t V, int64_t ld);
 
-/* ---- BART weights ----------------------------------------------------------------------------- */
+/* ---- BART-family weights (bart-large; Pegasus and mBART, the pre-LayerNorm family) ------------------ */
 
 typedef struct sealbart sealbart_t;
 
@@ -62,7 +63,34 @@ typedef struct {
                                   6 = 3xBF16 with bf16 weights (see below).  All wgmma + TMA. */
 } sealbart_config_t;
 
-int  sealbart_create(const sealbart_config_t* cfg, int device, sealbart_t** out);
+#define SEALBART_ACT_GELU 0            /* exact-erf GELU (bart-large, mBART, PegasusConfig() defaults) */
+#define SEALBART_ACT_RELU 1            /* ReLU (released Pegasus checkpoints)                          */
+
+typedef struct {
+    int32_t pre_layer_norm;            /* 1: h += SelfAttn(LN_self(h)); h += CrossAttn(LN_cross(h)); h += fc2(act(fc1(LN_final(h))))
+                                          and the stacks' final "model.{encoder,decoder}.layer_norm" (Pegasus, mBART);
+                                          0: bart-large's post-LayerNorm layer (then only {0, 2, 1, SEALBART_ACT_GELU}) */
+    int32_t position_offset;           /* 0: position p reads table row p (Pegasus's sinusoidal table); 2: row p + 2 (mBART, BART) */
+    int32_t layernorm_embedding;       /* 1: "model.{encoder,decoder}.layernorm_embedding" after the embedding (mBART); 0: none */
+    int32_t activation;                /* SEALBART_ACT_GELU or SEALBART_ACT_RELU, the fc1 epilogue                           */
+} sealbart_variant_t;
+
+/* Creates a BART-family model; every entry point below takes the handle.  variant NULL is bart-large's post-LayerNorm
+ * layer, as is {0, 2, 1, SEALBART_ACT_GELU}, the only variant with pre_layer_norm = 0.  cfg: d_model a multiple of 128
+ * up to 1024, 64-wide heads, ffn_dim % 64 == 0; for a pre-LayerNorm variant max_positions >= 1 is the number of
+ * positions the tables cover: each of "model.{encoder,decoder}.embed_positions.weight" has max_positions +
+ * position_offset rows (Pegasus's max_position_embeddings rows; mBART's max_position_embeddings + 2).  A pre-LayerNorm
+ * model's sealbart_set_tensor takes BART's keys plus "model.{encoder,decoder}.layer_norm.{weight,bias}";
+ * "model.{encoder,decoder}.layernorm_embedding.*" only with layernorm_embedding = 1.  Every other key is SEALFM_EINVAL.
+ * An unsupported variant or shape is SEALFM_EINVAL before any allocation.
+ * Position table (BART's learned table of max_positions + 2 rows too): sources longer than max_positions are refused,
+ * and sealdec_teacher_forced / sealdec_debug_step_logits refuse decoder inputs longer than max_positions.  A generate
+ * may reach decoder positions past the table (max_length - 2 >= max_positions); those steps read the table's last
+ * row, so the records of a beam that is still alive there are not the model's -- whether such a call may run is the
+ * caller's decision (seal_b200.beam_search raises the reference's IndexError exactly where the reference's forward
+ * would read past the table).
+ * ABI version 3 added the variant argument. */
+int  sealbart_create(const sealbart_config_t* cfg, const sealbart_variant_t* variant, int device, sealbart_t** out);
 void sealbart_free(sealbart_t* m);
 /* Copies one tensor of an HF BartForConditionalGeneration state_dict (float32, host pointer,
  * row-major, `numel` elements) by its state_dict key, e.g.
@@ -83,36 +111,6 @@ int  sealbart_set_tensor(sealbart_t* m, const char* key, const float* host, uint
  * given, derives fused/pre-split copies. */
 int  sealbart_finalize(sealbart_t* m);
 uint64_t sealbart_device_bytes(const sealbart_t* m);
-
-/* ---- pre-LayerNorm BART family (Pegasus, mBART) ---------------------------------------------------- */
-
-#define SEALBART_ACT_GELU 0            /* exact-erf GELU (bart-large, mBART, PegasusConfig() defaults) */
-#define SEALBART_ACT_RELU 1            /* ReLU (released Pegasus checkpoints)                          */
-
-typedef struct {
-    int32_t pre_layer_norm;            /* 1: h += SelfAttn(LN_self(h)); h += CrossAttn(LN_cross(h)); h += fc2(act(fc1(LN_final(h))))
-                                          and the stacks' final "model.{encoder,decoder}.layer_norm" (Pegasus, mBART);
-                                          0: bart-large's post-LayerNorm layer (then only {0, 2, 1, SEALBART_ACT_GELU}) */
-    int32_t position_offset;           /* 0: position p reads table row p (Pegasus's sinusoidal table); 2: row p + 2 (mBART, BART) */
-    int32_t layernorm_embedding;       /* 1: "model.{encoder,decoder}.layernorm_embedding" after the embedding (mBART); 0: none */
-    int32_t activation;                /* SEALBART_ACT_GELU or SEALBART_ACT_RELU, the fc1 epilogue                           */
-} sealbart_variant_t;
-
-/* A BART-family model behind the same handle: every entry point below takes it and behaves as documented for BART.
- * cfg as for sealbart_create (d_model a multiple of 128 up to 1024, 64-wide heads, ffn_dim % 64 == 0); for a
- * pre-LayerNorm variant max_positions >= 1 is the number of positions the tables cover: each of
- * "model.{encoder,decoder}.embed_positions.weight" has max_positions + position_offset rows (Pegasus's
- * max_position_embeddings rows; mBART's max_position_embeddings + 2).  sealbart_set_tensor takes BART's keys plus
- * "model.{encoder,decoder}.layer_norm.{weight,bias}"; "model.{encoder,decoder}.layernorm_embedding.*" only with
- * layernorm_embedding = 1.  Every other key is SEALFM_EINVAL.  An unsupported variant or shape is SEALFM_EINVAL before
- * any allocation.  sealbart_create is sealbart_create_ex with {0, 2, 1, SEALBART_ACT_GELU}.
- * Position table (BART's learned table of max_positions + 2 rows too): sources longer than max_positions are refused,
- * and sealdec_teacher_forced / sealdec_debug_step_logits refuse decoder inputs longer than max_positions.  A generate
- * may reach decoder positions past the table (max_length - 2 >= max_positions); those steps read the table's last
- * row, so the records of a beam that is still alive there are not the model's -- whether such a call may run is the
- * caller's decision (seal_b200.beam_search raises the reference's IndexError exactly where the reference's forward
- * would read past the table). */
-int  sealbart_create_ex(const sealbart_config_t* cfg, const sealbart_variant_t* variant, int device, sealbart_t** out);
 
 /* ---- T5 weights ------------------------------------------------------------------------------- */
 
@@ -192,8 +190,23 @@ typedef struct {
  * (max_length-1) * 2*num_beams + num_beams   (process :662-668 every step + finalize :717-725). */
 int64_t sealdec_hyps_per_query(const sealdec_params_t* p);
 
+/* ---- diverse beam groups (fm_index_generate's diverse_bs_groups / diverse_bs_penalty, seal/beam_search.py:447-532) ----
+ * With num_beam_groups = G > 1 the decode follows transformers 4.13's group_beam_search: the beams of a query form G
+ * groups of num_beams / G, chosen one group after the other at every step; the index mask is an ordinary logits
+ * processor there, so recorded scores are the constrained ones (tie-filled picks record -inf), and a positive
+ * diversity_penalty subtracts penalty * count(v) from group g's log-probability of token v, count(v) = how often the
+ * groups before g chose v at this step (HammingDiversityLogitsProcessor).  The record count and layout are those of
+ * one group: sealdec_hyps_per_query per query, each step's 2*num_beams records group by group, in rank order.
+ * The generate calls take this struct; NULL and {1, 0} are both the single-group decode, with bit-identical records.
+ * 1 <= num_beam_groups <= num_beams with num_beams % num_beam_groups == 0, else SEALFM_EINVAL. */
+typedef struct {
+    int32_t num_beam_groups;         /* G, 1 = one group                                             */
+    float   diversity_penalty;       /* <= 0: no Hamming penalty (only used with G > 1); finite      */
+} sealdec_groups_t;
+
 /* fm_index_generate(model, index, input_ids, attention_mask, ..., keep_history=True)
- * seal/beam_search.py:391-557.  HOST buffers in and out (copies are part of the call):
+ * seal/beam_search.py:391-557, with the beam groups of `groups` (NULL = one group).  HOST buffers in and out (copies
+ * are part of the call):
  *   input_ids, attention_mask  int64 [Q][S]
  *   out_scores   float32 [Q][H]      sum_logprobs of each recorded hypothesis (:667); caller applies
  *                                    score/len**lp * len**lp (:754,:555) — identity for lp = 0
@@ -205,72 +218,45 @@ int64_t sealdec_hyps_per_query(const sealdec_params_t* p);
  *                                    or FM index disabled); may be NULL
  * Every source must attend to at least one position, and every token id must lie in [0, vocab_size): an
  * attention_mask row that is all zero or an id outside that range is rejected with SEALFM_EINVAL (here, by
- * sealdec_teacher_forced and by the debug entry points); the device-buffer entry points below do not check either,
- * and their results for such a source are undefined.
+ * sealdec_teacher_forced and by the debug entry points); sealdec_generate_dx does not check either, and its results
+ * for such a source are undefined.
  * H = sealdec_hyps_per_query(p).  Returns SEALFM_EINVAL("beam") if some query had fewer than
  * num_beams non-EOS candidates (the reference raises ValueError, :687-690).  If an activation leaves the fp16
- * range of the default GEMM mode the pass is repeated with the 3xTF32 kernels (sealbart_get_stat "overflow_fallbacks"). */
+ * range of the default GEMM mode the pass is repeated with the 3xTF32 kernels (sealbart_get_stat "overflow_fallbacks").
+ * ABI version 3 added `groups`. */
 int sealdec_generate(sealbart_t* model, const sealfm_t* fm, const uint32_t* occurring_mask_host,
                      const sealdec_params_t* p, const int64_t* input_ids, const int64_t* attention_mask,
                      int64_t Q, int64_t S, float* out_scores, int32_t* out_len, int32_t* out_tokens,
-                     uint8_t* out_valid, uint64_t* out_lo, uint64_t* out_hi);
+                     uint8_t* out_valid, uint64_t* out_lo, uint64_t* out_hi, const sealdec_groups_t* groups);
 
-/* Same, inputs and outputs already resident on the model's device; asynchronous on `stream` except for
- * workspace (re)allocation and -- without a source-token count, see sealdec_generate_dx -- one 16-byte read-back
- * of the real source-token count.  *_d pointers are device pointers.
- * error_flag_d: int32[4] on the device, zeroed by the call and raised by its kernels:
- *   [0] some query had fewer than num_beams non-EOS candidates   (the reference raises ValueError, :687-690)
- *   [1] an activation left the fp16 range of the 3xFP16 GEMM modes (|x| > 65504; operands were saturated): the
- *       results are NOT to be used -- re-run after sealbart_set_option(model, "gemm_mode", 2) (3xTF32, fp32 range).
- *       sealdec_generate (host buffers) does that by itself.
- *   [2] src_tokens_hint did not match the attention mask
- *   [3] reserved */
-int sealdec_generate_d(sealbart_t* model, const sealfm_t* fm, const uint32_t* occurring_mask_d,
-                       const sealdec_params_t* p, const int64_t* input_ids_d,
-                       const int64_t* attention_mask_d, int64_t Q, int64_t S, sealfm_stream_t stream,
-                       float* out_scores_d, int32_t* out_len_d, int32_t* out_tokens_d,
-                       uint8_t* out_valid_d, uint64_t* out_lo_d, uint64_t* out_hi_d,
-                       int32_t* error_flag_d);
-/* sealdec_generate_d plus what the caller knows about the sources:
- *   src_tokens_hint >= 1  the number of non-zero attention_mask entries, masks right-padded (the only kind SEAL
+/* fm_index_generate as sealdec_generate computes it, on inputs and outputs already resident on the model's device:
+ * the arguments and outputs of sealdec_generate, as device pointers (*_d), and these:
+ *   stream          the call is asynchronous on it, except for workspace (re)allocation and -- with
+ *                   src_tokens_hint = -1 -- one 16-byte read-back of the real source-token count.
+ *   src_tokens_hint what the caller knows about the sources:
+ *                   >= 1  the number of non-zero attention_mask entries, masks right-padded (the only kind SEAL
  *                         builds): the encoder runs on the real tokens only and the call never touches the host;
  *                         a wrong count raises error_flag_d[2];
- *                   -1    unknown (sealdec_generate_d): one 16-byte device->host read to learn it;
+ *                   -1    unknown: one 16-byte device->host read to learn it;
  *                   -2    compute the padded positions too (no host access either).
+ *   error_flag_d    int32[4] on the device, zeroed by the call and raised by its kernels:
+ *                   [0] some query had fewer than num_beams non-EOS candidates (the reference raises ValueError,
+ *                       :687-690)
+ *                   [1] an activation left the fp16 range of the 3xFP16 GEMM modes (|x| > 65504; operands were
+ *                       saturated): the results are NOT to be used -- re-run after sealbart_set_option(model,
+ *                       "gemm_mode", 2) (3xTF32, fp32 range).  sealdec_generate (host buffers) does that by itself.
+ *                   [2] src_tokens_hint did not match the attention mask
+ *                   [3] reserved
  * On a non-default stream, batches of at most 4096 rows (queries x beams) are replayed from a CUDA graph of the
  * whole call from the third call with the same shapes, parameters and buffer addresses on (a generate of 20
  * queries is ~1 900 short kernels: launch-bound); sealbart_set_option(model, "cuda_graph", 0 / 1 / -1) forces it
- * off / on / back to automatic. */
+ * off / on / back to automatic.  ABI version 3 added `groups`. */
 int sealdec_generate_dx(sealbart_t* model, const sealfm_t* fm, const uint32_t* occurring_mask_d,
                         const sealdec_params_t* p, const int64_t* input_ids_d,
                         const int64_t* attention_mask_d, int64_t Q, int64_t S, sealfm_stream_t stream,
                         float* out_scores_d, int32_t* out_len_d, int32_t* out_tokens_d,
                         uint8_t* out_valid_d, uint64_t* out_lo_d, uint64_t* out_hi_d,
-                        int32_t* error_flag_d, int64_t src_tokens_hint);
-/* ---- diverse beam groups (fm_index_generate's diverse_bs_groups / diverse_bs_penalty, seal/beam_search.py:447-532) ----
- * With num_beam_groups = G > 1 the decode follows transformers 4.13's group_beam_search: the beams of a query form G
- * groups of num_beams / G, chosen one group after the other at every step; the index mask is an ordinary logits
- * processor there, so recorded scores are the constrained ones (tie-filled picks record -inf), and a positive
- * diversity_penalty subtracts penalty * count(v) from group g's log-probability of token v, count(v) = how often the
- * groups before g chose v at this step (HammingDiversityLogitsProcessor).  The record count and layout are those of
- * one group: sealdec_hyps_per_query per query, each step's 2*num_beams records group by group, in rank order.
- * The _ex entry points take this struct; NULL, or {1, 0}, is the single-group decode of the functions above, which
- * call them that way.  1 <= num_beam_groups <= num_beams with num_beams % num_beam_groups == 0, else SEALFM_EINVAL. */
-typedef struct {
-    int32_t num_beam_groups;         /* G, 1 = one group                                             */
-    float   diversity_penalty;       /* <= 0: no Hamming penalty (only used with G > 1); finite      */
-} sealdec_groups_t;
-
-int sealdec_generate_ex(sealbart_t* model, const sealfm_t* fm, const uint32_t* occurring_mask_host,
-                        const sealdec_params_t* p, const int64_t* input_ids, const int64_t* attention_mask,
-                        int64_t Q, int64_t S, float* out_scores, int32_t* out_len, int32_t* out_tokens,
-                        uint8_t* out_valid, uint64_t* out_lo, uint64_t* out_hi, const sealdec_groups_t* groups);
-int sealdec_generate_dx_ex(sealbart_t* model, const sealfm_t* fm, const uint32_t* occurring_mask_d,
-                           const sealdec_params_t* p, const int64_t* input_ids_d,
-                           const int64_t* attention_mask_d, int64_t Q, int64_t S, sealfm_stream_t stream,
-                           float* out_scores_d, int32_t* out_len_d, int32_t* out_tokens_d,
-                           uint8_t* out_valid_d, uint64_t* out_lo_d, uint64_t* out_hi_d,
-                           int32_t* error_flag_d, int64_t src_tokens_hint, const sealdec_groups_t* groups);
+                        int32_t* error_flag_d, int64_t src_tokens_hint, const sealdec_groups_t* groups);
 
 /* Options: "cuda_graph" (-1 auto, 0 off, 1 on), "gemm_mode" (switch between the 3xFP16 modes 3/5 and 2 = 3xTF32;
  * the TF32 operand copies are made on first use; never into or out of 6), "fused_head" (-1 = $SEALB200_FUSED_HEAD, default on; 0 = the
@@ -284,7 +270,9 @@ int sealdec_generate_dx_ex(sealbart_t* model, const sealfm_t* fm, const uint32_t
  * "overflow_fallbacks", "gemm_mode", "cached_graphs", "fused_head_steps" (decode steps of the last generate run
  * eagerly that used the statistics epilogue), "topk_cluster_steps" (decode steps of the last generate whose top-k
  * threshold ran one cluster per logits row, vocab_size > 53 248; a CUDA-graph replay reports the captured call's
- * count), "last_paths" (-1 for an unknown name).
+ * count), "launches" (kernel launches issued by the last generate / teacher-forced / debug-step call, own kernels
+ * only; a CUDA-graph replay reports the captured call's count; a stat since ABI version 3), "last_paths" (-1 for an
+ * unknown name).
  * "last_paths" is the OR, over the last generate / teacher-forced / debug-step call (a CUDA-graph replay reports
  * the call it was captured from), of one bit per kernel branch of the BART forward:
  *   0 encoder on the real tokens only (packed)         1 encoder on the padded rows (mask per key)
@@ -301,7 +289,7 @@ int sealdec_generate_dx_ex(sealbart_t* model, const sealfm_t* fm, const uint32_t
  *  18 embedding / add + RMSNorm (one CTA per row; folds a pending split-K GEMM), d_model <= 1024
  *  19 ReLU feed-forward (ReLU GEMM epilogue)          20 gated-gelu feed-forward (gelu_new(wi_0 x) * wi_1 x kernel)
  *  21 embedding / add + RMSNorm as 18, d_model 2048 .. 4096 ("t5_rms_wide"; such a model never sets 18)
- * and of the pre-LayerNorm forward (sealbart_create_ex; it also sets 0 .. 7 and 10 .. 15 as BART does, never 8 / 9;
+ * and of the pre-LayerNorm forward (a sealbart_create variant; it also sets 0 .. 7 and 10 .. 15 as BART does, never 8 / 9;
  * bit 19 names its ReLU feed-forward, e.g. Pegasus's):
  *  22 embedding / add + LayerNorm, one CTA per row (preln_row_kernel; folds a pending split-K GEMM)
  *  23 the embedding form of 22 with layernorm_embedding (mBART: two LayerNorms in one launch)
@@ -328,21 +316,19 @@ int sealdec_teacher_forced(sealbart_t* model, const int64_t* input_ids, const in
                            int64_t N, int64_t T, float temperature, float* out_logprob,
                            int64_t out_full_pos, float* out_full);
 
-/* Test / profiling hooks: one decoder step's logits for explicit decoder inputs (teacher forcing).
- * decoder_input_ids int64 [R][t] host, R = Q*num_beams rows laid out query-major like the
- * reference's expanded batch (:517-521); writes float32 [R][V] host logits of the last position. */
-int sealdec_debug_step_logits(sealbart_t* model, const int64_t* input_ids, const int64_t* attention_mask,
-                              int64_t Q, int64_t S, int32_t num_beams, const int64_t* decoder_input_ids,
-                              int64_t t, float* out_logits);
-/* The same with the beam ancestry and the encoder's packing as inputs:
- *   ancestry int32 [R][t] host, or NULL for every row its own ancestor: row r reads the decoder cache of position s
+/* Test / profiling hooks: one decoder step's logits for explicit decoder inputs (teacher forcing).  Host pointers:
+ *   decoder_input_ids int64 [R][t], R = Q*num_beams rows laid out query-major like the reference's expanded batch
+ *            (:517-521);
+ *   ancestry int32 [R][t], or NULL for every row its own ancestor: row r reads the decoder cache of position s
  *            from row ancestry[r][s] (in [0, R)), as a generate does after beams were reordered; entries at
  *            position t-1 are not read.  The caller keeps it consistent (equal decoder_input_ids[:s+1]).
  *   src_tokens_hint as in sealdec_generate_dx: -1 pack right-padded masks, -2 never pack, >= 1 the count of
- *            non-zero mask entries of right-padded masks (checked here). */
-int sealdec_debug_step_logits_ex(sealbart_t* model, const int64_t* input_ids, const int64_t* attention_mask,
-                                 int64_t Q, int64_t S, int32_t num_beams, const int64_t* decoder_input_ids,
-                                 int64_t t, const int32_t* ancestry, int64_t src_tokens_hint, float* out_logits);
+ *            non-zero mask entries of right-padded masks (checked here);
+ *   out_logits float32 [R][V], the logits of the last position.
+ * ABI version 3 added ancestry and src_tokens_hint. */
+int sealdec_debug_step_logits(sealbart_t* model, const int64_t* input_ids, const int64_t* attention_mask,
+                              int64_t Q, int64_t S, int32_t num_beams, const int64_t* decoder_input_ids,
+                              int64_t t, const int32_t* ancestry, int64_t src_tokens_hint, float* out_logits);
 /* Stand-alone GEMM C[M,N] = A[M,K] W[N,K]^T + bias (+ the epilogue activation) through the model's GEMM kernels
  * (mode 2 = 3xTF32, 3 = 3xFP16, 5 = 3xFP16 on CTA pairs, 6 = 3xBF16 with W rounded to bf16 as sealbart_set_tensor
  * rounds it), host pointers; gelu: 0 = no activation, 1 = exact-erf GELU, 2 = ReLU.  If iters > 0 also reports the
@@ -532,8 +518,6 @@ int sealdec_debug_gemm_trace(int enable, int64_t out20[20]);
  * 2 epilogue start, 3 epilogue end (0 where nothing was stamped).  Copies the first n <= 1 024 entries, then clears
  * the record.  Only in a library built with GEMM_UNIT_TRACE=1 (seal_b200/csrc/Makefile); otherwise SEALFM_EINVAL. */
 int sealdec_debug_gemm_units(int64_t* out, int32_t n);
-/* kernel launches issued by the last sealdec_generate* call on this model (own kernels only) */
-int64_t sealdec_last_launch_count(const sealbart_t* model);
 /* GEMM profiling: enable != 0 makes every following GEMM launch of this model be bracketed by CUDA
  * events on its stream.  When total_us/launches/flops are non-NULL the call first drains the device
  * and returns the summed device time, launch count and 2MNK flops recorded since the previous call,

@@ -150,8 +150,7 @@ class NormCase(C.Structure):              # sealdec_norm_case_t
 _DEC_SIGS = {
     "sealdec_apply_index_mask_d": (i32, [vp, vp, C.POINTER(ProcessorCfg), vp, C.c_int64, C.c_int64, vp, vp, vp,
                                          C.c_int64, C.c_int64]),
-    "sealbart_create": (i32, [C.POINTER(BartConfig), i32, C.POINTER(vp)]),
-    "sealbart_create_ex": (i32, [C.POINTER(BartConfig), C.POINTER(BartVariant), i32, C.POINTER(vp)]),
+    "sealbart_create": (i32, [C.POINTER(BartConfig), C.POINTER(BartVariant), i32, C.POINTER(vp)]),
     "sealbart_free": (None, [vp]),
     "sealt5_create": (i32, [C.POINTER(T5Config), i32, C.POINTER(vp)]),
     "sealt5_relative_buckets": (i32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp]),
@@ -159,22 +158,15 @@ _DEC_SIGS = {
     "sealbart_finalize": (i32, [vp]),
     "sealbart_device_bytes": (u64, [vp]),
     "sealdec_hyps_per_query": (C.c_int64, [C.POINTER(DecParams)]),
-    "sealdec_generate": (i32, [vp, vp, vp, C.POINTER(DecParams), vp, vp, C.c_int64, C.c_int64, vp, vp, vp, vp, vp, vp]),
-    "sealdec_generate_d": (i32, [vp, vp, vp, C.POINTER(DecParams), vp, vp, C.c_int64, C.c_int64, vp, vp, vp, vp, vp,
-                                 vp, vp, vp]),
+    "sealdec_generate": (i32, [vp, vp, vp, C.POINTER(DecParams), vp, vp, C.c_int64, C.c_int64, vp, vp, vp, vp, vp, vp,
+                               C.POINTER(GroupParams)]),
     "sealdec_generate_dx": (i32, [vp, vp, vp, C.POINTER(DecParams), vp, vp, C.c_int64, C.c_int64, vp, vp, vp, vp, vp,
-                                  vp, vp, vp, C.c_int64]),
-    "sealdec_generate_ex": (i32, [vp, vp, vp, C.POINTER(DecParams), vp, vp, C.c_int64, C.c_int64, vp, vp, vp, vp, vp, vp,
-                                  C.POINTER(GroupParams)]),
-    "sealdec_generate_dx_ex": (i32, [vp, vp, vp, C.POINTER(DecParams), vp, vp, C.c_int64, C.c_int64, vp, vp, vp, vp, vp,
-                                     vp, vp, vp, C.c_int64, C.POINTER(GroupParams)]),
+                                  vp, vp, vp, C.c_int64, C.POINTER(GroupParams)]),
     "sealbart_set_option": (i32, [vp, cp, C.c_int64]),
     "sealbart_get_stat": (C.c_int64, [vp, cp]),
     "sealdec_teacher_forced": (i32, [vp, vp, vp, C.c_int64, C.c_int64, vp, vp, C.c_int64, C.c_int64, C.c_float, vp,
                                      C.c_int64, vp]),
-    "sealdec_debug_step_logits": (i32, [vp, vp, vp, C.c_int64, C.c_int64, C.c_int32, vp, C.c_int64, vp]),
-    "sealdec_debug_step_logits_ex": (i32, [vp, vp, vp, C.c_int64, C.c_int64, C.c_int32, vp, C.c_int64, vp, C.c_int64,
-                                           vp]),
+    "sealdec_debug_step_logits": (i32, [vp, vp, vp, C.c_int64, C.c_int64, C.c_int32, vp, C.c_int64, vp, C.c_int64, vp]),
     "sealdec_debug_gemm": (i32, [i32, C.c_int64, C.c_int32, C.c_int32, vp, vp, vp, vp, C.c_int32, C.c_int32,
                                  C.POINTER(C.c_double)]),
     "sealdec_debug_gemm_ex": (i32, [i32, C.c_int64, C.c_int32, C.c_int32, vp, vp, vp, vp, C.c_int32, C.c_int32,
@@ -211,7 +203,6 @@ _DEC_SIGS = {
                                       i32, i32, C.c_double, C.c_double, vp, vp, C.c_int64, vp, vp, vp, vp, vp, vp,
                                       C.c_int64, vp]),
     "sealev_batch_phase_us": (None, [vp]),
-    "sealdec_last_launch_count": (C.c_int64, [vp]),
     "sealdec_profile_gemm": (i32, [vp, i32, C.POINTER(C.c_double), C.POINTER(C.c_int64), C.POINTER(C.c_double)]),
     "sealdec_last_phase_us": (i32, [vp, C.POINTER(C.c_double)]),
 }

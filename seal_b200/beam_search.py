@@ -119,6 +119,26 @@ def _weight_dtypes(model):
     return frozenset(p.dtype for p in model.parameters())
 
 
+def _hf_device(model):
+    """The CUDA device of an HF model's engine: that of its parameters, else the current device."""
+    p = next(model.parameters())
+    return p.device.index if p.is_cuda else _torch().cuda.current_device()
+
+
+def _load_weights(h, state_dict, shared_key):
+    """Copies every tensor of `state_dict` to the handle h and finalizes it.  When `shared_key` (the shared token
+    embedding) is present, its tied aliases are skipped: the embed_tokens keys, and an lm_head stored in the same
+    memory (the library ties that itself)."""
+    shared = state_dict.get(shared_key)
+    for k, v in state_dict.items():
+        if shared is not None and (k.endswith("embed_tokens.weight") or
+                                   (k == "lm_head.weight" and v.data_ptr() == shared.data_ptr())):
+            continue
+        a = np.ascontiguousarray(v.detach().to("cpu").float().numpy())
+        check(lib.sealbart_set_tensor(h, k.encode(), a.ctypes.data, a.size))
+    check(lib.sealbart_finalize(h))
+
+
 class SealBartEngine:
     """Device-resident BART weights + workspace (include/sealdec.h `sealbart_t`)."""
 
@@ -140,16 +160,9 @@ class SealBartEngine:
         if getattr(config, "activation_function", "gelu") != "gelu":
             raise ValueError("only the exact-erf 'gelu' activation of bart-large is implemented")
         h = vp()
-        check(lib.sealbart_create(C.byref(cfg), self.device, C.byref(h)))
+        check(lib.sealbart_create(C.byref(cfg), None, self.device, C.byref(h)))
         self._h = h.value
-        for k, v in state_dict.items():
-            if k.endswith("embed_tokens.weight") and "model.shared.weight" in state_dict:
-                continue                                    # tied aliases of model.shared.weight
-            if k == "lm_head.weight" and "model.shared.weight" in state_dict and v.data_ptr() == state_dict["model.shared.weight"].data_ptr():
-                continue
-            a = np.ascontiguousarray(v.detach().to("cpu").float().numpy())
-            check(lib.sealbart_set_tensor(self._h, k.encode(), a.ctypes.data, a.size))
-        check(lib.sealbart_finalize(self._h))
+        _load_weights(self._h, state_dict, "model.shared.weight")
 
     @classmethod
     def from_hf(cls, model, device=None, gemm_mode=None):
@@ -158,11 +171,8 @@ class SealBartEngine:
             return SealT5Engine.from_hf(model, device=device, gemm_mode=gemm_mode)
         if model_type in PRELN_MODEL_TYPES:
             return SealPreLnEngine.from_hf(model, device=device, gemm_mode=gemm_mode)
-        torch = _torch()
-        if device is None:
-            p = next(model.parameters())
-            device = p.device.index if p.is_cuda else torch.cuda.current_device()
-        return cls(model.state_dict(), model.config, device=device, gemm_mode=gemm_mode)
+        return cls(model.state_dict(), model.config, device=_hf_device(model) if device is None else device,
+                   gemm_mode=gemm_mode)
 
     @property
     def max_positions(self):
@@ -182,7 +192,7 @@ class SealBartEngine:
     def debug_step_logits(self, input_ids, attention_mask, num_beams, decoder_input_ids, anc=None, src_tokens=-1):
         """Teacher-forced logits of the last decoder position for explicit decoder inputs [R,t].
         anc: optional int32 [R,t] beam ancestry (row r reads the decoder cache of position s from row anc[r,s]);
-        src_tokens: -1 pack right-padded sources, -2 never pack (include/sealdec.h sealdec_debug_step_logits_ex)."""
+        src_tokens: -1 pack right-padded sources, -2 never pack (include/sealdec.h sealdec_debug_step_logits)."""
         ids = np.ascontiguousarray(np.asarray(input_ids, dtype=np.int64))
         am = np.ascontiguousarray(np.asarray(attention_mask, dtype=np.int64))
         dec = np.ascontiguousarray(np.asarray(decoder_input_ids, dtype=np.int64))
@@ -194,9 +204,9 @@ class SealBartEngine:
             a = np.ascontiguousarray(np.asarray(anc, dtype=np.int32))
             assert a.shape == (R, t)
         out = np.empty((R, int(self.config.vocab_size)), dtype=np.float32)
-        check(lib.sealdec_debug_step_logits_ex(self._h, ids.ctypes.data, am.ctypes.data, Q, S, num_beams,
-                                               dec.ctypes.data, t, a.ctypes.data if a is not None else None,
-                                               int(src_tokens), out.ctypes.data))
+        check(lib.sealdec_debug_step_logits(self._h, ids.ctypes.data, am.ctypes.data, Q, S, num_beams,
+                                            dec.ctypes.data, t, a.ctypes.data if a is not None else None,
+                                            int(src_tokens), out.ctypes.data))
         return out
 
     def stat(self, name):
@@ -218,7 +228,8 @@ class SealBartEngine:
         return {"total_us": us.value, "launches": n.value, "flops": fl.value}
 
     def last_launch_count(self):
-        return int(lib.sealdec_last_launch_count(self._h))
+        """kernel launches of the last generate / teacher-forced / debug-step call (the "launches" stat)"""
+        return self.stat("launches")
 
 
 T5_FFN_KINDS = {"relu": 0, "gated-gelu": 1}      # sealt5_config_t.ffn_kind
@@ -292,25 +303,13 @@ class SealT5Engine(SealBartEngine):
         h = vp()
         check(lib.sealt5_create(C.byref(cfg), self.device, C.byref(h)))
         self._h = h.value
-        shared = state_dict.get("shared.weight")
-        for k, v in state_dict.items():
-            if shared is not None and k in ("encoder.embed_tokens.weight", "decoder.embed_tokens.weight"):
-                continue                                    # tied aliases of shared.weight
-            if k == "lm_head.weight" and shared is not None and v.data_ptr() == shared.data_ptr():
-                continue                                    # tie_word_embeddings: the library ties it itself
-            a = np.ascontiguousarray(v.detach().to("cpu").float().numpy())
-            check(lib.sealbart_set_tensor(self._h, k.encode(), a.ctypes.data, a.size))
-        check(lib.sealbart_finalize(self._h))
+        _load_weights(self._h, state_dict, "shared.weight")
 
     @classmethod
     def from_hf(cls, model, device=None, gemm_mode=None):
         t5_native_config(model.config, 3 if gemm_mode is None else gemm_mode)      # ValueError before any device work
-        torch = _torch()
-        if device is None:
-            p = next(model.parameters())
-            device = p.device.index if p.is_cuda else torch.cuda.current_device()
-        return cls(model.state_dict(), model.config, device=device, gemm_mode=gemm_mode,
-                   generation_config=getattr(model, "generation_config", None))
+        return cls(model.state_dict(), model.config, device=_hf_device(model) if device is None else device,
+                   gemm_mode=gemm_mode, generation_config=getattr(model, "generation_config", None))
 
 
 PRELN_MODEL_TYPES = ("pegasus", "mbart")          # HF model types of the pre-LayerNorm BART family
@@ -340,7 +339,7 @@ class PreLnConfigView:
 
 def preln_native_config(config, gemm_mode):
     """(sealbart_config_t, sealbart_variant_t) for an HF Pegasus or mBART config; ValueError for an activation or shape
-    the kernels do not cover (the limits sealbart_create_ex enforces, include/sealdec.h), before anything touches the
+    the kernels do not cover (the limits sealbart_create enforces, include/sealdec.h), before anything touches the
     device."""
     mt = getattr(config, "model_type", None)
     if mt not in PRELN_MODEL_TYPES:
@@ -369,8 +368,8 @@ def preln_native_config(config, gemm_mode):
 
 class SealPreLnEngine(SealBartEngine):
     """Device-resident Pegasus / mBART weights + workspace behind the same handle (include/sealdec.h
-    `sealbart_create_ex`): every method of SealBartEngine, and every entry point that takes an engine, works the same
-    way.  `config` is a PreLnConfigView."""
+    `sealbart_create` with a `sealbart_variant_t`): every method of SealBartEngine, and every entry point that takes an
+    engine, works the same way.  `config` is a PreLnConfigView."""
 
     def __init__(self, state_dict, config, device=0, gemm_mode=None):
         if gemm_mode is None:
@@ -380,27 +379,16 @@ class SealPreLnEngine(SealBartEngine):
         self.gemm_mode = int(gemm_mode)
         self.device = int(device)
         h = vp()
-        check(lib.sealbart_create_ex(C.byref(cfg), C.byref(var), self.device, C.byref(h)))
+        check(lib.sealbart_create(C.byref(cfg), C.byref(var), self.device, C.byref(h)))
         self._h = h.value
-        shared = state_dict.get("model.shared.weight")
-        for k, v in state_dict.items():
-            if shared is not None and k.endswith("embed_tokens.weight"):
-                continue                                    # tied aliases of model.shared.weight
-            if k == "lm_head.weight" and shared is not None and v.data_ptr() == shared.data_ptr():
-                continue
-            a = np.ascontiguousarray(v.detach().to("cpu").float().numpy())
-            check(lib.sealbart_set_tensor(self._h, k.encode(), a.ctypes.data, a.size))
-        check(lib.sealbart_finalize(self._h))
+        _load_weights(self._h, state_dict, "model.shared.weight")
 
     @classmethod
     def from_hf(cls, model, device=None, gemm_mode=None):
         preln_native_config(model.config, 3 if gemm_mode is None else gemm_mode)   # ValueError before any device work
         PreLnConfigView(model.config)
-        torch = _torch()
-        if device is None:
-            p = next(model.parameters())
-            device = p.device.index if p.is_cuda else torch.cuda.current_device()
-        return cls(model.state_dict(), model.config, device=device, gemm_mode=gemm_mode)
+        return cls(model.state_dict(), model.config, device=_hf_device(model) if device is None else device,
+                   gemm_mode=gemm_mode)
 
 
 def _position_error():
@@ -490,7 +478,7 @@ def generate_records(model, index, input_ids, attention_mask, min_length=3, max_
                      num_beams=3, eos_token_id=None, force_decoding_from=None, always_allow_eos=False,
                      disable_fm_index=False, stop_at_count=0, forced_bos_token_id="config", want_ranges=True,
                      num_beam_groups=1, diversity_penalty=0.0, top_k=0):
-    """The C-ABI call with HOST buffers (sealdec_generate_ex): returns the packed hypothesis records
+    """The C-ABI call with HOST buffers (sealdec_generate): returns the packed hypothesis records
     (scores [Q,H] f32, lens [Q,H] i32, tokens [Q,H,T] i32, valid [Q,H] u8, lo/hi [Q,H] u64).
     num_beam_groups > 1: diverse beam groups (include/sealdec.h sealdec_groups_t), records group by group per step.
     top_k > 0: the top-k logits warp on every step (sealdec_params_t.top_k; one group only)."""
@@ -521,10 +509,10 @@ def generate_records(model, index, input_ids, attention_mask, min_length=3, max_
         occ = _occurring_mask(index, int(cfg.vocab_size))
         occ_ptr = occ.ctypes.data
     grp = _group_params(num_beam_groups, diversity_penalty)
-    check(lib.sealdec_generate_ex(eng._h, fm_h, occ_ptr, C.byref(p), ids.ctypes.data, am.ctypes.data, Q, S,
-                                  scores.ctypes.data, lens.ctypes.data, toks.ctypes.data, valid.ctypes.data,
-                                  lo.ctypes.data if want_ranges else None, hi.ctypes.data if want_ranges else None,
-                                  C.byref(grp)))
+    check(lib.sealdec_generate(eng._h, fm_h, occ_ptr, C.byref(p), ids.ctypes.data, am.ctypes.data, Q, S,
+                               scores.ctypes.data, lens.ctypes.data, toks.ctypes.data, valid.ctypes.data,
+                               lo.ctypes.data if want_ranges else None, hi.ctypes.data if want_ranges else None,
+                               C.byref(grp)))
     return {"scores": scores, "lens": lens, "tokens": toks, "valid": valid, "lo": lo, "hi": hi}
 
 
@@ -619,10 +607,10 @@ def generate_records_device(model, index, input_ids_d, attention_mask_d, min_len
         grp = _group_params(num_beam_groups, diversity_penalty)
         with torch.cuda.stream(stream):
             out.set_filled(Q)
-            check(lib.sealdec_generate_dx_ex(eng._h, fm_h, occ_ptr, C.byref(p), ids.data_ptr(), am.data_ptr(), Q, S,
-                                             stream.cuda_stream, out.ptr("scores"), out.ptr("lens"), out.ptr("tokens"),
-                                             out.ptr("valid"), out.ptr("lo"), out.ptr("hi"), out.err_ptr, int(src_tokens),
-                                             C.byref(grp)))
+            check(lib.sealdec_generate_dx(eng._h, fm_h, occ_ptr, C.byref(p), ids.data_ptr(), am.data_ptr(), Q, S,
+                                          stream.cuda_stream, out.ptr("scores"), out.ptr("lens"), out.ptr("tokens"),
+                                          out.ptr("valid"), out.ptr("lo"), out.ptr("hi"), out.err_ptr, int(src_tokens),
+                                          C.byref(grp)))
         for t in (ids, am, out.buf):
             t.record_stream(stream)
         if stream.cuda_stream != cur.cuda_stream:

@@ -73,7 +73,7 @@ struct sealbart {
     // architecture: 0 BART (sealbart_create), 1 T5 (sealt5_create).  For T5 the Lin biases stay zero, LNp::g holds the
     // T5LayerNorm weights (EncLayerW: ln_attn = layer.0, ln_final = layer.1; DecLayerW: ln_self / ln_cross / ln_final =
     // layer.0 / 1 / 2), enc_ln_emb / dec_ln_emb the final_layer_norm of each stack, and fc1 is wi or [wi_0; wi_1].
-    // 2 pre-LayerNorm BART family (sealbart_create_ex): BART's keys and biases; enc_ln_emb / dec_ln_emb hold
+    // 2 pre-LayerNorm BART family (sealbart_create with a variant): BART's keys and biases; enc_ln_emb / dec_ln_emb hold
     // layernorm_embedding (allocated only if variant.layernorm_embedding), enc_ln_out / dec_ln_out the stacks' final
     // layer_norm; the position tables have max_positions + variant.position_offset rows.
     int arch = 0;

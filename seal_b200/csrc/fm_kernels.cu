@@ -473,7 +473,7 @@ const std::vector<uint64_t>& sealfm_beginnings(const sealfm_t* h) {
 extern "C" {
 
 const char* sealfm_last_error(void) { return last_error().c_str(); }
-int sealfm_abi_version(void) { return 2; }
+int sealfm_abi_version(void) { return 3; }
 
 int sealfm_build(const uint64_t* symbols, uint64_t n, sealfm_t** out) {
     return guarded([&] {

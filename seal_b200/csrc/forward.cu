@@ -224,9 +224,8 @@ struct DecStep : Acts {
 // step, where a row stands for all beams, nor for ragged re-scoring groups, and only while the staged K / V of P = pos + 1
 // positions fit in 112 KB of shared memory.  It sums a split-K qkv itself.
 bool use_self_attn_query(int pos, int B, bool compact, bool ragged) {
-    static const bool sa_query = [] { const char* e = std::getenv("SEALB200_SELF_ATTN_QUERY"); return !e || std::atoi(e) != 0; }();
     const size_t saq_smem = self_attn_query_smem(pos + 1, B);
-    return sa_query && !compact && !ragged && pos >= 1 && B >= 2 && B <= 32 && pos + 1 <= 128 && saq_smem <= 112 * 1024;
+    return !compact && !ragged && pos >= 1 && B >= 2 && B <= 32 && pos + 1 <= 128 && saq_smem <= 112 * 1024;
 }
 
 // cross_attn_small_kernel for sources of at most kXKeys positions; it sums a split-K cq itself

@@ -7,7 +7,6 @@
 
 #include <algorithm>
 #include <cmath>
-#include <cstdlib>
 #include <cstring>
 #include <type_traits>
 #include <vector>
@@ -79,10 +78,8 @@ template <typename F> void with_act(int act, F&& f) {
 // so that the serial K loop of a tile is spread over up to 8 CTAs, then sum the partial tiles in a fixed order
 int split_k_slices(int tiles, int kblocks) {
     int k_slices = 1;
-    static const int force_slices = [] { const char* e = std::getenv("SEALB200_KSLICES"); return e ? std::atoi(e) : 0; }();
     if (tiles * 2 <= sm_count() && kblocks >= 4) {
         k_slices = std::min(8, std::min(kblocks / 2, sm_count() / tiles));
-        if (force_slices > 0) k_slices = std::min(force_slices, kblocks);     // experiments only
         while (k_slices > 1 && kblocks % k_slices) --k_slices;
     }
     return k_slices;

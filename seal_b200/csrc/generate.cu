@@ -417,10 +417,10 @@ int64_t sealdec_hyps_per_query(const sealdec_params_t* p) {
     return (int64_t)(p->max_length - 1) * 2 * p->num_beams + p->num_beams;
 }
 
-int sealdec_generate_dx_ex(sealbart_t* m, const sealfm_t* fm, const uint32_t* occ_d, const sealdec_params_t* p,
-                           const int64_t* ids_d, const int64_t* mask_d, int64_t Q, int64_t S, sealfm_stream_t stream,
-                           float* o_score, int32_t* o_len, int32_t* o_tok, uint8_t* o_valid, uint64_t* o_lo,
-                           uint64_t* o_hi, int32_t* err_d, int64_t src_tokens_hint, const sealdec_groups_t* groups) {
+int sealdec_generate_dx(sealbart_t* m, const sealfm_t* fm, const uint32_t* occ_d, const sealdec_params_t* p,
+                        const int64_t* ids_d, const int64_t* mask_d, int64_t Q, int64_t S, sealfm_stream_t stream,
+                        float* o_score, int32_t* o_len, int32_t* o_tok, uint8_t* o_valid, uint64_t* o_lo,
+                        uint64_t* o_hi, int32_t* err_d, int64_t src_tokens_hint, const sealdec_groups_t* groups) {
     return guarded([&] {
         check_model(m);
         if (!p || !ids_d || !mask_d || !o_score || !o_len || !o_tok || !o_valid || !err_d) throw ApiError(SEALFM_EINVAL, "null argument");
@@ -544,21 +544,6 @@ int sealdec_generate_dx_ex(sealbart_t* m, const sealfm_t* fm, const uint32_t* oc
     });
 }
 
-int sealdec_generate_dx(sealbart_t* m, const sealfm_t* fm, const uint32_t* occ_d, const sealdec_params_t* p,
-                        const int64_t* ids_d, const int64_t* mask_d, int64_t Q, int64_t S, sealfm_stream_t stream,
-                        float* o_score, int32_t* o_len, int32_t* o_tok, uint8_t* o_valid, uint64_t* o_lo,
-                        uint64_t* o_hi, int32_t* err_d, int64_t src_tokens_hint) {
-    return sealdec_generate_dx_ex(m, fm, occ_d, p, ids_d, mask_d, Q, S, stream, o_score, o_len, o_tok, o_valid, o_lo, o_hi,
-                                  err_d, src_tokens_hint, nullptr);
-}
-
-int sealdec_generate_d(sealbart_t* m, const sealfm_t* fm, const uint32_t* occ_d, const sealdec_params_t* p,
-                       const int64_t* ids_d, const int64_t* mask_d, int64_t Q, int64_t S, sealfm_stream_t stream,
-                       float* o_score, int32_t* o_len, int32_t* o_tok, uint8_t* o_valid, uint64_t* o_lo,
-                       uint64_t* o_hi, int32_t* err_d) {
-    return sealdec_generate_dx(m, fm, occ_d, p, ids_d, mask_d, Q, S, stream, o_score, o_len, o_tok, o_valid, o_lo, o_hi, err_d, -1);
-}
-
 int sealdec_last_phase_us(const sealbart_t* mc, double out5[5]) {
     return guarded([&] {
         sealbart* m = const_cast<sealbart*>(mc);
@@ -574,17 +559,9 @@ int sealdec_last_phase_us(const sealbart_t* mc, double out5[5]) {
     });
 }
 
-int64_t sealdec_last_launch_count(const sealbart_t* m) { return m ? m->launches : 0; }
-
 int sealdec_generate(sealbart_t* m, const sealfm_t* fm, const uint32_t* occ_host, const sealdec_params_t* p,
                      const int64_t* ids, const int64_t* mask, int64_t Q, int64_t S, float* o_score, int32_t* o_len,
-                     int32_t* o_tok, uint8_t* o_valid, uint64_t* o_lo, uint64_t* o_hi) {
-    return sealdec_generate_ex(m, fm, occ_host, p, ids, mask, Q, S, o_score, o_len, o_tok, o_valid, o_lo, o_hi, nullptr);
-}
-
-int sealdec_generate_ex(sealbart_t* m, const sealfm_t* fm, const uint32_t* occ_host, const sealdec_params_t* p,
-                        const int64_t* ids, const int64_t* mask, int64_t Q, int64_t S, float* o_score, int32_t* o_len,
-                        int32_t* o_tok, uint8_t* o_valid, uint64_t* o_lo, uint64_t* o_hi, const sealdec_groups_t* groups) {
+                     int32_t* o_tok, uint8_t* o_valid, uint64_t* o_lo, uint64_t* o_hi, const sealdec_groups_t* groups) {
     return guarded([&] {
         check_model(m);
         if (!p || !ids || !mask || Q <= 0 || S <= 0) throw ApiError(SEALFM_EINVAL, "null argument / empty batch");
@@ -606,10 +583,10 @@ int sealdec_generate_ex(sealbart_t* m, const sealfm_t* fm, const uint32_t* occ_h
         if (occ_host) CUDA_CHECK(cudaMemcpyAsync(m->in_occ.p, occ_host, (size_t)W * 4, cudaMemcpyHostToDevice, s));
         int32_t errs[4] = {0, 0, 0, 0};
         auto run = [&] {                                       // one pass on the staged inputs
-            return sealdec_generate_dx_ex(m, fm, occ_host ? m->in_occ.as<uint32_t>() : nullptr, p, m->in_ids.as<int64_t>(),
-                                          m->in_mask.as<int64_t>(), Q, S, s, m->hy_score.as<float>(), m->hy_len.as<int32_t>(),
-                                          m->hy_tok.as<int32_t>(), m->hy_valid.as<uint8_t>(), o_lo ? m->hy_lo.as<uint64_t>() : nullptr,
-                                          o_hi ? m->hy_hi.as<uint64_t>() : nullptr, m->err.as<int32_t>(), hint, groups);
+            return sealdec_generate_dx(m, fm, occ_host ? m->in_occ.as<uint32_t>() : nullptr, p, m->in_ids.as<int64_t>(),
+                                       m->in_mask.as<int64_t>(), Q, S, s, m->hy_score.as<float>(), m->hy_len.as<int32_t>(),
+                                       m->hy_tok.as<int32_t>(), m->hy_valid.as<uint8_t>(), o_lo ? m->hy_lo.as<uint64_t>() : nullptr,
+                                       o_hi ? m->hy_hi.as<uint64_t>() : nullptr, m->err.as<int32_t>(), hint, groups);
         };
         if (const int rc = run()) throw ApiError(rc, last_error());
         CUDA_CHECK(cudaMemcpyAsync(errs, m->err.p, 16, cudaMemcpyDeviceToHost, s));
@@ -811,13 +788,8 @@ int debug_topk_threshold(bool cluster, int64_t R, int32_t V, int64_t ld, const f
 extern "C" {
 
 int sealdec_debug_step_logits(sealbart_t* m, const int64_t* ids, const int64_t* mask, int64_t Q, int64_t S, int32_t B,
-                              const int64_t* dec_ids, int64_t t, float* out_logits) {
-    return sealdec_debug_step_logits_ex(m, ids, mask, Q, S, B, dec_ids, t, nullptr, -1, out_logits);
-}
-
-int sealdec_debug_step_logits_ex(sealbart_t* m, const int64_t* ids, const int64_t* mask, int64_t Q, int64_t S, int32_t B,
-                                 const int64_t* dec_ids, int64_t t, const int32_t* anc, int64_t src_tokens_hint,
-                                 float* out_logits) {
+                              const int64_t* dec_ids, int64_t t, const int32_t* anc, int64_t src_tokens_hint,
+                              float* out_logits) {
     return guarded([&] {
         check_model(m);
         if (!ids || !mask || !dec_ids || !out_logits || t < 1 || t > kMaxLen || Q <= 0 || S <= 0 || B < 1)

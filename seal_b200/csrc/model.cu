@@ -9,6 +9,7 @@
 #include <cstring>
 #include <memory>
 #include <string>
+#include <string_view>
 #include <vector>
 
 namespace {
@@ -191,7 +192,7 @@ void check_t5_config(const sealt5_config_t* c) {
     check_gemm_mode(c->gemm_mode);
 }
 
-// sealbart_create and sealbart_create_ex: var == nullptr is bart-large's post-LayerNorm layer
+// var == nullptr is bart-large's post-LayerNorm layer
 void create_bart(const sealbart_config_t* cfg, const sealbart_variant_t* var, int device, sealbart_t** out) {
     if (!cfg || !out) throw ApiError(SEALFM_EINVAL, "null argument");
     if (cfg->d_model % 128 || cfg->d_model > 1024 || cfg->heads * kHeadDim != cfg->d_model)
@@ -325,13 +326,9 @@ int sealt5_create(const sealt5_config_t* cfg, int device, sealbart_t** out) {
     });
 }
 
-int sealbart_create(const sealbart_config_t* cfg, int device, sealbart_t** out) {
-    return guarded([&] { create_bart(cfg, nullptr, device, out); });
-}
-
-int sealbart_create_ex(const sealbart_config_t* cfg, const sealbart_variant_t* variant, int device, sealbart_t** out) {
+int sealbart_create(const sealbart_config_t* cfg, const sealbart_variant_t* variant, int device, sealbart_t** out) {
     return guarded([&] {
-        if (!cfg || !variant || !out) throw ApiError(SEALFM_EINVAL, "null argument");
+        if (!variant) { create_bart(cfg, nullptr, device, out); return; }
         const sealbart_variant_t& v = *variant;
         if (v.activation != SEALBART_ACT_GELU && v.activation != SEALBART_ACT_RELU)
             throw ApiError(SEALFM_EINVAL, "activation must be SEALBART_ACT_GELU or SEALBART_ACT_RELU");
@@ -450,7 +447,7 @@ int sealbart_set_option(sealbart_t* m, const char* name, int64_t value) {
 
 int64_t sealbart_get_stat(const sealbart_t* m, const char* name) {
     if (!m || !name) return -1;
-    const std::string n(name);
+    const std::string_view n(name);                       // compared inline: no std::string operator== joins the exports
     if (n == "last_used_graph") return m->last_used_graph;
     if (n == "overflow_fallbacks") return m->overflow_fallbacks;
     if (n == "gemm_mode") return m->cfg.gemm_mode;
@@ -458,6 +455,7 @@ int64_t sealbart_get_stat(const sealbart_t* m, const char* name) {
     if (n == "fused_head_steps") return m->fused_head_steps;
     if (n == "topk_cluster_steps") return m->topk_cluster_steps;
     if (n == "last_paths") return m->last_paths;
+    if (n == "launches") return m->launches;
     return -1;
 }
 

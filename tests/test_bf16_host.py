@@ -121,7 +121,7 @@ def test_explicit_mode_wins_over_the_dtype(monkeypatch):
         seen.append(args[0]._obj.gemm_mode)
         return -1
 
-    for name in ("sealbart_create", "sealbart_create_ex", "sealt5_create"):
+    for name in ("sealbart_create", "sealt5_create"):
         monkeypatch.setattr(beam_search.lib, name, probe)
     monkeypatch.delenv("SEALB200_GEMM", raising=False)
     small = dict(vocab_size=64, d_model=128, encoder_layers=1, decoder_layers=1, encoder_attention_heads=2,
@@ -163,15 +163,15 @@ def test_engine_cache_sees_in_place_bf16_conversion(monkeypatch):
 # ---- the C ABI --------------------------------------------------------------------------------------------------------
 
 def create_rc(kind, gemm_mode):
-    """sealbart_create / sealbart_create_ex / sealt5_create of a tiny shape; returns (rc, message).  A device-less
-    host answers a valid configuration with SEALFM_ENODEVICE; a GPU host creates (and frees) the model."""
+    """sealbart_create (no variant, or a pre-LayerNorm one) / sealt5_create of a tiny shape; returns (rc, message).  A
+    device-less host answers a valid configuration with SEALFM_ENODEVICE; a GPU host creates (and frees) the model."""
     from seal_b200._lib import BartConfig, BartVariant, T5Config, lib
     h = C.c_void_p()
     if kind == "bart":
-        rc = lib.sealbart_create(C.byref(BartConfig(64, 128, 1, 1, 2, 256, 32, 0, gemm_mode)), 0, C.byref(h))
+        rc = lib.sealbart_create(C.byref(BartConfig(64, 128, 1, 1, 2, 256, 32, 0, gemm_mode)), None, 0, C.byref(h))
     elif kind == "preln":
-        rc = lib.sealbart_create_ex(C.byref(BartConfig(64, 128, 1, 1, 2, 256, 32, 0, gemm_mode)),
-                                    C.byref(BartVariant(1, 0, 0, 1)), 0, C.byref(h))
+        rc = lib.sealbart_create(C.byref(BartConfig(64, 128, 1, 1, 2, 256, 32, 0, gemm_mode)),
+                                 C.byref(BartVariant(1, 0, 0, 1)), 0, C.byref(h))
     else:
         rc = lib.sealt5_create(C.byref(T5Config(64, 128, 1, 1, 2, 64, 256, 1, 32, 128, 1e-6, 1, gemm_mode)), 0, C.byref(h))
     msg = lib.sealfm_last_error().decode()

@@ -114,8 +114,8 @@ def test_penalty_zero_groups_are_copies(tiny):
     assert np.isfinite(rec["scores"]).any()
 
 
-def test_generate_ex_one_group_is_generate(tiny):
-    """sealdec_generate_ex(..., {1, 0}) and sealdec_generate: bit-identical record buffers."""
+def test_generate_null_groups_is_one_group(tiny):
+    """sealdec_generate with groups NULL and with {1, 0}: bit-identical record buffers."""
     import ctypes as C
     from seal_b200._lib import GroupParams, check, lib
     from seal_b200.beam_search import _engine_for, _make_params, _occurring_mask
@@ -132,18 +132,18 @@ def test_generate_ex_one_group_is_generate(tiny):
         idx.to_device(eng.device)
     occ = _occurring_mask(idx, int(eng.config.vocab_size))
 
-    def run(ex):
+    def run(groups):
         out = [np.zeros((Q, H), np.float32), np.zeros((Q, H), np.int32), np.zeros((Q, H, T), np.int32),
                np.zeros((Q, H), np.uint8), np.zeros((Q, H), np.uint64), np.zeros((Q, H), np.uint64)]
         args = [eng._h, idx._dev(), occ.ctypes.data, C.byref(p), ids.ctypes.data, am.ctypes.data, Q, S] + [o.ctypes.data for o in out]
-        check(lib.sealdec_generate_ex(*args, C.byref(GroupParams(1, 0.0))) if ex else lib.sealdec_generate(*args))
+        check(lib.sealdec_generate(*args, groups))
         return out
 
-    for a, b in zip(run(False), run(True)):
+    for a, b in zip(run(None), run(C.byref(GroupParams(1, 0.0)))):
         assert a.tobytes() == b.tobytes()
     with pytest.raises(Exception):
-        check(lib.sealdec_generate_ex(eng._h, idx._dev(), occ.ctypes.data, C.byref(p), ids.ctypes.data, am.ctypes.data,
-                                      Q, S, *([None] * 6), C.byref(GroupParams(4, 0.0))))
+        check(lib.sealdec_generate(eng._h, idx._dev(), occ.ctypes.data, C.byref(p), ids.ctypes.data, am.ctypes.data,
+                                   Q, S, *([None] * 6), C.byref(GroupParams(4, 0.0))))
 
 
 def test_graph_replay_and_key_q20_beam15(tiny):

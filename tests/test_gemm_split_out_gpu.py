@@ -18,7 +18,6 @@ Every case asserts the last_paths bits of the branch it is meant to take, derive
 gemm.cu's split_k_slices derives the slice count; the fp32 outputs are also held to test_gemm_range_gpu.py's float64
 bound (test_bf16_gpu.py's in gemm_mode 6)."""
 import ctypes as C
-import os
 from types import SimpleNamespace
 
 import numpy as np
@@ -40,7 +39,6 @@ ACTS = {0: "none", 1: "gelu", 2: "relu"}
 def sms():
     import torch
     assert torch.cuda.is_available(), "-m gpu tests need a CUDA device"
-    assert "SEALB200_KSLICES" not in os.environ, "the library reads it once per process: the expected paths would not hold"
     return torch.cuda.get_device_properties(0).multi_processor_count
 
 

@@ -1,7 +1,8 @@
-"""GPU: the pre-LayerNorm BART-family forward (sealbart_create_ex: preln_kernels.cuh + BART's attention, GEMM and decode
-kernels) against transformers' Pegasus and mBART, and every entry point SEALSearcher reaches with such a backbone.
+"""GPU: the pre-LayerNorm BART-family forward (sealbart_create with a variant: preln_kernels.cuh + BART's attention,
+GEMM and decode kernels) against transformers' Pegasus and mBART, and every entry point SEALSearcher reaches with such a
+backbone.
 
-  - last-position logits (sealdec_debug_step_logits_ex) against a float64 forward of the same seeded model, with
+  - last-position logits (sealdec_debug_step_logits) against a float64 forward of the same seeded model, with
     test_t5_gpu.py's method: the finiteness pattern, |dlog-prob| <= 1e-4, |dlogit| <= 8 x fp32 HF's own error + 1e-6,
     and the last_paths bits restated from the shapes;
   - fm_index_generate against the decode oracles (flat_ties) on the fp32 HF models, the top-k warp on 96 103 and
@@ -153,7 +154,7 @@ def test_position_table_and_state_dict_keys():
         sd = model.state_dict()
         cfg, var = preln_native_config(model.config, 3)
         h = C.c_void_p()
-        check(lib.sealbart_create_ex(C.byref(cfg), C.byref(var), 0, C.byref(h)))
+        check(lib.sealbart_create(C.byref(cfg), C.byref(var), 0, C.byref(h)))
         try:
             w = np.zeros(128 * 320, dtype=np.float32)
             for bad in bad_keys:
@@ -169,7 +170,7 @@ def test_position_table_and_state_dict_keys():
     cfg, _ = preln_native_config(make_preln("pegasus_relu").config, 3)
     for v in ((1, 1, 0, 0), (1, 0, 2, 0), (1, 0, 0, 2), (2, 0, 0, 0), (0, 0, 0, 0), (0, 2, 1, 1)):
         h = C.c_void_p()
-        assert lib.sealbart_create_ex(C.byref(cfg), C.byref(BartVariant(*v)), 0, C.byref(h)) != 0 and not h.value, v
+        assert lib.sealbart_create(C.byref(cfg), C.byref(BartVariant(*v)), 0, C.byref(h)) != 0 and not h.value, v
 
 
 # ---- decode ---------------------------------------------------------------------------------------------------------

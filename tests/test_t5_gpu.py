@@ -1,7 +1,7 @@
 """GPU: the T5 forward (sealt5_create: t5_kernels.cuh + the shared GEMM, cross-attention and decode kernels) against
 transformers' T5ForConditionalGeneration, and every entry point SEALSearcher reaches with a T5 backbone.
 
-  - last-position logits (sealdec_debug_step_logits_ex) against a float64 forward of the same seeded model, with the
+  - last-position logits (sealdec_debug_step_logits) against a float64 forward of the same seeded model, with the
     method of test_bart_paths_gpu.py: the finiteness pattern, an absolute bound on the log-probs, a bound relative to
     fp32 HF's own error against float64, and the last_paths bits restated from the shapes;
   - fm_index_generate against the decode oracle (oracle/decode_oracle.py and the top-k / group oracles) on the fp32 HF

@@ -18,7 +18,7 @@ cyc = t[6] - t[0]; ns = t[8] - t[7]
 f = cyc / ns if ns > 0 else 1.9                      # cycles per ns
 names = ["prologue", "first operands", "MMA issue", "last chunk done", "tile stored", "exit"]
 d = [(t[i + 1] - t[i]) / f / 1000 for i in range(6)]
-print(f"{M}x{N}x{K} slices={os.environ.get('SEALB200_KSLICES','auto')}: {us.value:.2f} us/launch(+finish); CTA0 total {ns/1000:.2f} us @ {f:.2f} GHz: "
+print(f"{M}x{N}x{K}: {us.value:.2f} us/launch(+finish); CTA0 total {ns/1000:.2f} us @ {f:.2f} GHz: "
       + ", ".join(f"{n} {x:.2f}" for n, x in zip(names, d)))
 sub = [t[4]] + t[9:17]
 print("   epilogue passes (staged, stored) us:", " ".join(f"{(sub[i + 1] - sub[i]) / f / 1000:.2f}" for i in range(8)))
